@@ -3,7 +3,7 @@
 #   make            -> dump1090_b200/libmodes_b200.so + dump1090-b200 (C host)
 #   make oracle     -> oracle/_build/libmodes_oracle.so (+ oracle/_ref when /root/reference exists)
 NVCC      ?= /usr/local/cuda/bin/nvcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := $(ARCH) -O3 -lineinfo -std=c++17 -Iinclude -Xcompiler -fPIC,-Wall,-Wextra
 CSRC      := dump1090_b200/csrc
 LIB       := dump1090_b200/libmodes_b200.so

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — Msamples/s of the Mode S decode hot path on B200 (see DESIGN.md "Measurement").
+"""bench.py — Msamples/s of the Mode S decode hot path on H100 (see DESIGN.md "Measurement").
 
-    python bench.py --gpus N --steps K --warmup W            # this framework (CUDA, sm_100a)
+    python bench.py --gpus N --steps K --warmup W            # this framework (CUDA, sm_90a)
     python bench.py --impl reference --gpus N --steps K ...   # the reference's CPU path, all host cores
     python bench.py --workload df17_aggressive|tiled_64g|snr_sweep ...   # BASELINE.json configs[2..4]
     python bench.py --workload receivers --receivers 256               # SURVEY 8(f) item 4: many receivers, one GPU
@@ -16,7 +16,8 @@ r-th GiB of the tiled stream.  A step = one pass of the hot path over the rank's
           host: H2D, kernels, D2H of the records over the rank's own PCIe link, and the sequential
           half resolved by every rank for its own shard (sharded.resolve_distributed: only 4 KiB
           address caches travel between ranks); wall clock between barriers, max over ranks.
-One JSON line on stdout (rank 0).
+One JSON line on stdout (rank 0).  --dump-outputs DIR also writes what the timed paths computed in
+their last step as DIR/<name>.npy (see dump_outputs).
 """
 from __future__ import annotations
 
@@ -55,10 +56,10 @@ WORKLOADS = {
 
 
 def load_capture() -> tuple[np.ndarray, str]:
-    """The reference's sample capture if it travelled with the repo, else a synthetic stand-in."""
-    for p in (ROOT / "oracle" / "_ref" / "modes1.bin", Path("/root/reference/testfiles/modes1.bin")):
-        if p.exists():
-            return np.fromfile(p, dtype=np.uint8), "modes1.bin tiled"
+    """The reference's sample capture if `make oracle` copied it into oracle/_ref, else a synthetic stand-in."""
+    p = ROOT / "oracle" / "_ref" / "modes1.bin"
+    if p.exists():
+        return np.fromfile(p, dtype=np.uint8), "modes1.bin tiled"
     from dump1090_b200 import synth
     return synth.random_traffic(356868, 560, seed=1), "synthetic traffic (modes1.bin absent) tiled"
 
@@ -82,7 +83,7 @@ def workload_source(name: str):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons while the timed regions run (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons while the timed regions run (read-only queries)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -123,7 +124,7 @@ def base_config(name: str, world: int) -> dict:
     w = WORKLOADS[name]
     return {"workload": w["desc"], "flags": w["flags"], "samples_per_gpu_step": w["nbytes"] // 2,
             "samples_per_step": world * (w["nbytes"] // 2),
-            "l2_policy": "a step's input (>= 1 GiB per GPU) is larger than the 126 MB L2 (and than the host's last-level "
+            "l2_policy": "a step's input (>= 1 GiB per GPU) is larger than the 50 MB L2 (and than the host's last-level "
                          "cache for the CPU arm); no explicit flush"}
 
 
@@ -183,7 +184,7 @@ def run_reference(args) -> None:
     import checker
     name = args.workload
     if name == "receivers":
-        print(json.dumps({"impl": "reference", "unavailable": "the reference serves one receiver per process: its rate per core is the tiled_nofix figure of this arm (147 Msamples/s = 73 receivers per core)"}))
+        print(json.dumps({"impl": "reference", "unavailable": "the reference serves one receiver per process: its rate per core is the tiled_nofix figure of this arm (2 Msamples/s per receiver)"}))
         return
     if name == "snr_sweep":
         print(json.dumps({"impl": "reference", "unavailable": "snr_sweep compares detect rates; run --workload snr_sweep on the GPU arm, which times the oracle alongside"}))
@@ -256,22 +257,6 @@ def scan_source_digest() -> str:
     return h.hexdigest()[:16]
 
 
-def measured_traffic() -> tuple[float | None, str]:
-    """DRAM bytes per scan-kernel launch from the committed ncu capture — only if it was taken with
-    the scan kernel that is running now: profiles/scan_kernel_traffic.json records the digest of the
-    kernel's sources + compiler flags (and the digest of the .so it was captured with)."""
-    tp = ROOT / "profiles" / "scan_kernel_traffic.json"
-    if not tp.exists():
-        return None, "no capture committed"
-    doc = json.loads(tp.read_text())
-    if doc.get("so_sha256_16") == so_digest():
-        return doc.get("dram_bytes_per_launch"), "profiles/scan_kernel_traffic.json (same library file)"
-    if doc.get("scan_source_sha256_16") == scan_source_digest():
-        return doc.get("dram_bytes_per_launch"), "profiles/scan_kernel_traffic.json (same scan-kernel sources and flags)"
-    return None, (f"capture is of another scan kernel (sources {doc.get('scan_source_sha256_16')} != {scan_source_digest()}): "
-                  "re-run scripts/ncu_traffic.sh")
-
-
 def messages_digest(arr, n: int) -> str:
     """sha256 over (sample_pos, msgbits, msg) of the first n messages of a ctypes Message array."""
     h = hashlib.sha256()
@@ -280,6 +265,47 @@ def messages_digest(arr, n: int) -> str:
     h.update(np.ascontiguousarray(a[:, 16:24]).tobytes())                 # msgbits, msgtype
     h.update(np.ascontiguousarray(a[:, 192:200]).tobytes())               # sample_pos
     return h.hexdigest()
+
+
+DUMP_SAMPLE_ROWS = 65536           # rows kept of a longer output: a fixed, seeded sample (~40 MB in all, cap 64 MB)
+
+
+def _sample_rows(n: int) -> np.ndarray:
+    if n <= DUMP_SAMPLE_ROWS:
+        return np.arange(n)
+    return np.sort(np.random.default_rng(0).choice(n, size=DUMP_SAMPLE_ROWS, replace=False))
+
+
+def dump_outputs(out_dir: Path, cands: np.ndarray, tiles: np.ndarray, msgs, n_msgs: int) -> None:
+    """What the timed paths computed in their last step, as float32/float64 .npy files:
+    device path (rank 0's last device batch): the candidate records in stream order (tile by tile) and
+    the candidates per tile; e2e path: the delivered messages.  Longer arrays are sampled by _sample_rows."""
+    out_dir.mkdir(parents=True, exist_ok=True)
+    order = np.concatenate([np.arange(o, o + c) for o, c in tiles] or [np.zeros(0, int)]).astype(np.int64)
+    rec = cands[order]
+    ci = _sample_rows(rec.size)
+    p = rec["p"][ci]                                         # (rows, 2 attempts)
+    arrays = {
+        "candidate_count": np.array([rec.size], dtype=np.float64),
+        "tile_candidate_count": tiles["count"].astype(np.float32),
+        "candidate_row": ci.astype(np.float64),
+        "candidate_t": rec["t"][ci].astype(np.float64),
+        "candidate_msg": p["msg"].astype(np.float32),
+        "candidate_fields": np.stack([p[k].astype(np.float32) for k in ("msgtype", "flags", "errorbit", "nfixed", "crc")], -1),
+    }
+    raw = np.frombuffer(msgs, dtype=np.uint8, count=n_msgs * 200).reshape(n_msgs, 200)
+    mi = _sample_rows(n_msgs)
+    m = raw[mi]
+    i32 = m[:, 16:200 - 8].copy().view("<i4")                 # msgbits .. pad2 (int32 fields, flight bytes among them)
+    arrays.update({
+        "message_count": np.array([n_msgs], dtype=np.float64),
+        "message_row": mi.astype(np.float64),
+        "message_sample_pos": m[:, 192:200].copy().view("<i8")[:, 0].astype(np.float64),
+        "message_msg": m[:, :14].astype(np.float32),
+        "message_words": i32.astype(np.float64),
+    })
+    for name, a in arrays.items():
+        np.save(out_dir / f"{name}.npy", a)
 
 
 def run_ours(args) -> None:
@@ -385,6 +411,7 @@ def run_ours(args) -> None:
     launches = dec.launch_count() - l0
     ktimes = dec.kernel_times_ms()                  # per batch: scan, eval, both, batches
     n_cand = dec.detect_wait()
+    last_records = dec.detect_fetch(bbuf) if args.dump_outputs and rank == 0 else None
     dev_ms, slow_rank = allmax(dev_ms_rank)
     scan_max, scan_rank = allmax(ktimes[0] * nbatch)
     eval_max, eval_rank = allmax(ktimes[1] * nbatch)
@@ -602,6 +629,8 @@ def run_ours(args) -> None:
         dist.all_reduce(t)
         e2e_msgs = int(t.item())
     e2e_value = world * samples_per_gpu * e2e_steps / e2e_s / 1e6
+    if last_records is not None:
+        dump_outputs(Path(args.dump_outputs), *last_records, out_arr, (dec2 if world == 1 else resolver).output_count())
     d2h = n_cand * 56 * (nbytes // (bbuf * api.BUFFER_BYTES)) + api.tiles_for(nbuf) * 8 + 16
 
     clocks = sampler.stop() if rank == 0 else None
@@ -611,13 +640,11 @@ def run_ours(args) -> None:
         if peaks_path.exists():
             peak, peak_src = float(json.loads(peaks_path.read_text())["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (measured)"
         else:
-            peak, peak_src = 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+            peak, peak_src = 3350.0, "fallback 3.35 TB/s (H100 SXM data sheet, not measured)"
         scan_ms = ktimes[0]                                   # per launch (= per device batch) on rank 0
         alg_bytes = 2 * (bbuf * api.BUFFER_SAMPLES)
         achieved = alg_bytes / (scan_ms * 1e-3) / 1e9 if scan_ms > 0 else 0.0
-        traffic, traffic_src = measured_traffic()
-        if traffic is not None and nbatch > 1:
-            traffic, traffic_src = None, "capture is of the 1 GiB launch"
+        traffic, traffic_src = None, "not measured (DRAM counters need a profiler capture)"
 
         cpu_baseline = None
         if world == 1 and name != "tiled_64g":
@@ -885,7 +912,13 @@ def main():
     ap.add_argument("--receivers", type=int, default=256, help="receivers: independent streams, one buffer of each per step")
     ap.add_argument("--frames", type=int, default=10000, help="snr_sweep: frames per SNR point (whole job)")
     ap.add_argument("--gpu-resolve", type=int, default=0, help="N=1 e2e: 1 = the order-dependent half on the GPU too (modes_config.gpu_resolve)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed paths computed in their last step to DIR/<name>.npy: the last device "
+                         "batch's candidate records (of two per step for tiled_64g) and the e2e step's messages, a "
+                         "fixed sample of each when long; not for snr_sweep, receivers or --impl reference")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.workload in ("snr_sweep", "receivers")):
+        ap.error("--dump-outputs applies to the device workloads of this framework: " + ", ".join(WORKLOADS))
     if args.impl == "reference":
         run_reference(args)
     elif args.workload == "snr_sweep":

@@ -3,7 +3,7 @@
 Mirrors the reference's main-loop contract (dump1090.c:2968-2990): a `Decoder`
 is fed raw u8 I/Q bytes and hands back, in stream order, the messages the
 reference would pass to useModesMessage() (dump1090.c:1802).  Everything that
-computes runs in libmodes_b200.so (CUDA, sm_100a).  There is no CPU fallback:
+computes runs in libmodes_b200.so (CUDA, sm_90a).  There is no CPU fallback:
 constructing a Decoder without a usable GPU raises.
 """
 from __future__ import annotations

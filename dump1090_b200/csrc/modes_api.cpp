@@ -61,7 +61,7 @@ struct Slot {
 
 struct modes_ctx {
     modes_config cfg;
-    int sm_count = 148;
+    int sm_count = 132;
     uint16_t *d_lutn = nullptr;
     uint16_t *d_lut_iq = nullptr;
     uint32_t *d_bit_syn = nullptr;
@@ -544,7 +544,8 @@ static int create_impl(modes_ctx *ctx) {
     CK(nullptr, cudaSetDevice(ctx->cfg.device));
     cudaDeviceProp prop;
     CK(nullptr, cudaGetDeviceProperties(&prop, ctx->cfg.device));
-    if (prop.major < 10) return fail(nullptr, "device %d is sm_%d%d; kernels are built for sm_100a only", ctx->cfg.device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)          // sm_90a code runs on compute capability 9.0 only
+        return fail(nullptr, "device %d is sm_%d%d; kernels are built for sm_90a only", ctx->cfg.device, prop.major, prop.minor);
     ctx->sm_count = prop.multiProcessorCount;
     ctx->scratch = scratch_create();
     if (!ctx->scratch) return fail(nullptr, "out of memory");

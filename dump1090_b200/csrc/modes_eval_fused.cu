@@ -1,4 +1,4 @@
-// modes_eval_fused.cu — K2, frame evaluation as ONE walk per candidate (sm_100a).
+// modes_eval_fused.cu — K2, frame evaluation as ONE walk per candidate (sm_90a).
 //
 // Replaces the body of detectModeS after the preamble test (dump1090.c:1653-1735) and the
 // order-independent half of decodeModesMessage (:1099-1128), like eval_serial_kernel
@@ -298,8 +298,8 @@ void launch_fused(const BatchView &in, const DeviceTables &tab, const ScanOutput
 
 void launch_eval_fused(const BatchView &in, const DeviceTables &tab, const ScanOutputs &scan, modes_candidate *records,
                        int fix_errors, int aggressive, int sm_count, int parts, cudaStream_t stream) {
-    // measured on the bench's 845 458 candidates: whole windows, 12 warps per SM 0.166 ms; half windows, 16 warps
-    // 0.170 ms (20 warps: 0.195 ms, the register limit spills; 85 + 29 slots, 16 warps: 0.183 ms)
+    // measured on an H100 (400 W) over the bench's 845 458 candidates: whole windows, 12 warps per SM 0.293 ms;
+    // half windows, 16 warps 0.321 ms
     if (parts == 2) launch_fused<2, 16>(in, tab, scan, records, fix_errors, aggressive, sm_count, stream);
     else launch_fused<4, 12>(in, tab, scan, records, fix_errors, aggressive, sm_count, stream);
 }

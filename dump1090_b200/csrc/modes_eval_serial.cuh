@@ -613,7 +613,7 @@ struct Sweep {
 // or (-1, -1); a tie is -2^14 <= U < 0 either way.  No shift, no clamp, and the serial chain from
 // one decision to the next is multiply-add, multiply-add, multiply-add, compare, select.
 //
-// Pipes.  An sm_100 scheduler's integer ALU pipe and FMA pipe each take a warp instruction every
+// Pipes.  An sm_90 scheduler's integer ALU pipe and FMA pipe each take a warp instruction every
 // second cycle; the walk is ALU-heavy by nature (funnel shifts, byte permutes, absolute
 // differences), so every addition that can be a multiply-add with a register multiplier is one:
 // per pair 10 ALU + 10 FMA + 3 load instructions.

@@ -1,4 +1,4 @@
-// modes_kernels.cu — sm_100a kernels of the Mode S demodulator.
+// modes_kernels.cu — sm_90a kernels of the Mode S demodulator.
 //
 //   (K1, the fused magnitude + preamble scan, lives in modes_scan2.cu.)
 //   eval_kernel   (K2)  one warp per candidate: bit slicing (dump1090.c:1668-1706),
@@ -647,7 +647,7 @@ void launch_magnitude(const uint8_t *d_iq, uint16_t *d_mag, uint64_t n_samples, 
                       cudaStream_t stream) {
     if (!n_samples) return;
     uint64_t blocks = (n_samples + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     magnitude_kernel<<<(uint32_t)blocks, 256, 0, stream>>>(d_iq, d_mag, n_samples, lutn);
 }
 

@@ -3,8 +3,8 @@
 //
 // One dump1090 process serves one RTL-SDR: rtlsdrCallback (dump1090.c:442-456) hands it 131072
 // samples at a time, each buffer is prefixed with the last 238 samples of the previous one (:481),
-// and detectModeS keeps its ICAO address cache, skip state and statistics for that one stream.  A
-// B200 decodes ~12 000 such 2 MHz streams in real time (the limit is the PCIe link), but a single
+// and detectModeS keeps its ICAO address cache, skip state and statistics for that one stream.
+// A GPU decodes far more than one such 2 MHz stream in real time (the limit is the PCIe link), but a single
 // stream only fills it with seconds of data at a time.  The pool takes ONE buffer from each of many
 // receivers and decodes them in one batch, with everything per stream kept per receiver.
 //

@@ -1,4 +1,4 @@
-// modes_scan2.cu — K1, the fused magnitude + preamble scan kernel (sm_100a).
+// modes_scan2.cu — K1, the fused magnitude + preamble scan kernel (sm_90a).
 //
 // Replaces computeMagnitudeVector (dump1090.c:1454-1469) and the per-position tests of
 // detectModeS (dump1090.c:1602-1650).  HBM-bound by design: 2 bytes read per sample, nothing

@@ -13,7 +13,7 @@
 // on n.  n is held as 15-bit fields, two per register (n = 32768 clamps to 32767, which no other
 // sample reaches: 32767 = 3 mod 4 is not a sum of two squares).
 //
-// Pipe balance.  An sm_100 scheduler issues one instruction per cycle, but the integer ALU pipe
+// Pipe balance.  An sm_90 scheduler issues one instruction per cycle, but the integer ALU pipe
 // and the FMA pipe each take a warp instruction every second cycle: the loop only runs at the
 // issue rate if its instructions split evenly between the two.  The packed comparison
 // "L + 0x7fff - R has bit 15 set <=> L > R" is therefore written as a multiply-add with operands

@@ -1,4 +1,4 @@
-/* dump1090-b200 — C host for the B200 demodulator: the --ifile side of
+/* dump1090-b200 — C host for the H100 demodulator: the --ifile side of
  * dump1090's command line (dump1090.c:2849-3010) over the C ABI of
  * include/modes_b200.h.  Reads 8-bit unsigned I/Q at 2 MHz from a file (or '-'
  * for stdin), feeds it to the device library, prints what the reference prints.

@@ -1,4 +1,4 @@
-/* modes_b200.h — C ABI of the B200-native Mode S / ADS-B demodulator.
+/* modes_b200.h — C ABI of the H100-native Mode S / ADS-B demodulator.
  *
  * Drop-in boundary for dump1090's --ifile decode path.  The reference has no
  * plugin/FFI surface; the seam is its main loop (dump1090.c:2968-2990):

@@ -38,9 +38,10 @@ def histogram(ins, lo, hi):
 
 
 k1 = sass("modes_scan2.o")
+(ROOT / "profiles").mkdir(exist_ok=True)
 lo, hi, n = next(x for x in loops(k1) if x[2] > 500)
 head = (f"# scan_kernel, the row-pair loop: {n} SASS instructions in the loop body (the slow path of the first/last tile\n"
-        f"# included; 64 positions per lane and trip on the fast path).  sm_100a, nvcc 12.9.\n# opcodes: {histogram(k1, lo, hi)}\n")
+        f"# included; 64 positions per lane and trip on the fast path).  sm_90a, nvcc 12.9.\n# opcodes: {histogram(k1, lo, hi)}\n")
 (ROOT / "profiles" / f"{tag}_sass_k1_row_loop.txt").write_text(head + "\n".join(l for a, _, l in k1 if lo <= a <= hi) + "\n")
 
 # the default frame-evaluation kernel: eval_fused_kernel<4, 12>, the 28-pair block of the walk
@@ -56,7 +57,7 @@ for l in txt.splitlines():
         ins.append((int(m.group(1), 16), m.group(2).strip(), re.sub(r"\s+/\* 0x[0-9a-f]+ \*/$", "", l)))
 lo, hi, n = next(x for x in loops(ins) if 500 < x[2] < 1000)
 head = (f"# eval_fused_kernel<4, 12> (the default frame evaluation), one block of the walk = 28 sample pairs, both attempts\n"
-        f"# (dump1090.c:1667-1690 and :1498-1558): {n} instructions = {n / 28:.1f} per bit.  sm_100a, nvcc 12.9.\n"
+        f"# (dump1090.c:1667-1690 and :1498-1558): {n} instructions = {n / 28:.1f} per bit.  sm_90a, nvcc 12.9.\n"
         f"# opcodes: {histogram(ins, lo, hi)}\n")
 (ROOT / "profiles" / f"{tag}_sass_k2_walk_block.txt").write_text(head + "\n".join(l for a, _, l in ins if lo <= a <= hi) + "\n")
 print("written", tag)

@@ -2,14 +2,18 @@
 
 TEST INFRASTRUCTURE.  Only tests/, __graft_entry__.smoke() and bench.py's CPU
 baseline legs import this.  `libref` (the unmodified reference compiled into
-oracle/_ref/libref.so) exists only where `make -C oracle ref` ran with
-/root/reference present; the prebuilt file travels to the GPU box.
+oracle/_ref/libref.so) exists only where `make oracle` found the reference's
+sources; tests that need it are skipped elsewhere.
 """
 from __future__ import annotations
 
+import atexit
 import ctypes
+import lzma
 import os
+import shutil
 import subprocess
+import tempfile
 from pathlib import Path
 
 import numpy as np
@@ -18,7 +22,7 @@ ROOT = Path(__file__).resolve().parent.parent
 ORACLE_DIR = ROOT / "oracle"
 REF_SO = ORACLE_DIR / "_ref" / "libref.so"
 ORACLE_SO = ORACLE_DIR / "_build" / "libmodes_oracle.so"
-REFERENCE_ROOT = Path("/root/reference")
+MODES1_XZ = Path(__file__).resolve().parent / "golden" / "modes1_head.bin.xz"
 
 _I32 = ("errorbit aa1 aa2 aa3 phase_corrected ca iid metype mesub heading_is_valid heading "
         "aircraft_type fflag tflag raw_latitude raw_longitude").split()
@@ -96,10 +100,8 @@ def msg_fields(m: Msg, with_pos: bool = False) -> dict:
 
 
 def build_oracle() -> None:
-    """Compile the CPU restatement (and, where the reference is mounted, oracle/_ref)."""
-    subprocess.run(["make", "-C", str(ORACLE_DIR)], check=True, capture_output=True)
-    if REFERENCE_ROOT.exists():
-        subprocess.run(["make", "-C", str(ORACLE_DIR), "ref"], check=True, capture_output=True)
+    """Compile the CPU restatement (and, where the reference's sources are found, oracle/_ref)."""
+    subprocess.run(["make", "-C", str(ROOT), "oracle"], check=True, capture_output=True)
 
 
 _libs = {}
@@ -114,7 +116,7 @@ def _load(path: Path):
 
 
 def have_ref() -> bool:
-    return REF_SO.exists() or REFERENCE_ROOT.exists()
+    return REF_SO.exists()
 
 
 def oracle_lib():
@@ -200,17 +202,26 @@ def ref_time_phases(data, fix=1, aggressive=0, check_crc=1, loops=1):
     return float(out[0]), float(out[1])
 
 
-def modes1_path() -> Path:
-    """The reference's sample capture (testfiles/modes1.bin).  `make -C oracle ref`
-    copies it to oracle/_ref/ (git-ignored, shipped to the GPU box)."""
-    for p in (ORACLE_DIR / "_ref" / "modes1.bin", REFERENCE_ROOT / "testfiles" / "modes1.bin"):
-        if p.exists():
-            return p
-    raise FileNotFoundError("modes1.bin not found: run `make -C oracle ref` where /root/reference is mounted")
+_modes1 = {}
 
 
 def modes1() -> np.ndarray:
-    return np.fromfile(modes1_path(), dtype=np.uint8)
+    """The first 327 680 bytes (1.25 reference buffers) of the reference's sample capture
+    testfiles/modes1.bin, stored in tests/golden/."""
+    if "data" not in _modes1:
+        _modes1["data"] = np.frombuffer(lzma.decompress(MODES1_XZ.read_bytes()), dtype=np.uint8)
+    return _modes1["data"].copy()
+
+
+def modes1_path() -> Path:
+    """modes1() as a file (for --ifile), written once per process to a temporary directory."""
+    if "path" not in _modes1:
+        d = tempfile.mkdtemp(prefix="modes1_")
+        atexit.register(shutil.rmtree, d, ignore_errors=True)
+        p = Path(d) / "modes1_head.bin"
+        modes1().tofile(p)
+        _modes1["path"] = p
+    return _modes1["path"]
 
 
 # ---- tracker door of the reference harness (SURVEY.md 8(f) item 3) -----------------------------

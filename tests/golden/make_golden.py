@@ -1,11 +1,11 @@
 """Generate tests/golden/*.json.gz from the UNMODIFIED reference (oracle/_ref/libref.so).
 
-Run where /root/reference is mounted:   python tests/golden/make_golden.py
+Run where `make oracle` built oracle/_ref:   python tests/golden/make_golden.py
 
 For every (input, flags) case the reference's delivered messages are stored as
 the --raw lines plus the struct modesMessage fields the reference assigns for
-that DF (checker.defined_fields), and the eight statistics counters.  Inputs
-are not stored: modes1.bin is located by checker.modes1_path(); synthetic
+that DF (checker.defined_fields), and the eight statistics counters.  The one
+stored input is the head of modes1.bin (checker.modes1()); synthetic
 streams are regenerated from (generator, arguments, seed) by
 dump1090_b200.synth, whose output is deterministic, and their sha256 is
 recorded so drift is detected.

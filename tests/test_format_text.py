@@ -11,7 +11,7 @@ import checker as C
 from dump1090_b200 import api, synth
 
 REF_BIN = C.ORACLE_DIR / "_ref" / "ref_dump1090"
-needs_ref_bin = pytest.mark.skipif(not (REF_BIN.exists() or C.REFERENCE_ROOT.exists()), reason="oracle/_ref not built")
+needs_ref_bin = pytest.mark.skipif(not REF_BIN.exists(), reason="oracle/_ref not built")
 
 
 def _product_text(data, fix=1, aggressive=0, check_crc=1):

@@ -132,4 +132,4 @@ def test_chunked_feed_is_invariant(gpu_decoder_factory, checker_libs):
     whole = [m.raw_line() for m in dec.decode(data)]
     for chunk in (1000, 262144, 300001):
         assert [m.raw_line() for m in dec.decode(data, chunk=chunk)] == whole
-    assert len(whole) == 284
+    assert len(whole) == 147

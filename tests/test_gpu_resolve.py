@@ -60,7 +60,7 @@ def test_device_resolve_cache_crosses_batches(batch_buffers, gpu_decoder_factory
 
 
 def test_device_resolve_full_size_equals_host_resolve(gpu_decoder_factory, checker_libs):
-    """BASELINE.json configs[1] size: the 425 744 messages of the tiled capture, device resolve vs host resolve."""
+    """BASELINE.json configs[1] size: the 481 691 messages of the tiled capture, device resolve vs host resolve."""
     data = synth.tile_to(C.modes1(), 1 << 30)
     digests = []
     for gpu in (0, 1):
@@ -71,5 +71,5 @@ def test_device_resolve_full_size_equals_host_resolve(gpu_decoder_factory, check
         a = np.frombuffer(out, dtype=np.uint8, count=n * 200).reshape(n, 200)
         digests.append((n, hashlib.sha256(a.tobytes()).hexdigest(), dec.stats()))
         dec.set_output_array(0)
-    assert digests[0][0] == 425744
+    assert digests[0][0] == 481691
     assert digests[0] == digests[1]

@@ -12,13 +12,13 @@ from dump1090_b200 import synth
 FLAG_SETS = [dict(), dict(aggressive=1), dict(fix=0), dict(check_crc=0), dict(check_crc=0, aggressive=1),
              dict(drop_eof=1), dict(fix=0, drop_eof=1), dict(check_crc=0, aggressive=1, drop_eof=1)]
 
-# SURVEY.md §4 / BASELINE.md §2: line count and md5 of the --raw output of the reference on modes1.bin
+# line count and md5 of the --raw output of the reference on checker.modes1() (the stored head of modes1.bin)
 MODES1_PINS = {
-    (): (284, "4a81758c8bec"), (("drop_eof", 1),): (217, "7b1719f22374"),
-    (("aggressive", 1),): (284, "4a81758c8bec"), (("fix", 0),): (283, "ac539444a66e"),
-    (("drop_eof", 1), ("fix", 0)): (217, "a76c3fc95b9a"), (("check_crc", 0),): (765, "a6092d178fcf"),
-    (("aggressive", 1), ("check_crc", 0)): (824, "bec25488d6b8"),
-    (("aggressive", 1), ("check_crc", 0), ("drop_eof", 1)): (629, "16e26b0aa79f"),
+    (): (147, "f23b14fbd58d"), (("drop_eof", 1),): (119, "896cf3d1da7e"),
+    (("aggressive", 1),): (147, "f23b14fbd58d"), (("fix", 0),): (147, "a8c3b59364d7"),
+    (("drop_eof", 1), ("fix", 0)): (119, "896cf3d1da7e"), (("check_crc", 0),): (359, "5c32e315e805"),
+    (("aggressive", 1), ("check_crc", 0)): (385, "5c0d8b9ab062"),
+    (("aggressive", 1), ("check_crc", 0), ("drop_eof", 1)): (308, "412617cf2a6d"),
 }
 
 
@@ -30,7 +30,7 @@ def _fields(msgs):
     return [C.msg_fields(m) for m in msgs]
 
 
-needs_ref = pytest.mark.skipif(not C.have_ref(), reason="oracle/_ref not built and /root/reference absent")
+needs_ref = pytest.mark.skipif(not C.have_ref(), reason="oracle/_ref not built")
 
 
 @pytest.mark.parametrize("kw", FLAG_SETS, ids=str)
@@ -42,16 +42,16 @@ def test_oracle_modes1_pins(kw, checker_libs):
 
 
 def test_oracle_modes1_stats_pins(checker_libs):
-    # SURVEY.md §4 stat counters (single-bit fixes are double counted by the reference: 8 -> 16)
+    # the reference's stat counters (single-bit fixes are double counted by the reference: 2 -> 4)
     _, st = C.oracle_decode(C.modes1())
-    assert st == [546, 282, 535, 276, 259, 8, 16, 0]
+    assert st == [261, 125, 256, 145, 111, 2, 4, 0]
     _, st = C.oracle_decode(C.modes1(), fix=0)
-    assert st[:5] == [546, 287, 535, 283, 252]
+    assert st[:5] == [261, 126, 256, 147, 109]
     msgs, _ = C.oracle_decode(C.modes1())
     hist = {}
     for m in msgs:
         hist[m.msgtype] = hist.get(m.msgtype, 0) + 1
-    assert hist == {0: 10, 4: 4, 5: 10, 11: 82, 17: 159, 20: 13, 21: 6}
+    assert hist == {0: 9, 4: 2, 5: 4, 11: 43, 17: 79, 20: 7, 21: 3}
 
 
 @needs_ref
@@ -85,10 +85,10 @@ def test_oracle_equals_golden(name, cid, checker_libs):
 
 
 def test_magnitude_pins(checker_libs):
-    # SURVEY.md §4 kernel-level pins for modes1.bin
+    # kernel-level pins for checker.modes1()
     m = C.oracle_magnitude(C.modes1())
-    assert m.size == 356868 and int(m.astype(np.int64).sum()) == 1732288336 and int(m.max()) == 64913
-    assert hashlib.sha256(m.astype("<u2").tobytes()).hexdigest().startswith("f116ccd64c38ad15")
+    assert m.size == 163840 and int(m.astype(np.int64).sum()) == 938262314 and int(m.max()) == 64913
+    assert hashlib.sha256(m.astype("<u2").tobytes()).hexdigest().startswith("c8afd162f16f9d3f")
 
 
 @needs_ref
@@ -102,14 +102,14 @@ def test_magnitude_equals_reference(checker_libs):
 
 
 def test_candidate_pins(checker_libs):
-    # SURVEY.md §4: positions passing all preamble tests, every j, no skip
+    # positions passing all preamble tests, every j, no skip
     cands = C.oracle_scan_candidates(C.modes1())
     t = np.array([c.t for c in cands], dtype=np.int64)
     per_buffer = [int(((t >> 17) == k).sum()) for k in range(3)]
-    assert per_buffer == [215, 212, 135]
+    assert per_buffer == [215, 52, 0]
     pos = t - 238
     assert pos[:5].tolist() == [794, 1918, 2552, 4196, 4235]
-    assert hashlib.sha256(pos.astype("<i8").tobytes()).hexdigest().startswith("20d38768f8bae2fe")
+    assert hashlib.sha256(pos.astype("<i8").tobytes()).hexdigest().startswith("63573bbb8af89e26")
 
 
 def test_known_answer_frames(checker_libs):

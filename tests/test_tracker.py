@@ -1,9 +1,15 @@
 """SURVEY.md §8(f) item 3: the aircraft tracker (modes_tracker_*, pure host code) against the
 reference's own interactiveReceiveData / decodeCPR / decodeCPRSurface / modesSendSBSOutput /
 aircraftsToJson, driven message by message with the same explicit clock.  Positions are compared
-bit for bit (doubles), text byte for byte."""
+bit for bit (doubles), text byte for byte.  The reference's answers are replayed from
+tests/golden/tracker_ref.tape.gz (gzipped JSON); `MODES_RECORD_REFERENCE=1 python -m pytest tests/test_tracker.py`
+records them anew from oracle/_ref (built by `make oracle` where the reference's sources are found)."""
 import ctypes
+import gzip
+import json
 import math
+import os
+from pathlib import Path
 
 import numpy as np
 import pytest
@@ -12,11 +18,88 @@ import checker as C
 from dump1090_b200 import api, synth
 
 
+TAPE = Path(__file__).resolve().parent / "golden" / "tracker_ref.tape.gz"
+RECORD = os.environ.get("MODES_RECORD_REFERENCE") == "1"
+_tapes = {}
+
+
+class _Aircraft(tuple):
+    """A recorded struct aircraft: as_tuple() and the position fields the tests read."""
+    def as_tuple(self):
+        return tuple(self)
+
+    addr = property(lambda self: self[0])
+    lat = property(lambda self: self[12])
+    lon = property(lambda self: self[13])
+
+
+def _enc(v):
+    if hasattr(v, "as_tuple"):
+        return {"a": [x.decode("latin1") if isinstance(x, bytes) else x for x in v.as_tuple()]}
+    if isinstance(v, (list, tuple)):
+        return [_enc(x) for x in v]
+    return v
+
+
+def _dec(v):
+    if isinstance(v, dict):
+        return _Aircraft(x.encode("latin1") if i in (1, 2) else x for i, x in enumerate(v["a"]))
+    if isinstance(v, list):
+        return tuple(_dec(x) for x in v)
+    return v
+
+
+class _Reference:
+    """The reference's tracker door: its answers in call order, from the tape (or, recording, from oracle/_ref)."""
+
+    def __init__(self, name):
+        self.name, self.k = name, 0
+        if RECORD:
+            _tapes[name] = []
+        else:
+            if not _tapes:
+                with gzip.open(TAPE, "rb") as f:
+                    _tapes.update(json.loads(f.read().decode()))
+            self.tape = _tapes[name]
+
+    def _ask(self, call):
+        if RECORD:
+            v = call()
+            _tapes[self.name].append(_enc(v))
+            return v
+        self.k += 1
+        return _dec(self.tape[self.k - 1])
+
+    def tracker(self, check_crc=1):
+        ref, ask = (C.RefTracker(check_crc) if RECORD else None), self._ask
+
+        class T:
+            update = staticmethod(lambda m, now: ask(lambda: ref.update(m, now)))
+            aircraft = staticmethod(lambda: list(ask(lambda: ref.aircraft())))
+            reference = staticmethod(lambda: ask(lambda: ref.reference()))
+            json = staticmethod(lambda metric=0: ask(lambda: ref.json(metric)))
+            expire = staticmethod(lambda now, ttl: ask(lambda: ref.expire(now, ttl)))
+            table = staticmethod(lambda now, metric, rows: ask(lambda: C.ref_track_table(now, metric, rows)))
+        return T
+
+    def cpr_nl(self, lat):
+        return self._ask(lambda: C.ref_cpr_nl(lat))
+
+
+@pytest.fixture
+def reference(request):
+    yield _Reference(request.node.name)
+    if RECORD:
+        with gzip.GzipFile(TAPE, "wb", mtime=0) as f:
+            f.write(json.dumps(_tapes, sort_keys=True, separators=(",", ":")).encode())
+
+
 def _decode_frame(frame: bytes) -> C.Msg:
-    """decodeModesMessage on raw bytes through the reference (fresh ICAO cache)."""
+    """decodeModesMessage on raw bytes (fresh ICAO cache), through the oracle's restatement
+    (test_oracle.py::test_decode_bytes_matches_reference pins it to the reference)."""
     out = C.Msg()
     buf = (ctypes.c_uint8 * 14)(*(list(frame) + [0] * (14 - len(frame))))
-    C.ref_lib().ref_decode_bytes(buf, 1, 0, ctypes.byref(out))
+    C.oracle_lib().oracle_decode_bytes(buf, 1, 0, ctypes.byref(out))
     return out
 
 
@@ -26,9 +109,9 @@ def _as_product(m) -> api.Message:
     return p
 
 
-def _run_both(messages, times, check_crc=1):
+def _run_both(reference, messages, times, check_crc=1):
     """Feed both trackers; compare aircraft state and SBS line after every message."""
-    ref, got = C.RefTracker(check_crc), api.Tracker(check_crc)
+    ref, got = reference.tracker(check_crc), api.Tracker(check_crc)
     tracked = 0
     for k, (m, t) in enumerate(zip(messages, times)):
         r = ref.update(m, t)
@@ -45,11 +128,11 @@ def _run_both(messages, times, check_crc=1):
         assert got.json(metric) == ref.json(metric)
         for rows in (3, 15, 100):
             now = times[-1] + 4321 * (rows + metric)
-            assert got.table(now, metric, rows) == C.ref_track_table(now, metric, rows)
+            assert got.table(now, metric, rows) == ref.table(now, metric, rows)
     return ref, got, tracked
 
 
-def test_nl_function_matches_reference(checker_libs):
+def test_nl_function_matches_reference(checker_libs, reference):
     """The zone-count table is generated from its defining formula: identical to the reference's
     literal table everywhere, including one ulp either side of every transition latitude."""
     nz = 15.0
@@ -60,17 +143,17 @@ def test_nl_function_matches_reference(checker_libs):
         for d in (t, np.nextafter(t, 0), np.nextafter(t, 100), t - 1e-9, t + 1e-9):
             lats += [float(d), -float(d)]
     for lat in lats:
-        assert api.cpr_nl(lat) == C.ref_cpr_nl(lat), lat
+        assert api.cpr_nl(lat) == reference.cpr_nl(lat), lat
 
 
-def test_tracker_on_decoded_traffic(checker_libs):
+def test_tracker_on_decoded_traffic(checker_libs, reference):
     """Everything the decoder delivers from a mixed-traffic stream (identification, airborne and
     surface positions with random CPR fields, velocities, address/parity replies)."""
     data = synth.random_traffic(131072 * 12, 2600, 41, n_aircraft=25)
     for check_crc in (1, 0):
         msgs, _ = C.oracle_decode(data, check_crc=check_crc)
         times = [1_700_000_000_000 + 37 * k for k in range(len(msgs))]          # ~27 messages per second
-        _, _, tracked = _run_both(msgs, times, check_crc)
+        _, _, tracked = _run_both(reference, msgs, times, check_crc)
         assert tracked > 300
 
 
@@ -90,7 +173,7 @@ def _position_frame(icao, tc, odd, yz, xz, alt12=0x3A5):
     return synth.make_frame(17, 5, icao.to_bytes(3, "big") + bits.to_bytes(7, "big"))
 
 
-def test_tracker_decodes_real_positions(checker_libs):
+def test_tracker_decodes_real_positions(checker_libs, reference):
     """Aircraft flying real tracks: even/odd pairs decode to the encoded position (to CPR
     resolution), the reference position follows, surface frames decode against it — and every
     double equals the reference's."""
@@ -116,7 +199,7 @@ def test_tracker_decodes_real_positions(checker_libs):
                 t += 50
         if step == 30:
             t += 11_000                                                   # a gap longer than the 10 s pairing window
-    ref, got, tracked = _run_both(msgs, times)
+    ref, got, tracked = _run_both(reference, msgs, times)
     assert tracked == len(msgs)
     # sanity of the test itself: the airborne fleet ends up where it was flown to
     by_addr = {a.addr: a for a in got.aircraft()}
@@ -127,10 +210,10 @@ def test_tracker_decodes_real_positions(checker_libs):
     assert got.reference()[2] > 100
 
 
-def test_tracker_expiry_and_order(checker_libs):
+def test_tracker_expiry_and_order(checker_libs, reference):
     msgs = [_decode_frame(synth.make_frame(17, 5, (0x400000 + i).to_bytes(3, "big") + bytes([0x20, 0x10, 0x82, 0x0C, 0x30, 0xC3, 0x0C])))
             for i in range(20)]
-    ref, got = C.RefTracker(), api.Tracker()
+    ref, got = reference.tracker(), api.Tracker()
     t0 = 1_700_000_000_000
     for k, m in enumerate(msgs):
         ref.update(m, t0 + 1000 * k)
@@ -142,14 +225,14 @@ def test_tracker_expiry_and_order(checker_libs):
     assert got.aircraft() == []
 
 
-def test_tracker_ignores_bad_crc_when_checking(checker_libs):
+def test_tracker_ignores_bad_crc_when_checking(checker_libs, reference):
     bad = _decode_frame(bytes.fromhex("8D4840D6202CC371C32CE0576099"))       # last byte off: CRC fails, not fixable to DF17? either way
     bad.crcok = 0
-    assert api.Tracker(1).update(_as_product(bad), 1) is None and C.RefTracker(1).update(bad, 1) is None
-    assert api.Tracker(0).update(_as_product(bad), 1) is not None and C.RefTracker(0).update(bad, 1) is not None
+    assert api.Tracker(1).update(_as_product(bad), 1) is None and reference.tracker(1).update(bad, 1) is None
+    assert api.Tracker(0).update(_as_product(bad), 1) is not None and reference.tracker(0).update(bad, 1) is not None
 
 
-def test_stream_clock_starts_at_the_epoch(checker_libs):
+def test_stream_clock_starts_at_the_epoch(checker_libs, reference):
     """A file's stream clock (sample position / 2 MHz) starts at 0: fed to the tracker as is, the
     first airborne position of a new aircraft would be paired with the empty (time 0) slot of the
     other parity and decoded against zeros.  With MODES_STREAM_EPOCH_MS added — what the C host
@@ -161,7 +244,7 @@ def test_stream_clock_starts_at_the_epoch(checker_libs):
         frames.append(_decode_frame(_position_frame(icao, 11, odd, yz, xz)))
     stream_ms = [3, 450, 900]                                            # first seconds of a file
     # reference behaviour under its own (wall) clock: no position after one frame, a position after two
-    ref, got = C.RefTracker(), api.Tracker()
+    ref, got = reference.tracker(), api.Tracker()
     for m, t in zip(frames, stream_ms):
         r = ref.update(m, 1_700_000_000_000 + t)
         g = got.update(_as_product(m), api.STREAM_EPOCH_MS + t)
