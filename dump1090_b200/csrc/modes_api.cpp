@@ -247,10 +247,12 @@ int gpu_resolve_ensure(modes_ctx *ctx, Slot &s) {
         CK(ctx, cudaMalloc(&s.gr.stats_out, 8 * sizeof(uint64_t)));
         CK(ctx, cudaMallocHost(&s.h_gr_flags, (20 + 1024) * sizeof(uint32_t)));
     }
-    if (s.gr.capacity < s.cand_cap) {                     // at most two deliveries per candidate; one per candidate is 2x the dense capture
+    // at most two deliveries per candidate (check_crc = 0 delivers a failed first attempt and its
+    // retry), so the deliveries fit whenever the candidates do
+    if (s.gr.capacity < 2 * s.cand_cap) {
         cudaFree(s.gr.out); s.gr.out = nullptr; s.gr.capacity = 0;
-        CK(ctx, cudaMalloc(&s.gr.out, (size_t)s.cand_cap * sizeof(modes_delivery)));
-        s.gr.capacity = s.cand_cap;
+        CK(ctx, cudaMalloc(&s.gr.out, 2 * (size_t)s.cand_cap * sizeof(modes_delivery)));
+        s.gr.capacity = 2 * s.cand_cap;
     }
     return 0;
 }
@@ -318,7 +320,7 @@ int launch_batch(modes_ctx *ctx, Slot &s) {
         launch_gpu_resolve(s.gr, s.out_records, s.out_tiles, tiles_for(n_samples), (uint32_t)s.n_buffers, ctx->cfg.check_crc,
                            ctx->sm_count, s.stream);
         CK(ctx, cudaGetLastError());
-        ctx->launches += 3 + 2 * kGpuResolveRounds;
+        ctx->launches += 4 + 2 * kGpuResolveRounds;
         CK(ctx, cudaEventRecord(ctx->ev_resolved, s.stream));
         ctx->resolved_pending = true;
         CK(ctx, cudaMemcpyAsync(s.h_gr_flags, s.gr.flags, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
@@ -370,7 +372,8 @@ int collect(modes_ctx *ctx, Slot &s) {
     if (ctx->cfg.gpu_resolve) {
         // the verdicts were taken on the device: fetch the deliveries, build the structs
         if (s.h_counters[1] || s.h_counters[0] > s.out_cap) return fail(ctx, "gpu_resolve: candidate capacity exceeded (%u found)", s.h_counters[0]);
-        if (s.h_gr_flags[0]) return fail(ctx, "gpu_resolve: address caches did not settle in %d rounds", kGpuResolveRounds);
+        // internal check: the in-order fallback leaves every buffer's cache as the hand-over computes it
+        if (s.h_gr_flags[0]) return fail(ctx, "gpu_resolve: internal error: address caches did not settle after the in-order replay");
         if (s.h_gr_flags[1]) return fail(ctx, "gpu_resolve: delivery capacity exceeded (%u messages)", s.h_gr_flags[2]);
         const size_t nd = s.h_gr_flags[2];
         if (s.h_deliveries_cap < nd) {

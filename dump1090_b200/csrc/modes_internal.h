@@ -86,13 +86,15 @@ bool build_pair_hash(const uint32_t *bit_syn, uint32_t *out /*[kPairHashSlots]*/
 // extra = DF11 interrogator id, or the address recovered from an address/parity field.
 struct modes_delivery { int64_t t; modes_frame_eval eval; uint32_t extra; uint32_t bits; };
 static_assert(sizeof(modes_delivery) == 40, "delivery record layout");
-constexpr int kGpuResolveRounds = 4;                 // replay + hand-over rounds before the emit pass (two suffice on real traffic)
+// Replay + hand-over rounds before the in-order fallback (which then does nothing) and the emit pass.
+// Two suffice on real traffic; a chain through the address cache over n buffers needs about n.
+constexpr int kGpuResolveRounds = 4;
 
 struct GpuResolve {
     uint32_t *start, *end;       // [n_buffers][1024] address cache at the start / end of each buffer
     uint32_t *written, *readfirst;   // [n_buffers][32]  slots a buffer wrote / read before writing
     uint32_t *rerun, *n_deliv, *offsets;   // [n_buffers] (+1 for offsets)
-    uint32_t *flags;             // [0] a buffer still needed another replay, [1] delivery capacity exceeded, [2] deliveries
+    uint32_t *flags;             // [0] a buffer still needed another replay (0 after the fallback), [1] delivery capacity exceeded, [2] deliveries
     const uint32_t *cache_in;    // [1024] cache at the start of the batch
     uint32_t *cache_out;         // [1024] cache at its end
     uint64_t *stats_out;         // [8]

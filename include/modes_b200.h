@@ -65,8 +65,10 @@ typedef struct modes_config {
                                    statistics: dump1090.c:1769-1791, :898-983) is replayed on the host over the
                                    candidate records.  1: it runs on the GPU too — one warp per reference buffer,
                                    address caches handed from buffer to buffer and verified (SURVEY.md §8(f) item
-                                   4) — and only 40-byte records of the delivered messages cross PCIe; the host
-                                   builds the struct fields.  Same messages, same statistics.  Streaming decode
+                                   4); a batch whose caches do not settle in a few rounds is replayed in stream
+                                   order on the device — and only 40-byte records of the delivered messages cross
+                                   PCIe; the host builds the struct fields.  Same messages, same statistics, on
+                                   any input within the density below (all flags included).  Streaming decode
                                    on one GPU only; a batch denser than one candidate per 64 samples is an error
                                    in this mode. */
 } modes_config;

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 import checker as C
+import streams as S
 from dump1090_b200 import api, synth
 
 pytestmark = pytest.mark.gpu
@@ -232,6 +233,15 @@ def test_pathological_density(name, pattern, gpu_decoder_factory, checker_libs):
     order = np.concatenate([np.arange(o, o + c) for o, c in tiles]).astype(int)
     assert order.size == want_arr.size
     assert np.array_equal(cands.view(np.uint8).reshape(-1, 56)[order], want_arr.view(np.uint8).reshape(-1, 56))
+    # the device resolve cannot repeat a batch with larger buffers: beyond the documented density (one
+    # candidate per 64 samples) it is an error, never a shortened list
+    gdec = gpu_decoder_factory(check_crc=0, gpu_resolve=1)
+    if want_arr.size > nbuf * api.BUFFER_SAMPLES // 64:
+        with pytest.raises(RuntimeError, match="candidate capacity exceeded"):
+            gdec.decode(data)
+    else:
+        assert [m.raw_line() for m in gdec.decode(data)] == [m.hexline() for m in exp]
+        assert list(gdec.stats().values()) == st
 
 
 def test_caller_buffers_overflow_is_reported(gpu_decoder_factory):
@@ -246,12 +256,15 @@ def test_caller_buffers_overflow_is_reported(gpu_decoder_factory):
         dec.detect_wait()
 
 
-@pytest.mark.parametrize("n_gpus,batch_buffers", [(2, 1), (3, 2), (2, 256)])
-def test_multi_gpu_context(n_gpus, batch_buffers, gpu_decoder_factory, checker_libs):
+@pytest.mark.parametrize("n_gpus,batch_buffers,name",
+                         [pytest.param(n, b, name, id=f"{n}-{b}" if name == "traffic" else f"{n}-{b}-{name}")
+                          for name in ["traffic"] + list(S.CHAINS) for n, b in [(2, 1), (3, 2), (2, 256)]])
+def test_multi_gpu_context(n_gpus, batch_buffers, name, gpu_decoder_factory, checker_libs):
     """modes_config.n_gpus > 1: the streaming decode deals its batches to several GPUs (devices are
     reused round-robin when the box has fewer) and resolves each group of batches exactly; messages,
-    fields and statistics equal the oracle's, whatever the batch size and the feeding pattern."""
-    data = synth.random_traffic(131072 * 11 + 4321, 2400, 91, n_aircraft=18)
+    fields and statistics equal the oracle's, whatever the batch size and the feeding pattern, also
+    on chains through the address cache (tests/streams.address_chain)."""
+    data = synth.random_traffic(131072 * 11 + 4321, 2400, 91, n_aircraft=18) if name == "traffic" else S.chain(name)
     for kw in (dict(), dict(aggressive=1, check_crc=0)):
         exp, st = C.oracle_decode(data, aggressive=kw.get("aggressive", 0), check_crc=kw.get("check_crc", 1), cap=100000)
         dec = gpu_decoder_factory(n_gpus=n_gpus, max_batch_bytes=batch_buffers * api.BUFFER_BYTES, **kw)

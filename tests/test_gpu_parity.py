@@ -32,6 +32,7 @@ def _streams():
     for seed in (1, 2, 3):
         yield f"traffic{seed}", synth.random_traffic(300000, 400, seed)
     yield "grid", synth.df17_grid(280000, 700, 5)
+    yield from S.chain_streams()                                       # chains through the address cache
 
 
 def _nasty_streams():

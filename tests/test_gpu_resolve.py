@@ -28,6 +28,10 @@ def _streams():
     yield "grid", synth.df17_grid(280000, 700, 5)
     yield "ties", S.tie_rich(11)
     yield "retry_at_j0", S.retry_at_buffer_start()
+    # a preamble every 60 samples: within the documented density, but with check_crc = 0 nearly every
+    # candidate delivers both attempts
+    yield "dense_ties", S.tie_rich(21, n_frames=17800, levels=(0, 40, 100), period=60)
+    yield from S.chain_streams()
 
 
 STREAMS = dict(_streams())
@@ -45,16 +49,31 @@ def test_device_resolve_matches_oracle(name, kw, gpu_decoder_factory, checker_li
     assert list(dec.stats().values()) == exp_stats
 
 
-@pytest.mark.parametrize("batch_buffers", [1, 3, 64])
-def test_device_resolve_cache_crosses_batches(batch_buffers, gpu_decoder_factory, checker_libs):
+def _batch_cases():
+    """(batch buffers, stream), named by the batch size (0: the default) and the stream unless it is
+    the traffic stream."""
+    for name in ["traffic"] + list(S.CHAINS):
+        for b in (1, 3, 8, 64, 0):
+            bid = str(b) if b else "default"
+            yield pytest.param(b, name, id=bid if name == "traffic" else f"{bid}-{name}")
+
+
+@pytest.mark.parametrize("batch_buffers,name", list(_batch_cases()))
+def test_device_resolve_cache_crosses_batches(batch_buffers, name, gpu_decoder_factory, checker_libs):
     """Small batches: an address announced in one batch validates address/parity replies in later
-    ones — the cache is handed from batch to batch on the device, across the two pipeline slots."""
-    data = synth.random_traffic(131072 * 21 + 999, 5000, 13, n_aircraft=25)
+    ones — the cache is handed from batch to batch on the device, across the two pipeline slots.
+    The chains (tests/streams.address_chain) also run through whole batches longer than the fixed
+    rounds of guessing (batch_buffers >= 8, the default size)."""
+    if name == "traffic":
+        data = synth.random_traffic(131072 * 21 + 999, 5000, 13, n_aircraft=25)
+    else:
+        data = STREAMS[name]
     exp, st = C.oracle_decode(data, cap=100000)
-    assert any(m.msgtype in (0, 4, 5, 16, 20, 21) for m in exp)
+    assert any(m.msgtype in (0, 4, 5, 16, 20, 21) for m in exp) or name == "chain_df11_iid"
     dec = gpu_decoder_factory(gpu_resolve=1, max_batch_bytes=batch_buffers * api.BUFFER_BYTES)
     for chunk in (None, 300001):
         got = dec.decode(data, chunk=chunk)
+        assert [m.raw_line() for m in got] == [m.hexline() for m in exp]
         assert [C.msg_fields(m, with_pos=True) for m in got] == [C.msg_fields(m, with_pos=True) for m in exp]
         assert list(dec.stats().values()) == st
 

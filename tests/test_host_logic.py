@@ -9,6 +9,7 @@ import pytest
 
 import checker as C
 import golden_util as G
+import streams as S
 from dump1090_b200 import api, synth
 
 ROOT = Path(__file__).resolve().parent.parent
@@ -103,10 +104,12 @@ def test_synth_parity_against_known_frames():
         assert synth.make_frame(17, b[0] & 7, b[1:11]) == b
 
 
-@pytest.mark.parametrize("nshards", [2, 3, 8])
-def test_parallel_shard_resolve_is_exact(nshards, checker_libs):
-    """modes_resolver_run_shards (speculative ICAO cache at shard boundaries, verified) == sequential."""
-    data = synth.random_traffic(131072 * 9 + 4000, 1400, 23, n_aircraft=40)
+@pytest.mark.parametrize("nshards,name", [pytest.param(n, "traffic", id=str(n)) for n in (2, 3, 8)]
+                         + [pytest.param(n, name, id=f"{n}-{name}") for name in S.CHAINS for n in (2, 3, 8)])
+def test_parallel_shard_resolve_is_exact(nshards, name, checker_libs):
+    """modes_resolver_run_shards (speculative ICAO cache at shard boundaries, verified) == sequential,
+    also on chains through the address cache where every shard's guess depends on the previous one."""
+    data = synth.random_traffic(131072 * 9 + 4000, 1400, 23, n_aircraft=40) if name == "traffic" else S.chain(name)
     cands = C.oracle_scan_candidates(data, aggressive=1)
     arr = np.frombuffer(b"".join(bytes(c) for c in cands), dtype=api.CANDIDATE_DTYPE)
     seq = api.Resolver(aggressive=1)

@@ -7,6 +7,7 @@ import pytest
 
 import checker as C
 import golden_util as G
+import streams as S
 from dump1090_b200 import synth
 
 FLAG_SETS = [dict(), dict(aggressive=1), dict(fix=0), dict(check_crc=0), dict(check_crc=0, aggressive=1),
@@ -72,6 +73,23 @@ def test_oracle_equals_reference_synthetic(seed, kw, checker_libs):
     o, os_ = C.oracle_decode(data, **kw)
     assert _fields(r) == _fields(o)
     assert rs == os_
+
+
+@pytest.mark.parametrize("kind", S.CHAIN_KINDS)
+@pytest.mark.parametrize("n_buffers", [1, 4, 9])
+def test_address_chain_pattern(kind, n_buffers, checker_libs):
+    """tests/streams.address_chain proves what it claims: one message per buffer, alternately the
+    writer and the reader, each at its position and with its address; and the reference agrees."""
+    data, want = S.address_chain(n_buffers, kind, return_expected=True)
+    msgs, st = C.oracle_decode(data)
+    assert [(m.sample_pos, m.msgtype, (m.aa1 << 16) | (m.aa2 << 8) | m.aa3) for m in msgs] == want
+    assert all(m.crcok for m in msgs)
+    if kind == "df11_iid":
+        assert all(m.iid for m in msgs[1::2])                              # validated through the cache, not by its parity
+    if C.have_ref():
+        r, rs = C.ref_decode(data)
+        assert _fields(r) == _fields(msgs)
+        assert rs == st
 
 
 @pytest.mark.parametrize("name,cid", G.CASES)

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 import checker as C
+import streams as S
 from dump1090_b200 import api, synth
 
 BUF = api.BUFFER_BYTES
@@ -19,6 +20,22 @@ def _streams(n_rx, n_buf):
     out = []
     for r in range(n_rx):
         s = synth.random_traffic(n_buf * 131072, 120 * n_buf + 37 * r, seed=100 + r)
+        assert s.size == n_buf * BUF
+        out.append(s)
+    return out
+
+
+def _chain_streams(n_rx, n_buf):
+    """n_rx streams of n_buf whole buffers, each a chain through the address cache
+    (streams.address_chain) of its own kind, length and phase: receiver r is silent for r % 3
+    buffers, then runs a chain of the remaining buffers.  A cache shared or lost between batches
+    breaks the chain."""
+    out = []
+    for r in range(n_rx):
+        phase = r % 3
+        kind = S.CHAIN_KINDS[r % len(S.CHAIN_KINDS)]
+        quiet = synth.synth_stream(phase * 131072, [], sigma=1.0, seed=50 + r)
+        s = np.concatenate([quiet, S.address_chain(n_buf - phase, kind, seed=r + 1)])
         assert s.size == n_buf * BUF
         out.append(s)
     return out
@@ -55,11 +72,18 @@ def _check(pool, streams, kw):
         assert list(pool.stats(r).values()) == stats, f"receiver {r}"
 
 
-@pytest.mark.parametrize("kw", [dict(), dict(aggressive=1), dict(fix=0), dict(check_crc=0)],
-                         ids=lambda k: "-".join(f"{a}{b}" for a, b in k.items()) or "default")
-def test_pool_resolve_matches_single_stream_decodes(kw, checker_libs):
-    n_rx, n_buf = 5, 3
-    streams = _streams(n_rx, n_buf)
+def _pool_cases():
+    """(flags, stream mix), named by the flags for ordinary traffic and flags-chains for chains."""
+    for mix in ("traffic", "chains"):
+        for kw in (dict(), dict(aggressive=1), dict(fix=0), dict(check_crc=0)):
+            kid = "-".join(f"{a}{b}" for a, b in kw.items()) or "default"
+            yield pytest.param(kw, mix, id=kid if mix == "traffic" else f"{kid}-{mix}")
+
+
+@pytest.mark.parametrize("kw,mix", list(_pool_cases()))
+def test_pool_resolve_matches_single_stream_decodes(kw, mix, checker_libs):
+    n_rx, n_buf = (5, 3) if mix == "traffic" else (5, 8)
+    streams = _streams(n_rx, n_buf) if mix == "traffic" else _chain_streams(n_rx, n_buf)
     cfg = dict(fix_errors=kw.get("fix", 1), aggressive=kw.get("aggressive", 0), check_crc=kw.get("check_crc", 1))
     nxt = [0] * n_rx
     with api.ReceiverPool(n_rx, **cfg) as pool:
@@ -127,11 +151,12 @@ def test_pool_rejects_bad_calls(checker_libs):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("kw", [dict(), dict(aggressive=1), dict(fix=0)],
+@pytest.mark.parametrize("kw", [dict(), dict(aggressive=1), dict(fix=0), dict(check_crc=0)],
                          ids=lambda k: "-".join(f"{a}{b}" for a, b in k.items()) or "default")
 def test_pool_ingest_matches_single_stream_decodes(kw, checker_libs):
     n_rx, n_buf = 7, 3
     streams = _streams(n_rx, n_buf)
+    streams[-1] = _chain_streams(1, n_buf)[0]                           # a receiver whose cache carries a chain
     cfg = dict(fix_errors=kw.get("fix", 1), aggressive=kw.get("aggressive", 0), check_crc=kw.get("check_crc", 1))
     nxt = [0] * n_rx
     with api.ReceiverPool(n_rx, max_batch=5, **cfg) as pool:

@@ -46,18 +46,40 @@ def _streams():
     yield "grid", synth.df17_grid(280000, 700, 5)
     yield "ties", S.tie_rich(11)
     yield "retry_at_j0", S.retry_at_buffer_start()
+    yield from S.chain_streams()
 
 
 STREAMS = dict(_streams())
+_scans = {}
 
 
-@pytest.mark.parametrize("name", list(STREAMS))
-@pytest.mark.parametrize("kw", [dict(), dict(aggressive=1), dict(check_crc=0), dict(check_crc=0, aggressive=1), dict(fix=0)],
-                         ids=lambda k: "-".join(f"{a}{b}" for a, b in k.items()) or "default")
-def test_buffer_parallel_resolve_equals_sequential(name, kw, shim):
+def _candidates(name, fix, aggressive):
+    key = (name, fix, aggressive)
+    if key not in _scans:
+        _scans[key] = C.oracle_scan_candidates(STREAMS[name], fix=fix, aggressive=aggressive, cap=400000)
+    return _scans[key]
+
+
+FLAG_SETS = [dict(), dict(aggressive=1), dict(check_crc=0), dict(check_crc=0, aggressive=1), dict(fix=0)]
+
+
+def _cases():
+    """(flags, stream, max_rounds), named flags-stream for the rounds-until-settled runs and
+    flags-stream-roundsN for the device's schedule."""
+    for max_rounds in (0, 1, 2, 4):
+        for name in STREAMS:
+            for kw in FLAG_SETS:
+                kid = "-".join(f"{a}{b}" for a, b in kw.items()) or "default"
+                yield pytest.param(kw, name, max_rounds, id=f"{kid}-{name}" + (f"-rounds{max_rounds}" if max_rounds else ""))
+
+
+@pytest.mark.parametrize("kw,name,max_rounds", list(_cases()))
+def test_buffer_parallel_resolve_equals_sequential(kw, name, max_rounds, shim):
+    """max_rounds = 0: guess and verify until nothing changes; 1, 2, 4: the device's schedule, that
+    many rounds and then, if the caches are still changing, one replay in stream order."""
     data = STREAMS[name]
     nbuf = data.size // api.BUFFER_BYTES + 1
-    cands = C.oracle_scan_candidates(data, fix=kw.get("fix", 1), aggressive=kw.get("aggressive", 0), cap=400000)
+    cands = _candidates(name, kw.get("fix", 1), kw.get("aggressive", 0))
     arr = np.frombuffer(b"".join(bytes(c) for c in cands), dtype=api.CANDIDATE_DTYPE).copy()
     tiles = _tiled(arr, nbuf)
     # the rule: the product's sequential host resolver
@@ -69,11 +91,13 @@ def test_buffer_parallel_resolve_equals_sequential(name, kw, shim):
     stats = (ctypes.c_int64 * 8)()
     start = np.zeros(1024, dtype=np.uint32)
     end = np.zeros(1024, dtype=np.uint32)
-    rounds = ctypes.c_int(0)
+    rounds, fallback = ctypes.c_int(0), ctypes.c_int(0)
     n = shim.shim_resolve_buffers(arr.ctypes.data_as(ctypes.c_void_p), tiles.ctypes.data_as(ctypes.c_void_p),
                                   ctypes.c_size_t(tiles.size), ctypes.c_size_t(nbuf), int(kw.get("check_crc", 1)),
                                   start.ctypes.data_as(ctypes.c_void_p), out, ctypes.c_size_t(cap), stats,
-                                  end.ctypes.data_as(ctypes.c_void_p), ctypes.byref(rounds), api.TILE_SAMPLES)
+                                  end.ctypes.data_as(ctypes.c_void_p), ctypes.byref(rounds), api.TILE_SAMPLES,
+                                  max_rounds, ctypes.byref(fallback))
+    assert n >= 0, "did not settle" if n == -2 else "the hand-over after the in-order replay found a wrong cache"
     assert n == len(want)
     assert list(stats) == list(seq.stats().values())
     by_t = {int(c.t): c for c in cands}
@@ -87,3 +111,11 @@ def test_buffer_parallel_resolve_equals_sequential(name, kw, shim):
             assert d.extra == m.iid
     assert np.array_equal(end, seq.get_cache())
     assert 1 <= rounds.value <= nbuf
+    if max_rounds:
+        assert rounds.value <= max_rounds
+        if name.startswith("chain_"):
+            assert fallback.value                                         # the in-order replay was taken, and exact
+    else:
+        assert not fallback.value
+        if name.startswith("chain_") and nbuf > 8:
+            assert rounds.value > 4                                       # the chain defeats the device's fixed rounds

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 import checker as C
+import streams as S
 from dump1090_b200 import api, synth
 
 
@@ -56,11 +57,19 @@ def sequential(monkeypatch):
     return run
 
 
-@pytest.mark.parametrize("parts,part_tiles", [(2, 1), (3, 7), (5, 1), (16, 1), (64, 1)])
+@pytest.mark.parametrize("name,parts,part_tiles",
+                         [pytest.param("traffic", p, t, id=f"{p}-{t}") for p, t in [(2, 1), (3, 7), (5, 1), (16, 1), (64, 1)]]
+                         + [pytest.param(name, p, 1, id=f"{name}-{p}-1") for name in S.CHAINS for p in (2, 3, 16)])
 @pytest.mark.parametrize("flags", [dict(), dict(aggressive=1), dict(fix_errors=0), dict(check_crc=0)])
-def test_parts_equal_the_sequential_pass(parts, part_tiles, flags, checker_libs, monkeypatch, sequential):
-    nbuf = 9
-    data = synth.random_traffic(131072 * nbuf + 4000, 1500, 31, n_aircraft=40)
+def test_parts_equal_the_sequential_pass(name, parts, part_tiles, flags, checker_libs, monkeypatch, sequential):
+    """Random traffic, and chains through the address cache (tests/streams.address_chain) whose
+    every buffer decides what the next one reads: a guess is wrong part after part."""
+    if name == "traffic":
+        nbuf = 9
+        data = synth.random_traffic(131072 * nbuf + 4000, 1500, 31, n_aircraft=40)
+    else:
+        nbuf = S.CHAINS[name][1]
+        data = S.chain(name)
     arr = records_of(data, fix=flags.get("fix_errors", 1), aggressive=flags.get("aggressive", 0))
     arr, tiles = tiled(arr, nbuf + 1, scatter_seed=parts)
     more = records_of(synth.random_traffic(300000, 300, 32, n_aircraft=40), fix=flags.get("fix_errors", 1),
@@ -80,7 +89,7 @@ def test_parts_equal_the_sequential_pass(parts, part_tiles, flags, checker_libs,
     monkeypatch.setenv("MODES_RESOLVE_PARTS", str(parts))
     monkeypatch.setenv("MODES_RESOLVE_PART_TILES", str(part_tiles))
     got = both_calls()
-    assert got[0] == want[0] and len(got[0]) > 500
+    assert got[0] == want[0] and len(got[0]) >= (500 if name == "traffic" else nbuf)
     assert got[1] == want[1]
     assert np.array_equal(got[2], want[2])
     assert got[3] == want[3] and got[4] == want[4]

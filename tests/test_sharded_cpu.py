@@ -13,6 +13,7 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 import checker as C
+import streams as S
 from dump1090_b200 import api, sharded, synth
 
 
@@ -101,6 +102,9 @@ def _dist_worker(rank, world, port, kind, q):
         if kind.startswith("wrong_guess"):
             data = _wrong_guess_stream(24)
             total_buffers = 24
+        elif kind.startswith("chain"):
+            data = S.chain(kind)
+            total_buffers = data.size // api.BUFFER_BYTES + 1
         else:
             data = synth.random_traffic(131072 * 9 + 5000, 1500, 77, n_aircraft=20)
             total_buffers = data.size // api.BUFFER_BYTES + 1
@@ -134,11 +138,13 @@ def _dist_worker(rank, world, port, kind, q):
         dist.destroy_process_group()
 
 
-@pytest.mark.parametrize("world,kind", [(2, "traffic"), (3, "traffic"), (2, "wrong_guess"), (3, "traffic_shm"), (2, "wrong_guess_shm")])
+@pytest.mark.parametrize("world,kind", [(2, "traffic"), (3, "traffic"), (2, "wrong_guess"), (3, "traffic_shm"), (2, "wrong_guess_shm"),
+                                        (2, "chain_evict"), (3, "chain_df4")])
 def test_every_rank_resolves_its_own_shard(world, kind, checker_libs):
     """sharded.resolve_distributed over gloo: ranks exchange 4 KiB address caches only, never records,
     and the concatenation of their messages is exactly the sequential decode — also when the first
-    guess of a shard's starting cache is wrong (then a second round is needed, and taken)."""
+    guess of a shard's starting cache is wrong (then a second round is needed, and taken), and on a
+    chain through the address cache where every shard's outcome depends on the previous shard's."""
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
     port = _free_port()
