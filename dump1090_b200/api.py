@@ -160,6 +160,7 @@ def lib():
         L.modes_resolver_output_count.restype = C.c_size_t
         L.modes_resolver_output_count.argtypes = [C.c_void_p]
         L.modes_decode_frame.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(Message)]
+        L.modes_decode_frames.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
         L.modes_format_message.restype = C.c_size_t
         L.modes_format_message.argtypes = [C.POINTER(Message), C.c_int, C.c_char_p, C.c_size_t]
         L.modes_format_raw_net.restype = C.c_size_t
@@ -425,8 +426,16 @@ class Decoder:
         self._check(lib().modes_decode_frame(self._h, buf, C.byref(m)))
         return m
 
-    def decode_frames(self, frames) -> list:
-        """A batch of frames (each padded to 14 bytes) through the hex door in one launch."""
+    def decode_frames(self, frames):
+        """A batch of frames (each padded to 14 bytes) through the hex door in one launch, the
+        address cache carried from frame to frame.  A list of frames gives a list of Message; an
+        (n, 14) uint8 array is passed as it is and gives the ctypes array of n Message (view it
+        with np.frombuffer), without a Python object per byte or per frame."""
+        if isinstance(frames, np.ndarray):
+            a = np.ascontiguousarray(frames, dtype=np.uint8).reshape(-1, 14)
+            out = (Message * a.shape[0])()
+            self._check(lib().modes_decode_frames(self._h, _ptr(a), a.shape[0], out))
+            return out
         n = len(frames)
         buf = (C.c_uint8 * (14 * n))(*[b for f in frames for b in (list(f) + [0] * (14 - len(f)))])
         out = (Message * n)()

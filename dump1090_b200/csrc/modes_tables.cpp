@@ -11,7 +11,8 @@
 //   fix_hash open-addressed inverse of bit_syn over positions 5..111, the domain
 //            of the reference's bitErrorTable (dump1090.c:806)
 //   pair_hash open-addressed map from the syndrome of TWO flipped bits p < q (positions 5..111,
-//            5671 patterns, all syndromes distinct: dump1090.c:817-841) to p; q follows from
+//            5671 patterns, all syndromes distinct and none equal to a single's: dump1090.c:817-841,
+//            checked here) to p; q follows from
 //            fix_hash(S ^ bit_syn[p]).  One or two probes replace a 107-step search per frame.
 #include <cmath>
 #include <cstring>
@@ -61,6 +62,10 @@ bool build_pair_hash(const uint32_t *bit_syn, uint32_t *out) {
         for (int q = p + 1; q < 112; q++) {
             const uint32_t s = bit_syn[p] ^ bit_syn[q];
             if (s == 0 || s >= (1u << 24)) return false;
+            // nor may a pair share a single's syndrome: the kernels go on to this table when the
+            // single-bit hit lies outside a short frame, where the reference stops at the single
+            for (int r = 5; r < 112; r++)
+                if (s == bit_syn[r]) return false;
             const uint32_t h = (s * 0x9E3779B1u) >> (32 - kPairHashBits);
             int i = 0;
             for (; i < kPairHashMaxProbe; i++) {

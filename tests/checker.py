@@ -166,6 +166,75 @@ def oracle_scan_candidates(data, fix=1, aggressive=0, drop_eof=0, cap=None):
     return [out[i] for i in range(n)]
 
 
+def oracle_decode_frames(frames, fix=1, aggressive=0):
+    """(n, 14) frames through the oracle's hex door, the address cache carried from frame to frame:
+    (messages, the eight statistics counters; only the fix counters move)."""
+    f = np.ascontiguousarray(frames, dtype=np.uint8).reshape(-1, 14)
+    n = f.shape[0]
+    out = (Msg * max(n, 1))()
+    st = (ctypes.c_longlong * 8)()
+    fn = oracle_lib().oracle_decode_frames
+    fn.restype = None
+    fn(f.ctypes.data_as(ctypes.c_void_p), ctypes.c_size_t(n), int(fix), int(aggressive), out, st)
+    return [out[i] for i in range(n)], list(st)
+
+
+def ref_decode_frames(frames, fix=1, aggressive=0):
+    """(n, 14) frames through the reference's own decodeModesMessage, in order, with one reset for
+    the whole batch, so the address cache is carried from frame to frame.
+
+    The reset is ref_decode_bytes on an all-zero frame (a DF0, which leaves the cache empty): it
+    sets the flags and clears the cache.  The frames then go to decodeModesMessage directly, which
+    the reference library exports like every function of dump1090.c, so this works with a library
+    built by any version of the harness.  struct modesMessage (dump1090.c:211-260) is the leading
+    part of Msg (oracle/oracle_msg.h), which is how the harness's own doors read it."""
+    lib = ref_lib()
+    f = np.ascontiguousarray(frames, dtype=np.uint8).reshape(-1, 14)
+    lib.ref_decode_bytes.restype = None
+    lib.decodeModesMessage.restype = None
+    lib.ref_decode_bytes(bytes(14), int(fix), int(aggressive), ctypes.byref(Msg()))
+    out = []
+    for row in f:
+        m = Msg()                                   # zeroed, as the harness zeroes its modesMessage
+        lib.decodeModesMessage(ctypes.byref(m), row.tobytes())
+        m.sample_pos = -1
+        out.append(m)
+    return out
+
+
+class ErrorInfo(ctypes.Structure):
+    """struct errorinfo, dump1090.c:263-267."""
+    _fields_ = [("syndrome", ctypes.c_uint32), ("bits", ctypes.c_int32), ("pos", ctypes.c_int32 * 2)]
+
+
+NERRORINFO = 5778
+
+
+def ref_error_table() -> np.ndarray:
+    """The reference's bitErrorTable after modesInitErrorInfo(): (syndrome, bits, pos0, pos1) rows in
+    the reference's order (sorted by syndrome)."""
+    lib = ref_lib()
+    lib.modesInitErrorInfo.restype = None
+    lib.modesInitErrorInfo()
+    tab = (ErrorInfo * NERRORINFO).in_dll(lib, "bitErrorTable")
+    return np.frombuffer(bytes(tab), dtype=np.int32).reshape(NERRORINFO, 4).astype(np.int64)   # syndromes < 2^24
+
+
+def ref_checksum_table() -> list:
+    """The reference's modes_checksum_table[112]."""
+    return list((ctypes.c_uint32 * 112).in_dll(ref_lib(), "modes_checksum_table"))
+
+
+def ref_fix_bit_errors(msg14: bytes, bits: int, maxfix: int):
+    """The reference's fixBitErrors on a copy of msg14: (repaired bytes, number fixed, positions)."""
+    lib = ref_lib()
+    lib.fixBitErrors.restype = ctypes.c_int
+    buf = (ctypes.c_uint8 * 14).from_buffer_copy(msg14)
+    fixed = (ctypes.c_int * 2)()
+    n = lib.fixBitErrors(buf, int(bits), int(maxfix), fixed)
+    return bytes(buf), n, list(fixed)[:n]
+
+
 def oracle_magnitude(iq) -> np.ndarray:
     a = _as_u8(iq)
     out = np.empty(a.size // 2, dtype=np.uint16)

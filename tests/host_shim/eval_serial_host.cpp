@@ -15,25 +15,81 @@ bool build_fix_hash(const uint32_t *bit_syn, uint32_t *out);
 bool build_pair_hash(const uint32_t *bit_syn, uint32_t *out);
 }
 
-// virt: the virtual sample array as bytes: 480 halo bytes (2 unused samples + 238 carried) then the body.
-extern "C" int shim_eval_candidates(const uint8_t *virt, uint64_t n_virtual_samples, const uint32_t *cand_v, uint32_t n,
-                                    int fix_errors, int aggressive, int lean, modes_candidate *out) {
+// The constant tables, built once by the product's builders; false if a builder refused.
+static bool tables(modes::serial::Tables &tab) {
     using namespace modes::serial;
     static uint32_t bit_syn[112], fix_hash[256];
     static std::vector<uint32_t> nib_syn(28 * 16);
     static std::vector<uint16_t> lut_iq(kIqLutEntries);
     static std::vector<uint32_t> pair_hash(1u << kPairHashBits);
-    static bool ready = false;
+    static int ready = 0;                        // 0 not yet, 1 built, -1 refused
     if (!ready) {
         modes::build_bit_syndromes(bit_syn);
-        if (!modes::build_fix_hash(bit_syn, fix_hash)) return -1;
         for (int pos = 0; pos < 28; pos++)
             for (uint32_t v = 0; v < 16; v++) nib_syn[pos * 16 + v] = nibble_syndrome(bit_syn, pos, v);
         modes::build_lut_iq(lut_iq.data());
-        if (!modes::build_pair_hash(bit_syn, pair_hash.data())) return -1;
-        ready = true;
+        ready = modes::build_fix_hash(bit_syn, fix_hash) && modes::build_pair_hash(bit_syn, pair_hash.data()) ? 1 : -1;
     }
-    const Tables tab{lut_iq.data(), bit_syn, nib_syn.data(), fix_hash, pair_hash.data()};
+    tab = Tables{lut_iq.data(), bit_syn, nib_syn.data(), fix_hash, pair_hash.data()};
+    return ready == 1;
+}
+
+// The syndrome tables as the kernels see them: bit_syn[112], fix_hash[256], pair_hash[1 << kPairHashBits].
+// Returns 0, or -1 if a builder refused.
+extern "C" int shim_tables(uint32_t *bit_syn, uint32_t *fix_hash, uint32_t *pair_hash) {
+    using namespace modes::serial;
+    Tables tab;
+    const bool ok = tables(tab);
+    std::memcpy(bit_syn, tab.bit_syn, 112 * sizeof(uint32_t));
+    std::memcpy(fix_hash, tab.fix_hash, 256 * sizeof(uint32_t));
+    std::memcpy(pair_hash, tab.pair_hash, (1u << kPairHashBits) * sizeof(uint32_t));
+    return ok ? 0 : -1;
+}
+
+// The builders themselves on caller-supplied syndromes (returns what the builder returns).
+extern "C" int shim_build_bit_syndromes(uint32_t *out) { modes::build_bit_syndromes(out); return 0; }
+extern "C" int shim_build_fix_hash(const uint32_t *bit_syn, uint32_t *out) { return modes::build_fix_hash(bit_syn, out); }
+extern "C" int shim_build_pair_hash(const uint32_t *bit_syn, uint32_t *out) { return modes::build_pair_hash(bit_syn, out); }
+
+// The hash probes: position (or first position of a pair) with syndrome s[i], or -1.
+extern "C" void shim_probe(const uint32_t *s, uint32_t n, int32_t *single, int32_t *pair_first) {
+    using namespace modes::serial;
+    Tables tab;
+    tables(tab);
+    for (uint32_t i = 0; i < n; i++) {
+        single[i] = syndrome_pos(tab.fix_hash, s[i]);
+        pair_first[i] = modes::serial::pair_first(tab.pair_hash, s[i]);
+    }
+}
+
+// serial::crc_and_fix on n 14-byte frames (the DF field decides the length): out[i] is the
+// modes_frame_eval of the frame after the repair (flags GATE_OK | DECODED).
+extern "C" int shim_crc_and_fix(const uint8_t *frames, uint64_t n, int fix_errors, int aggressive, modes_frame_eval *out) {
+    using namespace modes::serial;
+    Tables tab;
+    if (!tables(tab)) return -1;
+    for (uint64_t i = 0; i < n; i++) {
+        const uint8_t *m = frames + 14 * i;
+        Verdict R;
+        R.F[0] = R.F[1] = R.F[2] = R.F[3] = 0;
+        for (int b = 0; b < 112; b++) R.F[b >> 5] |= (uint32_t)((m[b >> 3] >> (7 - (b & 7))) & 1) << (b & 31);
+        R.msgtype = m[0] >> 3;
+        const int msgbits = (R.msgtype >= 16 && R.msgtype <= 21) ? 112 : 56;
+        R.flags = MODES_EVAL_GATE_OK | MODES_EVAL_DECODED;
+        crc_and_fix(R.F, msgbits, R.msgtype, fix_errors, aggressive, tab, R.crc, R.errorbit, R.nfixed);
+        uint32_t w[6];
+        eval_words(R, w);
+        std::memcpy(&out[i], w, sizeof(w));
+    }
+    return 0;
+}
+
+// virt: the virtual sample array as bytes: 480 halo bytes (2 unused samples + 238 carried) then the body.
+extern "C" int shim_eval_candidates(const uint8_t *virt, uint64_t n_virtual_samples, const uint32_t *cand_v, uint32_t n,
+                                    int fix_errors, int aggressive, int lean, modes_candidate *out) {
+    using namespace modes::serial;
+    Tables tab;
+    if (!tables(tab)) return -1;
     auto s16 = [&](uint64_t idx) -> uint32_t { uint16_t w; std::memcpy(&w, virt + 2 * idx, 2); return w; };
     for (uint32_t c = 0; c < n; c++) {
         const uint32_t v = cand_v[c];

@@ -12,6 +12,7 @@ import pytest
 
 import checker as C
 from dump1090_b200 import api, synth
+import repair_corpus as R
 import streams as S
 
 SHIM = C.ROOT / "tests" / "_build" / "libeval_serial_host.so"
@@ -35,6 +36,8 @@ def _streams():
     yield "ties", S.tie_rich(11)
     yield "ties_weak", S.tie_rich(12, levels=(0, 0, 1, 3, 30))
     yield "retry_at_j0", S.retry_at_buffer_start()
+    yield "repair0", R.repair_stream(0.0)                              # tests/repair_corpus.py
+    yield "repair_frac", R.repair_stream(R.RETRY_FRAC)
 
 
 STREAMS = dict(_streams())

@@ -11,6 +11,7 @@ FLAG_SETS = [dict(), dict(aggressive=1), dict(fix=0), dict(check_crc=0), dict(ch
              dict(drop_eof=1), dict(fix=0, drop_eof=1)]
 
 
+import repair_corpus as R
 import streams as S
 
 # all frame-evaluation kernels: thread per candidate with both attempts in one walk (whole or half
@@ -33,6 +34,9 @@ def _streams():
         yield f"traffic{seed}", synth.random_traffic(300000, 400, seed)
     yield "grid", synth.df17_grid(280000, 700, 5)
     yield from S.chain_streams()                                       # chains through the address cache
+    # every repair path (tests/repair_corpus.py), in the first attempt and in the phase-corrected retry
+    yield "repair0", R.repair_stream(0.0)
+    yield "repair_frac", R.repair_stream(R.RETRY_FRAC)
 
 
 def _nasty_streams():

@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 import checker as C
+import repair_corpus as R
 import streams as S
 from dump1090_b200 import api, synth
 
@@ -32,6 +33,8 @@ def _streams():
     # candidate delivers both attempts
     yield "dense_ties", S.tie_rich(21, n_frames=17800, levels=(0, 40, 100), period=60)
     yield from S.chain_streams()
+    yield "repair0", R.repair_stream(0.0)                              # tests/repair_corpus.py
+    yield "repair_frac", R.repair_stream(R.RETRY_FRAC)
 
 
 STREAMS = dict(_streams())
