@@ -9,6 +9,7 @@ constructing a Decoder without a usable GPU raises.
 from __future__ import annotations
 
 import ctypes as C
+import math
 from pathlib import Path
 
 import numpy as np
@@ -36,7 +37,7 @@ _MSG_A = ("errorbit aa1 aa2 aa3 phase_corrected ca iid metype mesub heading_is_v
           "aircraft_type fflag tflag raw_latitude raw_longitude").split()
 _MSG_B = ("ew_dir ew_velocity ns_dir ns_velocity vert_rate_source vert_rate_sign vert_rate velocity "
           "movement movement_valid ground_track ground_track_valid fs dr um identity altitude unit "
-          "nfixed pad2").split()
+          "nfixed signal").split()
 
 
 class Message(C.Structure):
@@ -67,6 +68,17 @@ class Message(C.Structure):
         n = lib().modes_format_raw_net(C.byref(self), buf, 64)
         return buf.raw[:n].decode("latin1")
 
+    def rssi_dbfs(self):
+        """Signal level in dB relative to the largest magnitude (20 log10(signal / 65535)), or None
+        when it was not measured (signal measurement off, or a frame from the hex door)."""
+        return None if self.signal <= 0 else 20.0 * math.log10(self.signal / 65535.0)
+
+    def beast(self) -> bytes:
+        """The Beast binary frame of this message (modes_format_beast)."""
+        buf = (C.c_uint8 * 64)()
+        n = lib().modes_format_beast(C.byref(self), buf, 64)
+        return bytes(buf[:n])
+
     def copy(self) -> "Message":
         m = Message()
         C.memmove(C.byref(m), C.byref(self), C.sizeof(Message))
@@ -75,7 +87,7 @@ class Message(C.Structure):
 
 class FrameEval(C.Structure):
     _fields_ = [("msg", C.c_uint8 * 14), ("msgtype", C.c_uint8), ("flags", C.c_uint8),
-                ("errorbit", C.c_uint8), ("nfixed", C.c_uint8), ("crc", C.c_uint32)]
+                ("errorbit", C.c_uint8), ("nfixed", C.c_uint8), ("signal", C.c_uint16), ("crc", C.c_uint32)]
 
 
 class Candidate(C.Structure):
@@ -98,7 +110,7 @@ POOL_SINK_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_uint32, C.POINTER(Message))
 
 CANDIDATE_DTYPE = np.dtype([("t", "<i8"),
                             ("p", [("msg", "u1", 14), ("msgtype", "u1"), ("flags", "u1"), ("errorbit", "u1"),
-                                   ("nfixed", "u1"), ("crc", "<u4")], 2)], align=True)
+                                   ("nfixed", "u1"), ("signal", "<u2"), ("crc", "<u4")], 2)], align=True)
 TILE_DTYPE = np.dtype([("offset", "<u4"), ("count", "<u4")])
 assert CANDIDATE_DTYPE.itemsize == C.sizeof(Candidate) == 56
 
@@ -119,7 +131,7 @@ EXPORTS = ["modes_abi_version", "modes_default_config", "modes_create", "modes_d
            "modes_tracker_format_table", "modes_format_sbs", "modes_cpr_nl",
            "modes_pool_create", "modes_pool_destroy", "modes_pool_last_error", "modes_pool_ingest", "modes_pool_resolve",
            "modes_pool_stats", "modes_pool_reset", "modes_pool_buffers", "modes_pool_set_output", "modes_pool_output_count",
-           "modes_pool_submit", "modes_pool_collect"]
+           "modes_pool_submit", "modes_pool_collect", "modes_set_signal", "modes_pool_set_signal", "modes_format_beast"]
 
 
 def lib():
@@ -211,6 +223,10 @@ def lib():
         L.modes_pool_output_count.argtypes = [C.c_void_p]
         L.modes_pool_buffers.restype = C.c_int64
         L.modes_pool_buffers.argtypes = [C.c_void_p, C.c_uint32]
+        L.modes_set_signal.argtypes = [C.c_void_p, C.c_int]
+        L.modes_pool_set_signal.argtypes = [C.c_void_p, C.c_int]
+        L.modes_format_beast.restype = C.c_size_t
+        L.modes_format_beast.argtypes = [C.POINTER(Message), C.c_void_p, C.c_size_t]
         _lib = L
     return _lib
 
@@ -281,13 +297,16 @@ class PinnedBuffer:
 
 
 class Decoder:
-    """One GPU decode context (modes_create ... modes_destroy)."""
+    """One GPU decode context (modes_create ... modes_destroy).  signal=True measures the signal
+    level of every decoded frame on the GPU (modes_set_signal): Message.signal, rssi_dbfs(), beast()."""
 
-    def __init__(self, **cfg):
+    def __init__(self, signal: bool = False, **cfg):
         self.cfg = make_config(**cfg)
         self._h = lib().modes_create(C.byref(self.cfg))
         if not self._h:
             raise RuntimeError("modes_create failed: " + lib().modes_last_error(None).decode())
+        if signal:
+            self.set_signal(True)
         self._collector = _Collector()
         lib().modes_set_sink(self._h, self._collector.fn, None)
 
@@ -364,6 +383,10 @@ class Decoder:
 
     def output_count(self) -> int:
         return int(lib().modes_output_count(self._h))
+
+    def set_signal(self, on: bool) -> None:
+        """Measure the signal level for batches submitted from now on (modes_set_signal)."""
+        self._check(lib().modes_set_signal(self._h, int(bool(on))))
 
     def set_stream(self, cuda_stream: int) -> None:
         self._check(lib().modes_set_stream(self._h, C.c_void_p(cuda_stream)))
@@ -557,14 +580,16 @@ class Resolver:
 class ReceiverPool:
     """modes_pool_*: independent 2 MHz streams (one address cache, carry, skip state and set of
     statistics each, as one dump1090 process keeps per receiver), one buffer of each decoded per
-    batch.  Messages are collected per receiver (`take(receiver)`)."""
+    batch.  Messages are collected per receiver (`take(receiver)`).  signal=True: as for Decoder."""
 
-    def __init__(self, n_receivers: int, max_batch: int = 0, **cfg):
+    def __init__(self, n_receivers: int, max_batch: int = 0, signal: bool = False, **cfg):
         self.cfg = make_config(**cfg)
         self.n = n_receivers
         self._h = lib().modes_pool_create(C.byref(self.cfg), n_receivers, max_batch)
         if not self._h:
             raise RuntimeError("modes_pool_create failed")
+        if signal:
+            self.set_signal(True)
         self.messages = [[] for _ in range(n_receivers)]
         self._fn = POOL_SINK_FN(self._on)
 
@@ -635,6 +660,10 @@ class ReceiverPool:
         st = Stats()
         lib().modes_pool_stats(self._h, receiver, C.byref(st))
         return dict(zip(STAT_NAMES, [int(x) for x in st.v]))
+
+    def set_signal(self, on: bool) -> None:
+        """Measure the signal level for batches submitted from now on (modes_pool_set_signal)."""
+        self._check(lib().modes_pool_set_signal(self._h, int(bool(on))))
 
     def buffers(self, receiver: int) -> int:
         return int(lib().modes_pool_buffers(self._h, receiver))

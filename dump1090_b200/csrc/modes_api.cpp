@@ -94,6 +94,7 @@ struct modes_ctx {
     cudaStream_t own_detect_stream = nullptr;
     std::string err;
     uint64_t launches = 0;
+    bool signal = false;                  // modes_set_signal: measure the signal level of decoded attempts
     // cfg.profile: ring of CUDA-event triplets, one per batch, recorded on the launching stream
     static constexpr int kProfRing = 512;
     cudaEvent_t prof_ev[kProfRing][3];
@@ -308,8 +309,10 @@ int launch_batch(modes_ctx *ctx, Slot &s) {
     if (pe) CK(ctx, cudaEventRecord(pe[1], s.stream));
     launch_eval(in, ctx->tab, so, s.out_records, ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->sm_count, s.stream);
     if (pe) CK(ctx, cudaEventRecord(pe[2], s.stream));
+    // after pe[2]: the kernel times keep their meaning; before the device resolve, which copies the field
+    if (ctx->signal) launch_signal(in, ctx->tab, so, s.out_records, ctx->sm_count, s.stream);
     CK(ctx, cudaGetLastError());
-    ctx->launches += 2;
+    ctx->launches += ctx->signal ? 3 : 2;
     if (ctx->cfg.gpu_resolve && s.own_outputs && &s != &ctx->detect) {
         if (gpu_resolve_ensure(ctx, s)) return -1;
         // the address cache comes from the previous batch's resolve (other slot, other stream)
@@ -459,7 +462,7 @@ int run_buffers_multi(modes_ctx *ctx, const uint8_t *host_iq, size_t n_buffers) 
             ctx->buffers_done += (int64_t)nb;
             host_iq += nb * MODES_BUFFER_BYTES;
             n_buffers -= nb;
-            ctx->launches += 2;
+            ctx->launches += g->signal ? 3 : 2;
         }
         ctx->group_n[cur] = k;
         if (have_prev && collect_group(ctx, cur ^ 1)) return -1;
@@ -607,6 +610,13 @@ modes_ctx *modes_create(const modes_config *cfg) {
         cudaSetDevice(ctx->cfg.device);
     }
     return ctx;
+}
+
+int modes_set_signal(modes_ctx *ctx, int on) {
+    if (!ctx) return -1;
+    ctx->signal = on != 0;
+    for (modes_ctx *g : ctx->gpus) g->signal = on != 0;
+    return 0;
 }
 
 int modes_set_sink(modes_ctx *ctx, modes_sink_fn fn, void *user) {

@@ -167,6 +167,30 @@ extern "C" size_t modes_format_raw_net(const modes_message *mm, char *buf, size_
     return o.len;
 }
 
+// The Beast binary frame of the dump1090 descendants (their port 30005), Mode S frames only:
+// 0x1a, type '2' (7 bytes) or '3' (14 bytes), 48-bit 12 MHz timestamp, signal byte, frame; every
+// 0x1a after the leading one is doubled.  At 2 MHz one sample is 6 ticks of the 12 MHz clock.
+extern "C" size_t modes_format_beast(const modes_message *mm, uint8_t *buf, size_t capacity) {
+    const int nbytes = mm->msgbits == 112 ? 14 : 7;
+    uint8_t body[2 + 6 + 1 + 14];
+    size_t k = 0;
+    body[k++] = nbytes == 14 ? '3' : '2';
+    const uint64_t ts = mm->sample_pos < 0 ? 0 : ((uint64_t)mm->sample_pos * 6u) & ((1ull << 48) - 1);
+    for (int i = 5; i >= 0; i--) body[k++] = (uint8_t)(ts >> (8 * i));
+    const int64_t s = mm->signal < 0 ? 0 : mm->signal;
+    const int64_t level = (s * 255 + 32767) / 65535;
+    body[k++] = (uint8_t)(level > 255 ? 255 : level);
+    for (int i = 0; i < nbytes; i++) body[k++] = mm->msg[i];
+    size_t len = 0;
+    auto put = [&](uint8_t b) { if (len < capacity) buf[len] = b; len++; };
+    put(0x1a);
+    for (size_t i = 0; i < k; i++) {
+        put(body[i]);
+        if (body[i] == 0x1a) put(0x1a);
+    }
+    return len;
+}
+
 // The raw TCP input line (port 30001), the parsing half of decodeHexMessage dump1090.c:2472-2497:
 // surrounding white space ignored, "*" ... ";" required, at most 28 hex digits, any non-hex digit
 // (or an odd digit count, which makes the reference pair a digit with ';') discards the line.

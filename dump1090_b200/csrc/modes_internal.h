@@ -72,6 +72,15 @@ void launch_magnitude(const uint8_t *d_iq, uint16_t *d_mag, uint64_t n_samples, 
 // CRC / fix on raw frame bytes (hex door): n frames of 14 bytes -> n modes_frame_eval.
 void launch_eval_frames(const uint8_t *d_frames, modes_frame_eval *d_out, uint32_t n, const DeviceTables &tab,
                         int fix_errors, int aggressive, cudaStream_t stream);
+// Signal level of every decoded attempt (modes_signal.cu): writes pass[k].signal of the first
+// min(counters[0], cand_capacity) records over the same windows the scan and frame evaluation read.
+void launch_signal(const BatchView &in, const DeviceTables &tab, const ScanOutputs &scan, modes_candidate *records,
+                   int sm_count, cudaStream_t stream);
+
+// The record layouts are ABI: the signal field took the two bytes every evaluation kernel already wrote as zero.
+static_assert(sizeof(modes_frame_eval) == 24 && offsetof(modes_frame_eval, signal) == 18 && offsetof(modes_frame_eval, crc) == 20,
+              "frame evaluation record layout");
+static_assert(sizeof(modes_candidate) == 56, "candidate record layout");
 
 // Host-side table construction (modes_tables.cpp).
 void build_lutn(uint16_t *out /*[32769]*/);

@@ -100,6 +100,7 @@ struct modes_pool {
     modes_config cfg;
     std::vector<Receiver> rx;
     size_t max_batch = 0;
+    int signal = 0;                            // modes_pool_set_signal, applied to the slot contexts
     std::string err;
     // device half (created on the first modes_pool_submit / _ingest): two batches may be in flight, so
     // that one is uploaded and scanned while the one before it is resolved on the host
@@ -167,6 +168,7 @@ int ensure_device(modes_pool *p) {
     for (modes_pool::Slot &sl : p->slot) {
         sl.ctx = modes_create(&c);
         if (!sl.ctx) return fail(p, "%s", modes_last_error(nullptr));
+        modes_set_signal(sl.ctx, p->signal);
         sl.d_batch = static_cast<uint8_t *>(modes_device_alloc(bytes));
         sl.h_carry = static_cast<uint8_t *>(modes_host_alloc(p->max_batch * MODES_CARRY_BYTES));
         if (!sl.d_batch || !sl.h_carry) return fail(p, "out of memory for %zu receivers per batch", p->max_batch);
@@ -389,6 +391,14 @@ int modes_pool_set_output(modes_pool *p, modes_message *out, uint32_t *receiver_
 }
 
 size_t modes_pool_output_count(const modes_pool *p) { return p ? p->out_count : 0; }
+
+int modes_pool_set_signal(modes_pool *p, int on) {
+    if (!p) return -1;
+    p->signal = on != 0;
+    for (modes_pool::Slot &sl : p->slot)
+        if (sl.ctx) modes_set_signal(sl.ctx, p->signal);
+    return 0;
+}
 
 int64_t modes_pool_buffers(const modes_pool *p, uint32_t receiver) {
     if (!p || receiver >= p->rx.size()) return -1;

@@ -170,6 +170,7 @@ static void build_message(const modes_frame_eval &p, int crcok, uint32_t iid, ui
     o->msgbits = bits_by_type(p.msgtype);
     o->crc = p.crc;
     o->nfixed = p.nfixed;
+    o->signal = p.signal;
     o->errorbit = p.nfixed ? (int)p.errorbit : -1;
     o->crcok = crcok;
     o->iid = (int32_t)iid;

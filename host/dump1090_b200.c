@@ -11,6 +11,9 @@
  * line of every message instead (what the reference writes to port 30003, dump1090.c:2396) and
  * --aircraft-json prints the tracked aircraft as the reference's /data.json at the end (:2505),
  * both with stream time (MODES_STREAM_EPOCH_MS + sample position / 2 MHz) as the clock.
+ * --beast writes one Beast binary frame per message instead (what the dump1090 descendants send on
+ * port 30005: 12 MHz timestamp = 6 x sample position, signal level measured on the GPU); it excludes
+ * --raw, --onlyaddr, --sbs and --aircraft-json, which write to stdout as well.
  * The live-radio, networking and interactive options are out of scope.
  */
 #include <stdio.h>
@@ -18,7 +21,7 @@
 #include <string.h>
 #include "modes_b200.h"
 
-static int opt_raw = 0, opt_onlyaddr = 0, opt_stats = 0, opt_check_crc = 1, opt_sbs = 0, opt_json = 0;
+static int opt_raw = 0, opt_onlyaddr = 0, opt_stats = 0, opt_check_crc = 1, opt_sbs = 0, opt_json = 0, opt_beast = 0;
 static modes_tracker *tracker = NULL;
 
 /* Message sink: the --raw / --onlyaddr forms of displayModesMessage
@@ -26,6 +29,12 @@ static modes_tracker *tracker = NULL;
 static void on_message(void *user, const modes_message *mm) {
     (void)user;
     if (opt_stats) return;                                  /* dump1090.c:1803 */
+    if (opt_beast) {
+        uint8_t frame[64];
+        size_t n = modes_format_beast(mm, frame, sizeof(frame));
+        fwrite(frame, 1, n, stdout);
+        return;
+    }
     if (tracker) {                                          /* dump1090.c:1806-1809 */
         const modes_aircraft *a = modes_tracker_update(tracker, mm, MODES_STREAM_EPOCH_MS + mm->sample_pos / 2000);
         if (a && opt_sbs) {
@@ -68,6 +77,7 @@ int main(int argc, char **argv) {
         else if (!strcmp(argv[j], "--drop-eof-buffer")) cfg.drop_eof_buffer = 1;
         else if (!strcmp(argv[j], "--sbs")) opt_sbs = 1;
         else if (!strcmp(argv[j], "--aircraft-json")) opt_json = 1;
+        else if (!strcmp(argv[j], "--beast")) opt_beast = 1;
         else if (!strcmp(argv[j], "--device") && more) cfg.device = atoi(argv[++j]);
         else if (!strcmp(argv[j], "--gpus") && more) cfg.n_gpus = atoi(argv[++j]);
         else if (!strcmp(argv[j], "--chunk") && more) chunk = (size_t)strtoull(argv[++j], NULL, 10);
@@ -77,6 +87,10 @@ int main(int argc, char **argv) {
         }
     }
     if (!filename) { fprintf(stderr, "--ifile <filename> is required (use '-' for stdin)\n"); return 1; }
+    if (opt_beast && (opt_raw || opt_onlyaddr || opt_sbs || opt_json)) {
+        fprintf(stderr, "--beast writes binary frames to stdout: it cannot be combined with --raw, --onlyaddr, --sbs or --aircraft-json\n");
+        return 1;
+    }
     FILE *f = (filename[0] == '-' && filename[1] == 0) ? stdin : fopen(filename, "rb");
     if (!f) { perror("Opening data file"); return 1; }
 
@@ -86,6 +100,7 @@ int main(int argc, char **argv) {
         tracker = modes_tracker_create(cfg.check_crc);
         if (!tracker) { fprintf(stderr, "out of memory\n"); return 1; }
     }
+    if (opt_beast) modes_set_signal(ctx, 1);
     modes_set_sink(ctx, on_message, NULL);
     unsigned char *buf = (unsigned char *)modes_host_alloc(chunk);
     if (!buf) { fprintf(stderr, "out of memory\n"); return 1; }

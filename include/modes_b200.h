@@ -93,7 +93,7 @@ typedef struct modes_message {
     int32_t  fs, dr, um, identity;
     int32_t  altitude, unit;
     int32_t  nfixed;            /* bits repaired by the CRC fix (0/1/2) */
-    int32_t  pad2;
+    int32_t  signal;            /* RMS pulse magnitude of the frame (see modes_frame_eval.signal); 0 = not measured */
     int64_t  sample_pos;        /* stream sample index of the preamble start */
 } modes_message;
 
@@ -106,6 +106,10 @@ typedef struct modes_frame_eval {
     uint8_t  flags;             /* MODES_EVAL_* */
     uint8_t  errorbit;          /* first repaired bit, 0xFF = none */
     uint8_t  nfixed;
+    uint16_t signal;            /* with modes_set_signal on and MODES_EVAL_DECODED set: floor(sqrt(floor(S / b))),
+                                   S = sum over the b frame bits (b = 56 or 112 from msgtype) of the squared
+                                   larger magnitude of the bit's two uncorrected samples (dump1090.c:1670-1671,
+                                   magnitudes of :359-364); otherwise 0 */
     uint32_t crc;               /* 24-bit syndrome after the fix; 0 when not decoded */
 } modes_frame_eval;
 
@@ -386,6 +390,23 @@ size_t modes_pool_output_count(const modes_pool *p);
 int  modes_pool_stats(const modes_pool *p, uint32_t receiver, modes_stats *out);
 int  modes_pool_reset(modes_pool *p, uint32_t receiver);        /* the receiver starts a new stream */
 int64_t modes_pool_buffers(const modes_pool *p, uint32_t receiver);   /* buffers of it decoded so far */
+
+/* ---- signal level and the Beast binary feed ----------------------------------------------------
+ * Signal measurement is off by default.  When it is on, every batch submitted afterwards runs one
+ * more kernel after frame evaluation, which writes modes_frame_eval.signal for every decoded
+ * attempt; delivered messages carry it in modes_message.signal.  It is always measured on the
+ * uncorrected samples, also for a phase-corrected retry.  Messages from the hex door have no
+ * samples and keep signal = 0.  On an n_gpus > 1 context the setting reaches every GPU; a pool
+ * applies it to all its device contexts.  Returns 0, or -1 for a NULL handle. */
+int    modes_set_signal(modes_ctx *ctx, int on);
+int    modes_pool_set_signal(modes_pool *p, int on);
+/* One Beast frame for a message: 0x1a, '2' (7-byte frame) or '3' (14-byte frame), a 6-byte big-endian
+ * 12 MHz timestamp = (6 * sample_pos) mod 2^48 (0 when sample_pos < 0), one signal byte
+ * = min(255, (signal * 255 + 32767) / 65535), then the frame bytes; every 0x1a after the leading one
+ * is doubled.  sample_pos counts the samples of one stream (of one receiver in a pool), so each
+ * stream's clock is its own.  Returns the length the frame needs (at most 44); writes at most
+ * capacity bytes and no terminating NUL.  Pure host code. */
+size_t modes_format_beast(const modes_message *mm, uint8_t *buf, size_t capacity);
 
 #ifdef __cplusplus
 }
