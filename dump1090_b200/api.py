@@ -114,6 +114,38 @@ CANDIDATE_DTYPE = np.dtype([("t", "<i8"),
 TILE_DTYPE = np.dtype([("offset", "<u4"), ("count", "<u4")])
 assert CANDIDATE_DTYPE.itemsize == C.sizeof(Candidate) == 56
 
+
+class Level(C.Structure):
+    """struct modes_level: noise, peak and clipping sums of one reference buffer."""
+    _fields_ = [("buffer", C.c_int64), ("n_samples", C.c_uint32), ("clipped", C.c_uint32),
+                ("sum_mag", C.c_uint64), ("sum_power", C.c_uint64), ("peak", C.c_uint32), ("pad", C.c_uint32)]
+
+
+LEVEL_DTYPE = np.dtype([("buffer", "<i8"), ("n_samples", "<u4"), ("clipped", "<u4"), ("sum_mag", "<u8"),
+                        ("sum_power", "<u8"), ("peak", "<u4"), ("pad", "<u4")])
+assert LEVEL_DTYPE.itemsize == C.sizeof(Level) == 40
+FULL_SCALE = 65535                        # the dBFS reference of rssi_dbfs() and level_summary()
+
+
+def level_summary(records) -> dict:
+    """Totals of level records (LEVEL_DTYPE): buffers, n_samples, clipped, and on the scale of
+    Message.rssi_dbfs() (so that SNR = signal dB - noise dB)
+        noise_dbfs = 10 log10(sum sum_power / sum n_samples / 65535^2)   (mean power)
+        peak_dbfs  = 20 log10(max peak / 65535)
+        clipped_fraction = sum clipped / sum n_samples
+    With no samples the three derived values are None; with no power / a zero peak the dB values are -inf."""
+    r = np.asarray(records, dtype=LEVEL_DTYPE)
+    n = int(r["n_samples"].astype(np.uint64).sum()) if r.size else 0
+    power = int(sum(int(v) for v in r["sum_power"]))
+    peak = int(r["peak"].max()) if r.size else 0
+    clipped = int(r["clipped"].astype(np.uint64).sum()) if r.size else 0
+    out = dict(buffers=int(r.size), n_samples=n, clipped=clipped, noise_dbfs=None, peak_dbfs=None, clipped_fraction=None)
+    if n:
+        out["noise_dbfs"] = 10.0 * math.log10(power / n / FULL_SCALE ** 2) if power else -math.inf
+        out["peak_dbfs"] = 20.0 * math.log10(peak / FULL_SCALE) if peak else -math.inf
+        out["clipped_fraction"] = clipped / n
+    return out
+
 _lib = None
 
 # every symbol include/modes_b200.h declares
@@ -131,7 +163,9 @@ EXPORTS = ["modes_abi_version", "modes_default_config", "modes_create", "modes_d
            "modes_tracker_format_table", "modes_format_sbs", "modes_cpr_nl",
            "modes_pool_create", "modes_pool_destroy", "modes_pool_last_error", "modes_pool_ingest", "modes_pool_resolve",
            "modes_pool_stats", "modes_pool_reset", "modes_pool_buffers", "modes_pool_set_output", "modes_pool_output_count",
-           "modes_pool_submit", "modes_pool_collect", "modes_set_signal", "modes_pool_set_signal", "modes_format_beast"]
+           "modes_pool_submit", "modes_pool_collect", "modes_set_signal", "modes_pool_set_signal", "modes_format_beast",
+           "modes_set_levels", "modes_take_levels", "modes_levels_device", "modes_levels_fetch",
+           "modes_pool_set_levels", "modes_pool_take_levels"]
 
 
 def lib():
@@ -227,6 +261,14 @@ def lib():
         L.modes_pool_set_signal.argtypes = [C.c_void_p, C.c_int]
         L.modes_format_beast.restype = C.c_size_t
         L.modes_format_beast.argtypes = [C.POINTER(Message), C.c_void_p, C.c_size_t]
+        L.modes_set_levels.argtypes = [C.c_void_p, C.c_int]
+        L.modes_take_levels.restype = C.c_size_t
+        L.modes_take_levels.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+        L.modes_levels_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]
+        L.modes_levels_fetch.argtypes = [C.c_void_p, C.c_void_p]
+        L.modes_pool_set_levels.argtypes = [C.c_void_p, C.c_int]
+        L.modes_pool_take_levels.restype = C.c_size_t
+        L.modes_pool_take_levels.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t]
         _lib = L
     return _lib
 
@@ -298,15 +340,19 @@ class PinnedBuffer:
 
 class Decoder:
     """One GPU decode context (modes_create ... modes_destroy).  signal=True measures the signal
-    level of every decoded frame on the GPU (modes_set_signal): Message.signal, rssi_dbfs(), beast()."""
+    level of every decoded frame on the GPU (modes_set_signal): Message.signal, rssi_dbfs(), beast().
+    levels=True measures every decoded buffer's noise, peak and clipping on the GPU
+    (modes_set_levels): take_levels(), level_summary()."""
 
-    def __init__(self, signal: bool = False, **cfg):
+    def __init__(self, signal: bool = False, levels: bool = False, **cfg):
         self.cfg = make_config(**cfg)
         self._h = lib().modes_create(C.byref(self.cfg))
         if not self._h:
             raise RuntimeError("modes_create failed: " + lib().modes_last_error(None).decode())
         if signal:
             self.set_signal(True)
+        if levels:
+            self.set_levels(True)
         self._collector = _Collector()
         lib().modes_set_sink(self._h, self._collector.fn, None)
 
@@ -388,6 +434,17 @@ class Decoder:
         """Measure the signal level for batches submitted from now on (modes_set_signal)."""
         self._check(lib().modes_set_signal(self._h, int(bool(on))))
 
+    def set_levels(self, on: bool) -> None:
+        """Measure the buffers' levels for batches submitted from now on (modes_set_levels)."""
+        self._check(lib().modes_set_levels(self._h, int(bool(on))))
+
+    def take_levels(self) -> np.ndarray:
+        """The queued level records (LEVEL_DTYPE), oldest first, in stream order; the queue is emptied."""
+        n = int(lib().modes_take_levels(self._h, None, 0))
+        out = np.zeros(n, dtype=LEVEL_DTYPE)
+        got = int(lib().modes_take_levels(self._h, _ptr(out), n)) if n else 0
+        return out[:got]
+
     def set_stream(self, cuda_stream: int) -> None:
         self._check(lib().modes_set_stream(self._h, C.c_void_p(cuda_stream)))
 
@@ -464,6 +521,17 @@ class Decoder:
         out = (Message * n)()
         self._check(lib().modes_decode_frames(self._h, buf, n, out))
         return [out[i] for i in range(n)]
+
+    def levels_device(self, d_iq_ptr: int, n_buffers: int, stride_bytes: int = 0) -> None:
+        """Level records of n_buffers buffers in device memory, buffer k at d_iq_ptr + k * stride_bytes."""
+        self._check(lib().modes_levels_device(self._h, C.c_void_p(d_iq_ptr), n_buffers, stride_bytes))
+        self._levels_n = n_buffers
+
+    def levels_fetch(self) -> np.ndarray:
+        """The records of the last levels_device call (waits for them)."""
+        out = np.zeros(getattr(self, "_levels_n", 0), dtype=LEVEL_DTYPE)
+        self._check(lib().modes_levels_fetch(self._h, _ptr(out)))
+        return out
 
     def publish_count(self, dst_ptr: int) -> None:
         self._check(lib().modes_detect_publish_count(self._h, C.c_void_p(dst_ptr)))
@@ -580,9 +648,10 @@ class Resolver:
 class ReceiverPool:
     """modes_pool_*: independent 2 MHz streams (one address cache, carry, skip state and set of
     statistics each, as one dump1090 process keeps per receiver), one buffer of each decoded per
-    batch.  Messages are collected per receiver (`take(receiver)`).  signal=True: as for Decoder."""
+    batch.  Messages are collected per receiver (`take(receiver)`).  signal=True: as for Decoder.
+    levels=True: level records of every receiver's buffers (`take_levels(receiver)`)."""
 
-    def __init__(self, n_receivers: int, max_batch: int = 0, signal: bool = False, **cfg):
+    def __init__(self, n_receivers: int, max_batch: int = 0, signal: bool = False, levels: bool = False, **cfg):
         self.cfg = make_config(**cfg)
         self.n = n_receivers
         self._h = lib().modes_pool_create(C.byref(self.cfg), n_receivers, max_batch)
@@ -590,6 +659,8 @@ class ReceiverPool:
             raise RuntimeError("modes_pool_create failed")
         if signal:
             self.set_signal(True)
+        if levels:
+            self.set_levels(True)
         self.messages = [[] for _ in range(n_receivers)]
         self._fn = POOL_SINK_FN(self._on)
 
@@ -664,6 +735,17 @@ class ReceiverPool:
     def set_signal(self, on: bool) -> None:
         """Measure the signal level for batches submitted from now on (modes_pool_set_signal)."""
         self._check(lib().modes_pool_set_signal(self._h, int(bool(on))))
+
+    def set_levels(self, on: bool) -> None:
+        """Measure the levels of batches submitted from now on (modes_pool_set_levels)."""
+        self._check(lib().modes_pool_set_levels(self._h, int(bool(on))))
+
+    def take_levels(self, receiver: int) -> np.ndarray:
+        """The receiver's queued level records (LEVEL_DTYPE), its own buffer indices, oldest first."""
+        n = int(lib().modes_pool_take_levels(self._h, receiver, None, 0))
+        out = np.zeros(n, dtype=LEVEL_DTYPE)
+        got = int(lib().modes_pool_take_levels(self._h, receiver, _ptr(out), n)) if n else 0
+        return out[:got]
 
     def buffers(self, receiver: int) -> int:
         return int(lib().modes_pool_buffers(self._h, receiver))

@@ -44,12 +44,15 @@ struct Slot {
     size_t gr_buffers = 0;
     uint32_t *h_gr_flags = nullptr;       // pinned: flags[3] + pad, then stats[8] as u64, then the end cache [1024]
     modes_delivery *h_deliveries = nullptr; size_t h_deliveries_cap = 0;   // pinned
+    // modes_set_levels: one record per buffer of the batch (device, and its pinned host copy)
+    modes_level *d_levels = nullptr, *h_levels = nullptr; size_t levels_cap = 0;
     // in-flight batch
     bool busy = false;
     size_t n_buffers = 0;
     int64_t buffer_base = 0;
     const void *batch_iq = nullptr;   // device address the batch was scanned from
     bool own_outputs = true;          // results in this slot's own buffers (growable)
+    bool levels = false;              // the batch measures levels (the switch as it was at submit)
     uint32_t want_cap = 0;            // grow the candidate buffers to at least this on the next ensure
     // where this batch's results live (own workspace unless the caller supplied memory)
     modes_candidate *out_records = nullptr;
@@ -95,6 +98,14 @@ struct modes_ctx {
     std::string err;
     uint64_t launches = 0;
     bool signal = false;                  // modes_set_signal: measure the signal level of decoded attempts
+    bool levels = false;                  // modes_set_levels: measure every decoded buffer's levels
+    std::vector<modes_level> level_q;     // records not taken yet, oldest from level_head on
+    size_t level_head = 0;
+    int64_t eof_buffer = -1;              // modes_finish: stream index of the EOF buffer and its real samples
+    uint32_t eof_samples = 0;
+    // modes_levels_device: the records of the last call (device, pinned host copy)
+    modes_level *d_lv = nullptr, *h_lv = nullptr; size_t lv_cap = 0, lv_n = 0;
+    bool lv_fetched = true;               // no copy of them is pending
     // cfg.profile: ring of CUDA-event triplets, one per batch, recorded on the launching stream
     static constexpr int kProfRing = 512;
     cudaEvent_t prof_ev[kProfRing][3];
@@ -181,6 +192,7 @@ void slot_free(Slot &s) {
     cudaFree(s.gr.start); cudaFree(s.gr.end); cudaFree(s.gr.written); cudaFree(s.gr.readfirst); cudaFree(s.gr.rerun);
     cudaFree(s.gr.n_deliv); cudaFree(s.gr.offsets); cudaFree(s.gr.flags); cudaFree(s.gr.stats_out); cudaFree(s.gr.out);
     cudaFreeHost(s.h_gr_flags); cudaFreeHost(s.h_deliveries);
+    cudaFree(s.d_levels); cudaFreeHost(s.h_levels);
     for (auto &e : s.ev) if (e) cudaEventDestroy(e);
     for (auto &e : s.halo_ev) if (e) cudaEventDestroy(e);
     if (s.stream) cudaStreamDestroy(s.stream);
@@ -230,6 +242,30 @@ int host_ensure(modes_ctx *ctx, Slot &s, size_t n_records, size_t n_tiles) {
 
 int launch_batch(modes_ctx *ctx, Slot &s);
 
+// Room for n level records in device memory and in pinned host memory.  `queued`: a stream whose
+// copy into the old host block may still be pending, waited for before the block is replaced.
+int levels_ensure(modes_ctx *ctx, modes_level *&d, modes_level *&h, size_t &cap, size_t n, cudaStream_t queued) {
+    if (cap >= n) return 0;
+    if (queued) CK(ctx, wait_stream(queued));
+    cudaFree(d); cudaFreeHost(h);
+    d = h = nullptr; cap = 0;
+    CK(ctx, cudaMalloc(&d, n * sizeof(modes_level)));
+    CK(ctx, cudaMallocHost(&h, n * sizeof(modes_level)));
+    cap = n;
+    return 0;
+}
+
+// Queue the level records of the slot's finished batch, re-based to stream buffer indices.
+void append_levels(modes_ctx *ctx, const Slot &s) {
+    if (!s.levels) return;
+    for (size_t k = 0; k < s.n_buffers; k++) {
+        modes_level r = s.h_levels[k];
+        r.buffer = s.buffer_base + (int64_t)k;
+        if (r.buffer == ctx->eof_buffer) r.n_samples = ctx->eof_samples;
+        ctx->level_q.push_back(r);
+    }
+}
+
 // Workspace of the device resolve for the slot's current batch.
 int gpu_resolve_ensure(modes_ctx *ctx, Slot &s) {
     const size_t nb = s.n_buffers;
@@ -266,6 +302,8 @@ int submit(modes_ctx *ctx, Slot &s, const uint8_t *host_iq, const void *d_iq, si
     // caller-supplied record buffers: the slot's own position list must hold as many candidates
     if (d_records_ext && cap_ext > s.want_cap) s.want_cap = cap_ext;
     if (slot_ensure(ctx, s, n_samples, host_iq != nullptr, d_records_ext == nullptr)) return -1;
+    s.levels = ctx->levels && &s != &ctx->detect;
+    if (s.levels && levels_ensure(ctx, s.d_levels, s.h_levels, s.levels_cap, n_buffers, nullptr)) return -1;   // collected
     if (host_iq) {
         CK(ctx, cudaMemcpyAsync(s.d_iq, host_iq, n_samples * 2, cudaMemcpyHostToDevice, s.stream));
         d_iq = s.d_iq;
@@ -311,8 +349,12 @@ int launch_batch(modes_ctx *ctx, Slot &s) {
     if (pe) CK(ctx, cudaEventRecord(pe[2], s.stream));
     // after pe[2]: the kernel times keep their meaning; before the device resolve, which copies the field
     if (ctx->signal) launch_signal(in, ctx->tab, so, s.out_records, ctx->sm_count, s.stream);
+    // the buffers' own bytes (the body, not the carry block); one writer per record, so a repeated
+    // batch writes the same records
+    if (s.levels)
+        launch_levels(in.body, (uint32_t)s.n_buffers, MODES_BUFFER_BYTES, ctx->tab, s.d_levels, ctx->sm_count, s.stream);
     CK(ctx, cudaGetLastError());
-    ctx->launches += ctx->signal ? 3 : 2;
+    ctx->launches += (ctx->signal ? 3 : 2) + (s.levels ? 1 : 0);
     if (ctx->cfg.gpu_resolve && s.own_outputs && &s != &ctx->detect) {
         if (gpu_resolve_ensure(ctx, s)) return -1;
         // the address cache comes from the previous batch's resolve (other slot, other stream)
@@ -331,6 +373,7 @@ int launch_batch(modes_ctx *ctx, Slot &s) {
         CK(ctx, cudaMemcpyAsync(s.h_gr_flags + 20, s.gr.cache_out, 1024 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
     }
     CK(ctx, cudaMemcpyAsync(s.h_counters, s.d_counters, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
+    if (s.levels) CK(ctx, cudaMemcpyAsync(s.h_levels, s.d_levels, s.n_buffers * sizeof(modes_level), cudaMemcpyDeviceToHost, s.stream));
     CK(ctx, cudaEventRecord(s.ev[3], s.stream));
     s.busy = true;
     return 0;
@@ -371,6 +414,7 @@ int collect(modes_ctx *ctx, Slot &s) {
     const double t0 = dbg ? now_ms() : 0;
     if (wait_batch(ctx, s, &n)) return -1;
     s.busy = false;                                     // a repeated (overflowed) batch re-arms the flag
+    append_levels(ctx, s);                              // copied with the counters: on the host since ev[3]
     const double t1 = dbg ? now_ms() : 0;
     if (ctx->cfg.gpu_resolve) {
         // the verdicts were taken on the device: fetch the deliveries, build the structs
@@ -425,6 +469,7 @@ int collect_group(modes_ctx *ctx, int parity) {
         s.busy = false;
         if (wait_batch(g, s, &nc)) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
         s.busy = false;
+        append_levels(ctx, s);                          // groups and GPUs in stream order
         n_tiles[k] = tiles_for((uint64_t)s.n_buffers * kBufSamples);
         if (host_ensure(g, s, nc, n_tiles[k])) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
         if (nc) CK(ctx, cudaMemcpyAsync(s.h_records, s.out_records, nc * sizeof(modes_candidate), cudaMemcpyDeviceToHost, s.stream));
@@ -462,7 +507,7 @@ int run_buffers_multi(modes_ctx *ctx, const uint8_t *host_iq, size_t n_buffers) 
             ctx->buffers_done += (int64_t)nb;
             host_iq += nb * MODES_BUFFER_BYTES;
             n_buffers -= nb;
-            ctx->launches += g->signal ? 3 : 2;
+            ctx->launches += (g->signal ? 3 : 2) + (g->levels ? 1 : 0);
         }
         ctx->group_n[cur] = k;
         if (have_prev && collect_group(ctx, cur ^ 1)) return -1;
@@ -536,6 +581,7 @@ void modes_destroy(modes_ctx *ctx) {
     if (ctx->ev_resolved) cudaEventDestroy(ctx->ev_resolved);
     if (ctx->prof_ready) for (auto &trip : ctx->prof_ev) for (auto &e : trip) cudaEventDestroy(e);
     cudaFreeHost(ctx->pending);
+    cudaFree(ctx->d_lv); cudaFreeHost(ctx->h_lv);
     scratch_destroy(ctx->scratch);
     delete ctx;
 }
@@ -619,6 +665,59 @@ int modes_set_signal(modes_ctx *ctx, int on) {
     return 0;
 }
 
+int modes_set_levels(modes_ctx *ctx, int on) {
+    if (!ctx) return -1;
+    ctx->levels = on != 0;
+    for (modes_ctx *g : ctx->gpus) g->levels = on != 0;
+    return 0;
+}
+
+size_t modes_take_levels(modes_ctx *ctx, modes_level *out, size_t cap) {
+    if (!ctx) return 0;
+    std::vector<modes_level> &q = ctx->level_q;
+    const size_t queued = q.size() - ctx->level_head;
+    if (!out) return queued;
+    const size_t n = cap < queued ? cap : queued;
+    if (n) memcpy(out, q.data() + ctx->level_head, n * sizeof(modes_level));
+    ctx->level_head += n;
+    if (ctx->level_head == q.size()) { q.clear(); ctx->level_head = 0; }
+    else if (ctx->level_head >= 4096 && 2 * ctx->level_head >= q.size()) {
+        q.erase(q.begin(), q.begin() + (ptrdiff_t)ctx->level_head);
+        ctx->level_head = 0;
+    }
+    return n;
+}
+
+int modes_levels_device(modes_ctx *ctx, const void *d_iq, size_t n_buffers, size_t stride_bytes) {
+    if (!ctx) return -1;
+    if (!d_iq || !n_buffers) return fail(ctx, "modes_levels_device: empty input");
+    if (n_buffers > 0xFFFFFFFFu) return fail(ctx, "modes_levels_device: too many buffers: %zu", n_buffers);
+    if (!stride_bytes) stride_bytes = MODES_BUFFER_BYTES;
+    if (((reinterpret_cast<uintptr_t>(d_iq) | stride_bytes) & 15) != 0)
+        return fail(ctx, "modes_levels_device: buffers must be 16-byte aligned");
+    CK(ctx, cudaSetDevice(ctx->cfg.device));
+    cudaStream_t st = ctx->detect.stream;
+    if (levels_ensure(ctx, ctx->d_lv, ctx->h_lv, ctx->lv_cap, n_buffers, ctx->lv_fetched ? nullptr : st)) return -1;
+    launch_levels(static_cast<const uint8_t *>(d_iq), (uint32_t)n_buffers, stride_bytes, ctx->tab, ctx->d_lv, ctx->sm_count, st);
+    CK(ctx, cudaGetLastError());
+    ctx->launches++;
+    CK(ctx, cudaMemcpyAsync(ctx->h_lv, ctx->d_lv, n_buffers * sizeof(modes_level), cudaMemcpyDeviceToHost, st));
+    ctx->lv_n = n_buffers;
+    ctx->lv_fetched = false;
+    return 0;
+}
+
+int modes_levels_fetch(modes_ctx *ctx, modes_level *out) {
+    if (!ctx) return -1;
+    if (!ctx->lv_n) return fail(ctx, "modes_levels_fetch without modes_levels_device");
+    if (!out) return fail(ctx, "modes_levels_fetch: no output array");
+    CK(ctx, cudaSetDevice(ctx->cfg.device));
+    CK(ctx, wait_stream(ctx->detect.stream));
+    ctx->lv_fetched = true;
+    memcpy(out, ctx->h_lv, ctx->lv_n * sizeof(modes_level));
+    return 0;
+}
+
 int modes_set_sink(modes_ctx *ctx, modes_sink_fn fn, void *user) {
     if (!ctx) return -1;
     ctx->out.sink = fn; ctx->out.user = user;
@@ -655,6 +754,9 @@ int modes_reset(modes_ctx *ctx) {
     ctx->pending_len = 0;
     ctx->buffers_done = 0;
     ctx->finished = false;
+    ctx->level_q.clear();
+    ctx->level_head = 0;
+    ctx->eof_buffer = -1;
     memset(ctx->carry, 127, sizeof(ctx->carry));
     return 0;
 }
@@ -687,6 +789,8 @@ int modes_finish(modes_ctx *ctx) {
     // The read that hits EOF still hands a 127-padded buffer to the decoder (dump1090.c:496-510);
     // whether it is decoded is the reference's race, made a switch here.
     memset(ctx->pending + ctx->pending_len, 127, MODES_BUFFER_BYTES - ctx->pending_len);
+    ctx->eof_buffer = ctx->buffers_done;                 // its level record counts the real samples only
+    ctx->eof_samples = (uint32_t)((ctx->pending_len + 1) / 2);
     ctx->pending_len = 0;
     if (ctx->cfg.drop_eof_buffer) return 0;
     return run_buffers(ctx, ctx->pending, 1);

@@ -76,6 +76,12 @@ void launch_eval_frames(const uint8_t *d_frames, modes_frame_eval *d_out, uint32
 // min(counters[0], cand_capacity) records over the same windows the scan and frame evaluation read.
 void launch_signal(const BatchView &in, const DeviceTables &tab, const ScanOutputs &scan, modes_candidate *records,
                    int sm_count, cudaStream_t stream);
+// Levels of n_buffers whole buffers at d_iq + k * stride_bytes (modes_levels.cu): writes out[k],
+// k < n_buffers, with buffer = k and n_samples = kBufSamples.
+void launch_levels(const uint8_t *d_iq, uint32_t n_buffers, uint64_t stride_bytes, const DeviceTables &tab,
+                   modes_level *out, int sm_count, cudaStream_t stream);
+static_assert(sizeof(modes_level) == 40 && offsetof(modes_level, sum_mag) == 16 && offsetof(modes_level, peak) == 32,
+              "level record layout");
 
 // The record layouts are ABI: the signal field took the two bytes every evaluation kernel already wrote as zero.
 static_assert(sizeof(modes_frame_eval) == 24 && offsetof(modes_frame_eval, signal) == 18 && offsetof(modes_frame_eval, crc) == 20,

@@ -43,7 +43,10 @@ constexpr int64_t kBufSamples = MODES_BUFFER_SAMPLES;
 struct Receiver {
     modes_resolver *res = nullptr;
     int64_t buffers = 0;                       // buffers of this receiver decoded so far
+    int64_t submitted = 0;                     // buffers of this receiver submitted so far
     uint8_t carry[MODES_CARRY_BYTES];
+    std::vector<modes_level> levels;           // level records not taken yet, oldest from level_head on
+    size_t level_head = 0;
 };
 
 // A few persistent helper threads: run(n, f) executes f(0..n-1), f(0) on the calling thread.
@@ -101,6 +104,7 @@ struct modes_pool {
     std::vector<Receiver> rx;
     size_t max_batch = 0;
     int signal = 0;                            // modes_pool_set_signal, applied to the slot contexts
+    int levels = 0;                            // modes_pool_set_levels
     std::string err;
     // device half (created on the first modes_pool_submit / _ingest): two batches may be in flight, so
     // that one is uploaded and scanned while the one before it is resolved on the host
@@ -109,6 +113,9 @@ struct modes_pool {
         uint8_t *d_batch = nullptr;            // [2 * max_batch] buffers: pad, data, pad, data, ...
         uint8_t *h_carry = nullptr;            // pinned [max_batch][MODES_CARRY_BYTES]
         std::vector<uint32_t> ids;             // the receivers of the batch in flight
+        std::vector<int64_t> buf_index;        // with levels: each one's own index of its buffer
+        std::vector<modes_level> level_out;
+        bool levels = false;                   // the batch measures its data buffers' levels
         bool busy = false;
     } slot[2];
     unsigned submitted = 0, collected = 0;     // batches so far: slot = number & 1
@@ -338,6 +345,11 @@ int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *c
                 return fail(p, "buffer upload failed: %s", cudaGetErrorString(cudaGetLastError()));
     }
     if (modes_detect_device(sl.ctx, sl.d_batch, 2 * n, nullptr, nullptr, 0, nullptr)) return fail(p, "%s", modes_last_error(sl.ctx));
+    // the data buffers only (every second buffer), on the same stream: no wait before the collect
+    sl.levels = p->levels != 0;
+    if (sl.levels && modes_levels_device(sl.ctx, sl.d_batch + kBuf, n, 2 * kBuf)) return fail(p, "%s", modes_last_error(sl.ctx));
+    sl.buf_index.resize(n);
+    for (size_t i = 0; i < n; i++) sl.buf_index[i] = p->rx[receivers[i]].submitted++;
     // what each receiver carries into its next buffer (dump1090.c:481)
     for (size_t i = 0; i < n; i++)
         memcpy(p->rx[receivers[i]].carry, iq[i] + kBuf - MODES_CARRY_BYTES, MODES_CARRY_BYTES);
@@ -357,6 +369,15 @@ int modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user) {
     p->cands.resize(n_cand ? n_cand : 1);
     p->tiles.resize(modes_tile_count(2 * n));
     if (modes_detect_fetch(sl.ctx, p->cands.data(), p->tiles.data())) return fail(p, "%s", modes_last_error(sl.ctx));
+    if (sl.levels) {
+        sl.level_out.resize(n);
+        if (modes_levels_fetch(sl.ctx, sl.level_out.data())) return fail(p, "%s", modes_last_error(sl.ctx));
+        for (size_t i = 0; i < n; i++) {
+            modes_level r = sl.level_out[i];
+            r.buffer = sl.buf_index[i];
+            p->rx[sl.ids[i]].levels.push_back(r);
+        }
+    }
     sl.busy = false;
     p->collected++;
     return modes_pool_resolve(p, sl.ids.data(), n, p->cands.data(), p->tiles.data(), sink, user);
@@ -380,6 +401,9 @@ int modes_pool_reset(modes_pool *p, uint32_t receiver) {
     if (!p || receiver >= p->rx.size()) return -1;
     Receiver &r = p->rx[receiver];
     r.buffers = 0;
+    r.submitted = 0;
+    r.levels.clear();
+    r.level_head = 0;
     memset(r.carry, 127, sizeof r.carry);
     return modes_resolver_reset(r.res);
 }
@@ -398,6 +422,28 @@ int modes_pool_set_signal(modes_pool *p, int on) {
     for (modes_pool::Slot &sl : p->slot)
         if (sl.ctx) modes_set_signal(sl.ctx, p->signal);
     return 0;
+}
+
+int modes_pool_set_levels(modes_pool *p, int on) {
+    if (!p) return -1;
+    p->levels = on != 0;
+    return 0;
+}
+
+size_t modes_pool_take_levels(modes_pool *p, uint32_t receiver, modes_level *out, size_t cap) {
+    if (!p || receiver >= p->rx.size()) return 0;
+    Receiver &r = p->rx[receiver];
+    const size_t queued = r.levels.size() - r.level_head;
+    if (!out) return queued;
+    const size_t n = cap < queued ? cap : queued;
+    if (n) memcpy(out, r.levels.data() + r.level_head, n * sizeof(modes_level));
+    r.level_head += n;
+    if (r.level_head == r.levels.size()) { r.levels.clear(); r.level_head = 0; }
+    else if (r.level_head >= 4096 && 2 * r.level_head >= r.levels.size()) {
+        r.levels.erase(r.levels.begin(), r.levels.begin() + (ptrdiff_t)r.level_head);
+        r.level_head = 0;
+    }
+    return n;
 }
 
 int64_t modes_pool_buffers(const modes_pool *p, uint32_t receiver) {

@@ -14,15 +14,47 @@
  * --beast writes one Beast binary frame per message instead (what the dump1090 descendants send on
  * port 30005: 12 MHz timestamp = 6 x sample position, signal level measured on the GPU); it excludes
  * --raw, --onlyaddr, --sbs and --aircraft-json, which write to stdout as well.
+ * --levels measures every decoded buffer's noise, peak and clipping on the GPU and prints one
+ * summary line on stderr at the end (buffers, samples, noise floor and peak in dBFS on the scale of
+ * the Beast signal level, clipped samples and their fraction); it combines with every output mode
+ * and leaves stdout as it is.
  * The live-radio, networking and interactive options are out of scope.
  */
+#include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 #include "modes_b200.h"
 
 static int opt_raw = 0, opt_onlyaddr = 0, opt_stats = 0, opt_check_crc = 1, opt_sbs = 0, opt_json = 0, opt_beast = 0;
+static int opt_levels = 0;
 static modes_tracker *tracker = NULL;
+
+/* --levels: totals over the records taken so far */
+static struct { long long buffers; unsigned long long samples, clipped; unsigned __int128 power; unsigned peak; } lv;
+
+static void take_levels(modes_ctx *ctx) {
+    modes_level r[256];
+    size_t n;
+    while ((n = modes_take_levels(ctx, r, 256)) > 0)
+        for (size_t i = 0; i < n; i++) {
+            lv.buffers++;
+            lv.samples += r[i].n_samples;
+            lv.clipped += r[i].clipped;
+            lv.power += r[i].sum_power;
+            if (r[i].peak > lv.peak) lv.peak = r[i].peak;
+        }
+}
+
+static void print_levels(void) {
+    fprintf(stderr, "levels: %lld buffers, %llu samples, ", lv.buffers, lv.samples);
+    if (!lv.samples) { fprintf(stderr, "noise n/a, peak n/a, clipped 0\n"); return; }
+    const double fs2 = 65535.0 * 65535.0;
+    const double noise = lv.power ? 10.0 * log10((double)lv.power / (double)lv.samples / fs2) : -INFINITY;
+    const double peak = lv.peak ? 20.0 * log10(lv.peak / 65535.0) : -INFINITY;
+    fprintf(stderr, "noise %.2f dBFS, peak %.2f dBFS, clipped %llu (%.6f)\n", noise, peak, lv.clipped,
+            (double)lv.clipped / (double)lv.samples);
+}
 
 /* Message sink: the --raw / --onlyaddr forms of displayModesMessage
  * (dump1090.c:1318-1331) and, by default, the full text (:1314-1450) via modes_format_message(). */
@@ -78,6 +110,7 @@ int main(int argc, char **argv) {
         else if (!strcmp(argv[j], "--sbs")) opt_sbs = 1;
         else if (!strcmp(argv[j], "--aircraft-json")) opt_json = 1;
         else if (!strcmp(argv[j], "--beast")) opt_beast = 1;
+        else if (!strcmp(argv[j], "--levels")) opt_levels = 1;
         else if (!strcmp(argv[j], "--device") && more) cfg.device = atoi(argv[++j]);
         else if (!strcmp(argv[j], "--gpus") && more) cfg.n_gpus = atoi(argv[++j]);
         else if (!strcmp(argv[j], "--chunk") && more) chunk = (size_t)strtoull(argv[++j], NULL, 10);
@@ -101,14 +134,17 @@ int main(int argc, char **argv) {
         if (!tracker) { fprintf(stderr, "out of memory\n"); return 1; }
     }
     if (opt_beast) modes_set_signal(ctx, 1);
+    if (opt_levels) modes_set_levels(ctx, 1);
     modes_set_sink(ctx, on_message, NULL);
     unsigned char *buf = (unsigned char *)modes_host_alloc(chunk);
     if (!buf) { fprintf(stderr, "out of memory\n"); return 1; }
     size_t n;
     while ((n = fread(buf, 1, chunk, f)) > 0) {
         if (modes_process(ctx, buf, n)) { fprintf(stderr, "modes_process: %s\n", modes_last_error(ctx)); return 1; }
+        if (opt_levels) take_levels(ctx);
     }
     if (modes_finish(ctx)) { fprintf(stderr, "modes_finish: %s\n", modes_last_error(ctx)); return 1; }
+    if (opt_levels) { take_levels(ctx); print_levels(); }
     if (opt_stats) {                                        /* dump1090.c:2993-3006 */
         modes_stats st;
         modes_get_stats(ctx, &st);

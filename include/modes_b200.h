@@ -408,6 +408,49 @@ int    modes_pool_set_signal(modes_pool *p, int on);
  * capacity bytes and no terminating NUL.  Pure host code. */
 size_t modes_format_beast(const modes_message *mm, uint8_t *buf, size_t capacity);
 
+/* ---- receiver levels: noise floor, peak and clipping per buffer --------------------------------
+ * What an operator reads of a receiver besides its messages: how loud the channel is, how close the
+ * strongest samples come to full scale, and whether the ADC clips (gain too high).  One record per
+ * reference buffer decoded, over the buffer's own samples (the 238 it carries over belong to the
+ * buffer before it, so every stream sample is counted once), with m = the reference's magnitude
+ * round(360 * sqrt((I-127)^2 + (Q-127)^2)) (dump1090.c:359-364, :1454-1469), m <= 65167.
+ * Every field is an integer, so records do not depend on the order of the GPU's reduction.
+ * On the scale of modes_message.signal (so that SNR = signal dB - noise dB):
+ *     noise dBFS = 10 log10(sum sum_power / sum n_samples / 65535^2)
+ *     peak dBFS  = 20 log10(max peak / 65535)
+ *     clipped fraction = sum clipped / sum n_samples */
+typedef struct modes_level {
+    int64_t  buffer;            /* stream index of the buffer (in a pool: the receiver's own buffer index) */
+    uint32_t n_samples;         /* stream samples in it: MODES_BUFFER_SAMPLES, fewer only in the EOF buffer
+                                   (a trailing odd byte counts as a sample); the EOF padding adds nothing */
+    uint32_t clipped;           /* samples whose I or Q byte is 0 or 255 */
+    uint64_t sum_mag;           /* sum of m */
+    uint64_t sum_power;         /* sum of m^2 */
+    uint32_t peak;              /* max m, 0 for a buffer without signal */
+    uint32_t pad;
+} modes_level;
+
+/* Level measurement is off by default.  When it is on, every batch the streaming decode submits
+ * afterwards runs one more kernel over its buffers in HBM (one more launch per batch), and the
+ * records are queued on the context in stream order: one per buffer decoded, none for an EOF buffer
+ * dropped by drop_eof_buffer, n_samples = 0 for an all-padding EOF buffer that is decoded.  On an
+ * n_gpus > 1 context the setting reaches every GPU.  modes_reset drops the queue.
+ * modes_take_levels moves the oldest min(cap, queued) records to out and returns how many it moved;
+ * with out = NULL it moves nothing and returns how many are queued.  Returns 0 / -1 (NULL handle). */
+int    modes_set_levels(modes_ctx *ctx, int on);
+size_t modes_take_levels(modes_ctx *ctx, modes_level *out, size_t cap);
+/* Stage level: records of n_buffers whole buffers in device memory, buffer k at d_iq + k * stride_bytes
+ * (16-byte aligned; stride 0 = MODES_BUFFER_BYTES), queued on the context's stream without waiting.
+ * modes_levels_fetch waits and copies the n_buffers records of the last call to out in call order,
+ * with buffer = k and n_samples = MODES_BUFFER_SAMPLES.  Independent of modes_set_levels. */
+int    modes_levels_device(modes_ctx *ctx, const void *d_iq, size_t n_buffers, size_t stride_bytes);
+int    modes_levels_fetch(modes_ctx *ctx, modes_level *out);
+/* The pool measures the data buffers of every batch submitted while the switch is on (never the pad
+ * buffers) and queues each receiver's records, buffer = the receiver's own buffer index, in its stream
+ * order; modes_pool_reset clears the receiver's queue.  Same take convention as above. */
+int    modes_pool_set_levels(modes_pool *p, int on);
+size_t modes_pool_take_levels(modes_pool *p, uint32_t receiver, modes_level *out, size_t cap);
+
 #ifdef __cplusplus
 }
 #endif
