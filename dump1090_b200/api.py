@@ -42,7 +42,7 @@ _MSG_B = ("ew_dir ew_velocity ns_dir ns_velocity vert_rate_source vert_rate_sign
 
 class Message(C.Structure):
     """struct modes_message == fields of struct modesMessage (dump1090.c:211-260)."""
-    _fields_ = ([("msg", C.c_uint8 * 14), ("pad0", C.c_uint8 * 2), ("msgbits", C.c_int32),
+    _fields_ = ([("msg", C.c_uint8 * 14), ("recovered", C.c_uint8), ("pad0", C.c_uint8), ("msgbits", C.c_int32),
                  ("msgtype", C.c_int32), ("crcok", C.c_int32), ("crc", C.c_uint32)]
                 + [(n, C.c_int32) for n in _MSG_A]
                 + [("flight", C.c_char * 9), ("pad1", C.c_char * 3)]
@@ -126,6 +126,20 @@ LEVEL_DTYPE = np.dtype([("buffer", "<i8"), ("n_samples", "<u4"), ("clipped", "<u
 assert LEVEL_DTYPE.itemsize == C.sizeof(Level) == 40
 FULL_SCALE = 65535                        # the dBFS reference of rssi_dbfs() and level_summary()
 
+# struct modes_recovered: one soft-decision recovery record per candidate (modes_set_recovery)
+RECOVERED_DTYPE = np.dtype([("msg", "u1", 14), ("status", "u1"), ("nflips", "u1"), ("signal", "<u2"), ("pad", "u1", 2)])
+assert RECOVERED_DTYPE.itemsize == 20
+RECOVER_BITS = 10                         # MODES_RECOVER_BITS
+RECOVER_INELIGIBLE, RECOVER_FOUND, RECOVER_AMBIGUOUS, RECOVER_NOT_FOUND = 0, 1, 2, 3
+RECOVERY_STAT_NAMES = ["considered", "found", "ambiguous", "unknown_address", "dropped", "delivered"]
+
+
+class RecoveryStats(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in RECOVERY_STAT_NAMES]
+
+    def as_dict(self) -> dict:
+        return {n: int(getattr(self, n)) for n in RECOVERY_STAT_NAMES}
+
 
 def level_summary(records) -> dict:
     """Totals of level records (LEVEL_DTYPE): buffers, n_samples, clipped, and on the scale of
@@ -165,7 +179,10 @@ EXPORTS = ["modes_abi_version", "modes_default_config", "modes_create", "modes_d
            "modes_pool_stats", "modes_pool_reset", "modes_pool_buffers", "modes_pool_set_output", "modes_pool_output_count",
            "modes_pool_submit", "modes_pool_collect", "modes_set_signal", "modes_pool_set_signal", "modes_format_beast",
            "modes_set_levels", "modes_take_levels", "modes_levels_device", "modes_levels_fetch",
-           "modes_pool_set_levels", "modes_pool_take_levels"]
+           "modes_pool_set_levels", "modes_pool_take_levels",
+           "modes_set_recovery", "modes_get_recovery_stats", "modes_recover_device", "modes_recover_fetch",
+           "modes_resolver_run_recovered", "modes_resolver_run_shards_recovered", "modes_resolver_recovery_stats", "modes_pool_set_recovery",
+           "modes_pool_recovery_stats"]
 
 
 def lib():
@@ -269,6 +286,17 @@ def lib():
         L.modes_pool_set_levels.argtypes = [C.c_void_p, C.c_int]
         L.modes_pool_take_levels.restype = C.c_size_t
         L.modes_pool_take_levels.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t]
+        L.modes_set_recovery.argtypes = [C.c_void_p, C.c_int]
+        L.modes_get_recovery_stats.argtypes = [C.c_void_p, C.POINTER(RecoveryStats)]
+        L.modes_recover_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+        L.modes_recover_fetch.argtypes = [C.c_void_p, C.c_void_p]
+        L.modes_resolver_run_recovered.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int64,
+                                                   SINK_FN, C.c_void_p]
+        L.modes_resolver_run_shards_recovered.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                          C.c_void_p, C.c_void_p, SINK_FN, C.c_void_p]
+        L.modes_resolver_recovery_stats.argtypes = [C.c_void_p, C.POINTER(RecoveryStats)]
+        L.modes_pool_set_recovery.argtypes = [C.c_void_p, C.c_int]
+        L.modes_pool_recovery_stats.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(RecoveryStats)]
         _lib = L
     return _lib
 
@@ -342,9 +370,11 @@ class Decoder:
     """One GPU decode context (modes_create ... modes_destroy).  signal=True measures the signal
     level of every decoded frame on the GPU (modes_set_signal): Message.signal, rssi_dbfs(), beast().
     levels=True measures every decoded buffer's noise, peak and clipping on the GPU
-    (modes_set_levels): take_levels(), level_summary()."""
+    (modes_set_levels): take_levels(), level_summary().  recover=True adds weak DF17/DF18 frames of
+    known aircraft found by a soft-decision search on the GPU (modes_set_recovery), marked
+    Message.recovered: recovery_stats()."""
 
-    def __init__(self, signal: bool = False, levels: bool = False, **cfg):
+    def __init__(self, signal: bool = False, levels: bool = False, recover: bool = False, **cfg):
         self.cfg = make_config(**cfg)
         self._h = lib().modes_create(C.byref(self.cfg))
         if not self._h:
@@ -353,6 +383,8 @@ class Decoder:
             self.set_signal(True)
         if levels:
             self.set_levels(True)
+        if recover:
+            self.set_recovery(True)
         self._collector = _Collector()
         lib().modes_set_sink(self._h, self._collector.fn, None)
 
@@ -437,6 +469,15 @@ class Decoder:
     def set_levels(self, on: bool) -> None:
         """Measure the buffers' levels for batches submitted from now on (modes_set_levels)."""
         self._check(lib().modes_set_levels(self._h, int(bool(on))))
+
+    def set_recovery(self, on: bool) -> None:
+        """Recover weak DF17/DF18 frames in batches submitted from now on (modes_set_recovery)."""
+        self._check(lib().modes_set_recovery(self._h, int(bool(on))))
+
+    def recovery_stats(self) -> dict:
+        st = RecoveryStats()
+        self._check(lib().modes_get_recovery_stats(self._h, C.byref(st)))
+        return st.as_dict()
 
     def take_levels(self) -> np.ndarray:
         """The queued level records (LEVEL_DTYPE), oldest first, in stream order; the queue is emptied."""
@@ -533,6 +574,18 @@ class Decoder:
         self._check(lib().modes_levels_fetch(self._h, _ptr(out)))
         return out
 
+    def recover_device(self, d_out_ptr: int = 0, capacity: int = 0) -> None:
+        """Recovery records of the last detect_device / detect_host batch, into device memory, or (0) into
+        the context's own buffer for recover_fetch()."""
+        self._check(lib().modes_recover_device(self._h, C.c_void_p(d_out_ptr or None), capacity))
+
+    def recover_fetch(self) -> np.ndarray:
+        """The records of the last recover_device(0) call (RECOVERED_DTYPE), one per candidate record."""
+        n = self.detect_wait()
+        out = np.zeros(max(n, 1), dtype=RECOVERED_DTYPE)
+        self._check(lib().modes_recover_fetch(self._h, _ptr(out)))
+        return out[:n]
+
     def publish_count(self, dst_ptr: int) -> None:
         self._check(lib().modes_detect_publish_count(self._h, C.c_void_p(dst_ptr)))
 
@@ -549,6 +602,13 @@ class Decoder:
         return int(lib().modes_stream(self._h) or 0)
 
 
+def _recovery_records(recovered, cands: np.ndarray) -> np.ndarray:
+    rec = np.ascontiguousarray(recovered, dtype=RECOVERED_DTYPE)
+    if rec.size < cands.size:
+        raise ValueError(f"{rec.size} recovery records for {cands.size} candidates: one per candidate is needed")
+    return rec
+
+
 class Resolver:
     """The sequential half alone (no device): modes_resolver_*."""
 
@@ -557,19 +617,33 @@ class Resolver:
         self._h = lib().modes_resolver_create(C.byref(self.cfg))
         self._collector = _Collector()
 
-    def run(self, cands: np.ndarray, tiles: np.ndarray, buffer_base: int = 0) -> None:
+    def run(self, cands: np.ndarray, tiles: np.ndarray, buffer_base: int = 0, recovered: np.ndarray | None = None) -> None:
+        """recovered: RECOVERED_DTYPE records, one per candidate, to add recovered messages
+        (modes_resolver_run_recovered); None runs the reference's resolve alone."""
         cands = np.ascontiguousarray(cands)
         tiles = np.ascontiguousarray(tiles)
         fn = C.cast(None, SINK_FN) if getattr(self, "_native", False) else self._collector.fn
-        rc = lib().modes_resolver_run(self._h, _ptr(cands), _ptr(tiles), tiles.size, buffer_base, fn, None)
+        if recovered is None:
+            rc = lib().modes_resolver_run(self._h, _ptr(cands), _ptr(tiles), tiles.size, buffer_base, fn, None)
+        else:
+            rec = _recovery_records(recovered, cands)
+            rc = lib().modes_resolver_run_recovered(self._h, _ptr(cands), _ptr(rec), _ptr(tiles), tiles.size, buffer_base,
+                                                    fn, None)
         if rc:
             raise RuntimeError("modes_resolver_run failed")
+
+    def recovery_stats(self) -> dict:
+        st = RecoveryStats()
+        if lib().modes_resolver_recovery_stats(self._h, C.byref(st)):
+            raise RuntimeError("modes_resolver_recovery_stats failed")
+        return st.as_dict()
 
     def reset_state(self) -> None:
         lib().modes_resolver_reset(self._h)
 
-    def run_shards(self, shards) -> None:
-        """shards: [(cands ndarray, tiles ndarray, buffer_base)] in stream order; resolved concurrently."""
+    def run_shards(self, shards, recovered=None) -> None:
+        """shards: [(cands ndarray, tiles ndarray, buffer_base)] in stream order; resolved concurrently.
+        recovered: a list of RECOVERED_DTYPE arrays, one per shard (modes_resolver_run_shards_recovered)."""
         n = len(shards)
         keep = [(np.ascontiguousarray(c), np.ascontiguousarray(t)) for c, t, _ in shards]
         cp = (C.c_void_p * n)(*[c.ctypes.data for c, _ in keep])
@@ -577,7 +651,15 @@ class Resolver:
         nt = (C.c_size_t * n)(*[t.size for _, t in keep])
         bb = (C.c_int64 * n)(*[int(b) for _, _, b in shards])
         fn = C.cast(None, SINK_FN) if getattr(self, "_native", False) else self._collector.fn
-        if lib().modes_resolver_run_shards(self._h, n, cp, tp, nt, bb, fn, None):
+        if recovered is None:
+            rc = lib().modes_resolver_run_shards(self._h, n, cp, tp, nt, bb, fn, None)
+        else:
+            if len(recovered) != n:
+                raise ValueError(f"{len(recovered)} recovery arrays for {n} shards")
+            recs = [_recovery_records(r, c) for r, (c, _) in zip(recovered, keep)]
+            rp = (C.c_void_p * n)(*[r.ctypes.data for r in recs])
+            rc = lib().modes_resolver_run_shards_recovered(self._h, n, cp, rp, tp, nt, bb, fn, None)
+        if rc:
             raise RuntimeError("modes_resolver_run_shards failed")
 
     # ---- one shard of a sharded decode (see include/modes_b200.h and sharded.resolve_distributed)
@@ -649,9 +731,11 @@ class ReceiverPool:
     """modes_pool_*: independent 2 MHz streams (one address cache, carry, skip state and set of
     statistics each, as one dump1090 process keeps per receiver), one buffer of each decoded per
     batch.  Messages are collected per receiver (`take(receiver)`).  signal=True: as for Decoder.
-    levels=True: level records of every receiver's buffers (`take_levels(receiver)`)."""
+    levels=True: level records of every receiver's buffers (`take_levels(receiver)`).
+    recover=True: as for Decoder, with statistics per receiver (`recovery_stats(receiver)`)."""
 
-    def __init__(self, n_receivers: int, max_batch: int = 0, signal: bool = False, levels: bool = False, **cfg):
+    def __init__(self, n_receivers: int, max_batch: int = 0, signal: bool = False, levels: bool = False,
+                 recover: bool = False, **cfg):
         self.cfg = make_config(**cfg)
         self.n = n_receivers
         self._h = lib().modes_pool_create(C.byref(self.cfg), n_receivers, max_batch)
@@ -661,6 +745,8 @@ class ReceiverPool:
             self.set_signal(True)
         if levels:
             self.set_levels(True)
+        if recover:
+            self.set_recovery(True)
         self.messages = [[] for _ in range(n_receivers)]
         self._fn = POOL_SINK_FN(self._on)
 
@@ -739,6 +825,15 @@ class ReceiverPool:
     def set_levels(self, on: bool) -> None:
         """Measure the levels of batches submitted from now on (modes_pool_set_levels)."""
         self._check(lib().modes_pool_set_levels(self._h, int(bool(on))))
+
+    def set_recovery(self, on: bool) -> None:
+        """Recover weak DF17/DF18 frames in batches submitted from now on (modes_pool_set_recovery)."""
+        self._check(lib().modes_pool_set_recovery(self._h, int(bool(on))))
+
+    def recovery_stats(self, receiver: int) -> dict:
+        st = RecoveryStats()
+        self._check(lib().modes_pool_recovery_stats(self._h, receiver, C.byref(st)))
+        return st.as_dict()
 
     def take_levels(self, receiver: int) -> np.ndarray:
         """The receiver's queued level records (LEVEL_DTYPE), its own buffer indices, oldest first."""

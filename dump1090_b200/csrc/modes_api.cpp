@@ -46,6 +46,9 @@ struct Slot {
     modes_delivery *h_deliveries = nullptr; size_t h_deliveries_cap = 0;   // pinned
     // modes_set_levels: one record per buffer of the batch (device, and its pinned host copy)
     modes_level *d_levels = nullptr, *h_levels = nullptr; size_t levels_cap = 0;
+    // modes_set_recovery / modes_recover_device: one record per candidate (device, and its pinned host copy)
+    modes_recovered *d_recovered = nullptr; size_t rec_cap = 0;
+    modes_recovered *h_recovered = nullptr; size_t h_rec_cap = 0;
     // in-flight batch
     bool busy = false;
     size_t n_buffers = 0;
@@ -53,6 +56,9 @@ struct Slot {
     const void *batch_iq = nullptr;   // device address the batch was scanned from
     bool own_outputs = true;          // results in this slot's own buffers (growable)
     bool levels = false;              // the batch measures levels (the switch as it was at submit)
+    bool recover = false;             // the batch runs the recovery pass (streaming: the switch as it was at submit)
+    bool signal = false;              // the signal switch as it was at submit
+    modes_recovered *rec_ext = nullptr; uint32_t rec_ext_cap = 0;   // modes_recover_device's d_out (nullptr: own buffer)
     uint32_t want_cap = 0;            // grow the candidate buffers to at least this on the next ensure
     // where this batch's results live (own workspace unless the caller supplied memory)
     modes_candidate *out_records = nullptr;
@@ -99,6 +105,7 @@ struct modes_ctx {
     uint64_t launches = 0;
     bool signal = false;                  // modes_set_signal: measure the signal level of decoded attempts
     bool levels = false;                  // modes_set_levels: measure every decoded buffer's levels
+    bool recover = false;                 // modes_set_recovery: soft-decision recovery of weak DF17/18 frames
     std::vector<modes_level> level_q;     // records not taken yet, oldest from level_head on
     size_t level_head = 0;
     int64_t eof_buffer = -1;              // modes_finish: stream index of the EOF buffer and its real samples
@@ -193,6 +200,7 @@ void slot_free(Slot &s) {
     cudaFree(s.gr.n_deliv); cudaFree(s.gr.offsets); cudaFree(s.gr.flags); cudaFree(s.gr.stats_out); cudaFree(s.gr.out);
     cudaFreeHost(s.h_gr_flags); cudaFreeHost(s.h_deliveries);
     cudaFree(s.d_levels); cudaFreeHost(s.h_levels);
+    cudaFree(s.d_recovered); cudaFreeHost(s.h_recovered);
     for (auto &e : s.ev) if (e) cudaEventDestroy(e);
     for (auto &e : s.halo_ev) if (e) cudaEventDestroy(e);
     if (s.stream) cudaStreamDestroy(s.stream);
@@ -222,6 +230,16 @@ int slot_ensure(modes_ctx *ctx, Slot &s, uint64_t n_samples, bool need_iq, bool 
         CK(ctx, cudaMalloc(&s.d_tiles, (size_t)nt * sizeof(modes_tile)));
         s.tiles_cap = nt;
     }
+    return 0;
+}
+
+// Pinned room for the recovery records of n candidates.
+int recovered_ensure(modes_ctx *ctx, Slot &s, size_t n) {
+    if (s.h_rec_cap >= n) return 0;
+    cudaFreeHost(s.h_recovered); s.h_recovered = nullptr; s.h_rec_cap = 0;
+    const size_t cap = n + n / 2 + 1024;
+    CK(ctx, cudaMallocHost(&s.h_recovered, cap * sizeof(modes_recovered)));
+    s.h_rec_cap = cap;
     return 0;
 }
 
@@ -303,6 +321,9 @@ int submit(modes_ctx *ctx, Slot &s, const uint8_t *host_iq, const void *d_iq, si
     if (d_records_ext && cap_ext > s.want_cap) s.want_cap = cap_ext;
     if (slot_ensure(ctx, s, n_samples, host_iq != nullptr, d_records_ext == nullptr)) return -1;
     s.levels = ctx->levels && &s != &ctx->detect;
+    s.recover = ctx->recover && &s != &ctx->detect;       // the stage level asks with modes_recover_device
+    s.rec_ext = nullptr; s.rec_ext_cap = 0;
+    s.signal = ctx->signal;
     if (s.levels && levels_ensure(ctx, s.d_levels, s.h_levels, s.levels_cap, n_buffers, nullptr)) return -1;   // collected
     if (host_iq) {
         CK(ctx, cudaMemcpyAsync(s.d_iq, host_iq, n_samples * 2, cudaMemcpyHostToDevice, s.stream));
@@ -323,6 +344,26 @@ int submit(modes_ctx *ctx, Slot &s, const uint8_t *host_iq, const void *d_iq, si
     s.out_tiles = d_tiles_ext ? d_tiles_ext : s.d_tiles;
     s.out_cap = d_records_ext ? (cap_ext < s.cand_cap ? cap_ext : s.cand_cap) : s.cand_cap;
     return launch_batch(ctx, s);
+}
+
+// The recovery pass over the slot's batch and records, into the caller's array or the slot's own
+// (grown to the record capacity).
+int launch_recovery(modes_ctx *ctx, Slot &s, const BatchView &in, const ScanOutputs &so) {
+    modes_recovered *dst = s.rec_ext;
+    uint32_t cap = s.rec_ext_cap < s.out_cap ? s.rec_ext_cap : s.out_cap;
+    if (!dst) {
+        if (s.rec_cap < s.out_cap) {
+            cudaFree(s.d_recovered); s.d_recovered = nullptr; s.rec_cap = 0;
+            CK(ctx, cudaMalloc(&s.d_recovered, (size_t)s.out_cap * sizeof(modes_recovered)));
+            s.rec_cap = s.out_cap;
+        }
+        dst = s.d_recovered;
+        cap = s.out_cap;
+    }
+    launch_recover(in, ctx->tab, so, s.out_records, cap, dst, ctx->sm_count, s.stream);
+    CK(ctx, cudaGetLastError());
+    ctx->launches++;
+    return 0;
 }
 
 // The two kernels over the slot's staged batch (also used to repeat a batch that overflowed).
@@ -355,6 +396,7 @@ int launch_batch(modes_ctx *ctx, Slot &s) {
         launch_levels(in.body, (uint32_t)s.n_buffers, MODES_BUFFER_BYTES, ctx->tab, s.d_levels, ctx->sm_count, s.stream);
     CK(ctx, cudaGetLastError());
     ctx->launches += (ctx->signal ? 3 : 2) + (s.levels ? 1 : 0);
+    if (s.recover && launch_recovery(ctx, s, in, so)) return -1;
     if (ctx->cfg.gpu_resolve && s.own_outputs && &s != &ctx->detect) {
         if (gpu_resolve_ensure(ctx, s)) return -1;
         // the address cache comes from the previous batch's resolve (other slot, other stream)
@@ -440,12 +482,15 @@ int collect(modes_ctx *ctx, Slot &s) {
     }
     const size_t nt = tiles_for((uint64_t)s.n_buffers * kBufSamples);
     if (host_ensure(ctx, s, n, nt)) return -1;
+    if (s.recover && recovered_ensure(ctx, s, n)) return -1;
     if (n) CK(ctx, cudaMemcpyAsync(s.h_records, s.out_records, n * sizeof(modes_candidate), cudaMemcpyDeviceToHost, s.stream));
+    if (n && s.recover) CK(ctx, cudaMemcpyAsync(s.h_recovered, s.d_recovered, n * sizeof(modes_recovered), cudaMemcpyDeviceToHost, s.stream));
     CK(ctx, cudaMemcpyAsync(s.h_tiles, s.out_tiles, nt * sizeof(modes_tile), cudaMemcpyDeviceToHost, s.stream));
     CK(ctx, wait_stream(s.stream));
     const double t2 = dbg ? now_ms() : 0;
-    ResolveConfig rc{ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->cfg.check_crc};
-    resolve_candidates(ctx->rs, rc, s.h_records, s.h_tiles, nt, s.buffer_base, ctx->out, ctx->scratch);
+    ResolveConfig rc{ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->cfg.check_crc, s.signal ? 1 : 0};
+    resolve_candidates(ctx->rs, rc, s.h_records, s.h_tiles, nt, s.buffer_base, ctx->out, ctx->scratch,
+                       s.recover ? s.h_recovered : nullptr);
     if (dbg) fprintf(stderr, "[collect] %zu buffers, %llu cands: wait %.3f ms, d2h %.3f ms, resolve %.3f ms (t=%.3f)\n",
                      s.n_buffers, (unsigned long long)n, t1 - t0, t2 - t1, now_ms() - t2, now_ms());
     return 0;
@@ -461,6 +506,8 @@ int collect_group(modes_ctx *ctx, int parity) {
     std::vector<const modes_tile *> tiles(n);
     std::vector<size_t> n_tiles(n);
     std::vector<int64_t> base(n);
+    std::vector<const modes_recovered *> recovered(n, nullptr);
+    bool any_recover = false, signal = false;
     for (size_t k = 0; k < n; k++) {
         modes_ctx *g = ctx->gpus[k];
         Slot &s = g->slot[parity];
@@ -473,6 +520,13 @@ int collect_group(modes_ctx *ctx, int parity) {
         n_tiles[k] = tiles_for((uint64_t)s.n_buffers * kBufSamples);
         if (host_ensure(g, s, nc, n_tiles[k])) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
         if (nc) CK(ctx, cudaMemcpyAsync(s.h_records, s.out_records, nc * sizeof(modes_candidate), cudaMemcpyDeviceToHost, s.stream));
+        if (s.recover) {
+            if (recovered_ensure(g, s, nc)) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
+            if (nc) CK(ctx, cudaMemcpyAsync(s.h_recovered, s.d_recovered, nc * sizeof(modes_recovered), cudaMemcpyDeviceToHost, s.stream));
+            recovered[k] = s.h_recovered;
+            any_recover = true;
+        }
+        signal = s.signal;
         CK(ctx, cudaMemcpyAsync(s.h_tiles, s.out_tiles, n_tiles[k] * sizeof(modes_tile), cudaMemcpyDeviceToHost, s.stream));
         cands[k] = s.h_records; tiles[k] = s.h_tiles; base[k] = s.buffer_base;
     }
@@ -480,8 +534,12 @@ int collect_group(modes_ctx *ctx, int parity) {
         CK(ctx, cudaSetDevice(ctx->gpus[k]->cfg.device));
         CK(ctx, wait_stream(ctx->gpus[k]->slot[parity].stream));
     }
-    ResolveConfig rc{ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->cfg.check_crc};
-    resolve_shards(ctx->rs, rc, n, cands.data(), tiles.data(), n_tiles.data(), base.data(), ctx->out, ctx->scratch);
+    ResolveConfig rc{ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->cfg.check_crc, signal ? 1 : 0};
+    if (any_recover)   // the switch is the same on every GPU of a group: all or none of the shards have records
+        for (size_t k = 0; k < n; k++)
+            if (!recovered[k]) return fail(ctx, "internal: recovery records missing for GPU %d", ctx->gpus[k]->cfg.device);
+    resolve_shards(ctx->rs, rc, n, cands.data(), tiles.data(), n_tiles.data(), base.data(), ctx->out, ctx->scratch,
+                   any_recover ? recovered.data() : nullptr);
     return 0;
 }
 
@@ -507,7 +565,7 @@ int run_buffers_multi(modes_ctx *ctx, const uint8_t *host_iq, size_t n_buffers) 
             ctx->buffers_done += (int64_t)nb;
             host_iq += nb * MODES_BUFFER_BYTES;
             n_buffers -= nb;
-            ctx->launches += (g->signal ? 3 : 2) + (g->levels ? 1 : 0);
+            ctx->launches += (g->signal ? 3 : 2) + (g->levels ? 1 : 0) + (g->recover ? 1 : 0);
         }
         ctx->group_n[cur] = k;
         if (have_prev && collect_group(ctx, cur ^ 1)) return -1;
@@ -718,6 +776,50 @@ int modes_levels_fetch(modes_ctx *ctx, modes_level *out) {
     return 0;
 }
 
+int modes_set_recovery(modes_ctx *ctx, int on) {
+    if (!ctx) return -1;
+    // the device resolve's read-set bookkeeping has no recovery rule
+    if (on && ctx->cfg.gpu_resolve) return fail(ctx, "modes_set_recovery: recovery cannot be combined with gpu_resolve");
+    ctx->recover = on != 0;
+    for (modes_ctx *g : ctx->gpus) g->recover = on != 0;
+    return 0;
+}
+
+int modes_get_recovery_stats(const modes_ctx *ctx, modes_recovery_stats *out) {
+    if (!ctx || !out) return -1;
+    *out = ctx->rs.rstats;
+    return 0;
+}
+
+int modes_recover_device(modes_ctx *ctx, void *d_out, size_t capacity) {
+    if (!ctx) return -1;
+    Slot &s = ctx->detect;
+    if (!s.batch_iq) return fail(ctx, "modes_recover_device without modes_detect_device");
+    if (d_out && !capacity) return fail(ctx, "modes_recover_device: capacity 0");
+    if ((reinterpret_cast<uintptr_t>(d_out) & 3) != 0) return fail(ctx, "modes_recover_device: output must be 4-byte aligned");
+    CK(ctx, cudaSetDevice(ctx->cfg.device));
+    s.recover = true;
+    s.rec_ext = static_cast<modes_recovered *>(d_out);
+    s.rec_ext_cap = capacity > 0xFFFFFFF0ull ? 0xFFFFFFF0u : (uint32_t)capacity;
+    // a batch that wait_batch repeats after an overflow runs the pass again (launch_batch)
+    BatchView in{static_cast<const uint8_t *>(s.batch_iq), s.d_halo, (uint64_t)s.n_buffers * kBufSamples};
+    ScanOutputs so{s.d_cand_v, s.out_cap, s.out_tiles, s.d_counters};
+    return launch_recovery(ctx, s, in, so);
+}
+
+int modes_recover_fetch(modes_ctx *ctx, modes_recovered *out) {
+    if (!ctx) return -1;
+    Slot &s = ctx->detect;
+    if (!s.recover || s.rec_ext) return fail(ctx, "modes_recover_fetch without modes_recover_device(ctx, NULL, ...)");
+    if (!out) return fail(ctx, "modes_recover_fetch: no output array");
+    CK(ctx, cudaSetDevice(ctx->cfg.device));
+    uint64_t n = 0;
+    if (wait_batch(ctx, s, &n)) return -1;
+    if (n) CK(ctx, cudaMemcpyAsync(out, s.d_recovered, n * sizeof(modes_recovered), cudaMemcpyDeviceToHost, s.stream));
+    CK(ctx, wait_stream(s.stream));
+    return 0;
+}
+
 int modes_set_sink(modes_ctx *ctx, modes_sink_fn fn, void *user) {
     if (!ctx) return -1;
     ctx->out.sink = fn; ctx->out.user = user;
@@ -869,7 +971,7 @@ int modes_detect_fetch(modes_ctx *ctx, modes_candidate *candidates, modes_tile *
 int modes_resolve(modes_ctx *ctx, const modes_candidate *candidates, const modes_tile *tiles, size_t n_tiles,
                   int64_t buffer_base) {
     if (!ctx || !tiles) return -1;
-    ResolveConfig rc{ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->cfg.check_crc};
+    ResolveConfig rc{ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->cfg.check_crc, 0};
     resolve_candidates(ctx->rs, rc, candidates, tiles, n_tiles, buffer_base, ctx->out, ctx->scratch);
     return 0;
 }
@@ -885,7 +987,7 @@ modes_resolver *modes_resolver_create(const modes_config *cfg) {
     if (!r) return nullptr;
     modes_config c;
     if (cfg) c = *cfg; else modes_default_config(&c);
-    r->rc = ResolveConfig{c.fix_errors, c.aggressive, c.check_crc};
+    r->rc = ResolveConfig{c.fix_errors, c.aggressive, c.check_crc, 1};
     r->rs.reset();
     r->scratch = scratch_create();
     if (!r->scratch) { delete r; return nullptr; }
@@ -899,6 +1001,32 @@ int modes_resolver_run(modes_resolver *r, const modes_candidate *candidates, con
     if (!r || !tiles) return -1;
     r->out.sink = sink; r->out.user = user;
     resolve_candidates(r->rs, r->rc, candidates, tiles, n_tiles, buffer_base, r->out, r->scratch);
+    return 0;
+}
+
+int modes_resolver_run_recovered(modes_resolver *r, const modes_candidate *candidates, const modes_recovered *recovered,
+                                 const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, modes_sink_fn sink, void *user) {
+    if (!r || !tiles) return -1;
+    r->out.sink = sink; r->out.user = user;
+    resolve_candidates(r->rs, r->rc, candidates, tiles, n_tiles, buffer_base, r->out, r->scratch, recovered);
+    return 0;
+}
+
+int modes_resolver_run_shards_recovered(modes_resolver *r, size_t n_shards, const modes_candidate *const *candidates,
+                                        const modes_recovered *const *recovered, const modes_tile *const *tiles,
+                                        const size_t *n_tiles, const int64_t *buffer_base, modes_sink_fn sink, void *user) {
+    if (!r || (n_shards && (!candidates || !tiles || !n_tiles || !buffer_base))) return -1;
+    if (recovered)
+        for (size_t k = 0; k < n_shards; k++)
+            if (!recovered[k]) return -1;
+    r->out.sink = sink; r->out.user = user;
+    resolve_shards(r->rs, r->rc, n_shards, candidates, tiles, n_tiles, buffer_base, r->out, r->scratch, recovered);
+    return 0;
+}
+
+int modes_resolver_recovery_stats(const modes_resolver *r, modes_recovery_stats *out) {
+    if (!r || !out) return -1;
+    *out = r->rs.rstats;
     return 0;
 }
 
@@ -920,7 +1048,7 @@ int modes_resolver_get_cache(const modes_resolver *r, uint32_t cache[MODES_ICAO_
 int modes_resolver_set_cache(modes_resolver *r, const uint32_t cache[MODES_ICAO_CACHE_SLOTS]) {
     if (!r) return -1;
     if (cache) memcpy(r->rs.icao, cache, sizeof(r->rs.icao)); else memset(r->rs.icao, 0, sizeof(r->rs.icao));
-    r->rs.cur_buffer = -1; r->rs.next_j = 0;
+    r->rs.cur_buffer = -1; r->rs.next_j = 0; r->rs.next_j_recovered = 0;
     r->has_tentative = false;
     return 0;
 }
@@ -944,7 +1072,8 @@ int modes_resolver_run_tentative(modes_resolver *r, const modes_candidate *candi
     if (!r || !tiles) return -1;
     r->tentative = r->rs;
     memset(r->tentative.stats, 0, sizeof(r->tentative.stats));
-    r->tentative.cur_buffer = -1; r->tentative.next_j = 0;
+    memset(&r->tentative.rstats, 0, sizeof(r->tentative.rstats));
+    r->tentative.cur_buffer = -1; r->tentative.next_j = 0; r->tentative.next_j_recovered = 0;
     resolve_tentative(r->tentative, r->rc, candidates, tiles, n_tiles, buffer_base, r->scratch);
     r->has_tentative = true;
     return 0;
@@ -954,8 +1083,10 @@ int modes_resolver_commit(modes_resolver *r, modes_sink_fn sink, void *user) {
     if (!r || !r->has_tentative) return -1;
     r->out.sink = sink; r->out.user = user;
     for (int i = 0; i < 8; i++) r->rs.stats[i] += r->tentative.stats[i];
+    add_recovery_stats(r->rs.rstats, r->tentative.rstats);
     memcpy(r->rs.icao, r->tentative.icao, sizeof(r->rs.icao));
     r->rs.cur_buffer = r->tentative.cur_buffer; r->rs.next_j = r->tentative.next_j;
+    r->rs.next_j_recovered = r->tentative.next_j_recovered;
     resolve_commit(r->out, r->scratch);
     r->has_tentative = false;
     return 0;

@@ -82,6 +82,13 @@ void launch_levels(const uint8_t *d_iq, uint32_t n_buffers, uint64_t stride_byte
                    modes_level *out, int sm_count, cudaStream_t stream);
 static_assert(sizeof(modes_level) == 40 && offsetof(modes_level, sum_mag) == 16 && offsetof(modes_level, peak) == 32,
               "level record layout");
+// Recovery records (modes_recover.cu): writes out[k] for k < min(counters[0], capacity) from the
+// candidate records and the windows the scan and frame evaluation read.
+void launch_recover(const BatchView &in, const DeviceTables &tab, const ScanOutputs &scan, const modes_candidate *records,
+                    uint32_t capacity, modes_recovered *out, int sm_count, cudaStream_t stream);
+static_assert(sizeof(modes_recovered) == 20 && offsetof(modes_recovered, status) == 14 && offsetof(modes_recovered, signal) == 16,
+              "recovery record layout");
+static_assert(offsetof(modes_message, recovered) == 14 && offsetof(modes_message, msgbits) == 16, "message layout");
 
 // The record layouts are ABI: the signal field took the two bytes every evaluation kernel already wrote as zero.
 static_assert(sizeof(modes_frame_eval) == 24 && offsetof(modes_frame_eval, signal) == 18 && offsetof(modes_frame_eval, crc) == 20,
@@ -125,10 +132,13 @@ struct ResolveState {
     int64_t  stats[8];
     int64_t  cur_buffer;         // buffer whose skip state is live, -1 = none
     uint32_t next_j;             // first position not skipped in cur_buffer
+    uint32_t next_j_recovered;   // first position of cur_buffer not inside a recovered message (recovery only)
+    modes_recovery_stats rstats;
     void reset();
 };
 
-struct ResolveConfig { int fix_errors, aggressive, check_crc; };
+// recover_signal: recovered messages carry their record's signal (else 0)
+struct ResolveConfig { int fix_errors, aggressive, check_crc; int recover_signal; };
 
 // Where delivered messages go: a callback, and/or a caller-owned array that is
 // filled in place (count keeps running past capacity).
@@ -144,12 +154,13 @@ struct ResolveScratch;
 ResolveScratch *scratch_create();
 void scratch_destroy(ResolveScratch *s);
 
+// recovered: one record per candidate (modes_recover.cu), or nullptr with recovery off
 void resolve_candidates(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands,
                         const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, MessageOut &out,
-                        ResolveScratch *scratch);
+                        ResolveScratch *scratch, const modes_recovered *recovered = nullptr);
 void resolve_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards, const modes_candidate *const *cands,
                     const modes_tile *const *tiles, const size_t *n_tiles, const int64_t *buffer_base,
-                    MessageOut &out, ResolveScratch *scratch);
+                    MessageOut &out, ResolveScratch *scratch, const modes_recovered *const *recovered = nullptr);
 // A shard resolved from a GUESSED address cache (one rank / one GPU thread of a sharded decode):
 // verdicts only, deliveries held back in the scratch until the guess is verified.
 void resolve_tentative(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands, const modes_tile *tiles,
@@ -159,5 +170,6 @@ void resolve_commit(MessageOut &out, ResolveScratch *scratch);
 void deliver_gpu(const modes_delivery *d, size_t n, int64_t buffer_base, MessageOut &out);
 // The order-dependent tail of decodeModesMessage + field decode for one evaluated frame.
 int finish_message(ResolveState &st, const modes_frame_eval &p, modes_message *out);
+void add_recovery_stats(modes_recovery_stats &to, const modes_recovery_stats &from);
 
 }  // namespace modes

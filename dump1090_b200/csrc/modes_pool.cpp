@@ -105,6 +105,7 @@ struct modes_pool {
     size_t max_batch = 0;
     int signal = 0;                            // modes_pool_set_signal, applied to the slot contexts
     int levels = 0;                            // modes_pool_set_levels
+    int recover = 0;                           // modes_pool_set_recovery
     std::string err;
     // device half (created on the first modes_pool_submit / _ingest): two batches may be in flight, so
     // that one is uploaded and scanned while the one before it is resolved on the host
@@ -116,14 +117,17 @@ struct modes_pool {
         std::vector<int64_t> buf_index;        // with levels: each one's own index of its buffer
         std::vector<modes_level> level_out;
         bool levels = false;                   // the batch measures its data buffers' levels
+        bool recover = false, signal = false;  // the recovery / signal switches as they were at submit
         bool busy = false;
     } slot[2];
     unsigned submitted = 0, collected = 0;     // batches so far: slot = number & 1
     std::vector<modes_candidate> cands;
+    std::vector<modes_recovered> recovered;    // with recovery: one record per candidate
     std::vector<modes_tile> tiles;
     // the per-receiver resolve: one block of the receiver list per host thread
     struct Block {
         std::vector<modes_candidate> local;    // one receiver's records, re-based to its buffer
+        std::vector<modes_recovered> local_rec;   // and their recovery records
         std::vector<modes_tile> local_tiles;
         std::vector<modes_message> msgs;       // the block's messages, receiver by receiver
         std::vector<size_t> counts;            // messages of each receiver of the block
@@ -215,8 +219,11 @@ void modes_pool_destroy(modes_pool *p) {
 
 const char *modes_pool_last_error(const modes_pool *p) { return p ? p->err.c_str() : "no pool"; }
 
-int modes_pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, const modes_candidate *candidates,
-                       const modes_tile *tiles, modes_pool_sink_fn sink, void *user) {
+// The per-receiver resolve; recovered: the batch's recovery records (nullptr: off), whose signal the
+// messages carry only when the batch measured signals.
+static int pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, const modes_candidate *candidates,
+                        const modes_recovered *recovered, bool signal, const modes_tile *tiles, modes_pool_sink_fn sink,
+                        void *user) {
     if (!p) return -1;
     if (check_ids(p, receivers, n)) return -1;
     if (!n) return 0;
@@ -243,7 +250,10 @@ int modes_pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, const
         bl.counts.assign(i1 - i0, 0);
         size_t room = 0, ga, gb, gc, gd;
         tile_range(i0, ga, gb); tile_range(i1 - 1, gc, gd);
-        for (size_t g = ga; g <= gd; g++) room += 2 * (size_t)tiles[g].count;  // a candidate delivers at most two messages (both attempts without --check-crc... dump1090.c:1803)
+        // a candidate delivers at most two messages of the reference (both attempts without --check-crc,
+        // dump1090.c:1803) and, with recovery, one recovered message after them
+        const size_t per_candidate = recovered ? 3 : 2;
+        for (size_t g = ga; g <= gd; g++) room += per_candidate * (size_t)tiles[g].count;
         if (bl.msgs.size() < room) bl.msgs.resize(room);
         bl.local_tiles.resize(n_local);
         size_t used = 0;
@@ -253,6 +263,7 @@ int modes_pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, const
             size_t g0, g1;
             tile_range(i, g0, g1);
             bl.local.clear();
+            bl.local_rec.clear();
             for (modes_tile &lt : bl.local_tiles) { lt.offset = 0; lt.count = 0; }
             for (size_t g = g0; g <= g1; g++) {
                 const modes_candidate *c = candidates + tiles[g].offset;
@@ -264,16 +275,23 @@ int modes_pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, const
                     if (lg >= n_local) { bl.failed = (int64_t)i; return; }
                     bl.local_tiles[lg].count++;
                     bl.local.push_back(lc);
+                    if (recovered) {
+                        modes_recovered rc = recovered[tiles[g].offset + k];
+                        if (!signal) rc.signal = 0;
+                        bl.local_rec.push_back(rc);
+                    }
                 }
             }
             uint32_t off = 0;
             for (modes_tile &lt : bl.local_tiles) { lt.offset = off; off += lt.count; }
             modes_resolver_set_output(r.res, bl.msgs.data() + used, room - used);
-            if (modes_resolver_run(r.res, bl.local.data(), bl.local_tiles.data(), n_local, r.buffers, nullptr, nullptr)) {
+            if (modes_resolver_run_recovered(r.res, bl.local.data(), recovered ? bl.local_rec.data() : nullptr, bl.local_tiles.data(),
+                                             n_local, r.buffers, nullptr, nullptr)) {
                 bl.failed = (int64_t)i; return;
             }
             const size_t k = modes_resolver_output_count(r.res);
             modes_resolver_set_output(r.res, nullptr, 0);
+            if (k > room - used) { bl.failed = (int64_t)i; return; }   // the bound above is exact: never reached
             bl.counts[i - i0] = k;
             used += k;
             r.buffers++;
@@ -314,6 +332,11 @@ int modes_pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, const
     return 0;
 }
 
+int modes_pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, const modes_candidate *candidates,
+                       const modes_tile *tiles, modes_pool_sink_fn sink, void *user) {
+    return pool_resolve(p, receivers, n, candidates, nullptr, false, tiles, sink, user);
+}
+
 int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *const *iq, size_t n) {
     if (!p) return -1;
     if (check_ids(p, receivers, n)) return -1;
@@ -345,6 +368,9 @@ int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *c
                 return fail(p, "buffer upload failed: %s", cudaGetErrorString(cudaGetLastError()));
     }
     if (modes_detect_device(sl.ctx, sl.d_batch, 2 * n, nullptr, nullptr, 0, nullptr)) return fail(p, "%s", modes_last_error(sl.ctx));
+    sl.recover = p->recover != 0;
+    sl.signal = p->signal != 0;
+    if (sl.recover && modes_recover_device(sl.ctx, nullptr, 0)) return fail(p, "%s", modes_last_error(sl.ctx));
     // the data buffers only (every second buffer), on the same stream: no wait before the collect
     sl.levels = p->levels != 0;
     if (sl.levels && modes_levels_device(sl.ctx, sl.d_batch + kBuf, n, 2 * kBuf)) return fail(p, "%s", modes_last_error(sl.ctx));
@@ -369,6 +395,10 @@ int modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user) {
     p->cands.resize(n_cand ? n_cand : 1);
     p->tiles.resize(modes_tile_count(2 * n));
     if (modes_detect_fetch(sl.ctx, p->cands.data(), p->tiles.data())) return fail(p, "%s", modes_last_error(sl.ctx));
+    if (sl.recover) {
+        p->recovered.resize(n_cand ? n_cand : 1);
+        if (modes_recover_fetch(sl.ctx, p->recovered.data())) return fail(p, "%s", modes_last_error(sl.ctx));
+    }
     if (sl.levels) {
         sl.level_out.resize(n);
         if (modes_levels_fetch(sl.ctx, sl.level_out.data())) return fail(p, "%s", modes_last_error(sl.ctx));
@@ -380,7 +410,8 @@ int modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user) {
     }
     sl.busy = false;
     p->collected++;
-    return modes_pool_resolve(p, sl.ids.data(), n, p->cands.data(), p->tiles.data(), sink, user);
+    return pool_resolve(p, sl.ids.data(), n, p->cands.data(), sl.recover ? p->recovered.data() : nullptr, sl.signal, p->tiles.data(),
+                        sink, user);
 }
 
 int modes_pool_ingest(modes_pool *p, const uint32_t *receivers, const uint8_t *const *iq, size_t n,
@@ -422,6 +453,17 @@ int modes_pool_set_signal(modes_pool *p, int on) {
     for (modes_pool::Slot &sl : p->slot)
         if (sl.ctx) modes_set_signal(sl.ctx, p->signal);
     return 0;
+}
+
+int modes_pool_set_recovery(modes_pool *p, int on) {
+    if (!p) return -1;
+    p->recover = on != 0;
+    return 0;
+}
+
+int modes_pool_recovery_stats(const modes_pool *p, uint32_t receiver, modes_recovery_stats *out) {
+    if (!p || receiver >= p->rx.size() || !out) return -1;
+    return modes_resolver_recovery_stats(p->rx[receiver].res, out);
 }
 
 int modes_pool_set_levels(modes_pool *p, int on) {

@@ -35,6 +35,8 @@ void ResolveState::reset() {
     std::memset(stats, 0, sizeof(stats));
     cur_buffer = -1;
     next_j = 0;
+    next_j_recovered = 0;
+    std::memset(&rstats, 0, sizeof(rstats));
 }
 
 static inline uint32_t icao_slot(uint32_t a) {           // dump1090.c:898-905
@@ -195,12 +197,14 @@ struct Delivery {
     int64_t sample_pos;
     uint32_t iid, ap_addr;
     uint8_t crcok, phase_corrected;
+    uint8_t recovered;           // eval is a recovery record's frame: crc 0, nfixed = its flips
 };
 
 static inline void materialise(const Delivery &d, modes_message *mm) {
     build_message(d.eval, d.crcok, d.iid, d.ap_addr, mm);
     mm->sample_pos = d.sample_pos;
     mm->phase_corrected = d.phase_corrected;
+    if (d.recovered) { mm->recovered = 1; mm->errorbit = -1; }
 }
 
 // Cores this process may actually keep busy: the CPUs it is allowed on, cut down to the CPU-time
@@ -303,17 +307,70 @@ static inline bool attempt(ResolveState &st, const ResolveConfig &cfg, const mod
         else { st.stats[4]++; st.stats[5]++; st.stats[6]++; }
     }
     if (cfg.check_crc == 0 || crcok)                       // dump1090.c:1803; :1772-1773
-        deliveries.push_back(Delivery{p, sample_pos, iid, ap, (uint8_t)crcok, (uint8_t)(crcok && retry)});
+        deliveries.push_back(Delivery{p, sample_pos, iid, ap, (uint8_t)crcok, (uint8_t)(crcok && retry), (uint8_t)0});
     return crcok != 0;
+}
+
+// With recovery records (rec[k] belongs to cands[k]; include/modes_b200.h rules 1-6), a candidate the
+// walk visits where neither attempt was good may add a recovered message.  It goes into the list at
+// once, in stream order, and is taken out again if the reference delivers a good message within its
+// span (rule 6): only deliveries of the same buffer at later positions can follow it by then.
+constexpr uint32_t kRecoveredSpan = 241;                  // (8 + 112) * 2 + 1: the skip of a long message
+
+struct RecoveryPending {                                  // the recovered message rule 6 may still drop
+    size_t index = SIZE_MAX;                              // in the delivery list
+    int64_t buffer = -1;
+    uint32_t end = 0;                                     // first position of the buffer outside its span
+};
+
+// The recovery rules at one visited candidate, after the reference's attempts there (good: one of
+// them was judged crcok).
+static inline void recovery_step(ResolveState &st, const ResolveConfig &cfg, const modes_recovered &r, bool good,
+                                 int64_t buffer, uint32_t j, int64_t pos, std::vector<Delivery> &deliveries,
+                                 RecoveryPending &pend) {
+    if (good) {                                                            // rule 6
+        if (pend.index != SIZE_MAX && pend.buffer == buffer && j < pend.end) {
+            // what follows it in the list lies in this buffer within its span: a few entries move
+            deliveries.erase(deliveries.begin() + (ptrdiff_t)pend.index);
+            st.rstats.dropped++;
+            st.rstats.delivered--;
+            pend.index = SIZE_MAX;
+        }
+        return;
+    }
+    if (r.status == MODES_RECOVER_INELIGIBLE) return;                      // rule 2 holds
+    st.rstats.considered++;
+    if (j < st.next_j_recovered) return;                                   // rule 3
+    if (r.status == MODES_RECOVER_AMBIGUOUS) st.rstats.ambiguous++;
+    if (r.status != MODES_RECOVER_FOUND) return;                           // rule 4
+    st.rstats.found++;
+    const uint32_t addr = ((uint32_t)r.msg[1] << 16) | ((uint32_t)r.msg[2] << 8) | (uint32_t)r.msg[3];
+    if (!icao_seen(st, addr)) { st.rstats.unknown_address++; return; }     // rule 5
+    modes_frame_eval e{};
+    std::memcpy(e.msg, r.msg, 14);
+    e.msgtype = (uint8_t)(r.msg[0] >> 3);
+    e.nfixed = r.nflips;
+    e.errorbit = 0xFF;
+    e.signal = cfg.recover_signal ? r.signal : 0;
+    e.crc = 0;
+    pend.index = deliveries.size();
+    pend.buffer = buffer;
+    pend.end = j + kRecoveredSpan;
+    st.next_j_recovered = j + kRecoveredSpan;
+    deliveries.push_back(Delivery{e, pos, 0u, 0u, (uint8_t)1, (uint8_t)0, (uint8_t)1});
+    st.rstats.delivered++;
 }
 
 // The verdict pass over one run of tiles: everything order-dependent, no message structs yet.
 // `b_lo`, `b_hi`: only the candidates of the buffers [b_lo, b_hi) of this record array are judged (buffer
 // numbers as in the records: t >> 17); the walk ends at the first candidate of buffer b_hi or later
-// (records are in stream order).  The whole array: 0, UINT32_MAX.
-static void judge_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands, const modes_tile *tiles,
-                        size_t n_tiles, int64_t buffer_base, std::vector<Delivery> &deliveries,
-                        uint32_t b_lo = 0, uint32_t b_hi = UINT32_MAX) {
+// (records are in stream order).  The whole array: 0, UINT32_MAX.  kRecover: apply the recovery rules
+// with `rec` (the walk without them has no trace of them).
+template <bool kRecover>
+static void walk_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands, const modes_tile *tiles,
+                       size_t n_tiles, int64_t buffer_base, std::vector<Delivery> &deliveries, uint32_t b_lo, uint32_t b_hi,
+                       const modes_recovered *rec) {
+    RecoveryPending pend;
     // The kernels append a tile's records wherever the global cursor stands when the tile finishes:
     // records are contiguous per tile but the tiles lie scattered through the array, so walking them
     // in stream order is a chain of cache misses (the records were just written by DMA).  Request
@@ -325,28 +382,45 @@ static void judge_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_
             const size_t bytes = (size_t)tiles[ti + kAhead].count * sizeof(modes_candidate);
             for (size_t o = 0; o < bytes && o < 512; o += 64) __builtin_prefetch(p + o, 0, 1);
         }
-        const modes_candidate *c = cands + tiles[ti].offset;
-        for (uint32_t k = 0; k < tiles[ti].count; k++, c++) {
+        const size_t k0 = tiles[ti].offset;
+        for (uint32_t k = 0; k < tiles[ti].count; k++) {
+            const modes_candidate *c = cands + k0 + k;
             const uint32_t rb = (uint32_t)(c->t >> 17);
             if (rb < b_lo) continue;                       // the part before this one takes it
             if (rb >= b_hi) return;                        // the next part's
             const int64_t buffer = buffer_base + rb;
             const uint32_t j = (uint32_t)(c->t & (kBufSamples - 1));
-            if (buffer != st.cur_buffer) { st.cur_buffer = buffer; st.next_j = 0; }
-            if (j < st.next_j) continue;                   // inside a message already taken
+            if (buffer != st.cur_buffer) { st.cur_buffer = buffer; st.next_j = 0; st.next_j_recovered = 0; }
+            if (j < st.next_j) continue;                   // inside a message already taken (rule 1)
             st.stats[0]++;                                 // dump1090.c:1651
-            const modes_frame_eval &p1 = c->pass[0];
-            if (!(p1.flags & MODES_EVAL_GATE_OK)) continue;        // dump1090.c:1723-1726
             const int64_t pos = buffer * (int64_t)kBufSamples + j - MODES_CARRY_SAMPLES;
-            const uint32_t skip = (uint32_t)(8 + bits_by_type(p1.msgtype)) * 2 + 1;
-            if (attempt(st, cfg, p1, false, pos, deliveries)) { st.next_j = j + skip; continue; }
-            if (j) st.stats[1]++;                          // dump1090.c:1660-1663
-            const modes_frame_eval &p2 = c->pass[1];
-            if (!(p2.flags & MODES_EVAL_GATE_OK)) continue;
-            const uint32_t skip2 = (uint32_t)(8 + bits_by_type(p2.msgtype)) * 2 + 1;
-            if (attempt(st, cfg, p2, true, pos, deliveries)) st.next_j = j + skip2;
+            bool good = false;
+            const modes_frame_eval &p1 = c->pass[0];
+            if (p1.flags & MODES_EVAL_GATE_OK) {           // dump1090.c:1723-1726
+                const uint32_t skip = (uint32_t)(8 + bits_by_type(p1.msgtype)) * 2 + 1;
+                if (attempt(st, cfg, p1, false, pos, deliveries)) {
+                    st.next_j = j + skip;
+                    good = true;
+                } else {
+                    if (j) st.stats[1]++;                  // dump1090.c:1660-1663
+                    const modes_frame_eval &p2 = c->pass[1];
+                    if (p2.flags & MODES_EVAL_GATE_OK) {
+                        const uint32_t skip2 = (uint32_t)(8 + bits_by_type(p2.msgtype)) * 2 + 1;
+                        if (attempt(st, cfg, p2, true, pos, deliveries)) { st.next_j = j + skip2; good = true; }
+                    }
+                }
+            }
+            if constexpr (kRecover) recovery_step(st, cfg, rec[k0 + k], good, buffer, j, pos, deliveries, pend);
+            (void)good;
         }
     }
+}
+
+static void judge_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands, const modes_tile *tiles,
+                        size_t n_tiles, int64_t buffer_base, std::vector<Delivery> &deliveries,
+                        uint32_t b_lo = 0, uint32_t b_hi = UINT32_MAX, const modes_recovered *rec = nullptr) {
+    if (rec) walk_tiles<true>(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, b_lo, b_hi, rec);
+    else walk_tiles<false>(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, b_lo, b_hi, nullptr);
 }
 
 // Build the delivered structs: in place and in parallel for array output, then the callback
@@ -416,6 +490,7 @@ struct Part {
     uint32_t b_lo, b_hi;         // its buffers, as numbered in the records (t >> 17)
     int64_t buffer_base;
     bool first_of_shard;         // the tail pass for a shard's first part walks the previous SHARD's array
+    const modes_recovered *rec;  // the array's recovery records, or nullptr
 };
 struct PartRun { ResolveState start, end; std::vector<Delivery> deliveries; };
 struct ResolveScratch {
@@ -449,8 +524,8 @@ static size_t parts_for(size_t n_tiles) {
 // read from the records themselves: the buffer after the one the first candidate at or behind tile
 // k * n_tiles / want lies in (tiles do not line up with buffers; records are in stream order).
 static void cut_parts(const modes_candidate *cands, const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, size_t want,
-                      std::vector<Part> &parts) {
-    Part p{cands, tiles, n_tiles, 0, 0, UINT32_MAX, buffer_base, true};
+                      std::vector<Part> &parts, const modes_recovered *rec = nullptr) {
+    Part p{cands, tiles, n_tiles, 0, 0, UINT32_MAX, buffer_base, true, rec};
     for (size_t k = 1; k < want; k++) {
         size_t ti = k * n_tiles / want;
         while (ti < n_tiles && tiles[ti].count == 0) ti++;
@@ -464,6 +539,11 @@ static void cut_parts(const modes_candidate *cands, const modes_tile *tiles, siz
     parts.push_back(p);
 }
 
+void add_recovery_stats(modes_recovery_stats &to, const modes_recovery_stats &from) {
+    to.considered += from.considered; to.found += from.found; to.ambiguous += from.ambiguous;
+    to.unknown_address += from.unknown_address; to.dropped += from.dropped; to.delivered += from.delivered;
+}
+
 // Judge the parts (rounds of guess and verify, see above); runs[k] receives part k's deliveries
 // and statistics, `st` the state after the last part.
 static int judge_parts(ResolveState &st, const ResolveConfig &cfg, const std::vector<Part> &parts, PartRun *runs) {
@@ -475,10 +555,12 @@ static int judge_parts(ResolveState &st, const ResolveConfig &cfg, const std::ve
         const Part &p = parts[k];
         r.start = from;
         std::memset(r.start.stats, 0, sizeof(r.start.stats));
-        if (k) { r.start.cur_buffer = -1; r.start.next_j = 0; }           // a part starts a buffer
+        std::memset(&r.start.rstats, 0, sizeof(r.start.rstats));
+        if (k) { r.start.cur_buffer = -1; r.start.next_j = 0; r.start.next_j_recovered = 0; }   // a part starts a buffer
         r.end = r.start;
         r.deliveries.clear();
-        judge_tiles(r.end, cfg, p.cands, p.tiles + p.tile_lo, p.n_tiles - p.tile_lo, p.buffer_base, r.deliveries, p.b_lo, p.b_hi);
+        judge_tiles(r.end, cfg, p.cands, p.tiles + p.tile_lo, p.n_tiles - p.tile_lo, p.buffer_base, r.deliveries, p.b_lo, p.b_hi,
+                    p.rec);
     };
     int rounds = 0;
     size_t done = 0;                                       // parts [0, done) are final
@@ -497,7 +579,7 @@ static int judge_parts(ResolveState &st, const ResolveConfig &cfg, const std::ve
             // part has normally written every slot the whole part leaves changed).
             const Part &q = parts[k - 1];
             ResolveState g = st;
-            g.cur_buffer = -1; g.next_j = 0;
+            g.cur_buffer = -1; g.next_j = 0; g.next_j_recovered = 0;   // (recovery never writes the cache: the guess skips it)
             const size_t end_tile = parts[k].first_of_shard ? q.n_tiles : (parts[k].tile_lo + 1 < q.n_tiles ? parts[k].tile_lo + 1 : q.n_tiles);
             const size_t len = end_tile - q.tile_lo;
             size_t tail = len / 16 > 128 ? len / 16 : 128;             // at least ~1 M samples (half a second of stream)
@@ -522,13 +604,19 @@ static int judge_parts(ResolveState &st, const ResolveConfig &cfg, const std::ve
             if (std::memcmp(truth.icao, runs[done].start.icao, sizeof(truth.icao)) != 0) break;
         }
     }
-    for (size_t k = 0; k < n; k++)
+    for (size_t k = 0; k < n; k++) {
         for (int i = 0; i < 8; i++) st.stats[i] += runs[k].end.stats[i];
+        add_recovery_stats(st.rstats, runs[k].end.rstats);
+    }
     if (n) {
         std::memcpy(st.icao, runs[n - 1].end.icao, sizeof(st.icao));
         // the skip state is that of the last part that saw a candidate (an empty part leaves none)
         for (size_t k = n; k-- > 0;)
-            if (runs[k].end.cur_buffer != -1 || k == 0) { st.cur_buffer = runs[k].end.cur_buffer; st.next_j = runs[k].end.next_j; break; }
+            if (runs[k].end.cur_buffer != -1 || k == 0) {
+                st.cur_buffer = runs[k].end.cur_buffer; st.next_j = runs[k].end.next_j;
+                st.next_j_recovered = runs[k].end.next_j_recovered;
+                break;
+            }
     }
     return rounds;
 }
@@ -540,7 +628,7 @@ static PartRun *runs_for(ResolveScratch *scratch, size_t n) {
 
 void resolve_candidates(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands,
                         const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, MessageOut &out,
-                        ResolveScratch *scratch) {
+                        ResolveScratch *scratch, const modes_recovered *recovered) {
     const bool timing = std::getenv("MODES_RESOLVE_TIMING") != nullptr;
     auto now = [] { return std::chrono::steady_clock::now(); };
     auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) {
@@ -551,14 +639,14 @@ void resolve_candidates(ResolveState &st, const ResolveConfig &cfg, const modes_
     if (want <= 1) {
         std::vector<Delivery> &deliveries = scratch->deliveries;
         deliveries.clear();
-        judge_tiles(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries);
+        judge_tiles(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, 0, UINT32_MAX, recovered);
         const auto t1 = now();
         deliver(deliveries, out);
         if (timing) std::fprintf(stderr, "resolve_candidates: %zu tiles, verdicts %.2f ms, structs %.2f ms\n", n_tiles, ms(t0, t1), ms(t1, now()));
         return;
     }
     std::vector<Part> parts;
-    cut_parts(cands, tiles, n_tiles, buffer_base, want, parts);
+    cut_parts(cands, tiles, n_tiles, buffer_base, want, parts, recovered);
     PartRun *runs = runs_for(scratch, parts.size());
     const int rounds = judge_parts(st, cfg, parts, runs);
     const auto t1 = now();
@@ -597,7 +685,7 @@ void resolve_commit(MessageOut &out, ResolveScratch *scratch) {
 // is a part, long shards are cut once more (see judge_parts).
 void resolve_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards, const modes_candidate *const *cands,
                     const modes_tile *const *tiles, const size_t *n_tiles, const int64_t *buffer_base,
-                    MessageOut &out, ResolveScratch *scratch) {
+                    MessageOut &out, ResolveScratch *scratch, const modes_recovered *const *recovered) {
     const bool timing = std::getenv("MODES_RESOLVE_TIMING") != nullptr;
     auto now = [] { return std::chrono::steady_clock::now(); };
     auto t_start = now();
@@ -608,7 +696,7 @@ void resolve_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards,
         size_t want = parts_for(n_tiles[k]);
         const size_t share = threads_left / (n_shards - k) > 0 ? threads_left / (n_shards - k) : 1;
         if (want > share) want = share;
-        cut_parts(cands[k], tiles[k], n_tiles[k], buffer_base[k], want, parts);
+        cut_parts(cands[k], tiles[k], n_tiles[k], buffer_base[k], want, parts, recovered ? recovered[k] : nullptr);
         threads_left = threads_left > want ? threads_left - want : 0;
     }
     PartRun *runs = runs_for(scratch, parts.size());

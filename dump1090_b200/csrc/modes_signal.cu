@@ -24,10 +24,7 @@ namespace modes {
 constexpr int kSignalThreads = 256;
 constexpr int kSignalBlocksPerSm = 8;
 
-__device__ __forceinline__ uint32_t raw_sample16(const BatchView &in, uint32_t v) {
-    const uint8_t *p = (v < (uint32_t)kHaloSamples) ? in.halo + 2 * v : in.body + 2 * (v - kHaloSamples);
-    return *reinterpret_cast<const uint16_t *>(p);
-}
+using signal::load_pairs;
 
 // Bits of the longest decoded attempt of a record (0 = none), from the words holding msgtype / flags.
 __device__ __forceinline__ uint32_t bits_needed(uint32_t w0, uint32_t w1) {
@@ -38,29 +35,6 @@ __device__ __forceinline__ uint32_t bits_needed(uint32_t w0, uint32_t w1) {
     };
     const uint32_t a = bits(w0), b = bits(w1);
     return a > b ? a : b;
-}
-
-// The sample pairs of bits 32r + lane < nb of the frame whose first pair starts at virtual index s;
-// bits beyond nb read as no signal (magnitude 0).
-__device__ __forceinline__ void load_pairs(const BatchView &in, uint32_t s, uint32_t nb, int lane, uint32_t pair[4]) {
-    if (s >= (uint32_t)kHaloSamples) {
-        const uint32_t f = s - kHaloSamples;                              // body sample of the first pair
-        const uint32_t *wp = reinterpret_cast<const uint32_t *>(in.body) + (f >> 1);
-#pragma unroll
-        for (int r = 0; r < 4; r++) {
-            const uint32_t b = 32 * r + lane;
-            pair[r] = 0x7f7f7f7fu;
-            if (b < nb) pair[r] = (f & 1u) ? __byte_perm(wp[b], wp[b + 1], 0x5432) : wp[b];
-        }
-    } else {
-        // the window starts in the carry block (first positions of a batch): sample by sample
-#pragma unroll
-        for (int r = 0; r < 4; r++) {
-            const uint32_t b = 32 * r + lane;
-            pair[r] = 0x7f7f7f7fu;
-            if (b < nb) pair[r] = raw_sample16(in, s + 2 * b) | (raw_sample16(in, s + 2 * b + 1) << 16);
-        }
-    }
 }
 
 __global__ void __launch_bounds__(kSignalThreads)

@@ -47,15 +47,21 @@ MODES_SIGNAL_FN uint32_t dot4(uint32_t a, uint32_t b) {
 #endif
 }
 
-// Squared pulse of one bit: pair = the bit's two samples as one word (first sample in the low half),
-// lutn = magnitude keyed by I*I + Q*Q (modes_tables.cpp).
-MODES_SIGNAL_FN uint32_t pulse_sq(uint32_t pair, const uint16_t *lutn) {
+// The magnitudes of a bit's two samples: pair = the two samples as one word (first sample in the low
+// half), lutn = magnitude keyed by I*I + Q*Q (modes_tables.cpp).
+MODES_SIGNAL_FN void pair_mags(uint32_t pair, const uint16_t *lutn, uint32_t &first, uint32_t &second) {
     const uint32_t a = absdiff127x4(pair);
 #if defined(__CUDA_ARCH__)
-    const uint32_t lo = __ldg(lutn + dot4(a & 0x0000ffffu, a)), hi = __ldg(lutn + dot4(a & 0xffff0000u, a));
+    first = __ldg(lutn + dot4(a & 0x0000ffffu, a)); second = __ldg(lutn + dot4(a & 0xffff0000u, a));
 #else
-    const uint32_t lo = lutn[dot4(a & 0x0000ffffu, a)], hi = lutn[dot4(a & 0xffff0000u, a)];
+    first = lutn[dot4(a & 0x0000ffffu, a)]; second = lutn[dot4(a & 0xffff0000u, a)];
 #endif
+}
+
+// Squared pulse of one bit (the larger of its two magnitudes, squared).
+MODES_SIGNAL_FN uint32_t pulse_sq(uint32_t pair, const uint16_t *lutn) {
+    uint32_t lo, hi;
+    pair_mags(pair, lutn, lo, hi);
     const uint32_t p = lo > hi ? lo : hi;
     return p * p;
 }
@@ -82,3 +88,42 @@ MODES_SIGNAL_FN uint16_t signal_of(uint64_t sum_sq, uint32_t bits) {
 
 }  // namespace signal
 }  // namespace modes
+
+#if defined(__CUDACC__)
+// ---- the window loads the signal and recovery passes share (device only)
+#include "modes_internal.h"
+
+namespace modes {
+namespace signal {
+
+__device__ __forceinline__ uint32_t raw_sample16(const BatchView &in, uint32_t v) {
+    const uint8_t *p = (v < (uint32_t)kHaloSamples) ? in.halo + 2 * v : in.body + 2 * (v - kHaloSamples);
+    return *reinterpret_cast<const uint16_t *>(p);
+}
+
+// The sample pairs of bits 32r + lane < nb of the frame whose first pair starts at virtual index s;
+// bits beyond nb read as no signal (magnitude 0).
+__device__ __forceinline__ void load_pairs(const BatchView &in, uint32_t s, uint32_t nb, int lane, uint32_t pair[4]) {
+    if (s >= (uint32_t)kHaloSamples) {
+        const uint32_t f = s - kHaloSamples;                              // body sample of the first pair
+        const uint32_t *wp = reinterpret_cast<const uint32_t *>(in.body) + (f >> 1);
+#pragma unroll
+        for (int r = 0; r < 4; r++) {
+            const uint32_t b = 32 * r + lane;
+            pair[r] = 0x7f7f7f7fu;
+            if (b < nb) pair[r] = (f & 1u) ? __byte_perm(wp[b], wp[b + 1], 0x5432) : wp[b];
+        }
+    } else {
+        // the window starts in the carry block (first positions of a batch): sample by sample
+#pragma unroll
+        for (int r = 0; r < 4; r++) {
+            const uint32_t b = 32 * r + lane;
+            pair[r] = 0x7f7f7f7fu;
+            if (b < nb) pair[r] = raw_sample16(in, s + 2 * b) | (raw_sample16(in, s + 2 * b + 1) << 16);
+        }
+    }
+}
+
+}  // namespace signal
+}  // namespace modes
+#endif

@@ -272,6 +272,23 @@ def df17_grid(nsamples: int, period: int, seed: int, sigma: float = 1.5, amp: fl
     return synth_stream(nsamples, frames, sigma=sigma, seed=seed)
 
 
+def fleet_at(snr_db: float, nframes: int, seed: int, n_aircraft: int = 20, amp: float = 20.0, period: int = 400):
+    """DF17 extended squitters (identification, airborne position, velocity) of a fleet of n_aircraft,
+    each sending many frames, in noise at snr_db (pulse power / noise power = amp^2 / (2 sigma^2)), one
+    frame every ~period samples.  Returns (stream, set of the frames' hex)."""
+    sigma = amp / (np.sqrt(2.0) * 10 ** (snr_db / 20.0))
+    rng = Counter(seed)
+    fleet = [0x400000 + rng.below(0x3FFFFF) for _ in range(n_aircraft)]
+    frames, truth = [], set()
+    for k in range(nframes):
+        aa = fleet[rng.below(n_aircraft)].to_bytes(3, "big")
+        me = [_me_ident, _me_airborne, _me_airborne, _me_velocity][rng.below(4)](rng)
+        frame = make_frame(17, 5, aa + me)
+        frames.append((200 + k * period + rng.below(100), frame, amp, 2 * np.pi * rng.uniform(), 0.5 * rng.uniform()))
+        truth.add(frame.hex())
+    return synth_stream(200 + nframes * period + 400, frames, sigma=sigma, seed=seed), truth
+
+
 def tile_to(data: np.ndarray, nbytes: int) -> np.ndarray:
     """Tile a capture back-to-back to exactly nbytes (SURVEY §8(d) input 2)."""
     reps = -(-nbytes // data.size)

@@ -18,6 +18,11 @@
  * summary line on stderr at the end (buffers, samples, noise floor and peak in dBFS on the scale of
  * the Beast signal level, clipped samples and their fraction); it combines with every output mode
  * and leaves stdout as it is.
+ * --recover adds weak DF17/DF18 frames of already known aircraft that a soft-decision search on the
+ * GPU repairs (include/modes_b200.h, modes_set_recovery); they are not the reference's messages.  It
+ * combines with every output mode; with --stats the reference's lines stay as they are on stdout and
+ * one recovery line goes to stderr.  --gpu-resolve runs the order-dependent half on the GPU too
+ * (modes_config.gpu_resolve); it has no recovery rule, so it is refused together with --recover.
  * The live-radio, networking and interactive options are out of scope.
  */
 #include <math.h>
@@ -27,7 +32,7 @@
 #include "modes_b200.h"
 
 static int opt_raw = 0, opt_onlyaddr = 0, opt_stats = 0, opt_check_crc = 1, opt_sbs = 0, opt_json = 0, opt_beast = 0;
-static int opt_levels = 0;
+static int opt_levels = 0, opt_recover = 0;
 static modes_tracker *tracker = NULL;
 
 /* --levels: totals over the records taken so far */
@@ -111,6 +116,8 @@ int main(int argc, char **argv) {
         else if (!strcmp(argv[j], "--aircraft-json")) opt_json = 1;
         else if (!strcmp(argv[j], "--beast")) opt_beast = 1;
         else if (!strcmp(argv[j], "--levels")) opt_levels = 1;
+        else if (!strcmp(argv[j], "--recover")) opt_recover = 1;
+        else if (!strcmp(argv[j], "--gpu-resolve")) cfg.gpu_resolve = 1;
         else if (!strcmp(argv[j], "--device") && more) cfg.device = atoi(argv[++j]);
         else if (!strcmp(argv[j], "--gpus") && more) cfg.n_gpus = atoi(argv[++j]);
         else if (!strcmp(argv[j], "--chunk") && more) chunk = (size_t)strtoull(argv[++j], NULL, 10);
@@ -124,6 +131,10 @@ int main(int argc, char **argv) {
         fprintf(stderr, "--beast writes binary frames to stdout: it cannot be combined with --raw, --onlyaddr, --sbs or --aircraft-json\n");
         return 1;
     }
+    if (opt_recover && cfg.gpu_resolve) {
+        fprintf(stderr, "--recover cannot be combined with --gpu-resolve: the device resolve has no recovery rule\n");
+        return 1;
+    }
     FILE *f = (filename[0] == '-' && filename[1] == 0) ? stdin : fopen(filename, "rb");
     if (!f) { perror("Opening data file"); return 1; }
 
@@ -135,6 +146,7 @@ int main(int argc, char **argv) {
     }
     if (opt_beast) modes_set_signal(ctx, 1);
     if (opt_levels) modes_set_levels(ctx, 1);
+    if (opt_recover && modes_set_recovery(ctx, 1)) { fprintf(stderr, "--recover: %s\n", modes_last_error(ctx)); return 1; }
     modes_set_sink(ctx, on_message, NULL);
     unsigned char *buf = (unsigned char *)modes_host_alloc(chunk);
     if (!buf) { fprintf(stderr, "out of memory\n"); return 1; }
@@ -157,6 +169,13 @@ int main(int argc, char **argv) {
         printf("%lld single bit errors\n", (long long)st.v[6]);
         printf("%lld two bits errors\n", (long long)st.v[7]);
         printf("%lld total usable messages\n", (long long)(st.v[3] + st.v[5]));
+        if (opt_recover) {
+            modes_recovery_stats rs;
+            modes_get_recovery_stats(ctx, &rs);
+            fprintf(stderr, "recovery: %lld considered, %lld found, %lld ambiguous, %lld unknown address, %lld dropped, %lld delivered\n",
+                    (long long)rs.considered, (long long)rs.found, (long long)rs.ambiguous, (long long)rs.unknown_address,
+                    (long long)rs.dropped, (long long)rs.delivered);
+        }
     }
     if (opt_json) {
         size_t need = modes_tracker_format_json(tracker, 0, NULL, 0);

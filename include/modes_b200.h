@@ -78,7 +78,8 @@ typedef struct modes_config {
  * unassigned for a given DF are 0 here.  nfixed and sample_pos are additions. */
 typedef struct modes_message {
     uint8_t  msg[14];
-    uint8_t  pad0[2];
+    uint8_t  recovered;         /* 1: delivered by the soft-decision recovery (modes_set_recovery), not by the reference */
+    uint8_t  pad0;
     int32_t  msgbits, msgtype, crcok;
     uint32_t crc;
     int32_t  errorbit, aa1, aa2, aa3, phase_corrected;
@@ -450,6 +451,89 @@ int    modes_levels_fetch(modes_ctx *ctx, modes_level *out);
  * order; modes_pool_reset clears the receiver's queue.  Same take convention as above. */
 int    modes_pool_set_levels(modes_pool *p, int on);
 size_t modes_pool_take_levels(modes_pool *p, uint32_t receiver, modes_level *out, size_t cap);
+
+/* ---- soft-decision recovery of weak DF17/DF18 frames of known aircraft -------------------------
+ * Many weak frames pass the preamble test and fail the CRC because a few bits whose two half-bit
+ * samples were nearly equal were sliced the wrong way.  The recovery pass asks which bits were
+ * doubtful.  For a candidate at buffer position j, with the uncorrected magnitudes
+ * a_i = m[j+16+2i], c_i = m[j+17+2i] (i < 112; dump1090.c:359-364, :1670-1671):
+ *     hard bit b_i = a_i > c_i (a tie gives 0), confidence w_i = |a_i - c_i|
+ *     only DF = b_0..b_4 in {17, 18} is searched (extended squitters: the parity must be exactly 0)
+ *     s0 = the 24-bit syndrome of the 112 hard bits (dump1090.c:733-742)
+ *     P  = the MODES_RECOVER_BITS positions in [5, 112) with the smallest (w_i, i); the DF is never flipped
+ *     every subset S of P with XOR of the single-bit syndromes over S == s0 solves the frame:
+ *       FOUND      one solution of least |S| (S may be empty): msg = the hard frame with S flipped, nflips = |S|
+ *       AMBIGUOUS  two or more solutions share the least |S| (msg = the hard frame, nflips = that |S|)
+ *       NOT_FOUND  no subset solves it (msg = the hard frame, nflips = 0)
+ *     signal = floor(sqrt(floor(sum max(a_i, c_i)^2 / 112))) (the signal level of a long frame)
+ * Candidates with another DF get status INELIGIBLE, the hard frame, nflips 0 and the signal.
+ *
+ * What is delivered is decided in stream order by the host resolve.  A recovered message is
+ * delivered at candidate c (buffer b, position j) iff
+ *   1. the reference's walk visits c (it is not inside a message the reference took),
+ *   2. neither attempt at c was judged crcok (with check_crc = 0 the reference's crcok = 0
+ *      deliveries at c come first),
+ *   3. c is not within 241 positions after an earlier recovered message of the same buffer,
+ *   4. its status is FOUND,
+ *   5. its address (msg[1..3]) is in the ICAO address cache at that point (recovered messages never
+ *      write the cache: an aircraft with no clean frame yet gets none), and
+ *   6. the reference delivers no crcok message in the same buffer at j' with j < j' < j + 241
+ *      (the same frame decoded a sample later).
+ * It carries crcok = 1, crc = 0, errorbit = -1, phase_corrected = 0, iid = 0, nfixed = nflips,
+ * recovered = 1, the fields of the frame, and signal = the record's signal when signal measurement
+ * is on (0 otherwise).  The reference's messages and its eight statistics are unchanged.
+ * Recovered messages are not the reference's: they are frames it does not decode. */
+#define MODES_RECOVER_BITS 10
+enum { MODES_RECOVER_INELIGIBLE = 0, MODES_RECOVER_FOUND = 1, MODES_RECOVER_AMBIGUOUS = 2, MODES_RECOVER_NOT_FOUND = 3 };
+
+/* One record per candidate, at the candidate's index in the record array. */
+typedef struct modes_recovered {
+    uint8_t  msg[14];           /* the repaired frame if FOUND, otherwise the hard frame */
+    uint8_t  status;            /* MODES_RECOVER_* */
+    uint8_t  nflips;
+    uint16_t signal;
+    uint8_t  pad[2];
+} modes_recovered;
+
+typedef struct modes_recovery_stats {
+    int64_t considered;         /* rules 1-2 hold and the DF is 17 or 18 */
+    int64_t found;              /* of those, outside an earlier recovered message's span (rule 3) and FOUND */
+    int64_t ambiguous;          /* ... and AMBIGUOUS */
+    int64_t unknown_address;    /* FOUND, address not in the cache (rule 5) */
+    int64_t dropped;            /* passed rules 1-5, dropped by rule 6 */
+    int64_t delivered;
+} modes_recovery_stats;
+
+/* Recovery is off by default.  When it is on, every batch the streaming decode submits afterwards
+ * runs one more kernel after frame evaluation (one more launch per batch), its records come back
+ * with the candidate records, and the host resolve applies the rules above.  On an n_gpus > 1
+ * context the setting reaches every GPU.  It cannot be combined with gpu_resolve = 1: the call then
+ * fails and leaves the context as it was.  modes_reset clears the statistics. */
+int    modes_set_recovery(modes_ctx *ctx, int on);
+int    modes_get_recovery_stats(const modes_ctx *ctx, modes_recovery_stats *out);
+/* Stage level: the records of the batch and candidate records of the last modes_detect_device /
+ * _host call, queued on the context's stream after it without waiting.  d_out: capacity records in
+ * device memory, or NULL for the context's own buffer, read with modes_recover_fetch (which waits
+ * and copies as many records as modes_detect_wait reports).  Records beyond the capacity of either
+ * array are not written. */
+int    modes_recover_device(modes_ctx *ctx, void *d_out, size_t capacity);
+int    modes_recover_fetch(modes_ctx *ctx, modes_recovered *out);
+/* The host resolve with the rules above: recovered[k] belongs to candidates[k] (NULL: exactly
+ * modes_resolver_run).  The records' signal is delivered as it is.  Batches must end at buffer
+ * boundaries, as every decode path's do. */
+int    modes_resolver_run_recovered(modes_resolver *r, const modes_candidate *candidates, const modes_recovered *recovered,
+                                    const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, modes_sink_fn sink, void *user);
+/* modes_resolver_run_shards with recovery records, recovered[k][i] belonging to candidates[k][i]
+ * (recovered = NULL: exactly modes_resolver_run_shards); the same as running the shards one by one
+ * with modes_resolver_run_recovered. */
+int    modes_resolver_run_shards_recovered(modes_resolver *r, size_t n_shards, const modes_candidate *const *candidates,
+                                           const modes_recovered *const *recovered, const modes_tile *const *tiles,
+                                           const size_t *n_tiles, const int64_t *buffer_base, modes_sink_fn sink, void *user);
+int    modes_resolver_recovery_stats(const modes_resolver *r, modes_recovery_stats *out);
+/* The pool: recovery for every batch submitted while the switch is on; statistics per receiver,
+ * cleared by modes_pool_reset. */
+int    modes_pool_set_recovery(modes_pool *p, int on);
+int    modes_pool_recovery_stats(const modes_pool *p, uint32_t receiver, modes_recovery_stats *out);
 
 #ifdef __cplusplus
 }
