@@ -54,7 +54,16 @@ tests/_build/libeval_serial_host.so: tests/host_shim/eval_serial_host.cpp $(CSRC
 	g++ -O2 -std=c++17 -shared -fPIC -Wall -Wno-unknown-pragmas -x c++ -Iinclude -I$(CSRC) -I/usr/local/cuda/include \
 	    tests/host_shim/eval_serial_host.cpp $(CSRC)/modes_tables.cpp -o $@
 
+# test infrastructure: device harness over the product's own kernel objects (recovery and signal
+# passes on constructed corpora, and the exhaustive sweeps of the core headers' device build)
+DSHIM_OBJS := build/modes_recover.o build/modes_signal.o build/modes_levels.o build/modes_tables.o
+dshim: tests/_build/libkernels_device.so
+tests/_build/libkernels_device.so: tests/device_shim/kernels_device.cu $(DSHIM_OBJS) $(CSRC)/modes_internal.h $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_levels_core.cuh include/modes_b200.h
+	@mkdir -p tests/_build
+	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/kernels_device.cu -o tests/_build/kernels_device.o
+	$(NVCC) $(ARCH) -shared -o $@ tests/_build/kernels_device.o $(DSHIM_OBJS) -cudart static
+
 clean:
 	rm -rf build tests/_build $(LIB) dump1090-b200
 
-.PHONY: all oracle shim clean
+.PHONY: all oracle shim dshim clean

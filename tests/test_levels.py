@@ -18,6 +18,7 @@ import numpy as np
 import pytest
 
 import checker as C
+import edge_corpora as E
 import streams as S
 from dump1090_b200 import api, synth
 
@@ -84,18 +85,7 @@ def shim():
     return lib
 
 
-def _buffers(rng):
-    """(name, one buffer of I/Q bytes)."""
-    yield "random", rng.integers(0, 256, size=BUF, dtype=np.uint8)
-    yield "all_0", np.zeros(BUF, dtype=np.uint8)
-    yield "all_255", np.full(BUF, 255, dtype=np.uint8)                   # every sample at m = 65167: largest sums
-    yield "all_127", np.full(BUF, 127, dtype=np.uint8)
-    yield "alphabet", rng.choice(np.array([0, 1, 126, 127, 128, 254, 255], dtype=np.uint8), size=BUF)
-    yield "weak_noise", np.clip(rng.normal(127, 3, size=BUF).round(), 0, 255).astype(np.uint8)
-    yield "rails_254", rng.choice(np.array([254, 1, 127], dtype=np.uint8), size=BUF)   # near the rails, never on them
-    one = np.full(BUF, 127, dtype=np.uint8)
-    one[[0, 1001, BUF - 1]] = [0, 255, 0]                                 # I, Q, Q on a rail
-    yield "three_clipped", one
+_buffers = E.level_buffers
 
 
 def _shim_sums(shim, buf, threads=KERNEL_THREADS):

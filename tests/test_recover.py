@@ -14,8 +14,8 @@ import numpy as np
 import pytest
 
 import checker as C
+import edge_corpora as E
 import recover_model as R
-import repair_corpus
 import streams as S
 from dump1090_b200 import api, synth
 
@@ -48,10 +48,7 @@ def _shim_records(shim, wins):
     return out
 
 
-def _restated(wins):
-    wins = np.asarray(wins, dtype=np.uint8).reshape(-1, 448)
-    m = R.magnitudes(wins.reshape(-1)).reshape(-1, 224)
-    return R.restate(m[:, 0::2], m[:, 1::2])
+_restated = E.restated
 
 
 def _assert_same(got, want, what):
@@ -60,62 +57,15 @@ def _assert_same(got, want, what):
         assert bad.size == 0, f"{what}: field {f} differs at {bad[:5].tolist()}"
 
 
-def _window(frame: bytes, weak=(), flips=(), strong=(60, 0), soft=(40, 39), rng=None):
-    """448 I/Q bytes of a frame's 112 bit pairs: the pulse of bit i in its first (1) or second (0)
-    sample; `weak` bits get nearly equal samples, and `flips` are sent the wrong way round."""
-    out = np.full((112, 4), 127, dtype=np.int64)
-    for i in range(112):
-        bit = (frame[i >> 3] >> (7 - (i & 7))) & 1
-        hi, lo = soft if i in weak else strong
-        if rng is not None and i not in weak:
-            hi += int(rng.integers(0, 20))
-        if i in flips:
-            bit ^= 1
-        out[i, 0] += hi if bit else lo
-        out[i, 2] += lo if bit else hi
-    return out.astype(np.uint8).reshape(-1)
-
-
-def _frames(n, seed, df=17):
-    rng = synth.Counter(seed)
-    return [synth.make_frame(df, 5, (0x400000 + rng.below(0x3FFFFF)).to_bytes(3, "big") + synth._me_airborne(rng))
-            for _ in range(n)]
-
-
 def test_shim_equals_restatement_on_random_windows(shim):
-    rng = np.random.default_rng(3)
-    cases = {
-        "random": rng.integers(0, 256, size=(500, 448), dtype=np.uint8),
-        "saturated": rng.choice(np.array([0, 255], dtype=np.uint8), size=(300, 448)),
-        "alphabet": rng.choice(np.array([0, 1, 126, 127, 128, 200, 254, 255], dtype=np.uint8), size=(300, 448)),
-    }
-    # all-equal windows behind a DF17 / DF18 prefix: every w = 0, the tie-break on i decides P
-    for df in (17, 18):
-        w = np.full((40, 448), 127, dtype=np.uint8)
-        for k in range(40):
-            w[k] = np.full(448, 127 + k, dtype=np.uint8)
-            w[k, :20] = _window(bytes([df << 3]) + bytes(13))[:20]
-        cases[f"all_equal_df{df}"] = w
-    # random windows whose hard DF is 17: the search runs on noise
-    noise = rng.integers(100, 155, size=(400, 448), dtype=np.uint8)
-    noise[:, :20] = _window(bytes([17 << 3]) + bytes(13))[:20]
-    cases["noise_df17"] = noise
+    cases = E.recover_random_windows()
     for name, wins in cases.items():
         _assert_same(_shim_records(shim, wins), _restated(wins), name)
     assert (_restated(cases["all_equal_df17"])["status"] != api.RECOVER_INELIGIBLE).all()
 
 
 def test_clean_and_repaired_frames(shim):
-    rng = np.random.default_rng(4)
-    wins, sent, expect = [], [], []
-    for k, f in enumerate(_frames(60, 11) + _frames(20, 12, df=18)):
-        wins.append(_window(f, rng=rng))                                # clean: FOUND with no flip
-        sent.append(f); expect.append(0)
-        weak = set(int(x) for x in rng.choice(np.arange(5, 112), size=10, replace=False))
-        for e in (1 + k % 10, 1 + (k + 3) % 10):
-            flips = set(sorted(weak)[:e])
-            wins.append(_window(f, weak=weak, flips=flips, rng=rng))
-            sent.append(f); expect.append(e)
+    wins, sent, expect = E.recover_frame_windows()
     got = _shim_records(shim, wins)
     want = _restated(wins)
     _assert_same(got, want, "frames")
@@ -128,13 +78,7 @@ def test_clean_and_repaired_frames(shim):
 
 
 def test_confident_error_and_other_formats(shim):
-    rng = np.random.default_rng(5)
-    wins = []
-    for f in _frames(40, 13):
-        weak = set(range(20, 30))
-        wins.append(_window(f, weak=weak, flips={int(rng.integers(40, 112))}, rng=rng))   # a confident bit wrong
-    for df in (0, 4, 5, 11, 16, 19, 20, 21, 24):
-        wins.append(_window(bytes([df << 3]) + bytes(rng.integers(0, 256, 13, dtype=np.uint8)), rng=rng))
+    wins = E.recover_confident_windows()                                 # a confident bit wrong; other formats
     got, want = _shim_records(shim, wins), _restated(wins)
     _assert_same(got, want, "confident/other")
     assert (want["status"][:40] != api.RECOVER_FOUND).sum() >= 35
@@ -144,14 +88,8 @@ def test_confident_error_and_other_formats(shim):
 def test_constructed_ambiguity(shim):
     """Three bits of a weight-6 codeword flipped, its six positions among the ten least confident:
     two solutions of weight 3."""
-    cws = [c for c in repair_corpus.long_codewords6() if min(c) >= 5]
-    assert len(cws) == 155
-    rng = np.random.default_rng(6)
-    wins = []
-    for k, (cw, f) in enumerate(zip(cws, _frames(len(cws), 14))):
-        others = [p for p in range(5, 112) if p not in cw]
-        weak = set(cw) | set(int(x) for x in rng.choice(others, size=4, replace=False))
-        wins.append(_window(f, weak=weak, flips=set(cw[:3]), rng=rng))
+    wins = E.recover_ambiguity_windows()
+    assert len(wins) == 155
     got, want = _shim_records(shim, wins), _restated(wins)
     _assert_same(got, want, "ambiguity")
     assert (want["status"] == api.RECOVER_AMBIGUOUS).all() and (want["nflips"] == 3).all()

@@ -14,6 +14,7 @@ import numpy as np
 import pytest
 
 import checker as C
+import edge_corpora as E
 import streams as S
 from dump1090_b200 import api, synth
 
@@ -103,20 +104,10 @@ def shim():
     return lib
 
 
-def _windows(rng):
-    """(name, windows of 224 samples as I/Q bytes)."""
-    yield "random", rng.integers(0, 256, size=(400, 448), dtype=np.uint8)
-    yield "saturated", rng.choice(np.array([0, 255], dtype=np.uint8), size=(200, 448))
-    yield "saturated_max", np.full((1, 448), 255, dtype=np.uint8)
-    yield "no_signal", np.full((2, 448), 127, dtype=np.uint8)
-    yield "levels", rng.choice(np.array([0, 1, 126, 127, 128, 200, 254, 255], dtype=np.uint8), size=(200, 448))
-    yield "weak", np.clip(rng.normal(127, 4, size=(200, 448)).round(), 0, 255).astype(np.uint8)
-
-
 @pytest.mark.parametrize("bits", [56, 112])
 def test_shim_window_equals_restatement(shim, bits):
     rng = np.random.default_rng(bits)
-    for name, wins in _windows(rng):
+    for name, wins in E.signal_windows(rng):
         for w in wins:
             w = np.ascontiguousarray(w)
             want = expected_signal(magnitudes(w), [-16], [bits])[0]
