@@ -182,7 +182,9 @@ EXPORTS = ["modes_abi_version", "modes_default_config", "modes_create", "modes_d
            "modes_pool_set_levels", "modes_pool_take_levels",
            "modes_set_recovery", "modes_get_recovery_stats", "modes_recover_device", "modes_recover_fetch",
            "modes_resolver_run_recovered", "modes_resolver_run_shards_recovered", "modes_resolver_recovery_stats", "modes_pool_set_recovery",
-           "modes_pool_recovery_stats"]
+           "modes_pool_recovery_stats", "modes_set_weak_preambles", "modes_get_weak_recovery_stats", "modes_weak_device",
+           "modes_weak_fetch", "modes_resolver_run_weak", "modes_resolver_run_shards_weak", "modes_resolver_weak_stats",
+           "modes_pool_set_weak_preambles", "modes_pool_weak_stats"]
 
 
 def lib():
@@ -297,6 +299,17 @@ def lib():
         L.modes_resolver_recovery_stats.argtypes = [C.c_void_p, C.POINTER(RecoveryStats)]
         L.modes_pool_set_recovery.argtypes = [C.c_void_p, C.c_int]
         L.modes_pool_recovery_stats.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(RecoveryStats)]
+        L.modes_set_weak_preambles.argtypes = [C.c_void_p, C.c_int]
+        L.modes_get_weak_recovery_stats.argtypes = [C.c_void_p, C.POINTER(RecoveryStats)]
+        L.modes_weak_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
+        L.modes_weak_fetch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
+        L.modes_resolver_run_weak.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int64,
+                                              C.c_void_p, C.c_void_p, C.c_size_t, SINK_FN, C.c_void_p]
+        L.modes_resolver_run_shards_weak.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, SINK_FN, C.c_void_p]
+        L.modes_resolver_weak_stats.argtypes = [C.c_void_p, C.POINTER(RecoveryStats)]
+        L.modes_pool_set_weak_preambles.argtypes = [C.c_void_p, C.c_int]
+        L.modes_pool_weak_stats.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(RecoveryStats)]
         _lib = L
     return _lib
 
@@ -372,9 +385,12 @@ class Decoder:
     levels=True measures every decoded buffer's noise, peak and clipping on the GPU
     (modes_set_levels): take_levels(), level_summary().  recover=True adds weak DF17/DF18 frames of
     known aircraft found by a soft-decision search on the GPU (modes_set_recovery), marked
-    Message.recovered: recovery_stats()."""
+    Message.recovered: recovery_stats().  weak_preambles=True (with recover=True) also searches the weak
+    preambles the reference's preamble test rejects (modes_set_weak_preambles): Message.recovered = 2,
+    weak_recovery_stats()."""
 
-    def __init__(self, signal: bool = False, levels: bool = False, recover: bool = False, **cfg):
+    def __init__(self, signal: bool = False, levels: bool = False, recover: bool = False, weak_preambles: bool = False,
+                 **cfg):
         self.cfg = make_config(**cfg)
         self._h = lib().modes_create(C.byref(self.cfg))
         if not self._h:
@@ -385,6 +401,8 @@ class Decoder:
             self.set_levels(True)
         if recover:
             self.set_recovery(True)
+        if weak_preambles:
+            self.set_weak_preambles(True)
         self._collector = _Collector()
         lib().modes_set_sink(self._h, self._collector.fn, None)
 
@@ -477,6 +495,16 @@ class Decoder:
     def recovery_stats(self) -> dict:
         st = RecoveryStats()
         self._check(lib().modes_get_recovery_stats(self._h, C.byref(st)))
+        return st.as_dict()
+
+    def set_weak_preambles(self, on: bool) -> None:
+        """Also recover at weak preambles in batches submitted from now on, while recovery is on
+        (modes_set_weak_preambles)."""
+        self._check(lib().modes_set_weak_preambles(self._h, int(bool(on))))
+
+    def weak_recovery_stats(self) -> dict:
+        st = RecoveryStats()
+        self._check(lib().modes_get_weak_recovery_stats(self._h, C.byref(st)))
         return st.as_dict()
 
     def take_levels(self) -> np.ndarray:
@@ -586,6 +614,23 @@ class Decoder:
         self._check(lib().modes_recover_fetch(self._h, _ptr(out)))
         return out[:n]
 
+    def weak_device(self, d_pos_ptr: int = 0, d_rec_ptr: int = 0, capacity: int = 0) -> None:
+        """Weak positions and their recovery records of the last detect_device / detect_host batch, into
+        device memory (capacity entries each), or (0) into the context's own buffers for weak_fetch()."""
+        self._check(lib().modes_weak_device(self._h, C.c_void_p(d_pos_ptr or None), C.c_void_p(d_rec_ptr or None), capacity))
+        self._weak_ext = bool(d_pos_ptr)
+
+    def weak_fetch(self):
+        """(count, t, records) of the last weak_device call; t and records are empty for caller buffers."""
+        n = C.c_uint64(0)
+        self._check(lib().modes_weak_fetch(self._h, None, None, C.byref(n)))
+        if getattr(self, "_weak_ext", False):
+            return int(n.value), np.zeros(0, np.uint32), np.zeros(0, RECOVERED_DTYPE)
+        t = np.zeros(max(n.value, 1), dtype=np.uint32)
+        rec = np.zeros(max(n.value, 1), dtype=RECOVERED_DTYPE)
+        self._check(lib().modes_weak_fetch(self._h, _ptr(t), _ptr(rec), C.byref(n)))
+        return int(n.value), t[: n.value], rec[: n.value]
+
     def publish_count(self, dst_ptr: int) -> None:
         self._check(lib().modes_detect_publish_count(self._h, C.c_void_p(dst_ptr)))
 
@@ -600,6 +645,17 @@ class Decoder:
     @property
     def stream(self) -> int:
         return int(lib().modes_stream(self._h) or 0)
+
+
+def _weak_arrays(weak):
+    t, rec = weak
+    t = np.ascontiguousarray(t, dtype=np.uint32)
+    rec = np.ascontiguousarray(rec, dtype=RECOVERED_DTYPE)
+    if rec.size != t.size:
+        raise ValueError(f"{rec.size} weak records for {t.size} weak positions: one per position is needed")
+    if t.size > 1 and not (np.diff(t.astype(np.int64)) > 0).all():
+        raise ValueError("weak positions must be sorted and distinct")
+    return t, rec
 
 
 def _recovery_records(recovered, cands: np.ndarray) -> np.ndarray:
@@ -617,13 +673,22 @@ class Resolver:
         self._h = lib().modes_resolver_create(C.byref(self.cfg))
         self._collector = _Collector()
 
-    def run(self, cands: np.ndarray, tiles: np.ndarray, buffer_base: int = 0, recovered: np.ndarray | None = None) -> None:
+    def run(self, cands: np.ndarray, tiles: np.ndarray, buffer_base: int = 0, recovered: np.ndarray | None = None,
+            weak=None) -> None:
         """recovered: RECOVERED_DTYPE records, one per candidate, to add recovered messages
-        (modes_resolver_run_recovered); None runs the reference's resolve alone."""
+        (modes_resolver_run_recovered); None runs the reference's resolve alone.  weak: (t, records) of
+        the weak preambles, t sorted (modes_resolver_run_weak; needs recovered)."""
         cands = np.ascontiguousarray(cands)
         tiles = np.ascontiguousarray(tiles)
         fn = C.cast(None, SINK_FN) if getattr(self, "_native", False) else self._collector.fn
-        if recovered is None:
+        if weak is not None:
+            if recovered is None:
+                raise ValueError("weak preambles need the candidates' recovery records")
+            rec = _recovery_records(recovered, cands)
+            wt, wr = _weak_arrays(weak)
+            rc = lib().modes_resolver_run_weak(self._h, _ptr(cands), _ptr(rec), _ptr(tiles), tiles.size, buffer_base,
+                                               _ptr(wt), _ptr(wr), wt.size, fn, None)
+        elif recovered is None:
             rc = lib().modes_resolver_run(self._h, _ptr(cands), _ptr(tiles), tiles.size, buffer_base, fn, None)
         else:
             rec = _recovery_records(recovered, cands)
@@ -638,12 +703,19 @@ class Resolver:
             raise RuntimeError("modes_resolver_recovery_stats failed")
         return st.as_dict()
 
+    def weak_stats(self) -> dict:
+        st = RecoveryStats()
+        if lib().modes_resolver_weak_stats(self._h, C.byref(st)):
+            raise RuntimeError("modes_resolver_weak_stats failed")
+        return st.as_dict()
+
     def reset_state(self) -> None:
         lib().modes_resolver_reset(self._h)
 
-    def run_shards(self, shards, recovered=None) -> None:
+    def run_shards(self, shards, recovered=None, weak=None) -> None:
         """shards: [(cands ndarray, tiles ndarray, buffer_base)] in stream order; resolved concurrently.
-        recovered: a list of RECOVERED_DTYPE arrays, one per shard (modes_resolver_run_shards_recovered)."""
+        recovered: a list of RECOVERED_DTYPE arrays, one per shard (modes_resolver_run_shards_recovered).
+        weak: a list of (t, records) per shard (modes_resolver_run_shards_weak; needs recovered)."""
         n = len(shards)
         keep = [(np.ascontiguousarray(c), np.ascontiguousarray(t)) for c, t, _ in shards]
         cp = (C.c_void_p * n)(*[c.ctypes.data for c, _ in keep])
@@ -651,7 +723,17 @@ class Resolver:
         nt = (C.c_size_t * n)(*[t.size for _, t in keep])
         bb = (C.c_int64 * n)(*[int(b) for _, _, b in shards])
         fn = C.cast(None, SINK_FN) if getattr(self, "_native", False) else self._collector.fn
-        if recovered is None:
+        if weak is not None:
+            if recovered is None or len(recovered) != n or len(weak) != n:
+                raise ValueError("weak preambles need one recovery array and one weak pair per shard")
+            recs = [_recovery_records(r, c) for r, (c, _) in zip(recovered, keep)]
+            wks = [_weak_arrays(w) for w in weak]
+            rp = (C.c_void_p * n)(*[r.ctypes.data for r in recs])
+            wtp = (C.c_void_p * n)(*[t.ctypes.data for t, _ in wks])
+            wrp = (C.c_void_p * n)(*[r.ctypes.data for _, r in wks])
+            nw = (C.c_size_t * n)(*[t.size for t, _ in wks])
+            rc = lib().modes_resolver_run_shards_weak(self._h, n, cp, rp, tp, nt, bb, wtp, wrp, nw, fn, None)
+        elif recovered is None:
             rc = lib().modes_resolver_run_shards(self._h, n, cp, tp, nt, bb, fn, None)
         else:
             if len(recovered) != n:
@@ -732,10 +814,11 @@ class ReceiverPool:
     statistics each, as one dump1090 process keeps per receiver), one buffer of each decoded per
     batch.  Messages are collected per receiver (`take(receiver)`).  signal=True: as for Decoder.
     levels=True: level records of every receiver's buffers (`take_levels(receiver)`).
-    recover=True: as for Decoder, with statistics per receiver (`recovery_stats(receiver)`)."""
+    recover=True: as for Decoder, with statistics per receiver (`recovery_stats(receiver)`).
+    weak_preambles=True: as for Decoder (`weak_recovery_stats(receiver)`)."""
 
     def __init__(self, n_receivers: int, max_batch: int = 0, signal: bool = False, levels: bool = False,
-                 recover: bool = False, **cfg):
+                 recover: bool = False, weak_preambles: bool = False, **cfg):
         self.cfg = make_config(**cfg)
         self.n = n_receivers
         self._h = lib().modes_pool_create(C.byref(self.cfg), n_receivers, max_batch)
@@ -747,6 +830,8 @@ class ReceiverPool:
             self.set_levels(True)
         if recover:
             self.set_recovery(True)
+        if weak_preambles:
+            self.set_weak_preambles(True)
         self.messages = [[] for _ in range(n_receivers)]
         self._fn = POOL_SINK_FN(self._on)
 
@@ -833,6 +918,15 @@ class ReceiverPool:
     def recovery_stats(self, receiver: int) -> dict:
         st = RecoveryStats()
         self._check(lib().modes_pool_recovery_stats(self._h, receiver, C.byref(st)))
+        return st.as_dict()
+
+    def set_weak_preambles(self, on: bool) -> None:
+        """Also recover at weak preambles in batches submitted from now on (modes_pool_set_weak_preambles)."""
+        self._check(lib().modes_pool_set_weak_preambles(self._h, int(bool(on))))
+
+    def weak_recovery_stats(self, receiver: int) -> dict:
+        st = RecoveryStats()
+        self._check(lib().modes_pool_weak_stats(self._h, receiver, C.byref(st)))
         return st.as_dict()
 
     def take_levels(self, receiver: int) -> np.ndarray:

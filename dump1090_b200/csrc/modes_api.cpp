@@ -49,6 +49,14 @@ struct Slot {
     // modes_set_recovery / modes_recover_device: one record per candidate (device, and its pinned host copy)
     modes_recovered *d_recovered = nullptr; size_t rec_cap = 0;
     modes_recovered *h_recovered = nullptr; size_t h_rec_cap = 0;
+    // modes_set_weak_preambles / modes_weak_device: the weak positions and their records (device, own
+    // capacity weak_cap), the scan's scratch list, its per-tile words (source, count and destination of
+    // every tile's block) and counters, and pinned host copies
+    uint32_t *d_weak_pos = nullptr; modes_recovered *d_weak_rec = nullptr; uint32_t weak_cap = 0, want_weak_cap = 0;
+    uint32_t *d_weak_scratch = nullptr;   // weak_cap entries: the scan's unordered list
+    uint32_t *d_weak_tiles = nullptr; uint32_t weak_tiles_cap = 0;
+    uint32_t *d_weak_counters = nullptr, *h_weak_counters = nullptr;
+    uint32_t *h_weak_pos = nullptr; modes_recovered *h_weak_rec = nullptr; size_t h_weak_cap = 0;
     // in-flight batch
     bool busy = false;
     size_t n_buffers = 0;
@@ -58,6 +66,9 @@ struct Slot {
     bool levels = false;              // the batch measures levels (the switch as it was at submit)
     bool recover = false;             // the batch runs the recovery pass (streaming: the switch as it was at submit)
     bool signal = false;              // the signal switch as it was at submit
+    bool weak = false;                // the batch runs the weak-preamble passes (streaming: both switches as they were at submit)
+    uint32_t *weak_pos_ext = nullptr; modes_recovered *weak_rec_ext = nullptr; uint32_t weak_ext_cap = 0;   // modes_weak_device's buffers
+    uint32_t weak_first = 0, weak_step = 1;   // the buffers the weak scan reads: weak_first + i * weak_step
     modes_recovered *rec_ext = nullptr; uint32_t rec_ext_cap = 0;   // modes_recover_device's d_out (nullptr: own buffer)
     uint32_t want_cap = 0;            // grow the candidate buffers to at least this on the next ensure
     // where this batch's results live (own workspace unless the caller supplied memory)
@@ -106,6 +117,7 @@ struct modes_ctx {
     bool signal = false;                  // modes_set_signal: measure the signal level of decoded attempts
     bool levels = false;                  // modes_set_levels: measure every decoded buffer's levels
     bool recover = false;                 // modes_set_recovery: soft-decision recovery of weak DF17/18 frames
+    bool weak = false;                    // modes_set_weak_preambles: recovery at weak preambles too
     std::vector<modes_level> level_q;     // records not taken yet, oldest from level_head on
     size_t level_head = 0;
     int64_t eof_buffer = -1;              // modes_finish: stream index of the EOF buffer and its real samples
@@ -201,6 +213,8 @@ void slot_free(Slot &s) {
     cudaFreeHost(s.h_gr_flags); cudaFreeHost(s.h_deliveries);
     cudaFree(s.d_levels); cudaFreeHost(s.h_levels);
     cudaFree(s.d_recovered); cudaFreeHost(s.h_recovered);
+    cudaFree(s.d_weak_pos); cudaFree(s.d_weak_rec); cudaFree(s.d_weak_scratch); cudaFree(s.d_weak_tiles); cudaFree(s.d_weak_counters);
+    cudaFreeHost(s.h_weak_counters); cudaFreeHost(s.h_weak_pos); cudaFreeHost(s.h_weak_rec);
     for (auto &e : s.ev) if (e) cudaEventDestroy(e);
     for (auto &e : s.halo_ev) if (e) cudaEventDestroy(e);
     if (s.stream) cudaStreamDestroy(s.stream);
@@ -323,6 +337,9 @@ int submit(modes_ctx *ctx, Slot &s, const uint8_t *host_iq, const void *d_iq, si
     s.levels = ctx->levels && &s != &ctx->detect;
     s.recover = ctx->recover && &s != &ctx->detect;       // the stage level asks with modes_recover_device
     s.rec_ext = nullptr; s.rec_ext_cap = 0;
+    s.weak = s.recover && ctx->weak;                      // the stage level asks with modes_weak_device
+    s.weak_pos_ext = nullptr; s.weak_rec_ext = nullptr; s.weak_ext_cap = 0;
+    s.weak_first = 0; s.weak_step = 1;
     s.signal = ctx->signal;
     if (s.levels && levels_ensure(ctx, s.d_levels, s.h_levels, s.levels_cap, n_buffers, nullptr)) return -1;   // collected
     if (host_iq) {
@@ -366,6 +383,54 @@ int launch_recovery(modes_ctx *ctx, Slot &s, const BatchView &in, const ScanOutp
     return 0;
 }
 
+// The weak-preamble scan and the search at its positions over the slot's batch, into the caller's
+// arrays or the slot's own, and the count to pinned memory.  The slot's own arrays (the scan's scratch
+// list always) are grown to want_weak_cap.
+int launch_weak(modes_ctx *ctx, Slot &s, const BatchView &in) {
+    const uint32_t n_scan = s.weak_first < s.n_buffers ? (uint32_t)((s.n_buffers - 1 - s.weak_first) / s.weak_step + 1) : 0u;
+    const uint64_t scan_samples = (uint64_t)n_scan * kBufSamples;
+    const uint32_t nt = weak_tiles_for(n_scan);
+    if (s.weak_tiles_cap < nt) {
+        cudaFree(s.d_weak_tiles); s.d_weak_tiles = nullptr; s.weak_tiles_cap = 0;
+        CK(ctx, cudaMalloc(&s.d_weak_tiles, 3 * (size_t)nt * sizeof(uint32_t)));
+        s.weak_tiles_cap = nt;
+    }
+    if (!s.d_weak_counters) {
+        CK(ctx, cudaMalloc(&s.d_weak_counters, 2 * sizeof(uint32_t)));
+        CK(ctx, cudaMallocHost(&s.h_weak_counters, 2 * sizeof(uint32_t)));
+    }
+    // a weak position passes the shape test, which two neighbours never both pass: at most one in two
+    uint64_t want = scan_samples / 512 + 4096;
+    if (want < s.want_weak_cap) want = s.want_weak_cap;
+    if (want > scan_samples / 2 + 1) want = scan_samples / 2 + 1;
+    if (s.weak_cap < want) {
+        cudaFree(s.d_weak_pos); cudaFree(s.d_weak_rec); cudaFree(s.d_weak_scratch);
+        s.d_weak_pos = nullptr; s.d_weak_rec = nullptr; s.d_weak_scratch = nullptr; s.weak_cap = 0;
+        CK(ctx, cudaMalloc(&s.d_weak_pos, want * sizeof(uint32_t)));
+        CK(ctx, cudaMalloc(&s.d_weak_rec, want * sizeof(modes_recovered)));
+        CK(ctx, cudaMalloc(&s.d_weak_scratch, want * sizeof(uint32_t)));
+        s.weak_cap = (uint32_t)want;
+    }
+    uint32_t *pos = s.weak_pos_ext ? s.weak_pos_ext : s.d_weak_pos;
+    modes_recovered *rec = s.weak_pos_ext ? s.weak_rec_ext : s.d_weak_rec;
+    const uint32_t cap = s.weak_pos_ext ? s.weak_ext_cap : s.weak_cap;
+    launch_weak_scan(in, ctx->tab,
+                     WeakOutputs{s.weak_first, s.weak_step, n_scan, pos, cap, s.d_weak_scratch, s.weak_cap, s.d_weak_tiles,
+                                 s.d_weak_counters},
+                     ctx->sm_count, s.stream);
+    launch_recover_weak(in, ctx->tab, s.d_weak_counters + 1, cap, s.weak_cap, pos, rec, ctx->sm_count, s.stream);
+    CK(ctx, cudaGetLastError());
+    ctx->launches += 4;
+    CK(ctx, cudaMemcpyAsync(s.h_weak_counters, s.d_weak_counters, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
+    return 0;
+}
+
+// The weak positions of the slot's last batch exceed its scratch list (and its own output arrays):
+// the batch is repeated with larger ones.  A caller's smaller arrays only report the count.
+bool weak_overflowed(const Slot &s) {
+    return s.weak && s.h_weak_counters[1] > s.weak_cap;
+}
+
 // The two kernels over the slot's staged batch (also used to repeat a batch that overflowed).
 int launch_batch(modes_ctx *ctx, Slot &s) {
     const uint64_t n_samples = (uint64_t)s.n_buffers * kBufSamples;
@@ -397,6 +462,7 @@ int launch_batch(modes_ctx *ctx, Slot &s) {
     CK(ctx, cudaGetLastError());
     ctx->launches += (ctx->signal ? 3 : 2) + (s.levels ? 1 : 0);
     if (s.recover && launch_recovery(ctx, s, in, so)) return -1;
+    if (s.weak && launch_weak(ctx, s, in)) return -1;
     if (ctx->cfg.gpu_resolve && s.own_outputs && &s != &ctx->detect) {
         if (gpu_resolve_ensure(ctx, s)) return -1;
         // the address cache comes from the previous batch's resolve (other slot, other stream)
@@ -427,18 +493,41 @@ int launch_batch(modes_ctx *ctx, Slot &s) {
 int wait_batch(modes_ctx *ctx, Slot &s, uint64_t *n_out) {
     for (;;) {
         CK(ctx, cudaEventSynchronize(s.ev[3]));
-        if (!s.h_counters[1] && s.h_counters[0] <= s.out_cap) break;
+        const bool cand_over = s.h_counters[1] || s.h_counters[0] > s.out_cap;
+        if (!cand_over && !weak_overflowed(s)) break;
         if (ctx->cfg.gpu_resolve && &s != &ctx->detect) break;           // reported by collect(): the device resolve ran on a truncated list
-        const uint32_t found = s.h_counters[0];
-        if (!s.own_outputs)
-            return fail(ctx, "candidate capacity exceeded: %u found, room for %u", found, s.out_cap);
-        s.want_cap = found + found / 8 + 1024;
-        if (slot_ensure(ctx, s, (uint64_t)s.n_buffers * kBufSamples, false, true)) return -1;
-        s.out_records = s.d_records;
-        s.out_cap = s.cand_cap;
+        if (cand_over) {
+            const uint32_t found = s.h_counters[0];
+            if (!s.own_outputs)
+                return fail(ctx, "candidate capacity exceeded: %u found, room for %u", found, s.out_cap);
+            s.want_cap = found + found / 8 + 1024;
+            if (slot_ensure(ctx, s, (uint64_t)s.n_buffers * kBufSamples, false, true)) return -1;
+            s.out_records = s.d_records;
+            s.out_cap = s.cand_cap;
+        }
+        if (weak_overflowed(s)) s.want_weak_cap = s.h_weak_counters[1] + s.h_weak_counters[1] / 8 + 1024;
         if (launch_batch(ctx, s)) return -1;
     }
     *n_out = s.h_counters[0];
+    return 0;
+}
+
+// Pinned room for the slot's weak positions and records, and their copies queued on its stream;
+// returns the weak list of the batch.
+int weak_fetch_async(modes_ctx *ctx, Slot &s, WeakList &wl) {
+    const size_t n = s.h_weak_counters[1];
+    if (s.h_weak_cap < n) {
+        cudaFreeHost(s.h_weak_pos); cudaFreeHost(s.h_weak_rec); s.h_weak_pos = nullptr; s.h_weak_rec = nullptr; s.h_weak_cap = 0;
+        const size_t cap = n + n / 2 + 1024;
+        CK(ctx, cudaMallocHost(&s.h_weak_pos, cap * sizeof(uint32_t)));
+        CK(ctx, cudaMallocHost(&s.h_weak_rec, cap * sizeof(modes_recovered)));
+        s.h_weak_cap = cap;
+    }
+    if (n) {
+        CK(ctx, cudaMemcpyAsync(s.h_weak_pos, s.d_weak_pos, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
+        CK(ctx, cudaMemcpyAsync(s.h_weak_rec, s.d_weak_rec, n * sizeof(modes_recovered), cudaMemcpyDeviceToHost, s.stream));
+    }
+    wl = WeakList{s.h_weak_pos, s.h_weak_rec, n};
     return 0;
 }
 
@@ -485,12 +574,14 @@ int collect(modes_ctx *ctx, Slot &s) {
     if (s.recover && recovered_ensure(ctx, s, n)) return -1;
     if (n) CK(ctx, cudaMemcpyAsync(s.h_records, s.out_records, n * sizeof(modes_candidate), cudaMemcpyDeviceToHost, s.stream));
     if (n && s.recover) CK(ctx, cudaMemcpyAsync(s.h_recovered, s.d_recovered, n * sizeof(modes_recovered), cudaMemcpyDeviceToHost, s.stream));
+    WeakList wl;
+    if (s.weak && weak_fetch_async(ctx, s, wl)) return -1;
     CK(ctx, cudaMemcpyAsync(s.h_tiles, s.out_tiles, nt * sizeof(modes_tile), cudaMemcpyDeviceToHost, s.stream));
     CK(ctx, wait_stream(s.stream));
     const double t2 = dbg ? now_ms() : 0;
     ResolveConfig rc{ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->cfg.check_crc, s.signal ? 1 : 0};
     resolve_candidates(ctx->rs, rc, s.h_records, s.h_tiles, nt, s.buffer_base, ctx->out, ctx->scratch,
-                       s.recover ? s.h_recovered : nullptr);
+                       s.recover ? s.h_recovered : nullptr, wl);
     if (dbg) fprintf(stderr, "[collect] %zu buffers, %llu cands: wait %.3f ms, d2h %.3f ms, resolve %.3f ms (t=%.3f)\n",
                      s.n_buffers, (unsigned long long)n, t1 - t0, t2 - t1, now_ms() - t2, now_ms());
     return 0;
@@ -507,6 +598,7 @@ int collect_group(modes_ctx *ctx, int parity) {
     std::vector<size_t> n_tiles(n);
     std::vector<int64_t> base(n);
     std::vector<const modes_recovered *> recovered(n, nullptr);
+    std::vector<WeakList> weak(n);
     bool any_recover = false, signal = false;
     for (size_t k = 0; k < n; k++) {
         modes_ctx *g = ctx->gpus[k];
@@ -526,6 +618,7 @@ int collect_group(modes_ctx *ctx, int parity) {
             recovered[k] = s.h_recovered;
             any_recover = true;
         }
+        if (s.weak && weak_fetch_async(g, s, weak[k])) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
         signal = s.signal;
         CK(ctx, cudaMemcpyAsync(s.h_tiles, s.out_tiles, n_tiles[k] * sizeof(modes_tile), cudaMemcpyDeviceToHost, s.stream));
         cands[k] = s.h_records; tiles[k] = s.h_tiles; base[k] = s.buffer_base;
@@ -539,7 +632,7 @@ int collect_group(modes_ctx *ctx, int parity) {
         for (size_t k = 0; k < n; k++)
             if (!recovered[k]) return fail(ctx, "internal: recovery records missing for GPU %d", ctx->gpus[k]->cfg.device);
     resolve_shards(ctx->rs, rc, n, cands.data(), tiles.data(), n_tiles.data(), base.data(), ctx->out, ctx->scratch,
-                   any_recover ? recovered.data() : nullptr);
+                   any_recover ? recovered.data() : nullptr, weak.data());
     return 0;
 }
 
@@ -565,7 +658,7 @@ int run_buffers_multi(modes_ctx *ctx, const uint8_t *host_iq, size_t n_buffers) 
             ctx->buffers_done += (int64_t)nb;
             host_iq += nb * MODES_BUFFER_BYTES;
             n_buffers -= nb;
-            ctx->launches += (g->signal ? 3 : 2) + (g->levels ? 1 : 0) + (g->recover ? 1 : 0);
+            ctx->launches += (g->signal ? 3 : 2) + (g->levels ? 1 : 0) + (g->recover ? 1 : 0) + (g->recover && g->weak ? 4 : 0);
         }
         ctx->group_n[cur] = k;
         if (have_prev && collect_group(ctx, cur ^ 1)) return -1;
@@ -788,6 +881,68 @@ int modes_set_recovery(modes_ctx *ctx, int on) {
 int modes_get_recovery_stats(const modes_ctx *ctx, modes_recovery_stats *out) {
     if (!ctx || !out) return -1;
     *out = ctx->rs.rstats;
+    return 0;
+}
+
+int modes_set_weak_preambles(modes_ctx *ctx, int on) {
+    if (!ctx) return -1;
+    if (on && ctx->cfg.gpu_resolve) return fail(ctx, "modes_set_weak_preambles: recovery cannot be combined with gpu_resolve");
+    ctx->weak = on != 0;
+    for (modes_ctx *g : ctx->gpus) g->weak = on != 0;
+    return 0;
+}
+
+int modes_get_weak_recovery_stats(const modes_ctx *ctx, modes_recovery_stats *out) {
+    if (!ctx || !out) return -1;
+    *out = ctx->rs.wstats;
+    return 0;
+}
+
+int modes_weak_device(modes_ctx *ctx, void *d_pos, void *d_rec, size_t capacity) {
+    return modes::weak_device_strided(ctx, d_pos, d_rec, capacity, 0, 1);
+}
+
+}  // extern "C"
+
+int modes::weak_device_strided(modes_ctx *ctx, void *d_pos, void *d_rec, size_t capacity, uint32_t first_buffer,
+                               uint32_t buffer_step) {
+    if (!ctx) return -1;
+    Slot &s = ctx->detect;
+    if (!s.batch_iq) return fail(ctx, "modes_weak_device without modes_detect_device");
+    if (!buffer_step) return fail(ctx, "modes_weak_device: buffer step 0");
+    if ((d_pos == nullptr) != (d_rec == nullptr)) return fail(ctx, "modes_weak_device: give both output arrays or neither");
+    if (d_pos && !capacity) return fail(ctx, "modes_weak_device: capacity 0");
+    if (((reinterpret_cast<uintptr_t>(d_pos) | reinterpret_cast<uintptr_t>(d_rec)) & 3) != 0)
+        return fail(ctx, "modes_weak_device: outputs must be 4-byte aligned");
+    CK(ctx, cudaSetDevice(ctx->cfg.device));
+    s.weak = true;
+    s.weak_pos_ext = static_cast<uint32_t *>(d_pos);
+    s.weak_rec_ext = static_cast<modes_recovered *>(d_rec);
+    s.weak_ext_cap = !d_pos ? 0 : (capacity > 0xFFFFFFF0ull ? 0xFFFFFFF0u : (uint32_t)capacity);
+    s.weak_first = first_buffer; s.weak_step = buffer_step;
+    // a batch that wait_batch repeats (after a candidate or weak overflow) runs the passes again (launch_batch)
+    BatchView in{static_cast<const uint8_t *>(s.batch_iq), s.d_halo, (uint64_t)s.n_buffers * kBufSamples};
+    if (launch_weak(ctx, s, in)) return -1;
+    CK(ctx, cudaEventRecord(s.ev[3], s.stream));           // wait_batch sees the weak count too
+    return 0;
+}
+
+extern "C" {
+
+int modes_weak_fetch(modes_ctx *ctx, uint32_t *t, modes_recovered *rec, uint64_t *n) {
+    if (!ctx) return -1;
+    Slot &s = ctx->detect;
+    if (!s.weak) return fail(ctx, "modes_weak_fetch without modes_weak_device");
+    CK(ctx, cudaSetDevice(ctx->cfg.device));
+    uint64_t nc = 0;
+    if (wait_batch(ctx, s, &nc)) return -1;
+    const uint64_t nw = s.h_weak_counters[1];
+    if (n) *n = nw;
+    if (!s.weak_pos_ext && nw) {
+        if (t) CK(ctx, cudaMemcpyAsync(t, s.d_weak_pos, nw * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
+        if (rec) CK(ctx, cudaMemcpyAsync(rec, s.d_weak_rec, nw * sizeof(modes_recovered), cudaMemcpyDeviceToHost, s.stream));
+    }
+    CK(ctx, wait_stream(s.stream));
     return 0;
 }
 
@@ -1030,6 +1185,43 @@ int modes_resolver_recovery_stats(const modes_resolver *r, modes_recovery_stats 
     return 0;
 }
 
+int modes_resolver_run_weak(modes_resolver *r, const modes_candidate *candidates, const modes_recovered *recovered,
+                            const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, const uint32_t *weak_t,
+                            const modes_recovered *weak_rec, size_t n_weak, modes_sink_fn sink, void *user) {
+    if (!r || !tiles || (n_weak && (!recovered || !weak_t || !weak_rec))) return -1;
+    for (size_t k = 1; k < n_weak; k++)
+        if (weak_t[k] <= weak_t[k - 1]) return -1;                   // stream order, each position once
+    r->out.sink = sink; r->out.user = user;
+    resolve_candidates(r->rs, r->rc, candidates, tiles, n_tiles, buffer_base, r->out, r->scratch, recovered,
+                       WeakList{weak_t, weak_rec, n_weak});
+    return 0;
+}
+
+int modes_resolver_run_shards_weak(modes_resolver *r, size_t n_shards, const modes_candidate *const *candidates,
+                                   const modes_recovered *const *recovered, const modes_tile *const *tiles,
+                                   const size_t *n_tiles, const int64_t *buffer_base, const uint32_t *const *weak_t,
+                                   const modes_recovered *const *weak_rec, const size_t *n_weak, modes_sink_fn sink,
+                                   void *user) {
+    if (!r || (n_shards && (!candidates || !tiles || !n_tiles || !buffer_base || !recovered || !weak_t || !weak_rec || !n_weak)))
+        return -1;
+    std::vector<WeakList> wl(n_shards);
+    for (size_t k = 0; k < n_shards; k++) {
+        if (!recovered[k] || (n_weak[k] && (!weak_t[k] || !weak_rec[k]))) return -1;
+        for (size_t i = 1; i < n_weak[k]; i++)
+            if (weak_t[k][i] <= weak_t[k][i - 1]) return -1;
+        wl[k] = WeakList{weak_t[k], weak_rec[k], n_weak[k]};
+    }
+    r->out.sink = sink; r->out.user = user;
+    resolve_shards(r->rs, r->rc, n_shards, candidates, tiles, n_tiles, buffer_base, r->out, r->scratch, recovered, wl.data());
+    return 0;
+}
+
+int modes_resolver_weak_stats(const modes_resolver *r, modes_recovery_stats *out) {
+    if (!r || !out) return -1;
+    *out = r->rs.wstats;
+    return 0;
+}
+
 int modes_resolver_run_shards(modes_resolver *r, size_t n_shards, const modes_candidate *const *candidates,
                               const modes_tile *const *tiles, const size_t *n_tiles, const int64_t *buffer_base,
                               modes_sink_fn sink, void *user) {
@@ -1073,6 +1265,7 @@ int modes_resolver_run_tentative(modes_resolver *r, const modes_candidate *candi
     r->tentative = r->rs;
     memset(r->tentative.stats, 0, sizeof(r->tentative.stats));
     memset(&r->tentative.rstats, 0, sizeof(r->tentative.rstats));
+    memset(&r->tentative.wstats, 0, sizeof(r->tentative.wstats));
     r->tentative.cur_buffer = -1; r->tentative.next_j = 0; r->tentative.next_j_recovered = 0;
     resolve_tentative(r->tentative, r->rc, candidates, tiles, n_tiles, buffer_base, r->scratch);
     r->has_tentative = true;
@@ -1084,6 +1277,7 @@ int modes_resolver_commit(modes_resolver *r, modes_sink_fn sink, void *user) {
     r->out.sink = sink; r->out.user = user;
     for (int i = 0; i < 8; i++) r->rs.stats[i] += r->tentative.stats[i];
     add_recovery_stats(r->rs.rstats, r->tentative.rstats);
+    add_recovery_stats(r->rs.wstats, r->tentative.wstats);
     memcpy(r->rs.icao, r->tentative.icao, sizeof(r->rs.icao));
     r->rs.cur_buffer = r->tentative.cur_buffer; r->rs.next_j = r->tentative.next_j;
     r->rs.next_j_recovered = r->tentative.next_j_recovered;

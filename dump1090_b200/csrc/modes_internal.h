@@ -86,6 +86,32 @@ static_assert(sizeof(modes_level) == 40 && offsetof(modes_level, sum_mag) == 16 
 // candidate records and the windows the scan and frame evaluation read.
 void launch_recover(const BatchView &in, const DeviceTables &tab, const ScanOutputs &scan, const modes_candidate *records,
                     uint32_t capacity, modes_recovered *out, int sm_count, cudaStream_t stream);
+// Weak preambles (modes_weak.cu, three kernels): the positions of the scanned buffers of the batch
+// (buffers first_buffer + i * buffer_step, i < n_buffers) that meet the weak-preamble definition
+// (include/modes_b200.h), in stream order: pos[k] for k < min(counters[1], capacity).  counters[1] is
+// the exact count; when it exceeds scratch_cap the list is not complete and nothing is written to pos
+// (the caller repeats the batch with a larger scratch list).  tiles: 3 * weak_tiles_for(n_buffers)
+// words of per-tile bookkeeping; counters (two words) are cleared on the stream by the launcher.
+constexpr uint32_t kWeakTileSamples = 4096;
+inline uint32_t weak_tiles_for(uint64_t n_buffers) { return (uint32_t)(n_buffers * (kBufSamples / kWeakTileSamples)); }
+struct WeakOutputs {
+    uint32_t  first_buffer, buffer_step, n_buffers;
+    uint32_t *pos;
+    uint32_t  capacity;
+    uint32_t *scratch;           // the positions tile by tile, in no particular order of the tiles
+    uint32_t  scratch_cap;
+    uint32_t *tiles;
+    uint32_t *counters;          // [1] weak positions found (may exceed both capacities); [0] is not used
+};
+void launch_weak_scan(const BatchView &in, const DeviceTables &tab, const WeakOutputs &out, int sm_count, cudaStream_t stream);
+// The recovery records of the weak positions pos[k], k < min(*count, capacity), and none when *count
+// exceeds scratch_cap (the positions were not all written) (modes_recover.cu: the same per-position
+// search as launch_recover's).
+void launch_recover_weak(const BatchView &in, const DeviceTables &tab, const uint32_t *count, uint32_t capacity,
+                         uint32_t scratch_cap, const uint32_t *pos, modes_recovered *out, int sm_count, cudaStream_t stream);
+// modes_weak_device over the buffers first_buffer + i * buffer_step of the last batch only (the
+// receiver pool: its data buffers, never its pad buffers); modes_weak_device is (0, 1).
+int weak_device_strided(modes_ctx *ctx, void *d_pos, void *d_rec, size_t capacity, uint32_t first_buffer, uint32_t buffer_step);
 static_assert(sizeof(modes_recovered) == 20 && offsetof(modes_recovered, status) == 14 && offsetof(modes_recovered, signal) == 16,
               "recovery record layout");
 static_assert(offsetof(modes_message, recovered) == 14 && offsetof(modes_message, msgbits) == 16, "message layout");
@@ -134,6 +160,7 @@ struct ResolveState {
     uint32_t next_j;             // first position not skipped in cur_buffer
     uint32_t next_j_recovered;   // first position of cur_buffer not inside a recovered message (recovery only)
     modes_recovery_stats rstats;
+    modes_recovery_stats wstats; // recoveries at weak preambles (modes_set_weak_preambles)
     void reset();
 };
 
@@ -154,13 +181,18 @@ struct ResolveScratch;
 ResolveScratch *scratch_create();
 void scratch_destroy(ResolveScratch *s);
 
-// recovered: one record per candidate (modes_recover.cu), or nullptr with recovery off
+// The weak positions of a record array (sorted t, as the candidates' t) and their recovery records.
+struct WeakList { const uint32_t *t = nullptr; const modes_recovered *rec = nullptr; size_t n = 0; };
+
+// recovered: one record per candidate (modes_recover.cu), or nullptr with recovery off; weak: the
+// weak positions merged into the walk (only with recovered)
 void resolve_candidates(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands,
                         const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, MessageOut &out,
-                        ResolveScratch *scratch, const modes_recovered *recovered = nullptr);
+                        ResolveScratch *scratch, const modes_recovered *recovered = nullptr, const WeakList &weak = WeakList());
 void resolve_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards, const modes_candidate *const *cands,
                     const modes_tile *const *tiles, const size_t *n_tiles, const int64_t *buffer_base,
-                    MessageOut &out, ResolveScratch *scratch, const modes_recovered *const *recovered = nullptr);
+                    MessageOut &out, ResolveScratch *scratch, const modes_recovered *const *recovered = nullptr,
+                    const WeakList *weak = nullptr);
 // A shard resolved from a GUESSED address cache (one rank / one GPU thread of a sharded decode):
 // verdicts only, deliveries held back in the scratch until the guess is verified.
 void resolve_tentative(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands, const modes_tile *tiles,

@@ -21,6 +21,7 @@
 // The order-dependent half is the existing host resolver, one per receiver: the records of a data
 // buffer are re-based to that receiver's own stream position and replayed with its own address
 // cache.  Built on the public C ABI only (modes_detect_device / _fetch, modes_resolver_*).
+#include <algorithm>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -34,6 +35,7 @@
 #include <vector>
 #include <cuda_runtime.h>
 #include "modes_b200.h"
+#include "modes_internal.h"
 
 namespace {
 
@@ -106,6 +108,7 @@ struct modes_pool {
     int signal = 0;                            // modes_pool_set_signal, applied to the slot contexts
     int levels = 0;                            // modes_pool_set_levels
     int recover = 0;                           // modes_pool_set_recovery
+    int weak = 0;                              // modes_pool_set_weak_preambles
     std::string err;
     // device half (created on the first modes_pool_submit / _ingest): two batches may be in flight, so
     // that one is uploaded and scanned while the one before it is resolved on the host
@@ -118,16 +121,21 @@ struct modes_pool {
         std::vector<modes_level> level_out;
         bool levels = false;                   // the batch measures its data buffers' levels
         bool recover = false, signal = false;  // the recovery / signal switches as they were at submit
+        bool weak = false;                     // the batch runs the weak-preamble passes
         bool busy = false;
     } slot[2];
     unsigned submitted = 0, collected = 0;     // batches so far: slot = number & 1
     std::vector<modes_candidate> cands;
     std::vector<modes_recovered> recovered;    // with recovery: one record per candidate
+    std::vector<uint32_t> weak_t;              // with weak preambles: the batch's weak positions and records
+    std::vector<modes_recovered> weak_rec;
     std::vector<modes_tile> tiles;
     // the per-receiver resolve: one block of the receiver list per host thread
     struct Block {
         std::vector<modes_candidate> local;    // one receiver's records, re-based to its buffer
         std::vector<modes_recovered> local_rec;   // and their recovery records
+        std::vector<uint32_t> local_wt;        // the receiver's weak positions, re-based, and their records
+        std::vector<modes_recovered> local_wrec;
         std::vector<modes_tile> local_tiles;
         std::vector<modes_message> msgs;       // the block's messages, receiver by receiver
         std::vector<size_t> counts;            // messages of each receiver of the block
@@ -220,10 +228,11 @@ void modes_pool_destroy(modes_pool *p) {
 const char *modes_pool_last_error(const modes_pool *p) { return p ? p->err.c_str() : "no pool"; }
 
 // The per-receiver resolve; recovered: the batch's recovery records (nullptr: off), whose signal the
-// messages carry only when the batch measured signals.
+// messages carry only when the batch measured signals; weak_t / weak_rec / n_weak: its weak positions.
 static int pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, const modes_candidate *candidates,
                         const modes_recovered *recovered, bool signal, const modes_tile *tiles, modes_pool_sink_fn sink,
-                        void *user) {
+                        void *user, const uint32_t *weak_t = nullptr, const modes_recovered *weak_rec = nullptr,
+                        size_t n_weak = 0) {
     if (!p) return -1;
     if (check_ids(p, receivers, n)) return -1;
     if (!n) return 0;
@@ -251,9 +260,12 @@ static int pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, cons
         size_t room = 0, ga, gb, gc, gd;
         tile_range(i0, ga, gb); tile_range(i1 - 1, gc, gd);
         // a candidate delivers at most two messages of the reference (both attempts without --check-crc,
-        // dump1090.c:1803) and, with recovery, one recovered message after them
+        // dump1090.c:1803) and, with recovery, one recovered message after them; a weak position one
         const size_t per_candidate = recovered ? 3 : 2;
         for (size_t g = ga; g <= gd; g++) room += per_candidate * (size_t)tiles[g].count;
+        const uint32_t *wlo = std::lower_bound(weak_t, weak_t + n_weak, (uint32_t)(kBufSamples * (2 * i0 + 1)));
+        const uint32_t *whi = std::lower_bound(weak_t, weak_t + n_weak, (uint32_t)(kBufSamples * (2 * i1)));
+        room += (size_t)(whi - wlo);
         if (bl.msgs.size() < room) bl.msgs.resize(room);
         bl.local_tiles.resize(n_local);
         size_t used = 0;
@@ -284,9 +296,18 @@ static int pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, cons
             }
             uint32_t off = 0;
             for (modes_tile &lt : bl.local_tiles) { lt.offset = off; off += lt.count; }
+            bl.local_wt.clear();
+            bl.local_wrec.clear();
+            for (const uint32_t *w = std::lower_bound(weak_t, weak_t + n_weak, (uint32_t)t0); w < weak_t + n_weak && *w < t1; w++) {
+                modes_recovered rc = weak_rec[w - weak_t];
+                if (!signal) rc.signal = 0;
+                bl.local_wt.push_back(*w - (uint32_t)t0);
+                bl.local_wrec.push_back(rc);
+            }
             modes_resolver_set_output(r.res, bl.msgs.data() + used, room - used);
-            if (modes_resolver_run_recovered(r.res, bl.local.data(), recovered ? bl.local_rec.data() : nullptr, bl.local_tiles.data(),
-                                             n_local, r.buffers, nullptr, nullptr)) {
+            if (modes_resolver_run_weak(r.res, bl.local.data(), recovered ? bl.local_rec.data() : nullptr, bl.local_tiles.data(),
+                                        n_local, r.buffers, bl.local_wt.data(), bl.local_wrec.data(), bl.local_wt.size(),
+                                        nullptr, nullptr)) {
                 bl.failed = (int64_t)i; return;
             }
             const size_t k = modes_resolver_output_count(r.res);
@@ -371,6 +392,9 @@ int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *c
     sl.recover = p->recover != 0;
     sl.signal = p->signal != 0;
     if (sl.recover && modes_recover_device(sl.ctx, nullptr, 0)) return fail(p, "%s", modes_last_error(sl.ctx));
+    sl.weak = sl.recover && p->weak;
+    // the data buffers only (every second buffer), like the level pass
+    if (sl.weak && modes::weak_device_strided(sl.ctx, nullptr, nullptr, 0, 1, 2)) return fail(p, "%s", modes_last_error(sl.ctx));
     // the data buffers only (every second buffer), on the same stream: no wait before the collect
     sl.levels = p->levels != 0;
     if (sl.levels && modes_levels_device(sl.ctx, sl.d_batch + kBuf, n, 2 * kBuf)) return fail(p, "%s", modes_last_error(sl.ctx));
@@ -399,6 +423,13 @@ int modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user) {
         p->recovered.resize(n_cand ? n_cand : 1);
         if (modes_recover_fetch(sl.ctx, p->recovered.data())) return fail(p, "%s", modes_last_error(sl.ctx));
     }
+    uint64_t n_weak = 0;
+    if (sl.weak) {
+        if (modes_weak_fetch(sl.ctx, nullptr, nullptr, &n_weak)) return fail(p, "%s", modes_last_error(sl.ctx));
+        p->weak_t.resize(n_weak ? n_weak : 1);
+        p->weak_rec.resize(n_weak ? n_weak : 1);
+        if (modes_weak_fetch(sl.ctx, p->weak_t.data(), p->weak_rec.data(), &n_weak)) return fail(p, "%s", modes_last_error(sl.ctx));
+    }
     if (sl.levels) {
         sl.level_out.resize(n);
         if (modes_levels_fetch(sl.ctx, sl.level_out.data())) return fail(p, "%s", modes_last_error(sl.ctx));
@@ -411,7 +442,7 @@ int modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user) {
     sl.busy = false;
     p->collected++;
     return pool_resolve(p, sl.ids.data(), n, p->cands.data(), sl.recover ? p->recovered.data() : nullptr, sl.signal, p->tiles.data(),
-                        sink, user);
+                        sink, user, p->weak_t.data(), p->weak_rec.data(), (size_t)n_weak);
 }
 
 int modes_pool_ingest(modes_pool *p, const uint32_t *receivers, const uint8_t *const *iq, size_t n,
@@ -464,6 +495,17 @@ int modes_pool_set_recovery(modes_pool *p, int on) {
 int modes_pool_recovery_stats(const modes_pool *p, uint32_t receiver, modes_recovery_stats *out) {
     if (!p || receiver >= p->rx.size() || !out) return -1;
     return modes_resolver_recovery_stats(p->rx[receiver].res, out);
+}
+
+int modes_pool_set_weak_preambles(modes_pool *p, int on) {
+    if (!p) return -1;
+    p->weak = on != 0;
+    return 0;
+}
+
+int modes_pool_weak_stats(const modes_pool *p, uint32_t receiver, modes_recovery_stats *out) {
+    if (!p || receiver >= p->rx.size() || !out) return -1;
+    return modes_resolver_weak_stats(p->rx[receiver].res, out);
 }
 
 int modes_pool_set_levels(modes_pool *p, int on) {

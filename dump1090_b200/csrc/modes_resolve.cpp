@@ -37,6 +37,7 @@ void ResolveState::reset() {
     next_j = 0;
     next_j_recovered = 0;
     std::memset(&rstats, 0, sizeof(rstats));
+    std::memset(&wstats, 0, sizeof(wstats));
 }
 
 static inline uint32_t icao_slot(uint32_t a) {           // dump1090.c:898-905
@@ -197,14 +198,14 @@ struct Delivery {
     int64_t sample_pos;
     uint32_t iid, ap_addr;
     uint8_t crcok, phase_corrected;
-    uint8_t recovered;           // eval is a recovery record's frame: crc 0, nfixed = its flips
+    uint8_t recovered;           // eval is a recovery record's frame (1: at a candidate, 2: at a weak preamble): crc 0, nfixed = its flips
 };
 
 static inline void materialise(const Delivery &d, modes_message *mm) {
     build_message(d.eval, d.crcok, d.iid, d.ap_addr, mm);
     mm->sample_pos = d.sample_pos;
     mm->phase_corrected = d.phase_corrected;
-    if (d.recovered) { mm->recovered = 1; mm->errorbit = -1; }
+    if (d.recovered) { mm->recovered = d.recovered; mm->errorbit = -1; }
 }
 
 // Cores this process may actually keep busy: the CPUs it is allowed on, cut down to the CPU-time
@@ -321,31 +322,32 @@ struct RecoveryPending {                                  // the recovered messa
     size_t index = SIZE_MAX;                              // in the delivery list
     int64_t buffer = -1;
     uint32_t end = 0;                                     // first position of the buffer outside its span
+    modes_recovery_stats *stats = nullptr;                // the statistics it was counted in
 };
 
 // The recovery rules at one visited candidate, after the reference's attempts there (good: one of
-// them was judged crcok).
+// them was judged crcok), or at a visited weak position (good = false, stats = st.wstats, marker 2).
 static inline void recovery_step(ResolveState &st, const ResolveConfig &cfg, const modes_recovered &r, bool good,
                                  int64_t buffer, uint32_t j, int64_t pos, std::vector<Delivery> &deliveries,
-                                 RecoveryPending &pend) {
+                                 RecoveryPending &pend, modes_recovery_stats &stats, uint8_t marker) {
     if (good) {                                                            // rule 6
         if (pend.index != SIZE_MAX && pend.buffer == buffer && j < pend.end) {
             // what follows it in the list lies in this buffer within its span: a few entries move
             deliveries.erase(deliveries.begin() + (ptrdiff_t)pend.index);
-            st.rstats.dropped++;
-            st.rstats.delivered--;
+            pend.stats->dropped++;
+            pend.stats->delivered--;
             pend.index = SIZE_MAX;
         }
         return;
     }
     if (r.status == MODES_RECOVER_INELIGIBLE) return;                      // rule 2 holds
-    st.rstats.considered++;
+    stats.considered++;
     if (j < st.next_j_recovered) return;                                   // rule 3
-    if (r.status == MODES_RECOVER_AMBIGUOUS) st.rstats.ambiguous++;
+    if (r.status == MODES_RECOVER_AMBIGUOUS) stats.ambiguous++;
     if (r.status != MODES_RECOVER_FOUND) return;                           // rule 4
-    st.rstats.found++;
+    stats.found++;
     const uint32_t addr = ((uint32_t)r.msg[1] << 16) | ((uint32_t)r.msg[2] << 8) | (uint32_t)r.msg[3];
-    if (!icao_seen(st, addr)) { st.rstats.unknown_address++; return; }     // rule 5
+    if (!icao_seen(st, addr)) { stats.unknown_address++; return; }         // rule 5
     modes_frame_eval e{};
     std::memcpy(e.msg, r.msg, 14);
     e.msgtype = (uint8_t)(r.msg[0] >> 3);
@@ -356,21 +358,54 @@ static inline void recovery_step(ResolveState &st, const ResolveConfig &cfg, con
     pend.index = deliveries.size();
     pend.buffer = buffer;
     pend.end = j + kRecoveredSpan;
+    pend.stats = &stats;
     st.next_j_recovered = j + kRecoveredSpan;
-    deliveries.push_back(Delivery{e, pos, 0u, 0u, (uint8_t)1, (uint8_t)0, (uint8_t)1});
-    st.rstats.delivered++;
+    deliveries.push_back(Delivery{e, pos, 0u, 0u, (uint8_t)1, (uint8_t)0, marker});
+    stats.delivered++;
+}
+
+// The weak positions of the buffers [b_lo, b_hi) of a record array, merged into the walk: `next` is
+// the first one not visited yet.
+struct WeakCursor {
+    const WeakList *w = nullptr;
+    size_t next = 0;
+};
+
+// Visit the weak positions before record position `until` (and before buffer b_hi).
+static inline void weak_steps(ResolveState &st, const ResolveConfig &cfg, WeakCursor &wc, uint64_t until, uint32_t b_hi,
+                              int64_t buffer_base, std::vector<Delivery> &deliveries, RecoveryPending &pend) {
+    for (; wc.next < wc.w->n && wc.w->t[wc.next] < until; wc.next++) {
+        const uint32_t t = wc.w->t[wc.next];
+        if ((t >> 17) >= b_hi) { wc.next = wc.w->n; return; }
+        const int64_t buffer = buffer_base + (t >> 17);
+        const uint32_t j = t & (kBufSamples - 1);
+        if (buffer != st.cur_buffer) { st.cur_buffer = buffer; st.next_j = 0; st.next_j_recovered = 0; }
+        if (j < st.next_j) continue;                       // inside a message the reference took (rule 1)
+        const int64_t pos = buffer * (int64_t)kBufSamples + j - MODES_CARRY_SAMPLES;
+        recovery_step(st, cfg, wc.w->rec[wc.next], false, buffer, j, pos, deliveries, pend, st.wstats, 2);
+    }
 }
 
 // The verdict pass over one run of tiles: everything order-dependent, no message structs yet.
 // `b_lo`, `b_hi`: only the candidates of the buffers [b_lo, b_hi) of this record array are judged (buffer
 // numbers as in the records: t >> 17); the walk ends at the first candidate of buffer b_hi or later
 // (records are in stream order).  The whole array: 0, UINT32_MAX.  kRecover: apply the recovery rules
-// with `rec` (the walk without them has no trace of them).
+// with `rec` and merge the weak positions `weak` (may be nullptr) into the walk (the walk without
+// them has no trace of them).
 template <bool kRecover>
 static void walk_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands, const modes_tile *tiles,
                        size_t n_tiles, int64_t buffer_base, std::vector<Delivery> &deliveries, uint32_t b_lo, uint32_t b_hi,
-                       const modes_recovered *rec) {
+                       const modes_recovered *rec, const WeakList *weak) {
     RecoveryPending pend;
+    WeakCursor wc;
+    const bool merge = kRecover && weak && weak->n;
+    if (merge) {                                           // the first weak position of buffer b_lo or later
+        wc.w = weak;
+        const uint64_t lo = (uint64_t)b_lo << 17;
+        size_t a = 0, b = weak->n;
+        while (a < b) { const size_t m = (a + b) / 2; if (weak->t[m] < lo) a = m + 1; else b = m; }
+        wc.next = a;
+    }
     // The kernels append a tile's records wherever the global cursor stands when the tile finishes:
     // records are contiguous per tile but the tiles lie scattered through the array, so walking them
     // in stream order is a chain of cache misses (the records were just written by DMA).  Request
@@ -387,7 +422,11 @@ static void walk_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_c
             const modes_candidate *c = cands + k0 + k;
             const uint32_t rb = (uint32_t)(c->t >> 17);
             if (rb < b_lo) continue;                       // the part before this one takes it
-            if (rb >= b_hi) return;                        // the next part's
+            if (rb >= b_hi) {                              // the next part's
+                if (merge) weak_steps(st, cfg, wc, UINT64_MAX, b_hi, buffer_base, deliveries, pend);
+                return;
+            }
+            if (merge) weak_steps(st, cfg, wc, (uint64_t)c->t, b_hi, buffer_base, deliveries, pend);
             const int64_t buffer = buffer_base + rb;
             const uint32_t j = (uint32_t)(c->t & (kBufSamples - 1));
             if (buffer != st.cur_buffer) { st.cur_buffer = buffer; st.next_j = 0; st.next_j_recovered = 0; }
@@ -410,17 +449,19 @@ static void walk_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_c
                     }
                 }
             }
-            if constexpr (kRecover) recovery_step(st, cfg, rec[k0 + k], good, buffer, j, pos, deliveries, pend);
+            if constexpr (kRecover) recovery_step(st, cfg, rec[k0 + k], good, buffer, j, pos, deliveries, pend, st.rstats, 1);
             (void)good;
         }
     }
+    if (merge) weak_steps(st, cfg, wc, UINT64_MAX, b_hi, buffer_base, deliveries, pend);
 }
 
 static void judge_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands, const modes_tile *tiles,
                         size_t n_tiles, int64_t buffer_base, std::vector<Delivery> &deliveries,
-                        uint32_t b_lo = 0, uint32_t b_hi = UINT32_MAX, const modes_recovered *rec = nullptr) {
-    if (rec) walk_tiles<true>(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, b_lo, b_hi, rec);
-    else walk_tiles<false>(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, b_lo, b_hi, nullptr);
+                        uint32_t b_lo = 0, uint32_t b_hi = UINT32_MAX, const modes_recovered *rec = nullptr,
+                        const WeakList *weak = nullptr) {
+    if (rec) walk_tiles<true>(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, b_lo, b_hi, rec, weak);
+    else walk_tiles<false>(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, b_lo, b_hi, nullptr, nullptr);
 }
 
 // Build the delivered structs: in place and in parallel for array output, then the callback
@@ -491,6 +532,7 @@ struct Part {
     int64_t buffer_base;
     bool first_of_shard;         // the tail pass for a shard's first part walks the previous SHARD's array
     const modes_recovered *rec;  // the array's recovery records, or nullptr
+    const WeakList *weak;        // the array's weak positions, or nullptr
 };
 struct PartRun { ResolveState start, end; std::vector<Delivery> deliveries; };
 struct ResolveScratch {
@@ -524,8 +566,8 @@ static size_t parts_for(size_t n_tiles) {
 // read from the records themselves: the buffer after the one the first candidate at or behind tile
 // k * n_tiles / want lies in (tiles do not line up with buffers; records are in stream order).
 static void cut_parts(const modes_candidate *cands, const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, size_t want,
-                      std::vector<Part> &parts, const modes_recovered *rec = nullptr) {
-    Part p{cands, tiles, n_tiles, 0, 0, UINT32_MAX, buffer_base, true, rec};
+                      std::vector<Part> &parts, const modes_recovered *rec = nullptr, const WeakList *weak = nullptr) {
+    Part p{cands, tiles, n_tiles, 0, 0, UINT32_MAX, buffer_base, true, rec, weak};
     for (size_t k = 1; k < want; k++) {
         size_t ti = k * n_tiles / want;
         while (ti < n_tiles && tiles[ti].count == 0) ti++;
@@ -556,11 +598,12 @@ static int judge_parts(ResolveState &st, const ResolveConfig &cfg, const std::ve
         r.start = from;
         std::memset(r.start.stats, 0, sizeof(r.start.stats));
         std::memset(&r.start.rstats, 0, sizeof(r.start.rstats));
+        std::memset(&r.start.wstats, 0, sizeof(r.start.wstats));
         if (k) { r.start.cur_buffer = -1; r.start.next_j = 0; r.start.next_j_recovered = 0; }   // a part starts a buffer
         r.end = r.start;
         r.deliveries.clear();
         judge_tiles(r.end, cfg, p.cands, p.tiles + p.tile_lo, p.n_tiles - p.tile_lo, p.buffer_base, r.deliveries, p.b_lo, p.b_hi,
-                    p.rec);
+                    p.rec, p.weak);
     };
     int rounds = 0;
     size_t done = 0;                                       // parts [0, done) are final
@@ -607,6 +650,7 @@ static int judge_parts(ResolveState &st, const ResolveConfig &cfg, const std::ve
     for (size_t k = 0; k < n; k++) {
         for (int i = 0; i < 8; i++) st.stats[i] += runs[k].end.stats[i];
         add_recovery_stats(st.rstats, runs[k].end.rstats);
+        add_recovery_stats(st.wstats, runs[k].end.wstats);
     }
     if (n) {
         std::memcpy(st.icao, runs[n - 1].end.icao, sizeof(st.icao));
@@ -628,7 +672,7 @@ static PartRun *runs_for(ResolveScratch *scratch, size_t n) {
 
 void resolve_candidates(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands,
                         const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, MessageOut &out,
-                        ResolveScratch *scratch, const modes_recovered *recovered) {
+                        ResolveScratch *scratch, const modes_recovered *recovered, const WeakList &weak) {
     const bool timing = std::getenv("MODES_RESOLVE_TIMING") != nullptr;
     auto now = [] { return std::chrono::steady_clock::now(); };
     auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) {
@@ -639,14 +683,14 @@ void resolve_candidates(ResolveState &st, const ResolveConfig &cfg, const modes_
     if (want <= 1) {
         std::vector<Delivery> &deliveries = scratch->deliveries;
         deliveries.clear();
-        judge_tiles(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, 0, UINT32_MAX, recovered);
+        judge_tiles(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, 0, UINT32_MAX, recovered, &weak);
         const auto t1 = now();
         deliver(deliveries, out);
         if (timing) std::fprintf(stderr, "resolve_candidates: %zu tiles, verdicts %.2f ms, structs %.2f ms\n", n_tiles, ms(t0, t1), ms(t1, now()));
         return;
     }
     std::vector<Part> parts;
-    cut_parts(cands, tiles, n_tiles, buffer_base, want, parts, recovered);
+    cut_parts(cands, tiles, n_tiles, buffer_base, want, parts, recovered, &weak);
     PartRun *runs = runs_for(scratch, parts.size());
     const int rounds = judge_parts(st, cfg, parts, runs);
     const auto t1 = now();
@@ -685,7 +729,7 @@ void resolve_commit(MessageOut &out, ResolveScratch *scratch) {
 // is a part, long shards are cut once more (see judge_parts).
 void resolve_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards, const modes_candidate *const *cands,
                     const modes_tile *const *tiles, const size_t *n_tiles, const int64_t *buffer_base,
-                    MessageOut &out, ResolveScratch *scratch, const modes_recovered *const *recovered) {
+                    MessageOut &out, ResolveScratch *scratch, const modes_recovered *const *recovered, const WeakList *weak) {
     const bool timing = std::getenv("MODES_RESOLVE_TIMING") != nullptr;
     auto now = [] { return std::chrono::steady_clock::now(); };
     auto t_start = now();
@@ -696,7 +740,8 @@ void resolve_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards,
         size_t want = parts_for(n_tiles[k]);
         const size_t share = threads_left / (n_shards - k) > 0 ? threads_left / (n_shards - k) : 1;
         if (want > share) want = share;
-        cut_parts(cands[k], tiles[k], n_tiles[k], buffer_base[k], want, parts, recovered ? recovered[k] : nullptr);
+        cut_parts(cands[k], tiles[k], n_tiles[k], buffer_base[k], want, parts, recovered ? recovered[k] : nullptr,
+                  recovered && weak ? weak + k : nullptr);
         threads_left = threads_left > want ? threads_left - want : 0;
     }
     PartRun *runs = runs_for(scratch, parts.size());

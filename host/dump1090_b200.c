@@ -23,6 +23,8 @@
  * combines with every output mode; with --stats the reference's lines stay as they are on stdout and
  * one recovery line goes to stderr.  --gpu-resolve runs the order-dependent half on the GPU too
  * (modes_config.gpu_resolve); it has no recovery rule, so it is refused together with --recover.
+ * --recover-weak implies --recover and also searches weak preambles, positions the reference's
+ * preamble test rejects (modes_set_weak_preambles); with --stats a second line goes to stderr.
  * The live-radio, networking and interactive options are out of scope.
  */
 #include <math.h>
@@ -32,7 +34,7 @@
 #include "modes_b200.h"
 
 static int opt_raw = 0, opt_onlyaddr = 0, opt_stats = 0, opt_check_crc = 1, opt_sbs = 0, opt_json = 0, opt_beast = 0;
-static int opt_levels = 0, opt_recover = 0;
+static int opt_levels = 0, opt_recover = 0, opt_weak = 0;
 static modes_tracker *tracker = NULL;
 
 /* --levels: totals over the records taken so far */
@@ -117,6 +119,7 @@ int main(int argc, char **argv) {
         else if (!strcmp(argv[j], "--beast")) opt_beast = 1;
         else if (!strcmp(argv[j], "--levels")) opt_levels = 1;
         else if (!strcmp(argv[j], "--recover")) opt_recover = 1;
+        else if (!strcmp(argv[j], "--recover-weak")) opt_recover = opt_weak = 1;
         else if (!strcmp(argv[j], "--gpu-resolve")) cfg.gpu_resolve = 1;
         else if (!strcmp(argv[j], "--device") && more) cfg.device = atoi(argv[++j]);
         else if (!strcmp(argv[j], "--gpus") && more) cfg.n_gpus = atoi(argv[++j]);
@@ -132,6 +135,7 @@ int main(int argc, char **argv) {
         return 1;
     }
     if (opt_recover && cfg.gpu_resolve) {
+        if (opt_weak) fprintf(stderr, "--recover-weak implies --recover: ");
         fprintf(stderr, "--recover cannot be combined with --gpu-resolve: the device resolve has no recovery rule\n");
         return 1;
     }
@@ -147,6 +151,7 @@ int main(int argc, char **argv) {
     if (opt_beast) modes_set_signal(ctx, 1);
     if (opt_levels) modes_set_levels(ctx, 1);
     if (opt_recover && modes_set_recovery(ctx, 1)) { fprintf(stderr, "--recover: %s\n", modes_last_error(ctx)); return 1; }
+    if (opt_weak && modes_set_weak_preambles(ctx, 1)) { fprintf(stderr, "--recover-weak: %s\n", modes_last_error(ctx)); return 1; }
     modes_set_sink(ctx, on_message, NULL);
     unsigned char *buf = (unsigned char *)modes_host_alloc(chunk);
     if (!buf) { fprintf(stderr, "out of memory\n"); return 1; }
@@ -175,6 +180,13 @@ int main(int argc, char **argv) {
             fprintf(stderr, "recovery: %lld considered, %lld found, %lld ambiguous, %lld unknown address, %lld dropped, %lld delivered\n",
                     (long long)rs.considered, (long long)rs.found, (long long)rs.ambiguous, (long long)rs.unknown_address,
                     (long long)rs.dropped, (long long)rs.delivered);
+        }
+        if (opt_weak) {
+            modes_recovery_stats ws;
+            modes_get_weak_recovery_stats(ctx, &ws);
+            fprintf(stderr, "weak preambles: %lld considered, %lld found, %lld ambiguous, %lld unknown address, %lld dropped, %lld delivered\n",
+                    (long long)ws.considered, (long long)ws.found, (long long)ws.ambiguous, (long long)ws.unknown_address,
+                    (long long)ws.dropped, (long long)ws.delivered);
         }
     }
     if (opt_json) {

@@ -78,7 +78,8 @@ typedef struct modes_config {
  * unassigned for a given DF are 0 here.  nfixed and sample_pos are additions. */
 typedef struct modes_message {
     uint8_t  msg[14];
-    uint8_t  recovered;         /* 1: delivered by the soft-decision recovery (modes_set_recovery), not by the reference */
+    uint8_t  recovered;         /* 1: delivered by the soft-decision recovery (modes_set_recovery), not by the reference;
+                                   2: the same at a weak preamble (modes_set_weak_preambles) */
     uint8_t  pad0;
     int32_t  msgbits, msgtype, crcok;
     uint32_t crc;
@@ -534,6 +535,65 @@ int    modes_resolver_recovery_stats(const modes_resolver *r, modes_recovery_sta
  * cleared by modes_pool_reset. */
 int    modes_pool_set_recovery(modes_pool *p, int on);
 int    modes_pool_recovery_stats(const modes_pool *p, uint32_t receiver, modes_recovery_stats *out);
+
+/* ---- recovery at weak preambles ------------------------------------------------------------------
+ * The recovery above only searches positions that passed the reference's preamble test, and at low
+ * SNR that test rejects most weak frames before their bits are looked at.  A WEAK PREAMBLE is a
+ * buffer position j in [0, 131070) (the positions the reference scans, dump1090.c:1593) where, with
+ * m_x = m[j+x] (magnitudes of dump1090.c:359-364),
+ *   1. the pulse shape holds: m0 > m1, m2 > m1, m7 > m8, m9 > m8,
+ *   2. the mean pulse is more than twice the mean quiet sample:
+ *        7 (m0+m2+m7+m9) > 8 (m4+m5+m6+m11+m12+m13+m14)
+ *      (samples 1, 3, 8 and 10 are left out: a late pulse leaks into them),
+ *   3. the hard DF is 17 or 18: b_i = m[16+2i] > m[17+2i], i < 5, and
+ *   4. the reference's preamble test (dump1090.c:1602-1650, the "high" tests included) FAILS there,
+ *      so weak positions and candidates are disjoint.
+ * Every weak position gets the recovery record of a candidate at the same position (the same search,
+ * the same modes_recovered record).  In the host resolve, the weak positions are merged into the
+ * reference's walk in stream order.  A weak position (buffer b, j) starts the buffer's skip state like a
+ * candidate does, is visited iff j is not inside a message the reference took (rule 1), and then goes
+ * through rules 3-6 above as a candidate without a good attempt.  It shares the recovered-span skip
+ * (rule 3) and the rule-6 drop with the candidates' recoveries.  It never changes the reference's
+ * statistics or the address cache.
+ * Messages delivered from weak positions carry recovered = 2 and otherwise the fields of recovered
+ * messages.  Their statistics are kept apart: considered = weak positions visited, then found /
+ * ambiguous / unknown_address / dropped / delivered as above; the recovery statistics keep counting
+ * candidates only. */
+
+/* Off by default, effective only while recovery is on: every batch the streaming decode submits
+ * afterwards runs four more kernels (the weak-preamble scan, two that put its positions in stream order,
+ * and the search over them), one more copy brings the positions and records back, and the resolve
+ * merges them.  On an n_gpus > 1
+ * context the setting reaches every GPU.  Refused (and the context left as it was) with gpu_resolve = 1.
+ * modes_reset clears the statistics. */
+int    modes_set_weak_preambles(modes_ctx *ctx, int on);
+int    modes_get_weak_recovery_stats(const modes_ctx *ctx, modes_recovery_stats *out);
+/* Stage level: the weak positions of the batch of the last modes_detect_device / _host call, in stream
+ * order (t = 131072 * buffer + j, as modes_candidate.t), and their recovery records, queued on the
+ * context's stream after it without waiting.  d_pos (u32) and d_rec: capacity entries of device memory
+ * each, of which the first min(n, capacity) are written; both NULL: the context's own buffers, which
+ * grow to hold every position.  modes_weak_fetch waits and sets *n to the number of weak positions of
+ * the batch (which may exceed a caller's capacity); with the context's own buffers it also copies the
+ * n positions and records to t and rec (either may be NULL). */
+int    modes_weak_device(modes_ctx *ctx, void *d_pos, void *d_rec, size_t capacity);
+int    modes_weak_fetch(modes_ctx *ctx, uint32_t *t, modes_recovered *rec, uint64_t *n);
+/* modes_resolver_run_recovered with weak positions: weak_t[k] (sorted, t relative to buffer_base as
+ * the candidates' t) and weak_rec[k], k < n_weak.  recovered must not be NULL when n_weak > 0.  With
+ * n_weak = 0 it is exactly modes_resolver_run_recovered. */
+int    modes_resolver_run_weak(modes_resolver *r, const modes_candidate *candidates, const modes_recovered *recovered,
+                               const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, const uint32_t *weak_t,
+                               const modes_recovered *weak_rec, size_t n_weak, modes_sink_fn sink, void *user);
+/* The same over shards (as modes_resolver_run_shards_recovered): weak_t[k], weak_rec[k], n_weak[k] of shard k. */
+int    modes_resolver_run_shards_weak(modes_resolver *r, size_t n_shards, const modes_candidate *const *candidates,
+                                      const modes_recovered *const *recovered, const modes_tile *const *tiles,
+                                      const size_t *n_tiles, const int64_t *buffer_base, const uint32_t *const *weak_t,
+                                      const modes_recovered *const *weak_rec, const size_t *n_weak, modes_sink_fn sink,
+                                      void *user);
+int    modes_resolver_weak_stats(const modes_resolver *r, modes_recovery_stats *out);
+/* The pool: weak preambles for every batch submitted while both switches are on; statistics per
+ * receiver, cleared by modes_pool_reset. */
+int    modes_pool_set_weak_preambles(modes_pool *p, int on);
+int    modes_pool_weak_stats(const modes_pool *p, uint32_t receiver, modes_recovery_stats *out);
 
 #ifdef __cplusplus
 }

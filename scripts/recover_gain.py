@@ -2,11 +2,14 @@
 of a fleet of 20 aircraft that each send many frames, in noise at -3..+18 dB), decoded with --aggressive
 through the host resolve over the oracle's candidate records, with recovery records from the numpy
 restatement (tests/recover_model.py).  The GPU computes the same records (tests/test_recover.py).
+The weak columns add the weak preambles (modes_set_weak_preambles) from the numpy restatement of the
+weak-preamble scan (tests/weak_model.py; the GPU computes the same, tests/test_weak_preambles.py).
 
     python scripts/recover_gain.py [frames_per_point]      -> one JSON line per SNR point
 
 Per point: the reference's true frames, the extra true frames recovered, false recoveries (recovered
-frames that were never sent) and the recovery statistics."""
+frames that were never sent) and the recovery statistics; then, with weak preambles on, the extra true
+frames recovered at weak preambles, their false recoveries and the weak statistics."""
 import json
 import sys
 from pathlib import Path
@@ -16,6 +19,7 @@ sys.path.insert(0, str(ROOT))
 sys.path.insert(0, str(ROOT / "tests"))
 
 import recover_model as R
+import weak_model as W
 from dump1090_b200 import synth
 
 
@@ -29,7 +33,16 @@ def main():
         extra = set(rec) & truth - ref
         print(json.dumps({"snr_db": snr, "frames": nframes, "reference_true": len(ref), "recovered": len(rec),
                           "recovered_true_extra": len(extra), "false_recoveries": sum(h not in truth for h in rec),
-                          "gain": round(len(extra) / len(ref), 4) if ref else None, "stats": rstats}), flush=True)
+                          "gain": round(len(extra) / len(ref), 4) if ref else None, "stats": rstats,
+                          **weak_columns(data, truth)}), flush=True)
+
+
+def weak_columns(data, truth):
+    msgs, _, _, wstats, *_ = W.cpu_decode(data, dict(aggressive=1))
+    ref = {m.hex() for m in msgs if m.recovered != 2} & truth
+    weak = [m.hex() for m in msgs if m.recovered == 2]
+    return {"weak_recovered": len(weak), "weak_true_extra": len(set(weak) & truth - ref),
+            "weak_false_recoveries": sum(h not in truth for h in weak), "weak_stats": wstats}
 
 
 if __name__ == "__main__":
