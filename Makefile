@@ -11,7 +11,7 @@ OBJS      := build/modes_kernels.o build/modes_scan2.o build/modes_eval_fused.o 
 
 all: $(LIB) dump1090-b200
 
-build/%.o: $(CSRC)/%.cu $(CSRC)/modes_internal.h $(CSRC)/modes_eval_serial.cuh $(CSRC)/modes_scan_core.cuh $(CSRC)/modes_resolve_core.cuh $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_levels_core.cuh $(CSRC)/modes_recover_core.cuh $(CSRC)/modes_weak_core.cuh include/modes_b200.h
+build/%.o: $(CSRC)/%.cu $(CSRC)/modes_internal.h $(CSRC)/modes_eval_serial.cuh $(CSRC)/modes_scan_core.cuh $(CSRC)/modes_resolve_core.cuh $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_arrival_core.cuh $(CSRC)/modes_levels_core.cuh $(CSRC)/modes_recover_core.cuh $(CSRC)/modes_weak_core.cuh include/modes_b200.h
 	@mkdir -p build
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@
 
@@ -30,7 +30,11 @@ oracle:
 	if [ -d /root/reference ]; then $(MAKE) -C oracle ref; fi
 
 # test infrastructure: host build of the per-candidate evaluation (logic checked against the oracle on CPU)
-shim: tests/_build/libeval_serial_host.so tests/_build/libscan_core_host.so tests/_build/libresolve_core_host.so tests/_build/libsignal_core_host.so tests/_build/liblevels_core_host.so tests/_build/librecover_core_host.so tests/_build/libweak_core_host.so
+shim: tests/_build/libeval_serial_host.so tests/_build/libscan_core_host.so tests/_build/libresolve_core_host.so tests/_build/libsignal_core_host.so tests/_build/liblevels_core_host.so tests/_build/librecover_core_host.so tests/_build/libweak_core_host.so tests/_build/libarrival_core_host.so
+tests/_build/libarrival_core_host.so: tests/host_shim/arrival_core_host.cpp $(CSRC)/modes_arrival_core.cuh $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_tables.cpp include/modes_b200.h
+	@mkdir -p tests/_build
+	g++ -O2 -std=c++17 -shared -fPIC -Wall -Wno-unknown-pragmas -x c++ -Iinclude -I$(CSRC) -I/usr/local/cuda/include \
+	    tests/host_shim/arrival_core_host.cpp $(CSRC)/modes_tables.cpp -o $@
 tests/_build/libweak_core_host.so: tests/host_shim/weak_core_host.cpp $(CSRC)/modes_weak_core.cuh $(CSRC)/modes_tables.cpp include/modes_b200.h
 	@mkdir -p tests/_build
 	g++ -O2 -std=c++17 -shared -fPIC -Wall -Wno-unknown-pragmas -x c++ -Iinclude -I$(CSRC) -I/usr/local/cuda/include \
@@ -61,11 +65,16 @@ tests/_build/libeval_serial_host.so: tests/host_shim/eval_serial_host.cpp $(CSRC
 # test infrastructure: device harness over the product's own kernel objects (recovery and signal
 # passes on constructed corpora, and the exhaustive sweeps of the core headers' device build)
 DSHIM_OBJS := build/modes_recover.o build/modes_signal.o build/modes_levels.o build/modes_tables.o
-dshim: tests/_build/libkernels_device.so
+dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so
 tests/_build/libkernels_device.so: tests/device_shim/kernels_device.cu $(DSHIM_OBJS) $(CSRC)/modes_internal.h $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_levels_core.cuh include/modes_b200.h
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/kernels_device.cu -o tests/_build/kernels_device.o
 	$(NVCC) $(ARCH) -shared -o $@ tests/_build/kernels_device.o $(DSHIM_OBJS) -cudart static
+# the arrival-time measurement of the signal pass on constructed corpora (tests/test_arrival.py)
+tests/_build/libarrival_device.so: tests/device_shim/arrival_device.cu build/modes_signal.o build/modes_tables.o $(CSRC)/modes_internal.h include/modes_b200.h
+	@mkdir -p tests/_build
+	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/arrival_device.cu -o tests/_build/arrival_device.o
+	$(NVCC) $(ARCH) -shared -o $@ tests/_build/arrival_device.o build/modes_signal.o build/modes_tables.o -cudart static
 
 clean:
 	rm -rf build tests/_build $(LIB) dump1090-b200

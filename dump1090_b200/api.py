@@ -25,6 +25,7 @@ ICAO_CACHE_SLOTS = 1024                   # MODES_ICAO_CACHE_SLOTS
 STREAM_EPOCH_MS = 1_000_000_000_000      # MODES_STREAM_EPOCH_MS: start of a file's stream clock for the tracker
 
 EVAL_GATE_OK, EVAL_ERRORS, EVAL_DECODED, EVAL_P2_VALID = 1, 2, 4, 8
+EVAL_ARRIVAL_SHIFT = 4                    # flags >> 4: arrival code (0 = not measured, else offset + 8 ticks)
 
 
 class Config(C.Structure):
@@ -42,7 +43,7 @@ _MSG_B = ("ew_dir ew_velocity ns_dir ns_velocity vert_rate_source vert_rate_sign
 
 class Message(C.Structure):
     """struct modes_message == fields of struct modesMessage (dump1090.c:211-260)."""
-    _fields_ = ([("msg", C.c_uint8 * 14), ("recovered", C.c_uint8), ("pad0", C.c_uint8), ("msgbits", C.c_int32),
+    _fields_ = ([("msg", C.c_uint8 * 14), ("recovered", C.c_uint8), ("arrival", C.c_uint8), ("msgbits", C.c_int32),
                  ("msgtype", C.c_int32), ("crcok", C.c_int32), ("crc", C.c_uint32)]
                 + [(n, C.c_int32) for n in _MSG_A]
                 + [("flight", C.c_char * 9), ("pad1", C.c_char * 3)]
@@ -73,8 +74,16 @@ class Message(C.Structure):
         when it was not measured (signal measurement off, or a frame from the hex door)."""
         return None if self.signal <= 0 else 20.0 * math.log10(self.signal / 65535.0)
 
+    def timestamp_12mhz(self) -> int:
+        """The 12 MHz Beast timestamp of this message: 6 * sample_pos, moved by the measured arrival
+        offset (arrival - 8 ticks) when arrival != 0 (modes_set_arrival); clamped at 0 and taken
+        modulo 2^48 as modes_format_beast writes it."""
+        ticks = 6 * int(self.sample_pos) + (int(self.arrival) - 8 if self.arrival else 0)
+        return 0 if ticks < 0 else ticks % (1 << 48)
+
     def beast(self) -> bytes:
-        """The Beast binary frame of this message (modes_format_beast)."""
+        """The Beast binary frame of this message (modes_format_beast); its timestamp is
+        timestamp_12mhz()."""
         buf = (C.c_uint8 * 64)()
         n = lib().modes_format_beast(C.byref(self), buf, 64)
         return bytes(buf[:n])
@@ -184,7 +193,7 @@ EXPORTS = ["modes_abi_version", "modes_default_config", "modes_create", "modes_d
            "modes_resolver_run_recovered", "modes_resolver_run_shards_recovered", "modes_resolver_recovery_stats", "modes_pool_set_recovery",
            "modes_pool_recovery_stats", "modes_set_weak_preambles", "modes_get_weak_recovery_stats", "modes_weak_device",
            "modes_weak_fetch", "modes_resolver_run_weak", "modes_resolver_run_shards_weak", "modes_resolver_weak_stats",
-           "modes_pool_set_weak_preambles", "modes_pool_weak_stats"]
+           "modes_pool_set_weak_preambles", "modes_pool_weak_stats", "modes_set_arrival", "modes_pool_set_arrival"]
 
 
 def lib():
@@ -278,6 +287,8 @@ def lib():
         L.modes_pool_buffers.argtypes = [C.c_void_p, C.c_uint32]
         L.modes_set_signal.argtypes = [C.c_void_p, C.c_int]
         L.modes_pool_set_signal.argtypes = [C.c_void_p, C.c_int]
+        L.modes_set_arrival.argtypes = [C.c_void_p, C.c_int]
+        L.modes_pool_set_arrival.argtypes = [C.c_void_p, C.c_int]
         L.modes_format_beast.restype = C.c_size_t
         L.modes_format_beast.argtypes = [C.POINTER(Message), C.c_void_p, C.c_size_t]
         L.modes_set_levels.argtypes = [C.c_void_p, C.c_int]
@@ -387,16 +398,19 @@ class Decoder:
     known aircraft found by a soft-decision search on the GPU (modes_set_recovery), marked
     Message.recovered: recovery_stats().  weak_preambles=True (with recover=True) also searches the weak
     preambles the reference's preamble test rejects (modes_set_weak_preambles): Message.recovered = 2,
-    weak_recovery_stats()."""
+    weak_recovery_stats().  arrival=True measures every decoded frame's arrival time to a sixth of a
+    sample on the GPU (modes_set_arrival): Message.arrival, timestamp_12mhz(), beast()."""
 
     def __init__(self, signal: bool = False, levels: bool = False, recover: bool = False, weak_preambles: bool = False,
-                 **cfg):
+                 arrival: bool = False, **cfg):
         self.cfg = make_config(**cfg)
         self._h = lib().modes_create(C.byref(self.cfg))
         if not self._h:
             raise RuntimeError("modes_create failed: " + lib().modes_last_error(None).decode())
         if signal:
             self.set_signal(True)
+        if arrival:
+            self.set_arrival(True)
         if levels:
             self.set_levels(True)
         if recover:
@@ -483,6 +497,10 @@ class Decoder:
     def set_signal(self, on: bool) -> None:
         """Measure the signal level for batches submitted from now on (modes_set_signal)."""
         self._check(lib().modes_set_signal(self._h, int(bool(on))))
+
+    def set_arrival(self, on: bool) -> None:
+        """Measure the arrival time for batches submitted from now on (modes_set_arrival)."""
+        self._check(lib().modes_set_arrival(self._h, int(bool(on))))
 
     def set_levels(self, on: bool) -> None:
         """Measure the buffers' levels for batches submitted from now on (modes_set_levels)."""
@@ -815,10 +833,10 @@ class ReceiverPool:
     batch.  Messages are collected per receiver (`take(receiver)`).  signal=True: as for Decoder.
     levels=True: level records of every receiver's buffers (`take_levels(receiver)`).
     recover=True: as for Decoder, with statistics per receiver (`recovery_stats(receiver)`).
-    weak_preambles=True: as for Decoder (`weak_recovery_stats(receiver)`)."""
+    weak_preambles=True: as for Decoder (`weak_recovery_stats(receiver)`).  arrival=True: as for Decoder."""
 
     def __init__(self, n_receivers: int, max_batch: int = 0, signal: bool = False, levels: bool = False,
-                 recover: bool = False, weak_preambles: bool = False, **cfg):
+                 recover: bool = False, weak_preambles: bool = False, arrival: bool = False, **cfg):
         self.cfg = make_config(**cfg)
         self.n = n_receivers
         self._h = lib().modes_pool_create(C.byref(self.cfg), n_receivers, max_batch)
@@ -826,6 +844,8 @@ class ReceiverPool:
             raise RuntimeError("modes_pool_create failed")
         if signal:
             self.set_signal(True)
+        if arrival:
+            self.set_arrival(True)
         if levels:
             self.set_levels(True)
         if recover:
@@ -906,6 +926,10 @@ class ReceiverPool:
     def set_signal(self, on: bool) -> None:
         """Measure the signal level for batches submitted from now on (modes_pool_set_signal)."""
         self._check(lib().modes_pool_set_signal(self._h, int(bool(on))))
+
+    def set_arrival(self, on: bool) -> None:
+        """Measure the arrival time for batches submitted from now on (modes_pool_set_arrival)."""
+        self._check(lib().modes_pool_set_arrival(self._h, int(bool(on))))
 
     def set_levels(self, on: bool) -> None:
         """Measure the levels of batches submitted from now on (modes_pool_set_levels)."""

@@ -66,6 +66,7 @@ struct Slot {
     bool levels = false;              // the batch measures levels (the switch as it was at submit)
     bool recover = false;             // the batch runs the recovery pass (streaming: the switch as it was at submit)
     bool signal = false;              // the signal switch as it was at submit
+    bool arrival = false;             // the arrival switch as it was at submit
     bool weak = false;                // the batch runs the weak-preamble passes (streaming: both switches as they were at submit)
     uint32_t *weak_pos_ext = nullptr; modes_recovered *weak_rec_ext = nullptr; uint32_t weak_ext_cap = 0;   // modes_weak_device's buffers
     uint32_t weak_first = 0, weak_step = 1;   // the buffers the weak scan reads: weak_first + i * weak_step
@@ -115,6 +116,7 @@ struct modes_ctx {
     std::string err;
     uint64_t launches = 0;
     bool signal = false;                  // modes_set_signal: measure the signal level of decoded attempts
+    bool arrival = false;                 // modes_set_arrival: measure the arrival time of decoded attempts
     bool levels = false;                  // modes_set_levels: measure every decoded buffer's levels
     bool recover = false;                 // modes_set_recovery: soft-decision recovery of weak DF17/18 frames
     bool weak = false;                    // modes_set_weak_preambles: recovery at weak preambles too
@@ -341,6 +343,7 @@ int submit(modes_ctx *ctx, Slot &s, const uint8_t *host_iq, const void *d_iq, si
     s.weak_pos_ext = nullptr; s.weak_rec_ext = nullptr; s.weak_ext_cap = 0;
     s.weak_first = 0; s.weak_step = 1;
     s.signal = ctx->signal;
+    s.arrival = ctx->arrival;
     if (s.levels && levels_ensure(ctx, s.d_levels, s.h_levels, s.levels_cap, n_buffers, nullptr)) return -1;   // collected
     if (host_iq) {
         CK(ctx, cudaMemcpyAsync(s.d_iq, host_iq, n_samples * 2, cudaMemcpyHostToDevice, s.stream));
@@ -454,13 +457,13 @@ int launch_batch(modes_ctx *ctx, Slot &s) {
     launch_eval(in, ctx->tab, so, s.out_records, ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->sm_count, s.stream);
     if (pe) CK(ctx, cudaEventRecord(pe[2], s.stream));
     // after pe[2]: the kernel times keep their meaning; before the device resolve, which copies the field
-    if (ctx->signal) launch_signal(in, ctx->tab, so, s.out_records, ctx->sm_count, s.stream);
+    if (s.signal || s.arrival) launch_signal(in, ctx->tab, so, s.out_records, ctx->sm_count, s.stream, s.signal, s.arrival);
     // the buffers' own bytes (the body, not the carry block); one writer per record, so a repeated
     // batch writes the same records
     if (s.levels)
         launch_levels(in.body, (uint32_t)s.n_buffers, MODES_BUFFER_BYTES, ctx->tab, s.d_levels, ctx->sm_count, s.stream);
     CK(ctx, cudaGetLastError());
-    ctx->launches += (ctx->signal ? 3 : 2) + (s.levels ? 1 : 0);
+    ctx->launches += (s.signal || s.arrival ? 3 : 2) + (s.levels ? 1 : 0);
     if (s.recover && launch_recovery(ctx, s, in, so)) return -1;
     if (s.weak && launch_weak(ctx, s, in)) return -1;
     if (ctx->cfg.gpu_resolve && s.own_outputs && &s != &ctx->detect) {
@@ -658,7 +661,7 @@ int run_buffers_multi(modes_ctx *ctx, const uint8_t *host_iq, size_t n_buffers) 
             ctx->buffers_done += (int64_t)nb;
             host_iq += nb * MODES_BUFFER_BYTES;
             n_buffers -= nb;
-            ctx->launches += (g->signal ? 3 : 2) + (g->levels ? 1 : 0) + (g->recover ? 1 : 0) + (g->recover && g->weak ? 4 : 0);
+            ctx->launches += (g->signal || g->arrival ? 3 : 2) + (g->levels ? 1 : 0) + (g->recover ? 1 : 0) + (g->recover && g->weak ? 4 : 0);
         }
         ctx->group_n[cur] = k;
         if (have_prev && collect_group(ctx, cur ^ 1)) return -1;
@@ -813,6 +816,13 @@ int modes_set_signal(modes_ctx *ctx, int on) {
     if (!ctx) return -1;
     ctx->signal = on != 0;
     for (modes_ctx *g : ctx->gpus) g->signal = on != 0;
+    return 0;
+}
+
+int modes_set_arrival(modes_ctx *ctx, int on) {
+    if (!ctx) return -1;
+    ctx->arrival = on != 0;
+    for (modes_ctx *g : ctx->gpus) g->arrival = on != 0;
     return 0;
 }
 

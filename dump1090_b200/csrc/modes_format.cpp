@@ -169,13 +169,15 @@ extern "C" size_t modes_format_raw_net(const modes_message *mm, char *buf, size_
 
 // The Beast binary frame of the dump1090 descendants (their port 30005), Mode S frames only:
 // 0x1a, type '2' (7 bytes) or '3' (14 bytes), 48-bit 12 MHz timestamp, signal byte, frame; every
-// 0x1a after the leading one is doubled.  At 2 MHz one sample is 6 ticks of the 12 MHz clock.
+// 0x1a after the leading one is doubled.  At 2 MHz one sample is 6 ticks of the 12 MHz clock; a
+// measured arrival (modes_set_arrival) moves the timestamp by -7 .. +7 ticks.
 extern "C" size_t modes_format_beast(const modes_message *mm, uint8_t *buf, size_t capacity) {
     const int nbytes = mm->msgbits == 112 ? 14 : 7;
     uint8_t body[2 + 6 + 1 + 14];
     size_t k = 0;
     body[k++] = nbytes == 14 ? '3' : '2';
-    const uint64_t ts = mm->sample_pos < 0 ? 0 : ((uint64_t)mm->sample_pos * 6u) & ((1ull << 48) - 1);
+    const __int128 ticks = (__int128)mm->sample_pos * 6 + (mm->arrival ? (int)mm->arrival - 8 : 0);
+    const uint64_t ts = ticks < 0 ? 0 : (uint64_t)ticks & ((1ull << 48) - 1);
     for (int i = 5; i >= 0; i--) body[k++] = (uint8_t)(ts >> (8 * i));
     const int64_t s = mm->signal < 0 ? 0 : mm->signal;
     const int64_t level = (s * 255 + 32767) / 65535;

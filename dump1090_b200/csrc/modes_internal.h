@@ -72,10 +72,11 @@ void launch_magnitude(const uint8_t *d_iq, uint16_t *d_mag, uint64_t n_samples, 
 // CRC / fix on raw frame bytes (hex door): n frames of 14 bytes -> n modes_frame_eval.
 void launch_eval_frames(const uint8_t *d_frames, modes_frame_eval *d_out, uint32_t n, const DeviceTables &tab,
                         int fix_errors, int aggressive, cudaStream_t stream);
-// Signal level of every decoded attempt (modes_signal.cu): writes pass[k].signal of the first
-// min(counters[0], cand_capacity) records over the same windows the scan and frame evaluation read.
+// Signal level and arrival code of every decoded attempt (modes_signal.cu): writes pass[k].signal
+// (signal) and bits 4-7 of pass[k].flags (arrival) of the first min(counters[0], cand_capacity)
+// records over the same windows the scan and frame evaluation read.  Launches nothing when both are off.
 void launch_signal(const BatchView &in, const DeviceTables &tab, const ScanOutputs &scan, modes_candidate *records,
-                   int sm_count, cudaStream_t stream);
+                   int sm_count, cudaStream_t stream, bool signal = true, bool arrival = false);
 // Levels of n_buffers whole buffers at d_iq + k * stride_bytes (modes_levels.cu): writes out[k],
 // k < n_buffers, with buffer = k and n_samples = kBufSamples.
 void launch_levels(const uint8_t *d_iq, uint32_t n_buffers, uint64_t stride_bytes, const DeviceTables &tab,
@@ -114,7 +115,8 @@ void launch_recover_weak(const BatchView &in, const DeviceTables &tab, const uin
 int weak_device_strided(modes_ctx *ctx, void *d_pos, void *d_rec, size_t capacity, uint32_t first_buffer, uint32_t buffer_step);
 static_assert(sizeof(modes_recovered) == 20 && offsetof(modes_recovered, status) == 14 && offsetof(modes_recovered, signal) == 16,
               "recovery record layout");
-static_assert(offsetof(modes_message, recovered) == 14 && offsetof(modes_message, msgbits) == 16, "message layout");
+static_assert(offsetof(modes_message, recovered) == 14 && offsetof(modes_message, arrival) == 15 &&
+              offsetof(modes_message, msgbits) == 16, "message layout");
 
 // The record layouts are ABI: the signal field took the two bytes every evaluation kernel already wrote as zero.
 static_assert(sizeof(modes_frame_eval) == 24 && offsetof(modes_frame_eval, signal) == 18 && offsetof(modes_frame_eval, crc) == 20,

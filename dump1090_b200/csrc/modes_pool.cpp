@@ -106,6 +106,7 @@ struct modes_pool {
     std::vector<Receiver> rx;
     size_t max_batch = 0;
     int signal = 0;                            // modes_pool_set_signal, applied to the slot contexts
+    int arrival = 0;                           // modes_pool_set_arrival, the same
     int levels = 0;                            // modes_pool_set_levels
     int recover = 0;                           // modes_pool_set_recovery
     int weak = 0;                              // modes_pool_set_weak_preambles
@@ -188,6 +189,7 @@ int ensure_device(modes_pool *p) {
         sl.ctx = modes_create(&c);
         if (!sl.ctx) return fail(p, "%s", modes_last_error(nullptr));
         modes_set_signal(sl.ctx, p->signal);
+        modes_set_arrival(sl.ctx, p->arrival);
         sl.d_batch = static_cast<uint8_t *>(modes_device_alloc(bytes));
         sl.h_carry = static_cast<uint8_t *>(modes_host_alloc(p->max_batch * MODES_CARRY_BYTES));
         if (!sl.d_batch || !sl.h_carry) return fail(p, "out of memory for %zu receivers per batch", p->max_batch);
@@ -477,6 +479,14 @@ int modes_pool_set_output(modes_pool *p, modes_message *out, uint32_t *receiver_
 }
 
 size_t modes_pool_output_count(const modes_pool *p) { return p ? p->out_count : 0; }
+
+int modes_pool_set_arrival(modes_pool *p, int on) {
+    if (!p) return -1;
+    p->arrival = on != 0;
+    for (modes_pool::Slot &sl : p->slot)
+        if (sl.ctx) modes_set_arrival(sl.ctx, p->arrival);
+    return 0;
+}
 
 int modes_pool_set_signal(modes_pool *p, int on) {
     if (!p) return -1;

@@ -174,6 +174,7 @@ static void build_message(const modes_frame_eval &p, int crcok, uint32_t iid, ui
     o->crc = p.crc;
     o->nfixed = p.nfixed;
     o->signal = p.signal;
+    o->arrival = (uint8_t)(p.flags >> MODES_EVAL_ARRIVAL_SHIFT);
     o->errorbit = p.nfixed ? (int)p.errorbit : -1;
     o->crcok = crcok;
     o->iid = (int32_t)iid;

@@ -14,6 +14,8 @@
  * --beast writes one Beast binary frame per message instead (what the dump1090 descendants send on
  * port 30005: 12 MHz timestamp = 6 x sample position, signal level measured on the GPU); it excludes
  * --raw, --onlyaddr, --sbs and --aircraft-json, which write to stdout as well.
+ * --arrival refines the Beast timestamps to a sixth of a sample with the arrival time measured on the
+ * GPU (modes_set_arrival); it needs --beast, the only output mode that prints a time.
  * --levels measures every decoded buffer's noise, peak and clipping on the GPU and prints one
  * summary line on stderr at the end (buffers, samples, noise floor and peak in dBFS on the scale of
  * the Beast signal level, clipped samples and their fraction); it combines with every output mode
@@ -34,7 +36,7 @@
 #include "modes_b200.h"
 
 static int opt_raw = 0, opt_onlyaddr = 0, opt_stats = 0, opt_check_crc = 1, opt_sbs = 0, opt_json = 0, opt_beast = 0;
-static int opt_levels = 0, opt_recover = 0, opt_weak = 0;
+static int opt_levels = 0, opt_recover = 0, opt_weak = 0, opt_arrival = 0;
 static modes_tracker *tracker = NULL;
 
 /* --levels: totals over the records taken so far */
@@ -117,6 +119,7 @@ int main(int argc, char **argv) {
         else if (!strcmp(argv[j], "--sbs")) opt_sbs = 1;
         else if (!strcmp(argv[j], "--aircraft-json")) opt_json = 1;
         else if (!strcmp(argv[j], "--beast")) opt_beast = 1;
+        else if (!strcmp(argv[j], "--arrival")) opt_arrival = 1;
         else if (!strcmp(argv[j], "--levels")) opt_levels = 1;
         else if (!strcmp(argv[j], "--recover")) opt_recover = 1;
         else if (!strcmp(argv[j], "--recover-weak")) opt_recover = opt_weak = 1;
@@ -134,6 +137,10 @@ int main(int argc, char **argv) {
         fprintf(stderr, "--beast writes binary frames to stdout: it cannot be combined with --raw, --onlyaddr, --sbs or --aircraft-json\n");
         return 1;
     }
+    if (opt_arrival && !opt_beast) {
+        fprintf(stderr, "--arrival refines the timestamps of --beast, the only output mode that prints a time: it needs --beast\n");
+        return 1;
+    }
     if (opt_recover && cfg.gpu_resolve) {
         if (opt_weak) fprintf(stderr, "--recover-weak implies --recover: ");
         fprintf(stderr, "--recover cannot be combined with --gpu-resolve: the device resolve has no recovery rule\n");
@@ -149,6 +156,7 @@ int main(int argc, char **argv) {
         if (!tracker) { fprintf(stderr, "out of memory\n"); return 1; }
     }
     if (opt_beast) modes_set_signal(ctx, 1);
+    if (opt_arrival) modes_set_arrival(ctx, 1);
     if (opt_levels) modes_set_levels(ctx, 1);
     if (opt_recover && modes_set_recovery(ctx, 1)) { fprintf(stderr, "--recover: %s\n", modes_last_error(ctx)); return 1; }
     if (opt_weak && modes_set_weak_preambles(ctx, 1)) { fprintf(stderr, "--recover-weak: %s\n", modes_last_error(ctx)); return 1; }

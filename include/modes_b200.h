@@ -80,7 +80,8 @@ typedef struct modes_message {
     uint8_t  msg[14];
     uint8_t  recovered;         /* 1: delivered by the soft-decision recovery (modes_set_recovery), not by the reference;
                                    2: the same at a weak preamble (modes_set_weak_preambles) */
-    uint8_t  pad0;
+    uint8_t  arrival;           /* MODES_EVAL_ARRIVAL code of the delivered attempt (modes_set_arrival): 0 = not measured,
+                                   otherwise the arrival is (arrival - 8) 12 MHz ticks after 6 * sample_pos */
     int32_t  msgbits, msgtype, crcok;
     uint32_t crc;
     int32_t  errorbit, aa1, aa2, aa3, phase_corrected;
@@ -105,7 +106,7 @@ typedef struct modes_message {
 typedef struct modes_frame_eval {
     uint8_t  msg[14];           /* frame bytes, after the CRC fix if one was applied */
     uint8_t  msgtype;           /* DF of the demodulated frame (before any fix) */
-    uint8_t  flags;             /* MODES_EVAL_* */
+    uint8_t  flags;             /* MODES_EVAL_* in bits 0-3; bits 4-7: the arrival code (MODES_EVAL_ARRIVAL_*) */
     uint8_t  errorbit;          /* first repaired bit, 0xFF = none */
     uint8_t  nfixed;
     uint16_t signal;            /* with modes_set_signal on and MODES_EVAL_DECODED set: floor(sqrt(floor(S / b))),
@@ -119,6 +120,8 @@ typedef struct modes_frame_eval {
 #define MODES_EVAL_ERRORS    2  /* demodulation error in first 56 bits dump1090.c:1682 */
 #define MODES_EVAL_DECODED   4  /* decodeModesMessage reached          dump1090.c:1731 */
 #define MODES_EVAL_P2_VALID  8  /* pass[1] (phase-corrected retry) was evaluated */
+#define MODES_EVAL_ARRIVAL_SHIFT 4      /* flags >> 4: arrival code, modes_set_arrival; 0 with the switch off */
+#define MODES_EVAL_ARRIVAL_MASK  0xF0
 
 /* One preamble candidate: a position that passes the tests of
  * dump1090.c:1602-1650, with the first attempt and the phase-corrected retry
@@ -403,12 +406,41 @@ int64_t modes_pool_buffers(const modes_pool *p, uint32_t receiver);   /* buffers
 int    modes_set_signal(modes_ctx *ctx, int on);
 int    modes_pool_set_signal(modes_pool *p, int on);
 /* One Beast frame for a message: 0x1a, '2' (7-byte frame) or '3' (14-byte frame), a 6-byte big-endian
- * 12 MHz timestamp = (6 * sample_pos) mod 2^48 (0 when sample_pos < 0), one signal byte
+ * 12 MHz timestamp = (6 * sample_pos) mod 2^48 (0 when sample_pos < 0) when arrival = 0, and
+ * max(6 * sample_pos + arrival - 8, 0) mod 2^48 otherwise (modes_set_arrival), one signal byte
  * = min(255, (signal * 255 + 32767) / 65535), then the frame bytes; every 0x1a after the leading one
  * is doubled.  sample_pos counts the samples of one stream (of one receiver in a pool), so each
  * stream's clock is its own.  Returns the length the frame needs (at most 44); writes at most
  * capacity bytes and no terminating NUL.  Pure host code. */
 size_t modes_format_beast(const modes_message *mm, uint8_t *buf, size_t capacity);
+
+/* ---- arrival time to a sixth of a sample (multilateration-grade Beast timestamps) -------------
+ * The Beast timestamp of a frame is 6 * sample_pos 12 MHz ticks: the preamble's sample, 500 ns coarse.
+ * A pulse that starts d samples after a sample boundary puts about (1 - d) of its amplitude into that
+ * sample and d into the next one, so the decoded frame's samples tell d.  For a decoded attempt
+ * (MODES_EVAL_DECODED) of b bits (56 or 112, from msgtype) at buffer position j, with its frame bits
+ * = its msg after any CRC fix and m = the reference's uncorrected magnitudes (dump1090.c:359-364):
+ *   1. e = the nominal pulse pattern over the samples j .. j+17+2b: preamble pulses at 0, 2, 7 and 9;
+ *      bit i puts a pulse at 16+2i when it is 1 and at 17+2i when it is 0; every other sample is empty.
+ *   2. Every sample s in j+1 .. j+16+2b is classified by (e[s-1], e[s], e[s+1]):
+ *        main (0,1,0), late (1,0,0), early (0,0,1), quiet (0,0,0); any other sample is not used.
+ *      Every class is non-empty (the preamble alone has 3 main, 2 late, 1 early, 6 quiet samples).
+ *   3. With mu = mean of m over quiet:  A = mean(main) - mu,  L = max(mean(late) - mu, 0),
+ *      E = max(mean(early) - mu, 0).
+ *   4. offset = round(6 (L - E) / (A + L + E)) ticks, halves rounded away from zero, clamped to
+ *      [-7, 7]; the frame is not measured when A + L + E <= 0.  It is computed exactly in 64-bit
+ *      integers from the class sums and counts (csrc/modes_arrival_core.cuh).
+ * The code is 0 (not measured) or offset + 8 (1..15) and sits in bits 4-7 of modes_frame_eval.flags;
+ * delivered messages carry it in modes_message.arrival.  The arrival of the frame is then
+ * 6 * sample_pos + offset ticks.  Recovered messages (modes_message.recovered != 0) and frames from the
+ * hex door are not measured (arrival = 0) and keep the coarse timestamp.
+ *
+ * Arrival measurement is off by default.  When it is on, every batch submitted afterwards runs the
+ * signal pass's kernel (one more launch per batch when signal measurement is off, none more when it is
+ * on).  On an n_gpus > 1 context the setting reaches every GPU; a pool applies it to all its device
+ * contexts.  Returns 0, or -1 for a NULL handle. */
+int    modes_set_arrival(modes_ctx *ctx, int on);
+int    modes_pool_set_arrival(modes_pool *p, int on);
 
 /* ---- receiver levels: noise floor, peak and clipping per buffer --------------------------------
  * What an operator reads of a receiver besides its messages: how loud the channel is, how close the
