@@ -21,53 +21,100 @@ namespace {
 
 thread_local std::string g_create_error;
 
+// An owning, grow-only array of T in device memory (DevBuf) or pinned host memory (PinnedBuf).
+// ensure(n) replaces the array with one of exactly n elements when n exceeds its capacity, without
+// keeping the contents; the caller chooses n, so each growth policy stays where the array is used.
+template <typename T, bool Pinned>
+class CudaBuf {
+public:
+    CudaBuf() = default;
+    CudaBuf(CudaBuf &&o) noexcept : p_(o.p_), cap_(o.cap_) { o.p_ = nullptr; o.cap_ = 0; }
+    CudaBuf &operator=(CudaBuf &&o) noexcept {
+        if (this != &o) { release(); p_ = o.p_; cap_ = o.cap_; o.p_ = nullptr; o.cap_ = 0; }
+        return *this;
+    }
+    ~CudaBuf() { release(); }
+    cudaError_t ensure(size_t n) {
+        if (n <= cap_) return cudaSuccess;
+        release();
+        void *p = nullptr;
+        const cudaError_t e = Pinned ? cudaMallocHost(&p, n * sizeof(T)) : cudaMalloc(&p, n * sizeof(T));
+        if (e != cudaSuccess) return e;
+        p_ = static_cast<T *>(p);
+        cap_ = n;
+        return cudaSuccess;
+    }
+    T *get() const { return p_; }
+    T &operator[](size_t i) const { return p_[i]; }
+    size_t capacity() const { return cap_; }
+private:
+    void release() {
+        if (p_) { if (Pinned) cudaFreeHost(p_); else cudaFree(p_); }
+        p_ = nullptr;
+        cap_ = 0;
+    }
+    T *p_ = nullptr;
+    size_t cap_ = 0;
+};
+template <typename T> using DevBuf = CudaBuf<T, false>;
+template <typename T> using PinnedBuf = CudaBuf<T, true>;
+
+// Pinned room for a host copy of n records, with half as much again to spare so that slowly rising
+// counts do not reallocate every batch.
+template <typename T>
+cudaError_t ensure_spare(PinnedBuf<T> &b, size_t n) { return b.capacity() >= n ? cudaSuccess : b.ensure(n + n / 2 + 1024); }
+
 struct Slot {
     cudaStream_t stream = nullptr;
-    uint8_t *d_iq = nullptr;         size_t iq_bytes = 0;
-    uint8_t *d_halo = nullptr;
-    uint32_t *d_cand_v = nullptr;    uint32_t cand_cap = 0;
-    modes_candidate *d_records = nullptr;
-    modes_tile *d_tiles = nullptr;   uint32_t tiles_cap = 0;
-    uint32_t *d_counters = nullptr;
+    DevBuf<uint8_t> d_iq;
+    DevBuf<uint8_t> d_halo;
+    DevBuf<uint32_t> d_cand_v;       // its capacity is the slot's candidate capacity
+    DevBuf<modes_candidate> d_records;
+    DevBuf<modes_tile> d_tiles;
+    DevBuf<uint32_t> d_counters;
     // pinned carry blocks: a ring, because modes_detect_device/_host return without waiting and the
     // next call must not rewrite a block whose host-to-device copy is still queued
     static constexpr int kHaloRing = 8;
-    uint8_t *h_halo = nullptr;       // kHaloRing x kHaloAlloc
+    PinnedBuf<uint8_t> h_halo;       // kHaloRing x kHaloAlloc
     cudaEvent_t halo_ev[kHaloRing] = {};
     unsigned halo_next = 0;
-    uint32_t *h_counters = nullptr;  // pinned
-    modes_candidate *h_records = nullptr; size_t h_records_cap = 0;   // pinned
-    modes_tile *h_tiles = nullptr;   size_t h_tiles_cap = 0;          // pinned
+    PinnedBuf<uint32_t> h_counters;
+    PinnedBuf<modes_candidate> h_records;
+    PinnedBuf<modes_tile> h_tiles;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-    // cfg.gpu_resolve: workspace of the device resolve, sized for gr_buffers buffers / gr.capacity deliveries
-    GpuResolve gr{};
-    size_t gr_buffers = 0;
-    uint32_t *h_gr_flags = nullptr;       // pinned: flags[3] + pad, then stats[8] as u64, then the end cache [1024]
-    modes_delivery *h_deliveries = nullptr; size_t h_deliveries_cap = 0;   // pinned
+    // cfg.gpu_resolve: workspace of the device resolve (the storage behind a GpuResolve view)
+    DevBuf<uint32_t> gr_start, gr_end, gr_written, gr_readfirst, gr_rerun, gr_n_deliv, gr_offsets, gr_flags;
+    DevBuf<uint64_t> gr_stats;
+    DevBuf<modes_delivery> gr_out;
+    PinnedBuf<uint32_t> h_gr_flags;  // flags[3] + pad, then stats[8] as u64, then the end cache [1024]
+    PinnedBuf<modes_delivery> h_deliveries;
     // modes_set_levels: one record per buffer of the batch (device, and its pinned host copy)
-    modes_level *d_levels = nullptr, *h_levels = nullptr; size_t levels_cap = 0;
+    DevBuf<modes_level> d_levels;
+    PinnedBuf<modes_level> h_levels;
     // modes_set_recovery / modes_recover_device: one record per candidate (device, and its pinned host copy)
-    modes_recovered *d_recovered = nullptr; size_t rec_cap = 0;
-    modes_recovered *h_recovered = nullptr; size_t h_rec_cap = 0;
-    // modes_set_weak_preambles / modes_weak_device: the weak positions and their records (device, own
-    // capacity weak_cap), the scan's scratch list, its per-tile words (source, count and destination of
-    // every tile's block) and counters, and pinned host copies
-    uint32_t *d_weak_pos = nullptr; modes_recovered *d_weak_rec = nullptr; uint32_t weak_cap = 0, want_weak_cap = 0;
-    uint32_t *d_weak_scratch = nullptr;   // weak_cap entries: the scan's unordered list
-    uint32_t *d_weak_tiles = nullptr; uint32_t weak_tiles_cap = 0;
-    uint32_t *d_weak_counters = nullptr, *h_weak_counters = nullptr;
-    uint32_t *h_weak_pos = nullptr; modes_recovered *h_weak_rec = nullptr; size_t h_weak_cap = 0;
+    DevBuf<modes_recovered> d_recovered;
+    PinnedBuf<modes_recovered> h_recovered;
+    // modes_set_weak_preambles / modes_weak_device: the weak positions and their records (device), the
+    // scan's unordered scratch list (its capacity is the slot's weak capacity), its per-tile words
+    // (source, count and destination of every tile's block) and counters, and pinned host copies
+    DevBuf<uint32_t> d_weak_pos;
+    DevBuf<modes_recovered> d_weak_rec;
+    DevBuf<uint32_t> d_weak_scratch;
+    uint32_t want_weak_cap = 0;
+    DevBuf<uint32_t> d_weak_tiles;
+    DevBuf<uint32_t> d_weak_counters;
+    PinnedBuf<uint32_t> h_weak_counters;
+    PinnedBuf<uint32_t> h_weak_pos;
+    PinnedBuf<modes_recovered> h_weak_rec;
     // in-flight batch
     bool busy = false;
     size_t n_buffers = 0;
     int64_t buffer_base = 0;
     const void *batch_iq = nullptr;   // device address the batch was scanned from
     bool own_outputs = true;          // results in this slot's own buffers (growable)
-    bool levels = false;              // the batch measures levels (the switch as it was at submit)
-    bool recover = false;             // the batch runs the recovery pass (streaming: the switch as it was at submit)
-    bool signal = false;              // the signal switch as it was at submit
-    bool arrival = false;             // the arrival switch as it was at submit
-    bool weak = false;                // the batch runs the weak-preamble passes (streaming: both switches as they were at submit)
+    // the batch's passes: the switches as they were at submit (the stage level adds recovery and weak
+    // preambles with modes_recover_device / modes_weak_device)
+    Features feat;
     uint32_t *weak_pos_ext = nullptr; modes_recovered *weak_rec_ext = nullptr; uint32_t weak_ext_cap = 0;   // modes_weak_device's buffers
     uint32_t weak_first = 0, weak_step = 1;   // the buffers the weak scan reads: weak_first + i * weak_step
     modes_recovered *rec_ext = nullptr; uint32_t rec_ext_cap = 0;   // modes_recover_device's d_out (nullptr: own buffer)
@@ -76,6 +123,8 @@ struct Slot {
     modes_candidate *out_records = nullptr;
     modes_tile *out_tiles = nullptr;
     uint32_t out_cap = 0;
+    uint32_t cand_cap() const { return (uint32_t)d_cand_v.capacity(); }
+    uint32_t weak_cap() const { return (uint32_t)d_weak_scratch.capacity(); }
 };
 
 }  // namespace
@@ -83,28 +132,27 @@ struct Slot {
 struct modes_ctx {
     modes_config cfg;
     int sm_count = 132;
-    uint16_t *d_lutn = nullptr;
-    uint16_t *d_lut_iq = nullptr;
-    uint32_t *d_bit_syn = nullptr;
-    uint32_t *d_fix_hash = nullptr;
-    uint32_t *d_pair_hash = nullptr;
+    DevBuf<uint16_t> d_lutn, d_lut_iq;
+    DevBuf<uint32_t> d_bit_syn, d_fix_hash, d_pair_hash;
     DeviceTables tab{};
     Slot slot[2];
     Slot detect;                      // stage-level API workspace
     // cfg.n_gpus > 1: this context is the front of a multi-GPU decode and owns one single-GPU
     // context per device; it keeps the stream state, the resolve state and the outputs itself
     // cfg.gpu_resolve: the address cache lives on the device, handed from batch to batch
-    uint32_t *d_cache[2] = {nullptr, nullptr};
+    DevBuf<uint32_t> d_cache[2];
     int cache_cur = 0;
     cudaEvent_t ev_resolved = nullptr;    // the last batch's device resolve has finished (its cache_out is valid)
     bool resolved_pending = false;
     // hex door staging (modes_decode_frames)
-    uint8_t *d_frames = nullptr; modes_frame_eval *d_frame_evals = nullptr, *h_frame_evals = nullptr; size_t frames_cap = 0;
+    DevBuf<uint8_t> d_frames;
+    DevBuf<modes_frame_eval> d_frame_evals;
+    PinnedBuf<modes_frame_eval> h_frame_evals;
     std::vector<modes_ctx *> gpus;
     size_t group_n[2] = {0, 0};       // batches in flight per slot parity
     uint64_t last_detect_count = 0;
     // stream state
-    uint8_t *pending = nullptr;       // pinned, one reference buffer
+    PinnedBuf<uint8_t> pending;       // one reference buffer
     size_t pending_len = 0;
     uint8_t carry[MODES_CARRY_BYTES];
     int64_t buffers_done = 0;
@@ -114,18 +162,17 @@ struct modes_ctx {
     MessageOut out;                       // modes_set_sink / modes_set_output
     cudaStream_t own_detect_stream = nullptr;
     std::string err;
-    uint64_t launches = 0;
-    bool signal = false;                  // modes_set_signal: measure the signal level of decoded attempts
-    bool arrival = false;                 // modes_set_arrival: measure the arrival time of decoded attempts
-    bool levels = false;                  // modes_set_levels: measure every decoded buffer's levels
-    bool recover = false;                 // modes_set_recovery: soft-decision recovery of weak DF17/18 frames
-    bool weak = false;                    // modes_set_weak_preambles: recovery at weak preambles too
-    std::vector<modes_level> level_q;     // records not taken yet, oldest from level_head on
-    size_t level_head = 0;
+    uint64_t launches = 0;                // this context's own; a multi-GPU front adds its GPUs' (modes_launch_count)
+    // signal, arrival: measured on decoded attempts; levels: of every decoded buffer; recover:
+    // soft-decision recovery of weak DF17/18 frames; weak: recovery at weak preambles too
+    Features feat;
+    LevelQueue level_q;
     int64_t eof_buffer = -1;              // modes_finish: stream index of the EOF buffer and its real samples
     uint32_t eof_samples = 0;
     // modes_levels_device: the records of the last call (device, pinned host copy)
-    modes_level *d_lv = nullptr, *h_lv = nullptr; size_t lv_cap = 0, lv_n = 0;
+    DevBuf<modes_level> d_lv;
+    PinnedBuf<modes_level> h_lv;
+    size_t lv_n = 0;
     bool lv_fetched = true;               // no copy of them is pending
     // cfg.profile: ring of CUDA-event triplets, one per batch, recorded on the launching stream
     static constexpr int kProfRing = 512;
@@ -196,135 +243,62 @@ uint32_t default_cand_capacity(uint64_t n_samples) {
 
 int slot_init(modes_ctx *ctx, Slot &s) {
     CK(ctx, cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
-    CK(ctx, cudaMalloc(&s.d_halo, kHaloAlloc));
-    CK(ctx, cudaMalloc(&s.d_counters, 4 * sizeof(uint32_t)));
-    CK(ctx, cudaMallocHost(&s.h_halo, (size_t)kHaloAlloc * Slot::kHaloRing));
+    CK(ctx, s.d_halo.ensure(kHaloAlloc));
+    CK(ctx, s.d_counters.ensure(4));
+    CK(ctx, s.h_halo.ensure((size_t)kHaloAlloc * Slot::kHaloRing));
     for (auto &e : s.halo_ev) CK(ctx, cudaEventCreateWithFlags(&e, event_flags(false)));
-    CK(ctx, cudaMallocHost(&s.h_counters, 4 * sizeof(uint32_t)));
+    CK(ctx, s.h_counters.ensure(4));
     for (auto &e : s.ev) CK(ctx, cudaEventCreateWithFlags(&e, event_flags(true)));
     return 0;
 }
 
 void slot_free(Slot &s) {
     if (s.stream) wait_stream(s.stream);
-    cudaFree(s.d_iq); cudaFree(s.d_halo); cudaFree(s.d_cand_v); cudaFree(s.d_records);
-    cudaFree(s.d_tiles); cudaFree(s.d_counters);
-    cudaFreeHost(s.h_halo); cudaFreeHost(s.h_counters); cudaFreeHost(s.h_records); cudaFreeHost(s.h_tiles);
-    cudaFree(s.gr.start); cudaFree(s.gr.end); cudaFree(s.gr.written); cudaFree(s.gr.readfirst); cudaFree(s.gr.rerun);
-    cudaFree(s.gr.n_deliv); cudaFree(s.gr.offsets); cudaFree(s.gr.flags); cudaFree(s.gr.stats_out); cudaFree(s.gr.out);
-    cudaFreeHost(s.h_gr_flags); cudaFreeHost(s.h_deliveries);
-    cudaFree(s.d_levels); cudaFreeHost(s.h_levels);
-    cudaFree(s.d_recovered); cudaFreeHost(s.h_recovered);
-    cudaFree(s.d_weak_pos); cudaFree(s.d_weak_rec); cudaFree(s.d_weak_scratch); cudaFree(s.d_weak_tiles); cudaFree(s.d_weak_counters);
-    cudaFreeHost(s.h_weak_counters); cudaFreeHost(s.h_weak_pos); cudaFreeHost(s.h_weak_rec);
     for (auto &e : s.ev) if (e) cudaEventDestroy(e);
     for (auto &e : s.halo_ev) if (e) cudaEventDestroy(e);
     if (s.stream) cudaStreamDestroy(s.stream);
-    s = Slot();
+    s = Slot();                       // releases its buffers: nothing queued uses them any more
 }
 
 // Make sure the slot can hold a batch of n_samples (device staging only if need_iq).
 int slot_ensure(modes_ctx *ctx, Slot &s, uint64_t n_samples, bool need_iq, bool need_records) {
-    if (need_iq && s.iq_bytes < n_samples * 2) {
-        cudaFree(s.d_iq); s.d_iq = nullptr; s.iq_bytes = 0;
-        CK(ctx, cudaMalloc(&s.d_iq, n_samples * 2));
-        s.iq_bytes = n_samples * 2;
-    }
+    if (need_iq) CK(ctx, s.d_iq.ensure(n_samples * 2));
     uint32_t cap = default_cand_capacity(n_samples);
     if (cap < s.want_cap) cap = s.want_cap;
-    if (s.cand_cap < cap) {
-        cudaFree(s.d_cand_v); s.d_cand_v = nullptr;
-        cudaFree(s.d_records); s.d_records = nullptr;
-        s.cand_cap = 0;
-        CK(ctx, cudaMalloc(&s.d_cand_v, (size_t)cap * sizeof(uint32_t)));
-        s.cand_cap = cap;
-    }
-    if (need_records && !s.d_records) CK(ctx, cudaMalloc(&s.d_records, (size_t)s.cand_cap * sizeof(modes_candidate)));
-    uint32_t nt = tiles_for(n_samples);
-    if (s.tiles_cap < nt) {
-        cudaFree(s.d_tiles); s.d_tiles = nullptr;
-        CK(ctx, cudaMalloc(&s.d_tiles, (size_t)nt * sizeof(modes_tile)));
-        s.tiles_cap = nt;
-    }
-    return 0;
-}
-
-// Pinned room for the recovery records of n candidates.
-int recovered_ensure(modes_ctx *ctx, Slot &s, size_t n) {
-    if (s.h_rec_cap >= n) return 0;
-    cudaFreeHost(s.h_recovered); s.h_recovered = nullptr; s.h_rec_cap = 0;
-    const size_t cap = n + n / 2 + 1024;
-    CK(ctx, cudaMallocHost(&s.h_recovered, cap * sizeof(modes_recovered)));
-    s.h_rec_cap = cap;
-    return 0;
-}
-
-int host_ensure(modes_ctx *ctx, Slot &s, size_t n_records, size_t n_tiles) {
-    if (s.h_records_cap < n_records) {
-        cudaFreeHost(s.h_records); s.h_records = nullptr; s.h_records_cap = 0;
-        size_t cap = n_records + n_records / 2 + 1024;
-        CK(ctx, cudaMallocHost(&s.h_records, cap * sizeof(modes_candidate)));
-        s.h_records_cap = cap;
-    }
-    if (s.h_tiles_cap < n_tiles) {
-        cudaFreeHost(s.h_tiles); s.h_tiles = nullptr; s.h_tiles_cap = 0;
-        CK(ctx, cudaMallocHost(&s.h_tiles, n_tiles * sizeof(modes_tile)));
-        s.h_tiles_cap = n_tiles;
-    }
+    CK(ctx, s.d_cand_v.ensure(cap));
+    if (need_records) CK(ctx, s.d_records.ensure(s.cand_cap()));
+    CK(ctx, s.d_tiles.ensure(tiles_for(n_samples)));
     return 0;
 }
 
 int launch_batch(modes_ctx *ctx, Slot &s);
 
-// Room for n level records in device memory and in pinned host memory.  `queued`: a stream whose
-// copy into the old host block may still be pending, waited for before the block is replaced.
-int levels_ensure(modes_ctx *ctx, modes_level *&d, modes_level *&h, size_t &cap, size_t n, cudaStream_t queued) {
-    if (cap >= n) return 0;
-    if (queued) CK(ctx, wait_stream(queued));
-    cudaFree(d); cudaFreeHost(h);
-    d = h = nullptr; cap = 0;
-    CK(ctx, cudaMalloc(&d, n * sizeof(modes_level)));
-    CK(ctx, cudaMallocHost(&h, n * sizeof(modes_level)));
-    cap = n;
-    return 0;
-}
-
 // Queue the level records of the slot's finished batch, re-based to stream buffer indices.
 void append_levels(modes_ctx *ctx, const Slot &s) {
-    if (!s.levels) return;
+    if (!s.feat.levels) return;
     for (size_t k = 0; k < s.n_buffers; k++) {
         modes_level r = s.h_levels[k];
         r.buffer = s.buffer_base + (int64_t)k;
         if (r.buffer == ctx->eof_buffer) r.n_samples = ctx->eof_samples;
-        ctx->level_q.push_back(r);
+        ctx->level_q.push(r);
     }
 }
 
-// Workspace of the device resolve for the slot's current batch.
-int gpu_resolve_ensure(modes_ctx *ctx, Slot &s) {
+// The device resolve's view of the slot's workspace, grown for its current batch.
+int gpu_resolve_ensure(modes_ctx *ctx, Slot &s, GpuResolve &g) {
     const size_t nb = s.n_buffers;
-    if (s.gr_buffers < nb) {
-        cudaFree(s.gr.start); cudaFree(s.gr.end); cudaFree(s.gr.written); cudaFree(s.gr.readfirst); cudaFree(s.gr.rerun);
-        cudaFree(s.gr.n_deliv); cudaFree(s.gr.offsets);
-        s.gr.start = s.gr.end = s.gr.written = s.gr.readfirst = s.gr.rerun = s.gr.n_deliv = s.gr.offsets = nullptr;
-        s.gr_buffers = 0;
-        CK(ctx, cudaMalloc(&s.gr.start, nb * 4096)); CK(ctx, cudaMalloc(&s.gr.end, nb * 4096));
-        CK(ctx, cudaMalloc(&s.gr.written, nb * 128)); CK(ctx, cudaMalloc(&s.gr.readfirst, nb * 128));
-        CK(ctx, cudaMalloc(&s.gr.rerun, nb * 4)); CK(ctx, cudaMalloc(&s.gr.n_deliv, nb * 4)); CK(ctx, cudaMalloc(&s.gr.offsets, (nb + 1) * 4));
-        s.gr_buffers = nb;
-    }
-    if (!s.gr.flags) {
-        CK(ctx, cudaMalloc(&s.gr.flags, 4 * sizeof(uint32_t)));
-        CK(ctx, cudaMalloc(&s.gr.stats_out, 8 * sizeof(uint64_t)));
-        CK(ctx, cudaMallocHost(&s.h_gr_flags, (20 + 1024) * sizeof(uint32_t)));
-    }
+    CK(ctx, s.gr_start.ensure(nb * 1024)); CK(ctx, s.gr_end.ensure(nb * 1024));
+    CK(ctx, s.gr_written.ensure(nb * 32)); CK(ctx, s.gr_readfirst.ensure(nb * 32));
+    CK(ctx, s.gr_rerun.ensure(nb)); CK(ctx, s.gr_n_deliv.ensure(nb)); CK(ctx, s.gr_offsets.ensure(nb + 1));
+    CK(ctx, s.gr_flags.ensure(4));
+    CK(ctx, s.gr_stats.ensure(8));
+    CK(ctx, s.h_gr_flags.ensure(20 + 1024));
     // at most two deliveries per candidate (check_crc = 0 delivers a failed first attempt and its
     // retry), so the deliveries fit whenever the candidates do
-    if (s.gr.capacity < 2 * s.cand_cap) {
-        cudaFree(s.gr.out); s.gr.out = nullptr; s.gr.capacity = 0;
-        CK(ctx, cudaMalloc(&s.gr.out, 2 * (size_t)s.cand_cap * sizeof(modes_delivery)));
-        s.gr.capacity = 2 * s.cand_cap;
-    }
+    CK(ctx, s.gr_out.ensure(2 * (size_t)s.cand_cap()));
+    g = GpuResolve{s.gr_start.get(), s.gr_end.get(), s.gr_written.get(), s.gr_readfirst.get(), s.gr_rerun.get(),
+                   s.gr_n_deliv.get(), s.gr_offsets.get(), s.gr_flags.get(), nullptr, nullptr, s.gr_stats.get(),
+                   s.gr_out.get(), (uint32_t)s.gr_out.capacity()};
     return 0;
 }
 
@@ -336,33 +310,35 @@ int submit(modes_ctx *ctx, Slot &s, const uint8_t *host_iq, const void *d_iq, si
     // caller-supplied record buffers: the slot's own position list must hold as many candidates
     if (d_records_ext && cap_ext > s.want_cap) s.want_cap = cap_ext;
     if (slot_ensure(ctx, s, n_samples, host_iq != nullptr, d_records_ext == nullptr)) return -1;
-    s.levels = ctx->levels && &s != &ctx->detect;
-    s.recover = ctx->recover && &s != &ctx->detect;       // the stage level asks with modes_recover_device
+    s.feat = ctx->feat;
+    s.feat.levels &= &s != &ctx->detect;
+    s.feat.recover &= &s != &ctx->detect;                 // the stage level asks with modes_recover_device
     s.rec_ext = nullptr; s.rec_ext_cap = 0;
-    s.weak = s.recover && ctx->weak;                      // the stage level asks with modes_weak_device
+    s.feat.weak &= s.feat.recover;                        // the stage level asks with modes_weak_device
     s.weak_pos_ext = nullptr; s.weak_rec_ext = nullptr; s.weak_ext_cap = 0;
     s.weak_first = 0; s.weak_step = 1;
-    s.signal = ctx->signal;
-    s.arrival = ctx->arrival;
-    if (s.levels && levels_ensure(ctx, s.d_levels, s.h_levels, s.levels_cap, n_buffers, nullptr)) return -1;   // collected
+    if (s.feat.levels) {                                  // the slot's previous batch is collected: no copy is queued
+        CK(ctx, s.d_levels.ensure(n_buffers));
+        CK(ctx, s.h_levels.ensure(n_buffers));
+    }
     if (host_iq) {
-        CK(ctx, cudaMemcpyAsync(s.d_iq, host_iq, n_samples * 2, cudaMemcpyHostToDevice, s.stream));
-        d_iq = s.d_iq;
+        CK(ctx, cudaMemcpyAsync(s.d_iq.get(), host_iq, n_samples * 2, cudaMemcpyHostToDevice, s.stream));
+        d_iq = s.d_iq.get();
     }
     if ((reinterpret_cast<uintptr_t>(d_iq) & 15) != 0) return fail(ctx, "device I/Q pointer must be 16-byte aligned");
     const unsigned hi = s.halo_next++ % Slot::kHaloRing;
-    uint8_t *h_halo = s.h_halo + (size_t)hi * kHaloAlloc;
+    uint8_t *h_halo = s.h_halo.get() + (size_t)hi * kHaloAlloc;
     CK(ctx, cudaEventSynchronize(s.halo_ev[hi]));                         // its previous copy (8 submits ago) has left the host
     memset(h_halo, 127, kHaloAlloc);                                      // dump1090.c:344 no-signal
     if (carry476) memcpy(h_halo + (kHaloBytes - MODES_CARRY_BYTES), carry476, MODES_CARRY_BYTES);
-    CK(ctx, cudaMemcpyAsync(s.d_halo, h_halo, kHaloAlloc, cudaMemcpyHostToDevice, s.stream));
+    CK(ctx, cudaMemcpyAsync(s.d_halo.get(), h_halo, kHaloAlloc, cudaMemcpyHostToDevice, s.stream));
     CK(ctx, cudaEventRecord(s.halo_ev[hi], s.stream));
     s.batch_iq = d_iq;
     s.n_buffers = n_buffers;
     s.own_outputs = d_records_ext == nullptr;
-    s.out_records = d_records_ext ? d_records_ext : s.d_records;
-    s.out_tiles = d_tiles_ext ? d_tiles_ext : s.d_tiles;
-    s.out_cap = d_records_ext ? (cap_ext < s.cand_cap ? cap_ext : s.cand_cap) : s.cand_cap;
+    s.out_records = d_records_ext ? d_records_ext : s.d_records.get();
+    s.out_tiles = d_tiles_ext ? d_tiles_ext : s.d_tiles.get();
+    s.out_cap = d_records_ext ? (cap_ext < s.cand_cap() ? cap_ext : s.cand_cap()) : s.cand_cap();
     return launch_batch(ctx, s);
 }
 
@@ -372,12 +348,8 @@ int launch_recovery(modes_ctx *ctx, Slot &s, const BatchView &in, const ScanOutp
     modes_recovered *dst = s.rec_ext;
     uint32_t cap = s.rec_ext_cap < s.out_cap ? s.rec_ext_cap : s.out_cap;
     if (!dst) {
-        if (s.rec_cap < s.out_cap) {
-            cudaFree(s.d_recovered); s.d_recovered = nullptr; s.rec_cap = 0;
-            CK(ctx, cudaMalloc(&s.d_recovered, (size_t)s.out_cap * sizeof(modes_recovered)));
-            s.rec_cap = s.out_cap;
-        }
-        dst = s.d_recovered;
+        CK(ctx, s.d_recovered.ensure(s.out_cap));
+        dst = s.d_recovered.get();
         cap = s.out_cap;
     }
     launch_recover(in, ctx->tab, so, s.out_records, cap, dst, ctx->sm_count, s.stream);
@@ -392,54 +364,42 @@ int launch_recovery(modes_ctx *ctx, Slot &s, const BatchView &in, const ScanOutp
 int launch_weak(modes_ctx *ctx, Slot &s, const BatchView &in) {
     const uint32_t n_scan = s.weak_first < s.n_buffers ? (uint32_t)((s.n_buffers - 1 - s.weak_first) / s.weak_step + 1) : 0u;
     const uint64_t scan_samples = (uint64_t)n_scan * kBufSamples;
-    const uint32_t nt = weak_tiles_for(n_scan);
-    if (s.weak_tiles_cap < nt) {
-        cudaFree(s.d_weak_tiles); s.d_weak_tiles = nullptr; s.weak_tiles_cap = 0;
-        CK(ctx, cudaMalloc(&s.d_weak_tiles, 3 * (size_t)nt * sizeof(uint32_t)));
-        s.weak_tiles_cap = nt;
-    }
-    if (!s.d_weak_counters) {
-        CK(ctx, cudaMalloc(&s.d_weak_counters, 2 * sizeof(uint32_t)));
-        CK(ctx, cudaMallocHost(&s.h_weak_counters, 2 * sizeof(uint32_t)));
-    }
+    CK(ctx, s.d_weak_tiles.ensure(3 * (size_t)weak_tiles_for(n_scan)));
+    CK(ctx, s.d_weak_counters.ensure(2));
+    CK(ctx, s.h_weak_counters.ensure(2));
     // a weak position passes the shape test, which two neighbours never both pass: at most one in two
     uint64_t want = scan_samples / 512 + 4096;
     if (want < s.want_weak_cap) want = s.want_weak_cap;
     if (want > scan_samples / 2 + 1) want = scan_samples / 2 + 1;
-    if (s.weak_cap < want) {
-        cudaFree(s.d_weak_pos); cudaFree(s.d_weak_rec); cudaFree(s.d_weak_scratch);
-        s.d_weak_pos = nullptr; s.d_weak_rec = nullptr; s.d_weak_scratch = nullptr; s.weak_cap = 0;
-        CK(ctx, cudaMalloc(&s.d_weak_pos, want * sizeof(uint32_t)));
-        CK(ctx, cudaMalloc(&s.d_weak_rec, want * sizeof(modes_recovered)));
-        CK(ctx, cudaMalloc(&s.d_weak_scratch, want * sizeof(uint32_t)));
-        s.weak_cap = (uint32_t)want;
-    }
-    uint32_t *pos = s.weak_pos_ext ? s.weak_pos_ext : s.d_weak_pos;
-    modes_recovered *rec = s.weak_pos_ext ? s.weak_rec_ext : s.d_weak_rec;
-    const uint32_t cap = s.weak_pos_ext ? s.weak_ext_cap : s.weak_cap;
+    CK(ctx, s.d_weak_pos.ensure(want));
+    CK(ctx, s.d_weak_rec.ensure(want));
+    CK(ctx, s.d_weak_scratch.ensure(want));
+    uint32_t *pos = s.weak_pos_ext ? s.weak_pos_ext : s.d_weak_pos.get();
+    modes_recovered *rec = s.weak_pos_ext ? s.weak_rec_ext : s.d_weak_rec.get();
+    const uint32_t cap = s.weak_pos_ext ? s.weak_ext_cap : s.weak_cap();
     launch_weak_scan(in, ctx->tab,
-                     WeakOutputs{s.weak_first, s.weak_step, n_scan, pos, cap, s.d_weak_scratch, s.weak_cap, s.d_weak_tiles,
-                                 s.d_weak_counters},
+                     WeakOutputs{s.weak_first, s.weak_step, n_scan, pos, cap, s.d_weak_scratch.get(), s.weak_cap(),
+                                 s.d_weak_tiles.get(), s.d_weak_counters.get()},
                      ctx->sm_count, s.stream);
-    launch_recover_weak(in, ctx->tab, s.d_weak_counters + 1, cap, s.weak_cap, pos, rec, ctx->sm_count, s.stream);
+    launch_recover_weak(in, ctx->tab, s.d_weak_counters.get() + 1, cap, s.weak_cap(), pos, rec, ctx->sm_count, s.stream);
     CK(ctx, cudaGetLastError());
     ctx->launches += 4;
-    CK(ctx, cudaMemcpyAsync(s.h_weak_counters, s.d_weak_counters, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
+    CK(ctx, cudaMemcpyAsync(s.h_weak_counters.get(), s.d_weak_counters.get(), 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
     return 0;
 }
 
 // The weak positions of the slot's last batch exceed its scratch list (and its own output arrays):
 // the batch is repeated with larger ones.  A caller's smaller arrays only report the count.
 bool weak_overflowed(const Slot &s) {
-    return s.weak && s.h_weak_counters[1] > s.weak_cap;
+    return s.feat.weak && s.h_weak_counters[1] > s.weak_cap();
 }
 
 // The two kernels over the slot's staged batch (also used to repeat a batch that overflowed).
 int launch_batch(modes_ctx *ctx, Slot &s) {
     const uint64_t n_samples = (uint64_t)s.n_buffers * kBufSamples;
-    CK(ctx, cudaMemsetAsync(s.d_counters, 0, 4 * sizeof(uint32_t), s.stream));
-    BatchView in{static_cast<const uint8_t *>(s.batch_iq), s.d_halo, n_samples};
-    ScanOutputs so{s.d_cand_v, s.out_cap, s.out_tiles, s.d_counters};
+    CK(ctx, cudaMemsetAsync(s.d_counters.get(), 0, 4 * sizeof(uint32_t), s.stream));
+    BatchView in{static_cast<const uint8_t *>(s.batch_iq), s.d_halo.get(), n_samples};
+    ScanOutputs so{s.d_cand_v.get(), s.out_cap, s.out_tiles, s.d_counters.get()};
 
     cudaEvent_t *pe = nullptr;
     if (ctx->cfg.profile) {
@@ -457,34 +417,38 @@ int launch_batch(modes_ctx *ctx, Slot &s) {
     launch_eval(in, ctx->tab, so, s.out_records, ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->sm_count, s.stream);
     if (pe) CK(ctx, cudaEventRecord(pe[2], s.stream));
     // after pe[2]: the kernel times keep their meaning; before the device resolve, which copies the field
-    if (s.signal || s.arrival) launch_signal(in, ctx->tab, so, s.out_records, ctx->sm_count, s.stream, s.signal, s.arrival);
+    const Features &f = s.feat;
+    if (f.signal || f.arrival) launch_signal(in, ctx->tab, so, s.out_records, ctx->sm_count, s.stream, f.signal, f.arrival);
     // the buffers' own bytes (the body, not the carry block); one writer per record, so a repeated
     // batch writes the same records
-    if (s.levels)
-        launch_levels(in.body, (uint32_t)s.n_buffers, MODES_BUFFER_BYTES, ctx->tab, s.d_levels, ctx->sm_count, s.stream);
+    if (f.levels)
+        launch_levels(in.body, (uint32_t)s.n_buffers, MODES_BUFFER_BYTES, ctx->tab, s.d_levels.get(), ctx->sm_count, s.stream);
     CK(ctx, cudaGetLastError());
-    ctx->launches += (s.signal || s.arrival ? 3 : 2) + (s.levels ? 1 : 0);
-    if (s.recover && launch_recovery(ctx, s, in, so)) return -1;
-    if (s.weak && launch_weak(ctx, s, in)) return -1;
+    ctx->launches += (f.signal || f.arrival ? 3 : 2) + (f.levels ? 1 : 0);
+    if (f.recover && launch_recovery(ctx, s, in, so)) return -1;
+    if (f.weak && launch_weak(ctx, s, in)) return -1;
     if (ctx->cfg.gpu_resolve && s.own_outputs && &s != &ctx->detect) {
-        if (gpu_resolve_ensure(ctx, s)) return -1;
+        GpuResolve g;
+        if (gpu_resolve_ensure(ctx, s, g)) return -1;
         // the address cache comes from the previous batch's resolve (other slot, other stream)
         if (ctx->resolved_pending) CK(ctx, cudaStreamWaitEvent(s.stream, ctx->ev_resolved, 0));
-        s.gr.cache_in = ctx->d_cache[ctx->cache_cur];
-        s.gr.cache_out = ctx->d_cache[ctx->cache_cur ^ 1];
+        g.cache_in = ctx->d_cache[ctx->cache_cur].get();
+        g.cache_out = ctx->d_cache[ctx->cache_cur ^ 1].get();
         ctx->cache_cur ^= 1;
-        launch_gpu_resolve(s.gr, s.out_records, s.out_tiles, tiles_for(n_samples), (uint32_t)s.n_buffers, ctx->cfg.check_crc,
+        launch_gpu_resolve(g, s.out_records, s.out_tiles, tiles_for(n_samples), (uint32_t)s.n_buffers, ctx->cfg.check_crc,
                            ctx->sm_count, s.stream);
         CK(ctx, cudaGetLastError());
         ctx->launches += 4 + 2 * kGpuResolveRounds;
         CK(ctx, cudaEventRecord(ctx->ev_resolved, s.stream));
         ctx->resolved_pending = true;
-        CK(ctx, cudaMemcpyAsync(s.h_gr_flags, s.gr.flags, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
-        CK(ctx, cudaMemcpyAsync(s.h_gr_flags + 4, s.gr.stats_out, 8 * sizeof(uint64_t), cudaMemcpyDeviceToHost, s.stream));
-        CK(ctx, cudaMemcpyAsync(s.h_gr_flags + 20, s.gr.cache_out, 1024 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
+        uint32_t *h = s.h_gr_flags.get();
+        CK(ctx, cudaMemcpyAsync(h, g.flags, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
+        CK(ctx, cudaMemcpyAsync(h + 4, g.stats_out, 8 * sizeof(uint64_t), cudaMemcpyDeviceToHost, s.stream));
+        CK(ctx, cudaMemcpyAsync(h + 20, g.cache_out, 1024 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
     }
-    CK(ctx, cudaMemcpyAsync(s.h_counters, s.d_counters, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
-    if (s.levels) CK(ctx, cudaMemcpyAsync(s.h_levels, s.d_levels, s.n_buffers * sizeof(modes_level), cudaMemcpyDeviceToHost, s.stream));
+    CK(ctx, cudaMemcpyAsync(s.h_counters.get(), s.d_counters.get(), 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
+    if (f.levels)
+        CK(ctx, cudaMemcpyAsync(s.h_levels.get(), s.d_levels.get(), s.n_buffers * sizeof(modes_level), cudaMemcpyDeviceToHost, s.stream));
     CK(ctx, cudaEventRecord(s.ev[3], s.stream));
     s.busy = true;
     return 0;
@@ -505,8 +469,8 @@ int wait_batch(modes_ctx *ctx, Slot &s, uint64_t *n_out) {
                 return fail(ctx, "candidate capacity exceeded: %u found, room for %u", found, s.out_cap);
             s.want_cap = found + found / 8 + 1024;
             if (slot_ensure(ctx, s, (uint64_t)s.n_buffers * kBufSamples, false, true)) return -1;
-            s.out_records = s.d_records;
-            s.out_cap = s.cand_cap;
+            s.out_records = s.d_records.get();
+            s.out_cap = s.cand_cap();
         }
         if (weak_overflowed(s)) s.want_weak_cap = s.h_weak_counters[1] + s.h_weak_counters[1] / 8 + 1024;
         if (launch_batch(ctx, s)) return -1;
@@ -515,22 +479,40 @@ int wait_batch(modes_ctx *ctx, Slot &s, uint64_t *n_out) {
     return 0;
 }
 
-// Pinned room for the slot's weak positions and records, and their copies queued on its stream;
-// returns the weak list of the batch.
-int weak_fetch_async(modes_ctx *ctx, Slot &s, WeakList &wl) {
-    const size_t n = s.h_weak_counters[1];
-    if (s.h_weak_cap < n) {
-        cudaFreeHost(s.h_weak_pos); cudaFreeHost(s.h_weak_rec); s.h_weak_pos = nullptr; s.h_weak_rec = nullptr; s.h_weak_cap = 0;
-        const size_t cap = n + n / 2 + 1024;
-        CK(ctx, cudaMallocHost(&s.h_weak_pos, cap * sizeof(uint32_t)));
-        CK(ctx, cudaMallocHost(&s.h_weak_rec, cap * sizeof(modes_recovered)));
-        s.h_weak_cap = cap;
+// One finished batch's results in pinned host memory, as the host resolve takes them.
+struct ShardView {
+    const modes_candidate *cands = nullptr;
+    const modes_tile *tiles = nullptr;
+    size_t n_tiles = 0;
+    int64_t buffer_base = 0;
+    const modes_recovered *recovered = nullptr;   // the batch ran no recovery: nullptr
+    WeakList weak;
+};
+
+// Queue the copies of the slot's finished batch (n candidate records) to pinned memory on its
+// stream; the view is valid once the stream has been waited for.
+int fetch_async(modes_ctx *ctx, Slot &s, uint64_t n, ShardView &v) {
+    const size_t nt = tiles_for((uint64_t)s.n_buffers * kBufSamples);
+    CK(ctx, ensure_spare(s.h_records, n));
+    CK(ctx, s.h_tiles.ensure(nt));
+    if (n) CK(ctx, cudaMemcpyAsync(s.h_records.get(), s.out_records, n * sizeof(modes_candidate), cudaMemcpyDeviceToHost, s.stream));
+    if (s.feat.recover) {
+        CK(ctx, ensure_spare(s.h_recovered, n));
+        if (n) CK(ctx, cudaMemcpyAsync(s.h_recovered.get(), s.d_recovered.get(), n * sizeof(modes_recovered), cudaMemcpyDeviceToHost, s.stream));
     }
-    if (n) {
-        CK(ctx, cudaMemcpyAsync(s.h_weak_pos, s.d_weak_pos, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
-        CK(ctx, cudaMemcpyAsync(s.h_weak_rec, s.d_weak_rec, n * sizeof(modes_recovered), cudaMemcpyDeviceToHost, s.stream));
+    WeakList wl;
+    if (s.feat.weak) {
+        const size_t nw = s.h_weak_counters[1];
+        CK(ctx, ensure_spare(s.h_weak_pos, nw));
+        CK(ctx, ensure_spare(s.h_weak_rec, nw));
+        if (nw) {
+            CK(ctx, cudaMemcpyAsync(s.h_weak_pos.get(), s.d_weak_pos.get(), nw * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
+            CK(ctx, cudaMemcpyAsync(s.h_weak_rec.get(), s.d_weak_rec.get(), nw * sizeof(modes_recovered), cudaMemcpyDeviceToHost, s.stream));
+        }
+        wl = WeakList{s.h_weak_pos.get(), s.h_weak_rec.get(), nw};
     }
-    wl = WeakList{s.h_weak_pos, s.h_weak_rec, n};
+    CK(ctx, cudaMemcpyAsync(s.h_tiles.get(), s.out_tiles, nt * sizeof(modes_tile), cudaMemcpyDeviceToHost, s.stream));
+    v = ShardView{s.h_records.get(), s.h_tiles.get(), nt, s.buffer_base, s.feat.recover ? s.h_recovered.get() : nullptr, wl};
     return 0;
 }
 
@@ -557,34 +539,22 @@ int collect(modes_ctx *ctx, Slot &s) {
         if (s.h_gr_flags[0]) return fail(ctx, "gpu_resolve: internal error: address caches did not settle after the in-order replay");
         if (s.h_gr_flags[1]) return fail(ctx, "gpu_resolve: delivery capacity exceeded (%u messages)", s.h_gr_flags[2]);
         const size_t nd = s.h_gr_flags[2];
-        if (s.h_deliveries_cap < nd) {
-            cudaFreeHost(s.h_deliveries); s.h_deliveries = nullptr; s.h_deliveries_cap = 0;
-            const size_t cap = nd + nd / 2 + 1024;
-            CK(ctx, cudaMallocHost(&s.h_deliveries, cap * sizeof(modes_delivery)));
-            s.h_deliveries_cap = cap;
-        }
-        if (nd) CK(ctx, cudaMemcpyAsync(s.h_deliveries, s.gr.out, nd * sizeof(modes_delivery), cudaMemcpyDeviceToHost, s.stream));
+        CK(ctx, ensure_spare(s.h_deliveries, nd));
+        if (nd) CK(ctx, cudaMemcpyAsync(s.h_deliveries.get(), s.gr_out.get(), nd * sizeof(modes_delivery), cudaMemcpyDeviceToHost, s.stream));
         CK(ctx, wait_stream(s.stream));
         uint64_t st8[8];
-        memcpy(st8, s.h_gr_flags + 4, sizeof(st8));
+        memcpy(st8, s.h_gr_flags.get() + 4, sizeof(st8));
         for (int i = 0; i < 8; i++) ctx->rs.stats[i] += (int64_t)st8[i];
-        memcpy(ctx->rs.icao, s.h_gr_flags + 20, sizeof(ctx->rs.icao));    // host copy for the hex door / a later host resolve
-        deliver_gpu(s.h_deliveries, nd, s.buffer_base, ctx->out);
+        memcpy(ctx->rs.icao, s.h_gr_flags.get() + 20, sizeof(ctx->rs.icao));    // host copy for the hex door / a later host resolve
+        deliver_gpu(s.h_deliveries.get(), nd, s.buffer_base, ctx->out);
         return 0;
     }
-    const size_t nt = tiles_for((uint64_t)s.n_buffers * kBufSamples);
-    if (host_ensure(ctx, s, n, nt)) return -1;
-    if (s.recover && recovered_ensure(ctx, s, n)) return -1;
-    if (n) CK(ctx, cudaMemcpyAsync(s.h_records, s.out_records, n * sizeof(modes_candidate), cudaMemcpyDeviceToHost, s.stream));
-    if (n && s.recover) CK(ctx, cudaMemcpyAsync(s.h_recovered, s.d_recovered, n * sizeof(modes_recovered), cudaMemcpyDeviceToHost, s.stream));
-    WeakList wl;
-    if (s.weak && weak_fetch_async(ctx, s, wl)) return -1;
-    CK(ctx, cudaMemcpyAsync(s.h_tiles, s.out_tiles, nt * sizeof(modes_tile), cudaMemcpyDeviceToHost, s.stream));
+    ShardView v;
+    if (fetch_async(ctx, s, n, v)) return -1;
     CK(ctx, wait_stream(s.stream));
     const double t2 = dbg ? now_ms() : 0;
-    ResolveConfig rc{ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->cfg.check_crc, s.signal ? 1 : 0};
-    resolve_candidates(ctx->rs, rc, s.h_records, s.h_tiles, nt, s.buffer_base, ctx->out, ctx->scratch,
-                       s.recover ? s.h_recovered : nullptr, wl);
+    ResolveConfig rc{ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->cfg.check_crc, s.feat.signal ? 1 : 0};
+    resolve_candidates(ctx->rs, rc, v.cands, v.tiles, v.n_tiles, v.buffer_base, ctx->out, ctx->scratch, v.recovered, v.weak);
     if (dbg) fprintf(stderr, "[collect] %zu buffers, %llu cands: wait %.3f ms, d2h %.3f ms, resolve %.3f ms (t=%.3f)\n",
                      s.n_buffers, (unsigned long long)n, t1 - t0, t2 - t1, now_ms() - t2, now_ms());
     return 0;
@@ -612,19 +582,12 @@ int collect_group(modes_ctx *ctx, int parity) {
         if (wait_batch(g, s, &nc)) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
         s.busy = false;
         append_levels(ctx, s);                          // groups and GPUs in stream order
-        n_tiles[k] = tiles_for((uint64_t)s.n_buffers * kBufSamples);
-        if (host_ensure(g, s, nc, n_tiles[k])) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
-        if (nc) CK(ctx, cudaMemcpyAsync(s.h_records, s.out_records, nc * sizeof(modes_candidate), cudaMemcpyDeviceToHost, s.stream));
-        if (s.recover) {
-            if (recovered_ensure(g, s, nc)) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
-            if (nc) CK(ctx, cudaMemcpyAsync(s.h_recovered, s.d_recovered, nc * sizeof(modes_recovered), cudaMemcpyDeviceToHost, s.stream));
-            recovered[k] = s.h_recovered;
-            any_recover = true;
-        }
-        if (s.weak && weak_fetch_async(g, s, weak[k])) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
-        signal = s.signal;
-        CK(ctx, cudaMemcpyAsync(s.h_tiles, s.out_tiles, n_tiles[k] * sizeof(modes_tile), cudaMemcpyDeviceToHost, s.stream));
-        cands[k] = s.h_records; tiles[k] = s.h_tiles; base[k] = s.buffer_base;
+        ShardView v;
+        if (fetch_async(g, s, nc, v)) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
+        cands[k] = v.cands; tiles[k] = v.tiles; n_tiles[k] = v.n_tiles; base[k] = v.buffer_base;
+        recovered[k] = v.recovered; weak[k] = v.weak;
+        any_recover |= s.feat.recover;
+        signal = s.feat.signal;
     }
     for (size_t k = 0; k < n; k++) {
         CK(ctx, cudaSetDevice(ctx->gpus[k]->cfg.device));
@@ -661,7 +624,6 @@ int run_buffers_multi(modes_ctx *ctx, const uint8_t *host_iq, size_t n_buffers) 
             ctx->buffers_done += (int64_t)nb;
             host_iq += nb * MODES_BUFFER_BYTES;
             n_buffers -= nb;
-            ctx->launches += (g->signal || g->arrival ? 3 : 2) + (g->levels ? 1 : 0) + (g->recover ? 1 : 0) + (g->recover && g->weak ? 4 : 0);
         }
         ctx->group_n[cur] = k;
         if (have_prev && collect_group(ctx, cur ^ 1)) return -1;
@@ -700,6 +662,14 @@ int run_buffers(modes_ctx *ctx, const uint8_t *host_iq, size_t n_buffers) {
     return 0;
 }
 
+// One switch of the context and of its GPUs' contexts; each batch runs as the switches were at submit.
+int set_feature(modes_ctx *ctx, bool Features::*f, int on) {
+    if (!ctx) return -1;
+    ctx->feat.*f = on != 0;
+    for (modes_ctx *g : ctx->gpus) g->feat.*f = on != 0;
+    return 0;
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------- C ABI
@@ -729,15 +699,10 @@ void modes_destroy(modes_ctx *ctx) {
     cudaSetDevice(ctx->cfg.device);
     if (ctx->own_detect_stream) { wait_stream(ctx->detect.stream); ctx->detect.stream = ctx->own_detect_stream; }
     slot_free(ctx->slot[0]); slot_free(ctx->slot[1]); slot_free(ctx->detect);
-    cudaFree(ctx->d_lutn); cudaFree(ctx->d_lut_iq); cudaFree(ctx->d_bit_syn); cudaFree(ctx->d_fix_hash); cudaFree(ctx->d_pair_hash);
-    cudaFree(ctx->d_frames); cudaFree(ctx->d_frame_evals); cudaFreeHost(ctx->h_frame_evals);
-    cudaFree(ctx->d_cache[0]); cudaFree(ctx->d_cache[1]);
     if (ctx->ev_resolved) cudaEventDestroy(ctx->ev_resolved);
     if (ctx->prof_ready) for (auto &trip : ctx->prof_ev) for (auto &e : trip) cudaEventDestroy(e);
-    cudaFreeHost(ctx->pending);
-    cudaFree(ctx->d_lv); cudaFreeHost(ctx->h_lv);
     scratch_destroy(ctx->scratch);
-    delete ctx;
+    delete ctx;                       // and with it the context's own buffers
 }
 
 static int create_impl(modes_ctx *ctx) {
@@ -763,23 +728,24 @@ static int create_impl(modes_ctx *ctx) {
     build_lut_iq(lut_iq.data());
     build_bit_syndromes(syn);
     if (!build_fix_hash(syn, hash)) return fail(nullptr, "internal: syndrome hash construction failed");
-    CK(nullptr, cudaMalloc(&ctx->d_lutn, kNLutEntries * sizeof(uint16_t)));
-    CK(nullptr, cudaMalloc(&ctx->d_lut_iq, kLutIqEntries * sizeof(uint16_t)));
-    CK(nullptr, cudaMemcpy(ctx->d_lut_iq, lut_iq.data(), kLutIqEntries * sizeof(uint16_t), cudaMemcpyHostToDevice));
-    CK(nullptr, cudaMalloc(&ctx->d_bit_syn, sizeof(syn)));
-    CK(nullptr, cudaMalloc(&ctx->d_fix_hash, sizeof(hash)));
-    CK(nullptr, cudaMemcpy(ctx->d_lutn, lutn.data(), kNLutEntries * sizeof(uint16_t), cudaMemcpyHostToDevice));
-    CK(nullptr, cudaMemcpy(ctx->d_bit_syn, syn, sizeof(syn), cudaMemcpyHostToDevice));
-    CK(nullptr, cudaMemcpy(ctx->d_fix_hash, hash, sizeof(hash), cudaMemcpyHostToDevice));
+    CK(nullptr, ctx->d_lutn.ensure(kNLutEntries));
+    CK(nullptr, ctx->d_lut_iq.ensure(kLutIqEntries));
+    CK(nullptr, cudaMemcpy(ctx->d_lut_iq.get(), lut_iq.data(), kLutIqEntries * sizeof(uint16_t), cudaMemcpyHostToDevice));
+    CK(nullptr, ctx->d_bit_syn.ensure(112));
+    CK(nullptr, ctx->d_fix_hash.ensure(kFixHashSlots));
+    CK(nullptr, cudaMemcpy(ctx->d_lutn.get(), lutn.data(), kNLutEntries * sizeof(uint16_t), cudaMemcpyHostToDevice));
+    CK(nullptr, cudaMemcpy(ctx->d_bit_syn.get(), syn, sizeof(syn), cudaMemcpyHostToDevice));
+    CK(nullptr, cudaMemcpy(ctx->d_fix_hash.get(), hash, sizeof(hash), cudaMemcpyHostToDevice));
     std::vector<uint32_t> pair(kPairHashSlots);
     if (!build_pair_hash(syn, pair.data())) return fail(nullptr, "internal: two-bit syndrome table construction failed");
-    CK(nullptr, cudaMalloc(&ctx->d_pair_hash, pair.size() * sizeof(uint32_t)));
-    CK(nullptr, cudaMemcpy(ctx->d_pair_hash, pair.data(), pair.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-    ctx->tab = DeviceTables{ctx->d_lutn, ctx->d_lut_iq, ctx->d_bit_syn, ctx->d_fix_hash, ctx->d_pair_hash};
-    CK(nullptr, cudaMallocHost(&ctx->pending, MODES_BUFFER_BYTES));
+    CK(nullptr, ctx->d_pair_hash.ensure(pair.size()));
+    CK(nullptr, cudaMemcpy(ctx->d_pair_hash.get(), pair.data(), pair.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    ctx->tab = DeviceTables{ctx->d_lutn.get(), ctx->d_lut_iq.get(), ctx->d_bit_syn.get(), ctx->d_fix_hash.get(),
+                            ctx->d_pair_hash.get()};
+    CK(nullptr, ctx->pending.ensure(MODES_BUFFER_BYTES));
     if (ctx->cfg.gpu_resolve) {
         if (ctx->cfg.n_gpus > 1) return fail(nullptr, "gpu_resolve and n_gpus > 1 cannot be combined");
-        for (auto &c : ctx->d_cache) { CK(nullptr, cudaMalloc(&c, 4096)); CK(nullptr, cudaMemset(c, 0, 4096)); }
+        for (auto &c : ctx->d_cache) { CK(nullptr, c.ensure(1024)); CK(nullptr, cudaMemset(c.get(), 0, 4096)); }
         CK(nullptr, cudaEventCreateWithFlags(&ctx->ev_resolved, cudaEventDisableTiming));
     }
     for (Slot *s : {&ctx->slot[0], &ctx->slot[1], &ctx->detect})
@@ -812,42 +778,13 @@ modes_ctx *modes_create(const modes_config *cfg) {
     return ctx;
 }
 
-int modes_set_signal(modes_ctx *ctx, int on) {
-    if (!ctx) return -1;
-    ctx->signal = on != 0;
-    for (modes_ctx *g : ctx->gpus) g->signal = on != 0;
-    return 0;
-}
+int modes_set_signal(modes_ctx *ctx, int on) { return set_feature(ctx, &Features::signal, on); }
 
-int modes_set_arrival(modes_ctx *ctx, int on) {
-    if (!ctx) return -1;
-    ctx->arrival = on != 0;
-    for (modes_ctx *g : ctx->gpus) g->arrival = on != 0;
-    return 0;
-}
+int modes_set_arrival(modes_ctx *ctx, int on) { return set_feature(ctx, &Features::arrival, on); }
 
-int modes_set_levels(modes_ctx *ctx, int on) {
-    if (!ctx) return -1;
-    ctx->levels = on != 0;
-    for (modes_ctx *g : ctx->gpus) g->levels = on != 0;
-    return 0;
-}
+int modes_set_levels(modes_ctx *ctx, int on) { return set_feature(ctx, &Features::levels, on); }
 
-size_t modes_take_levels(modes_ctx *ctx, modes_level *out, size_t cap) {
-    if (!ctx) return 0;
-    std::vector<modes_level> &q = ctx->level_q;
-    const size_t queued = q.size() - ctx->level_head;
-    if (!out) return queued;
-    const size_t n = cap < queued ? cap : queued;
-    if (n) memcpy(out, q.data() + ctx->level_head, n * sizeof(modes_level));
-    ctx->level_head += n;
-    if (ctx->level_head == q.size()) { q.clear(); ctx->level_head = 0; }
-    else if (ctx->level_head >= 4096 && 2 * ctx->level_head >= q.size()) {
-        q.erase(q.begin(), q.begin() + (ptrdiff_t)ctx->level_head);
-        ctx->level_head = 0;
-    }
-    return n;
-}
+size_t modes_take_levels(modes_ctx *ctx, modes_level *out, size_t cap) { return ctx ? ctx->level_q.take(out, cap) : 0; }
 
 int modes_levels_device(modes_ctx *ctx, const void *d_iq, size_t n_buffers, size_t stride_bytes) {
     if (!ctx) return -1;
@@ -858,11 +795,14 @@ int modes_levels_device(modes_ctx *ctx, const void *d_iq, size_t n_buffers, size
         return fail(ctx, "modes_levels_device: buffers must be 16-byte aligned");
     CK(ctx, cudaSetDevice(ctx->cfg.device));
     cudaStream_t st = ctx->detect.stream;
-    if (levels_ensure(ctx, ctx->d_lv, ctx->h_lv, ctx->lv_cap, n_buffers, ctx->lv_fetched ? nullptr : st)) return -1;
-    launch_levels(static_cast<const uint8_t *>(d_iq), (uint32_t)n_buffers, stride_bytes, ctx->tab, ctx->d_lv, ctx->sm_count, st);
+    // a copy into the pinned block may still be queued: wait for it before the block is replaced
+    if (!ctx->lv_fetched && ctx->h_lv.capacity() < n_buffers) CK(ctx, wait_stream(st));
+    CK(ctx, ctx->d_lv.ensure(n_buffers));
+    CK(ctx, ctx->h_lv.ensure(n_buffers));
+    launch_levels(static_cast<const uint8_t *>(d_iq), (uint32_t)n_buffers, stride_bytes, ctx->tab, ctx->d_lv.get(), ctx->sm_count, st);
     CK(ctx, cudaGetLastError());
     ctx->launches++;
-    CK(ctx, cudaMemcpyAsync(ctx->h_lv, ctx->d_lv, n_buffers * sizeof(modes_level), cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaMemcpyAsync(ctx->h_lv.get(), ctx->d_lv.get(), n_buffers * sizeof(modes_level), cudaMemcpyDeviceToHost, st));
     ctx->lv_n = n_buffers;
     ctx->lv_fetched = false;
     return 0;
@@ -875,17 +815,14 @@ int modes_levels_fetch(modes_ctx *ctx, modes_level *out) {
     CK(ctx, cudaSetDevice(ctx->cfg.device));
     CK(ctx, wait_stream(ctx->detect.stream));
     ctx->lv_fetched = true;
-    memcpy(out, ctx->h_lv, ctx->lv_n * sizeof(modes_level));
+    memcpy(out, ctx->h_lv.get(), ctx->lv_n * sizeof(modes_level));
     return 0;
 }
 
 int modes_set_recovery(modes_ctx *ctx, int on) {
-    if (!ctx) return -1;
     // the device resolve's read-set bookkeeping has no recovery rule
-    if (on && ctx->cfg.gpu_resolve) return fail(ctx, "modes_set_recovery: recovery cannot be combined with gpu_resolve");
-    ctx->recover = on != 0;
-    for (modes_ctx *g : ctx->gpus) g->recover = on != 0;
-    return 0;
+    if (ctx && on && ctx->cfg.gpu_resolve) return fail(ctx, "modes_set_recovery: recovery cannot be combined with gpu_resolve");
+    return set_feature(ctx, &Features::recover, on);
 }
 
 int modes_get_recovery_stats(const modes_ctx *ctx, modes_recovery_stats *out) {
@@ -895,11 +832,8 @@ int modes_get_recovery_stats(const modes_ctx *ctx, modes_recovery_stats *out) {
 }
 
 int modes_set_weak_preambles(modes_ctx *ctx, int on) {
-    if (!ctx) return -1;
-    if (on && ctx->cfg.gpu_resolve) return fail(ctx, "modes_set_weak_preambles: recovery cannot be combined with gpu_resolve");
-    ctx->weak = on != 0;
-    for (modes_ctx *g : ctx->gpus) g->weak = on != 0;
-    return 0;
+    if (ctx && on && ctx->cfg.gpu_resolve) return fail(ctx, "modes_set_weak_preambles: recovery cannot be combined with gpu_resolve");
+    return set_feature(ctx, &Features::weak, on);
 }
 
 int modes_get_weak_recovery_stats(const modes_ctx *ctx, modes_recovery_stats *out) {
@@ -925,13 +859,13 @@ int modes::weak_device_strided(modes_ctx *ctx, void *d_pos, void *d_rec, size_t 
     if (((reinterpret_cast<uintptr_t>(d_pos) | reinterpret_cast<uintptr_t>(d_rec)) & 3) != 0)
         return fail(ctx, "modes_weak_device: outputs must be 4-byte aligned");
     CK(ctx, cudaSetDevice(ctx->cfg.device));
-    s.weak = true;
+    s.feat.weak = true;
     s.weak_pos_ext = static_cast<uint32_t *>(d_pos);
     s.weak_rec_ext = static_cast<modes_recovered *>(d_rec);
     s.weak_ext_cap = !d_pos ? 0 : (capacity > 0xFFFFFFF0ull ? 0xFFFFFFF0u : (uint32_t)capacity);
     s.weak_first = first_buffer; s.weak_step = buffer_step;
     // a batch that wait_batch repeats (after a candidate or weak overflow) runs the passes again (launch_batch)
-    BatchView in{static_cast<const uint8_t *>(s.batch_iq), s.d_halo, (uint64_t)s.n_buffers * kBufSamples};
+    BatchView in{static_cast<const uint8_t *>(s.batch_iq), s.d_halo.get(), (uint64_t)s.n_buffers * kBufSamples};
     if (launch_weak(ctx, s, in)) return -1;
     CK(ctx, cudaEventRecord(s.ev[3], s.stream));           // wait_batch sees the weak count too
     return 0;
@@ -942,15 +876,15 @@ extern "C" {
 int modes_weak_fetch(modes_ctx *ctx, uint32_t *t, modes_recovered *rec, uint64_t *n) {
     if (!ctx) return -1;
     Slot &s = ctx->detect;
-    if (!s.weak) return fail(ctx, "modes_weak_fetch without modes_weak_device");
+    if (!s.feat.weak) return fail(ctx, "modes_weak_fetch without modes_weak_device");
     CK(ctx, cudaSetDevice(ctx->cfg.device));
     uint64_t nc = 0;
     if (wait_batch(ctx, s, &nc)) return -1;
     const uint64_t nw = s.h_weak_counters[1];
     if (n) *n = nw;
     if (!s.weak_pos_ext && nw) {
-        if (t) CK(ctx, cudaMemcpyAsync(t, s.d_weak_pos, nw * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
-        if (rec) CK(ctx, cudaMemcpyAsync(rec, s.d_weak_rec, nw * sizeof(modes_recovered), cudaMemcpyDeviceToHost, s.stream));
+        if (t) CK(ctx, cudaMemcpyAsync(t, s.d_weak_pos.get(), nw * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
+        if (rec) CK(ctx, cudaMemcpyAsync(rec, s.d_weak_rec.get(), nw * sizeof(modes_recovered), cudaMemcpyDeviceToHost, s.stream));
     }
     CK(ctx, wait_stream(s.stream));
     return 0;
@@ -963,24 +897,24 @@ int modes_recover_device(modes_ctx *ctx, void *d_out, size_t capacity) {
     if (d_out && !capacity) return fail(ctx, "modes_recover_device: capacity 0");
     if ((reinterpret_cast<uintptr_t>(d_out) & 3) != 0) return fail(ctx, "modes_recover_device: output must be 4-byte aligned");
     CK(ctx, cudaSetDevice(ctx->cfg.device));
-    s.recover = true;
+    s.feat.recover = true;
     s.rec_ext = static_cast<modes_recovered *>(d_out);
     s.rec_ext_cap = capacity > 0xFFFFFFF0ull ? 0xFFFFFFF0u : (uint32_t)capacity;
     // a batch that wait_batch repeats after an overflow runs the pass again (launch_batch)
-    BatchView in{static_cast<const uint8_t *>(s.batch_iq), s.d_halo, (uint64_t)s.n_buffers * kBufSamples};
-    ScanOutputs so{s.d_cand_v, s.out_cap, s.out_tiles, s.d_counters};
+    BatchView in{static_cast<const uint8_t *>(s.batch_iq), s.d_halo.get(), (uint64_t)s.n_buffers * kBufSamples};
+    ScanOutputs so{s.d_cand_v.get(), s.out_cap, s.out_tiles, s.d_counters.get()};
     return launch_recovery(ctx, s, in, so);
 }
 
 int modes_recover_fetch(modes_ctx *ctx, modes_recovered *out) {
     if (!ctx) return -1;
     Slot &s = ctx->detect;
-    if (!s.recover || s.rec_ext) return fail(ctx, "modes_recover_fetch without modes_recover_device(ctx, NULL, ...)");
+    if (!s.feat.recover || s.rec_ext) return fail(ctx, "modes_recover_fetch without modes_recover_device(ctx, NULL, ...)");
     if (!out) return fail(ctx, "modes_recover_fetch: no output array");
     CK(ctx, cudaSetDevice(ctx->cfg.device));
     uint64_t n = 0;
     if (wait_batch(ctx, s, &n)) return -1;
-    if (n) CK(ctx, cudaMemcpyAsync(out, s.d_recovered, n * sizeof(modes_recovered), cudaMemcpyDeviceToHost, s.stream));
+    if (n) CK(ctx, cudaMemcpyAsync(out, s.d_recovered.get(), n * sizeof(modes_recovered), cudaMemcpyDeviceToHost, s.stream));
     CK(ctx, wait_stream(s.stream));
     return 0;
 }
@@ -1015,14 +949,13 @@ int modes_reset(modes_ctx *ctx) {
     if (ctx->cfg.gpu_resolve) {
         cudaSetDevice(ctx->cfg.device);
         cudaDeviceSynchronize();
-        for (auto &c : ctx->d_cache) cudaMemset(c, 0, 4096);
+        for (auto &c : ctx->d_cache) cudaMemset(c.get(), 0, 4096);
         ctx->resolved_pending = false;
     }
     ctx->pending_len = 0;
     ctx->buffers_done = 0;
     ctx->finished = false;
     ctx->level_q.clear();
-    ctx->level_head = 0;
     ctx->eof_buffer = -1;
     memset(ctx->carry, 127, sizeof(ctx->carry));
     return 0;
@@ -1035,16 +968,16 @@ int modes_process(modes_ctx *ctx, const uint8_t *iq, size_t nbytes) {
     if (ctx->pending_len) {
         size_t take = MODES_BUFFER_BYTES - ctx->pending_len;
         if (take > nbytes) take = nbytes;
-        memcpy(ctx->pending + ctx->pending_len, iq, take);
+        memcpy(ctx->pending.get() + ctx->pending_len, iq, take);
         ctx->pending_len += take; iq += take; nbytes -= take;
         if (ctx->pending_len < MODES_BUFFER_BYTES) return 0;
-        if (run_buffers(ctx, ctx->pending, 1)) return -1;
+        if (run_buffers(ctx, ctx->pending.get(), 1)) return -1;
         ctx->pending_len = 0;
     }
     size_t whole = nbytes / MODES_BUFFER_BYTES;
     if (whole && run_buffers(ctx, iq, whole)) return -1;
     iq += whole * MODES_BUFFER_BYTES; nbytes -= whole * MODES_BUFFER_BYTES;
-    if (nbytes) { memcpy(ctx->pending, iq, nbytes); ctx->pending_len = nbytes; }
+    if (nbytes) { memcpy(ctx->pending.get(), iq, nbytes); ctx->pending_len = nbytes; }
     return 0;
 }
 
@@ -1055,12 +988,12 @@ int modes_finish(modes_ctx *ctx) {
     ctx->finished = true;
     // The read that hits EOF still hands a 127-padded buffer to the decoder (dump1090.c:496-510);
     // whether it is decoded is the reference's race, made a switch here.
-    memset(ctx->pending + ctx->pending_len, 127, MODES_BUFFER_BYTES - ctx->pending_len);
+    memset(ctx->pending.get() + ctx->pending_len, 127, MODES_BUFFER_BYTES - ctx->pending_len);
     ctx->eof_buffer = ctx->buffers_done;                 // its level record counts the real samples only
     ctx->eof_samples = (uint32_t)((ctx->pending_len + 1) / 2);
     ctx->pending_len = 0;
     if (ctx->cfg.drop_eof_buffer) return 0;
-    return run_buffers(ctx, ctx->pending, 1);
+    return run_buffers(ctx, ctx->pending.get(), 1);
 }
 
 int modes_get_stats(const modes_ctx *ctx, modes_stats *out) {
@@ -1073,18 +1006,18 @@ int modes_compute_magnitude(modes_ctx *ctx, const uint8_t *iq, size_t nsamples, 
     if (!ctx) return -1;
     if (!nsamples) return 0;
     CK(ctx, cudaSetDevice(ctx->cfg.device));
-    uint8_t *d_iq = nullptr; uint16_t *d_mag = nullptr;
+    DevBuf<uint8_t> d_iq;
+    DevBuf<uint16_t> d_mag;
     cudaStream_t st = ctx->detect.stream;
-    cudaError_t e = cudaMalloc(&d_iq, nsamples * 2);
-    if (e == cudaSuccess) e = cudaMalloc(&d_mag, nsamples * 2);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_iq, iq, nsamples * 2, cudaMemcpyHostToDevice, st);
+    cudaError_t e = d_iq.ensure(nsamples * 2);
+    if (e == cudaSuccess) e = d_mag.ensure(nsamples);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_iq.get(), iq, nsamples * 2, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) {
-        launch_magnitude(d_iq, d_mag, nsamples, ctx->d_lutn, st);
+        launch_magnitude(d_iq.get(), d_mag.get(), nsamples, ctx->d_lutn.get(), st);
         ctx->launches++;
-        e = cudaMemcpyAsync(mag, d_mag, nsamples * 2, cudaMemcpyDeviceToHost, st);
+        e = cudaMemcpyAsync(mag, d_mag.get(), nsamples * 2, cudaMemcpyDeviceToHost, st);
     }
     if (e == cudaSuccess) e = wait_stream(st);
-    cudaFree(d_iq); cudaFree(d_mag);
     if (e != cudaSuccess) return fail(ctx, "magnitude kernel failed: %s", cudaGetErrorString(e));
     return 0;
 }
@@ -1325,22 +1258,19 @@ int modes_decode_frames(modes_ctx *ctx, const uint8_t *frames, size_t n, modes_m
     CK(ctx, cudaSetDevice(ctx->cfg.device));
     // persistent device / pinned staging, grown on demand (the hex door is called per line by a
     // network feeder: no allocation per call)
-    if (ctx->frames_cap < n) {
-        cudaFree(ctx->d_frames); cudaFree(ctx->d_frame_evals); cudaFreeHost(ctx->h_frame_evals);
-    cudaFree(ctx->d_cache[0]); cudaFree(ctx->d_cache[1]);
-    if (ctx->ev_resolved) cudaEventDestroy(ctx->ev_resolved);
-        ctx->d_frames = nullptr; ctx->d_frame_evals = nullptr; ctx->h_frame_evals = nullptr; ctx->frames_cap = 0;
+    if (ctx->h_frame_evals.capacity() < n) {
         const size_t cap = n < 64 ? 64 : n + n / 2;
-        CK(ctx, cudaMalloc(&ctx->d_frames, cap * 14));
-        CK(ctx, cudaMalloc(&ctx->d_frame_evals, cap * sizeof(modes_frame_eval)));
-        CK(ctx, cudaMallocHost(&ctx->h_frame_evals, cap * sizeof(modes_frame_eval)));
-        ctx->frames_cap = cap;
+        CK(ctx, ctx->d_frames.ensure(cap * 14));
+        CK(ctx, ctx->d_frame_evals.ensure(cap));
+        CK(ctx, ctx->h_frame_evals.ensure(cap));
     }
     cudaStream_t st = ctx->detect.stream;
-    CK(ctx, cudaMemcpyAsync(ctx->d_frames, frames, n * 14, cudaMemcpyHostToDevice, st));
-    launch_eval_frames(ctx->d_frames, ctx->d_frame_evals, (uint32_t)n, ctx->tab, ctx->cfg.fix_errors, ctx->cfg.aggressive, st);
+    CK(ctx, cudaMemcpyAsync(ctx->d_frames.get(), frames, n * 14, cudaMemcpyHostToDevice, st));
+    launch_eval_frames(ctx->d_frames.get(), ctx->d_frame_evals.get(), (uint32_t)n, ctx->tab, ctx->cfg.fix_errors,
+                       ctx->cfg.aggressive, st);
     ctx->launches++;
-    CK(ctx, cudaMemcpyAsync(ctx->h_frame_evals, ctx->d_frame_evals, n * sizeof(modes_frame_eval), cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaMemcpyAsync(ctx->h_frame_evals.get(), ctx->d_frame_evals.get(), n * sizeof(modes_frame_eval),
+                            cudaMemcpyDeviceToHost, st));
     CK(ctx, wait_stream(st));
     for (size_t i = 0; i < n; i++) {                       // in order: the address cache is sequential
         finish_message(ctx->rs, ctx->h_frame_evals[i], &out[i]);
@@ -1409,7 +1339,7 @@ int modes_device_memset(void *dst_device, int value, size_t nbytes) {
 
 int modes_detect_publish_count(modes_ctx *ctx, void *dst) {
     if (!ctx || !dst) return -1;
-    CK(ctx, cudaMemcpyAsync(dst, ctx->detect.d_counters, 4 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->detect.stream));
+    CK(ctx, cudaMemcpyAsync(dst, ctx->detect.d_counters.get(), 4 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->detect.stream));
     return 0;
 }
 
@@ -1437,7 +1367,12 @@ int modes_get_kernel_times(modes_ctx *ctx, float ms[4]) {
     return 0;
 }
 
-uint64_t modes_launch_count(const modes_ctx *ctx) { return ctx ? ctx->launches : 0; }
+uint64_t modes_launch_count(const modes_ctx *ctx) {
+    if (!ctx) return 0;
+    uint64_t n = ctx->launches;
+    for (const modes_ctx *g : ctx->gpus) n += g->launches;
+    return n;
+}
 
 size_t modes_tile_count(size_t n_buffers) { return tiles_for((uint64_t)n_buffers * kBufSamples); }
 

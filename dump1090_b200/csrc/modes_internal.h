@@ -4,6 +4,8 @@
 #pragma once
 #include <cstddef>
 #include <cstdint>
+#include <cstring>
+#include <vector>
 #include <cuda_runtime.h>
 #include "modes_b200.h"
 
@@ -205,5 +207,33 @@ void deliver_gpu(const modes_delivery *d, size_t n, int64_t buffer_base, Message
 // The order-dependent tail of decodeModesMessage + field decode for one evaluated frame.
 int finish_message(ResolveState &st, const modes_frame_eval &p, modes_message *out);
 void add_recovery_stats(modes_recovery_stats &to, const modes_recovery_stats &from);
+
+// ---- host glue shared by the context (modes_api.cpp) and the receiver pool (modes_pool.cpp) ----
+// The optional measurements and searches of a decode (modes_set_* / modes_pool_set_*).
+struct Features { bool signal = false, arrival = false, levels = false, recover = false, weak = false; };
+
+// Level records not taken yet, oldest first.
+class LevelQueue {
+public:
+    void push(const modes_level &r) { q_.push_back(r); }
+    void clear() { q_.clear(); head_ = 0; }
+    // Moves up to cap of the oldest records to out; out == nullptr: how many are queued.
+    size_t take(modes_level *out, size_t cap) {
+        const size_t queued = q_.size() - head_;
+        if (!out) return queued;
+        const size_t n = cap < queued ? cap : queued;
+        if (n) memcpy(out, q_.data() + head_, n * sizeof(modes_level));
+        head_ += n;
+        if (head_ == q_.size()) clear();
+        else if (head_ >= 4096 && 2 * head_ >= q_.size()) {   // compact when the taken records are half the queue
+            q_.erase(q_.begin(), q_.begin() + (ptrdiff_t)head_);
+            head_ = 0;
+        }
+        return n;
+    }
+private:
+    std::vector<modes_level> q_;
+    size_t head_ = 0;
+};
 
 }  // namespace modes

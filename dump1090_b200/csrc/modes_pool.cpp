@@ -47,8 +47,7 @@ struct Receiver {
     int64_t buffers = 0;                       // buffers of this receiver decoded so far
     int64_t submitted = 0;                     // buffers of this receiver submitted so far
     uint8_t carry[MODES_CARRY_BYTES];
-    std::vector<modes_level> levels;           // level records not taken yet, oldest from level_head on
-    size_t level_head = 0;
+    modes::LevelQueue levels;
 };
 
 // A few persistent helper threads: run(n, f) executes f(0..n-1), f(0) on the calling thread.
@@ -105,11 +104,9 @@ struct modes_pool {
     modes_config cfg;
     std::vector<Receiver> rx;
     size_t max_batch = 0;
-    int signal = 0;                            // modes_pool_set_signal, applied to the slot contexts
-    int arrival = 0;                           // modes_pool_set_arrival, the same
-    int levels = 0;                            // modes_pool_set_levels
-    int recover = 0;                           // modes_pool_set_recovery
-    int weak = 0;                              // modes_pool_set_weak_preambles
+    // signal and arrival are measured by the slot contexts' own passes and reach them at once;
+    // recovery, weak preambles and levels are run by the pool per batch, as they were at submit
+    modes::Features feat;
     std::string err;
     // device half (created on the first modes_pool_submit / _ingest): two batches may be in flight, so
     // that one is uploaded and scanned while the one before it is resolved on the host
@@ -120,9 +117,7 @@ struct modes_pool {
         std::vector<uint32_t> ids;             // the receivers of the batch in flight
         std::vector<int64_t> buf_index;        // with levels: each one's own index of its buffer
         std::vector<modes_level> level_out;
-        bool levels = false;                   // the batch measures its data buffers' levels
-        bool recover = false, signal = false;  // the recovery / signal switches as they were at submit
-        bool weak = false;                     // the batch runs the weak-preamble passes
+        modes::Features feat;                  // the switches as they were at submit
         bool busy = false;
     } slot[2];
     unsigned submitted = 0, collected = 0;     // batches so far: slot = number & 1
@@ -180,6 +175,21 @@ size_t pool_threads() {
     return n;
 }
 
+// The switches a slot context measures itself.
+void share_features(const modes_pool *p, modes_ctx *ctx) {
+    modes_set_signal(ctx, p->feat.signal);
+    modes_set_arrival(ctx, p->feat.arrival);
+}
+
+// One switch of the pool.
+int set_feature(modes_pool *p, bool modes::Features::*f, int on) {
+    if (!p) return -1;
+    p->feat.*f = on != 0;
+    for (modes_pool::Slot &sl : p->slot)
+        if (sl.ctx) share_features(p, sl.ctx);
+    return 0;
+}
+
 int ensure_device(modes_pool *p) {
     if (p->slot[0].ctx) return 0;
     modes_config c = p->cfg;
@@ -188,8 +198,7 @@ int ensure_device(modes_pool *p) {
     for (modes_pool::Slot &sl : p->slot) {
         sl.ctx = modes_create(&c);
         if (!sl.ctx) return fail(p, "%s", modes_last_error(nullptr));
-        modes_set_signal(sl.ctx, p->signal);
-        modes_set_arrival(sl.ctx, p->arrival);
+        share_features(p, sl.ctx);
         sl.d_batch = static_cast<uint8_t *>(modes_device_alloc(bytes));
         sl.h_carry = static_cast<uint8_t *>(modes_host_alloc(p->max_batch * MODES_CARRY_BYTES));
         if (!sl.d_batch || !sl.h_carry) return fail(p, "out of memory for %zu receivers per batch", p->max_batch);
@@ -391,15 +400,13 @@ int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *c
                 return fail(p, "buffer upload failed: %s", cudaGetErrorString(cudaGetLastError()));
     }
     if (modes_detect_device(sl.ctx, sl.d_batch, 2 * n, nullptr, nullptr, 0, nullptr)) return fail(p, "%s", modes_last_error(sl.ctx));
-    sl.recover = p->recover != 0;
-    sl.signal = p->signal != 0;
-    if (sl.recover && modes_recover_device(sl.ctx, nullptr, 0)) return fail(p, "%s", modes_last_error(sl.ctx));
-    sl.weak = sl.recover && p->weak;
+    sl.feat = p->feat;
+    sl.feat.weak &= sl.feat.recover;
+    if (sl.feat.recover && modes_recover_device(sl.ctx, nullptr, 0)) return fail(p, "%s", modes_last_error(sl.ctx));
     // the data buffers only (every second buffer), like the level pass
-    if (sl.weak && modes::weak_device_strided(sl.ctx, nullptr, nullptr, 0, 1, 2)) return fail(p, "%s", modes_last_error(sl.ctx));
+    if (sl.feat.weak && modes::weak_device_strided(sl.ctx, nullptr, nullptr, 0, 1, 2)) return fail(p, "%s", modes_last_error(sl.ctx));
     // the data buffers only (every second buffer), on the same stream: no wait before the collect
-    sl.levels = p->levels != 0;
-    if (sl.levels && modes_levels_device(sl.ctx, sl.d_batch + kBuf, n, 2 * kBuf)) return fail(p, "%s", modes_last_error(sl.ctx));
+    if (sl.feat.levels && modes_levels_device(sl.ctx, sl.d_batch + kBuf, n, 2 * kBuf)) return fail(p, "%s", modes_last_error(sl.ctx));
     sl.buf_index.resize(n);
     for (size_t i = 0; i < n; i++) sl.buf_index[i] = p->rx[receivers[i]].submitted++;
     // what each receiver carries into its next buffer (dump1090.c:481)
@@ -421,30 +428,30 @@ int modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user) {
     p->cands.resize(n_cand ? n_cand : 1);
     p->tiles.resize(modes_tile_count(2 * n));
     if (modes_detect_fetch(sl.ctx, p->cands.data(), p->tiles.data())) return fail(p, "%s", modes_last_error(sl.ctx));
-    if (sl.recover) {
+    if (sl.feat.recover) {
         p->recovered.resize(n_cand ? n_cand : 1);
         if (modes_recover_fetch(sl.ctx, p->recovered.data())) return fail(p, "%s", modes_last_error(sl.ctx));
     }
     uint64_t n_weak = 0;
-    if (sl.weak) {
+    if (sl.feat.weak) {
         if (modes_weak_fetch(sl.ctx, nullptr, nullptr, &n_weak)) return fail(p, "%s", modes_last_error(sl.ctx));
         p->weak_t.resize(n_weak ? n_weak : 1);
         p->weak_rec.resize(n_weak ? n_weak : 1);
         if (modes_weak_fetch(sl.ctx, p->weak_t.data(), p->weak_rec.data(), &n_weak)) return fail(p, "%s", modes_last_error(sl.ctx));
     }
-    if (sl.levels) {
+    if (sl.feat.levels) {
         sl.level_out.resize(n);
         if (modes_levels_fetch(sl.ctx, sl.level_out.data())) return fail(p, "%s", modes_last_error(sl.ctx));
         for (size_t i = 0; i < n; i++) {
             modes_level r = sl.level_out[i];
             r.buffer = sl.buf_index[i];
-            p->rx[sl.ids[i]].levels.push_back(r);
+            p->rx[sl.ids[i]].levels.push(r);
         }
     }
     sl.busy = false;
     p->collected++;
-    return pool_resolve(p, sl.ids.data(), n, p->cands.data(), sl.recover ? p->recovered.data() : nullptr, sl.signal, p->tiles.data(),
-                        sink, user, p->weak_t.data(), p->weak_rec.data(), (size_t)n_weak);
+    return pool_resolve(p, sl.ids.data(), n, p->cands.data(), sl.feat.recover ? p->recovered.data() : nullptr, sl.feat.signal,
+                        p->tiles.data(), sink, user, p->weak_t.data(), p->weak_rec.data(), (size_t)n_weak);
 }
 
 int modes_pool_ingest(modes_pool *p, const uint32_t *receivers, const uint8_t *const *iq, size_t n,
@@ -467,7 +474,6 @@ int modes_pool_reset(modes_pool *p, uint32_t receiver) {
     r.buffers = 0;
     r.submitted = 0;
     r.levels.clear();
-    r.level_head = 0;
     memset(r.carry, 127, sizeof r.carry);
     return modes_resolver_reset(r.res);
 }
@@ -480,64 +486,29 @@ int modes_pool_set_output(modes_pool *p, modes_message *out, uint32_t *receiver_
 
 size_t modes_pool_output_count(const modes_pool *p) { return p ? p->out_count : 0; }
 
-int modes_pool_set_arrival(modes_pool *p, int on) {
-    if (!p) return -1;
-    p->arrival = on != 0;
-    for (modes_pool::Slot &sl : p->slot)
-        if (sl.ctx) modes_set_arrival(sl.ctx, p->arrival);
-    return 0;
-}
+int modes_pool_set_arrival(modes_pool *p, int on) { return set_feature(p, &modes::Features::arrival, on); }
 
-int modes_pool_set_signal(modes_pool *p, int on) {
-    if (!p) return -1;
-    p->signal = on != 0;
-    for (modes_pool::Slot &sl : p->slot)
-        if (sl.ctx) modes_set_signal(sl.ctx, p->signal);
-    return 0;
-}
+int modes_pool_set_signal(modes_pool *p, int on) { return set_feature(p, &modes::Features::signal, on); }
 
-int modes_pool_set_recovery(modes_pool *p, int on) {
-    if (!p) return -1;
-    p->recover = on != 0;
-    return 0;
-}
+int modes_pool_set_recovery(modes_pool *p, int on) { return set_feature(p, &modes::Features::recover, on); }
 
 int modes_pool_recovery_stats(const modes_pool *p, uint32_t receiver, modes_recovery_stats *out) {
     if (!p || receiver >= p->rx.size() || !out) return -1;
     return modes_resolver_recovery_stats(p->rx[receiver].res, out);
 }
 
-int modes_pool_set_weak_preambles(modes_pool *p, int on) {
-    if (!p) return -1;
-    p->weak = on != 0;
-    return 0;
-}
+int modes_pool_set_weak_preambles(modes_pool *p, int on) { return set_feature(p, &modes::Features::weak, on); }
 
 int modes_pool_weak_stats(const modes_pool *p, uint32_t receiver, modes_recovery_stats *out) {
     if (!p || receiver >= p->rx.size() || !out) return -1;
     return modes_resolver_weak_stats(p->rx[receiver].res, out);
 }
 
-int modes_pool_set_levels(modes_pool *p, int on) {
-    if (!p) return -1;
-    p->levels = on != 0;
-    return 0;
-}
+int modes_pool_set_levels(modes_pool *p, int on) { return set_feature(p, &modes::Features::levels, on); }
 
 size_t modes_pool_take_levels(modes_pool *p, uint32_t receiver, modes_level *out, size_t cap) {
     if (!p || receiver >= p->rx.size()) return 0;
-    Receiver &r = p->rx[receiver];
-    const size_t queued = r.levels.size() - r.level_head;
-    if (!out) return queued;
-    const size_t n = cap < queued ? cap : queued;
-    if (n) memcpy(out, r.levels.data() + r.level_head, n * sizeof(modes_level));
-    r.level_head += n;
-    if (r.level_head == r.levels.size()) { r.levels.clear(); r.level_head = 0; }
-    else if (r.level_head >= 4096 && 2 * r.level_head >= r.levels.size()) {
-        r.levels.erase(r.levels.begin(), r.levels.begin() + (ptrdiff_t)r.level_head);
-        r.level_head = 0;
-    }
-    return n;
+    return p->rx[receiver].levels.take(out, cap);
 }
 
 int64_t modes_pool_buffers(const modes_pool *p, uint32_t receiver) {
