@@ -18,8 +18,13 @@
 //  * The next chunk's windows are copied while the current chunk's verdicts (mask assembly, CRC,
 //    repair) are worked out: the rows are free as soon as every lane has finished its walk, and
 //    the verdicts leave straight from registers.  Chunks of 32 candidates are handed out from a
-//    global counter three ahead: chunk i+2's positions are loaded, its preamble words copied and
-//    its windows prefetched into L2 while chunk i is walked.
+//    global counter three ahead: chunk i+2's positions are loaded and its preamble words copied
+//    while chunk i is walked.  The windows themselves are not prefetched into L2 (see look_ahead).
+//  * Copying each block's slots of the next chunk into the rows as soon as every lane has walked
+//    that block of the current one (a rolling refill: each copy gets three blocks of walk and the
+//    verdicts to land) measured slower on an H100: 0.294 ms against 0.231 ms, both without the L2
+//    prefetch.  Our reading, not profiled: the copies then run beside the walk's shared-memory
+//    loads, and four times as many shuffles hand the row positions round.
 //  * MODES_EVAL_VARIANT=fused2 stages half a window at a time into the same rows (57 slots, then
 //    the other 57, slot 56 twice): 8.4 KB per warp instead of 15.6, 16 warps per SM instead of 12.
 //    The second half's copy is exposed (it cannot start before all lanes finished the first half);
@@ -185,7 +190,7 @@ eval_fused_kernel(BatchView in, DeviceTables tab, const uint32_t *__restrict__ c
 
     // Chunks of 32 candidates are handed out from a global counter, requested three chunks ahead:
     // while chunk i is evaluated, chunk i+1's first part is staged (behind the verdicts of chunk i),
-    // chunk i+2's positions are loaded, its preamble words copied and its windows prefetched into L2.
+    // chunk i+2's positions are loaded and its preamble words copied.
     // (The counter values are used untouched until a chunk later: arithmetic on them right away
     // would wait for the atomic's round trip.)
     auto positions = [&](uint32_t c) -> uint32_t {
@@ -193,17 +198,14 @@ eval_fused_kernel(BatchView in, DeviceTables tab, const uint32_t *__restrict__ c
         const uint32_t nc = n_cand - c * 32 < 32u ? n_cand - c * 32 : 32u;   // idle lanes of the last chunk duplicate its last candidate
         return cand_v[c * 32 + ((uint32_t)lane < nc ? lane : nc - 1)];
     };
-    auto look_ahead = [&](uint32_t c, uint32_t v) {      // chunk c (positions v): preamble words -> preamble area, windows -> L2
+    // Chunk c (positions v): preamble words -> preamble area.  Its windows are not prefetched into
+    // L2: on an H100 (400 W) a prefetch of chunk i+2's windows (five lines per lane) made the kernel
+    // 0.292 ms against 0.231 ms without, and a prefetch of chunk i+1's at the top of walk i 0.254 ms
+    // (scripts/eval_time.py, DESIGN §6).  The prefetch reads five whole 128-byte lines per 484-byte
+    // window, and its lines wait a chunk in L2 for their copy.
+    auto look_ahead = [&](uint32_t c, uint32_t v) {
         if (c >= n_chunks) return;
         prestage(in, body32, v, pre, pre_s);
-        if (v > (uint32_t)kHaloSamples) {
-            // 484 bytes from a 4-byte aligned address: five 128-byte lines
-            const uint8_t *wp = in.body + 4ull * ((v - 1 - kHaloSamples) >> 1);
-            if ((uint64_t)(wp - in.body) + 640u <= 2ull * in.n_samples) {
-#pragma unroll
-                for (int k = 0; k < 5; k++) asm volatile("prefetch.global.L2 [%0];" ::"l"(wp + 128 * k));
-            }
-        }
     };
     // this lane's walk of the chunk whose preamble words are in the preamble area, and the chunk's first part on its way
     auto setup_and_stage = [&](uint32_t v, fz::Lane &L, uint32_t &rev_mask, bool &fast) {
@@ -298,8 +300,8 @@ void launch_fused(const BatchView &in, const DeviceTables &tab, const ScanOutput
 
 void launch_eval_fused(const BatchView &in, const DeviceTables &tab, const ScanOutputs &scan, modes_candidate *records,
                        int fix_errors, int aggressive, int sm_count, int parts, cudaStream_t stream) {
-    // measured on an H100 (400 W) over the bench's 845 458 candidates: whole windows, 12 warps per SM 0.293 ms;
-    // half windows, 16 warps 0.321 ms
+    // measured on an H100 (400 W) over the bench's 845 458 candidates: whole windows, 12 warps per SM 0.231 ms
+    // (0.292 ms with the L2 prefetch); half windows, 16 warps 0.238 ms (0.320 ms)
     if (parts == 2) launch_fused<2, 16>(in, tab, scan, records, fix_errors, aggressive, sm_count, stream);
     else launch_fused<4, 12>(in, tab, scan, records, fix_errors, aggressive, sm_count, stream);
 }
