@@ -84,15 +84,6 @@ __device__ __forceinline__ void load_row(const BatchView &in, const TileSrc &t, 
     }
 }
 
-// Ask L2 for rows r, r+1 of a tile (4 KB) with one bulk-prefetch instruction.  Issued four rows ahead
-// (a few microseconds: prefetched further ahead, lines were evicted again before their use and
-// DRAM traffic went up by 70 %), it turns the row load's DRAM latency into an L2 hit, which the
-// one-row-ahead register reload covers.
-constexpr int kPrefetchRows = 4;                         // = two steps of two rows
-__device__ __forceinline__ void prefetch_rows2_l2(const TileSrc &t, int r) {
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(t.flat + kRowStrideChunks * r), "r"(16 * kRowStrideChunks + 2048) : "memory");
-}
-
 // Squared magnitude of one sample (I in byte 0, Q in byte 1, upper bytes zero: they come out of
 // the byte-wise |x - 127| as 127 each, which the dot product's addend takes off again).
 __device__ __forceinline__ uint32_t n_of(uint32_t iq16) {
@@ -231,7 +222,9 @@ __device__ __noinline__ void dense_tile(const uint8_t *body, const uint8_t *halo
     __syncwarp();
 }
 
-__global__ void __launch_bounds__(32, 16)
+// 12 warps per SM (3 per scheduler) at up to 168 registers: the kernel needs about 160 and then has no
+// spill.  On the H100 that is faster than 16 warps at the 128-register cap with a spill (DESIGN §6).
+__global__ void __launch_bounds__(32, 12)
 scan_kernel(BatchView in, const uint16_t *__restrict__ lutn, ScanOutputs out, uint32_t n_tiles, uint32_t one,
              uint32_t minus_one, uint32_t c65536) {
     __shared__ __align__(16) uint32_t s_mask[kRows * 32];
@@ -295,10 +288,6 @@ scan_kernel(BatchView in, const uint16_t *__restrict__ lutn, ScanOutputs out, ui
             else if (g_next < n_tiles) load_row(in, ts, 0, lane, n_vchunks, x);
             if (r + 2 < kRows) load_row(in, ts_cur, r + 3, lane, n_vchunks, x + 4);
             else if (g_next < n_tiles) load_row(in, ts, 1, lane, n_vchunks, x + 4);
-            if (lane == 0) {
-                if (r + kPrefetchRows < kRows) { if (ts_cur.interior) prefetch_rows2_l2(ts_cur, r + kPrefetchRows); }
-                else if (g_next < n_tiles && ts.interior) prefetch_rows2_l2(ts, r + kPrefetchRows - kRows);
-            }
 #pragma unroll
             for (int k = 0; k < scan2::kPairLook; k++) X[32 + k] = __shfl_down_sync(0xffffffffu, X[k], 1);
             uint32_t ma, mb;
@@ -467,7 +456,7 @@ void launch_scan(const BatchView &in, const DeviceTables &tab, const ScanOutputs
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
     if (!ctas_per_sm[dev]) {
         int n = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, scan_kernel, 32, 0) != cudaSuccess || n < 1) n = 16;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, scan_kernel, 32, 0) != cudaSuccess || n < 1) n = 12;
         ctas_per_sm[dev] = n;
     }
     const uint32_t n_tiles = tiles_for(in.n_samples);

@@ -1,5 +1,5 @@
-"""Device time of the frame-evaluation kernel (K2) over the 1 GiB bench workload, for one or more builds of
-the library in alternation, and the DRAM floor of the kernel.
+"""Device time of the scan (K1) and frame-evaluation (K2) kernels over the 1 GiB bench workload, for one or
+more builds of the library in alternation, and the floors of both kernels.
 
     python scripts/eval_time.py [--workload tiled_nofix|df17_aggressive] [NAME=path/to/libmodes_b200.so ...]
 
@@ -11,7 +11,8 @@ candidate records are identical to the first build's.
 
 The DRAM floor: the distinct 32-byte sectors of all candidate windows (the 121 words the kernel reads
 per candidate, samples -1 .. 240 rounded out to whole words) and the 56-byte records it writes, over
-the rate of a device-to-device copy (read + write) measured in the same run.  The card's name, power
+the rate of a device-to-device copy (read + write) measured in the same run.  The scan's read floor: one
+read-only pass over the same GiB (a sum of it as int64), timed in the same run.  The card's name, power
 limit and median SM clock under the timed steps are read in the same run."""
 import argparse
 import hashlib
@@ -77,8 +78,20 @@ def worker(lib_path: str, workload: str) -> None:
                 if k:
                     rates.append(2 * d.numel() / (a.elapsed_time(b) * 1e-3) / 1e12)
             del dst
+            # read-only pass over the GiB (K1's floor: it reads every byte once and writes almost nothing)
+            words = d.view(torch.int64)
+            reads = []
+            for k in range(11):
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record()
+                words.sum()
+                b.record()
+                b.synchronize()
+                if k:
+                    reads.append(a.elapsed_time(b))
             reply({"cands": int(v.size), "in_carry": int(v.size - body.size), "window_bytes": int(sectors.size) * 32,
-                   "record_bytes": int(v.size) * 56, "copy_tbs": statistics.median(rates)})
+                   "record_bytes": int(v.size) * 56, "copy_tbs": statistics.median(rates),
+                   "read_ms": reads, "read_bytes": d.numel()})
         elif cmd == "quit":
             break
 
@@ -166,6 +179,11 @@ def main() -> None:
           f"distinct window sectors {fl['window_bytes'] / 1e9:.4f} GB + records {fl['record_bytes'] / 1e9:.4f} GB; "
           f"device-to-device copy {fl['copy_tbs']:.2f} TB/s (read + write) -> windows {floor_ms:.4f} ms, "
           f"with records {floor_ms + rec_ms:.4f} ms")
+    read_ms = statistics.median(fl["read_ms"])
+    print(f"read floor of scan: one read-only pass over the GiB (sum as int64) {spread(fl['read_ms'])}, "
+          f"{fl['read_bytes'] / (read_ms * 1e-3) / 1e12:.2f} TB/s")
+    for w in workers:
+        print(f"  {w.name:>12}: scan median {statistics.median(times[w.name]['scan']) / read_ms:.2f}x the read floor")
 
 
 if __name__ == "__main__":
