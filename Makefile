@@ -65,7 +65,7 @@ tests/_build/libeval_serial_host.so: tests/host_shim/eval_serial_host.cpp $(CSRC
 # test infrastructure: device harness over the product's own kernel objects (recovery and signal
 # passes on constructed corpora, and the exhaustive sweeps of the core headers' device build)
 DSHIM_OBJS := build/modes_recover.o build/modes_signal.o build/modes_levels.o build/modes_tables.o
-dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so
+dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so tests/_build/libscan_eval_device.so
 tests/_build/libkernels_device.so: tests/device_shim/kernels_device.cu $(DSHIM_OBJS) $(CSRC)/modes_internal.h $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_levels_core.cuh include/modes_b200.h
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/kernels_device.cu -o tests/_build/kernels_device.o
@@ -75,6 +75,12 @@ tests/_build/libarrival_device.so: tests/device_shim/arrival_device.cu build/mod
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/arrival_device.cu -o tests/_build/arrival_device.o
 	$(NVCC) $(ARCH) -shared -o $@ tests/_build/arrival_device.o build/modes_signal.o build/modes_tables.o -cudart static
+# the scan, frame-evaluation and weak-preamble kernels with a chosen SM count (tests/test_persistent_kernels.py)
+SCAN_EVAL_OBJS := build/modes_scan2.o build/modes_eval_fused.o build/modes_kernels.o build/modes_weak.o build/modes_tables.o
+tests/_build/libscan_eval_device.so: tests/device_shim/scan_eval_device.cu $(SCAN_EVAL_OBJS) $(CSRC)/modes_internal.h include/modes_b200.h
+	@mkdir -p tests/_build
+	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/scan_eval_device.cu -o tests/_build/scan_eval_device.o
+	$(NVCC) $(ARCH) -shared -o $@ tests/_build/scan_eval_device.o $(SCAN_EVAL_OBJS) -cudart static
 
 clean:
 	rm -rf build tests/_build $(LIB) dump1090-b200
