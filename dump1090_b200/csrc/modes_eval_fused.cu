@@ -26,7 +26,7 @@
 //    prefetch.  Our reading, not profiled: the copies then run beside the walk's shared-memory
 //    loads, and four times as many shuffles hand the row positions round.
 //  * MODES_EVAL_VARIANT=fused2 stages half a window at a time into the same rows (57 slots, then
-//    the other 57, slot 56 twice): 8.4 KB per warp instead of 15.6, 16 warps per SM instead of 12.
+//    the other 57, slot 56 twice): 8.4 KB per warp instead of 15.6, 16 warps per SM instead of at most 12.
 //    The second half's copy is exposed (it cannot start before all lanes finished the first half);
 //    measured slightly slower than whole windows (0.170 against 0.166 ms).
 #include <cstdint>
@@ -47,7 +47,8 @@ static_assert(serial::kIqLutStride == kLutIqStride && serial::kIqLutEntries % 8 
 static_assert(kTableWords % 2 == 0, "record staging uses 8-byte stores");
 
 // kFirst = blocks of the walk (of 4) whose slots are staged first; the rest follows into the same
-// rows once every lane is through them.  4: the whole walk (113 slots) at once, 12 warps per SM;
+// rows once every lane is through them.  4: the whole walk (113 slots) at once, 8 warps per SM
+// (up to 12 fit);
 // 3: 85 slots, then 29 (16 warps); 2: two halves of 57 (slot 56 twice: a part starts with the word
 // its first pair begins in).
 template <int kFirst, int kWarpsPerSm> struct Geom {
@@ -301,9 +302,14 @@ void launch_fused(const BatchView &in, const DeviceTables &tab, const ScanOutput
 void launch_eval_fused(const BatchView &in, const DeviceTables &tab, const ScanOutputs &scan, modes_candidate *records,
                        int fix_errors, int aggressive, int sm_count, int parts, cudaStream_t stream) {
     // measured on an H100 (400 W) over the bench's 845 458 candidates: whole windows, 12 warps per SM 0.231 ms
-    // (0.292 ms with the L2 prefetch); half windows, 16 warps 0.238 ms (0.320 ms)
+    // (0.292 ms with the L2 prefetch); half windows, 16 warps 0.238 ms (0.320 ms).
+    // Whole windows by warps per SM on an H100 (700 W), same candidates: 4: 0.227 ms, 6: 0.206, 7: 0.205,
+    // 8: 0.195, 9: 0.203, 10: 0.202, 11: 0.218, 12: 0.216 (DESIGN §6), the same records.  Our reading,
+    // not profiled: the times follow the L1 that the shared-memory carve-out leaves (92 KB at 7-8 warps,
+    // 60 KB at 9-10, 28 KB at 11-12; the copies are cp.async.ca, through L1), and below 8 warps fewer
+    // copies are in flight.
     if (parts == 2) launch_fused<2, 16>(in, tab, scan, records, fix_errors, aggressive, sm_count, stream);
-    else launch_fused<4, 12>(in, tab, scan, records, fix_errors, aggressive, sm_count, stream);
+    else launch_fused<4, 8>(in, tab, scan, records, fix_errors, aggressive, sm_count, stream);
 }
 
 }  // namespace modes
