@@ -193,7 +193,17 @@ EXPORTS = ["modes_abi_version", "modes_default_config", "modes_create", "modes_d
            "modes_resolver_run_recovered", "modes_resolver_run_shards_recovered", "modes_resolver_recovery_stats", "modes_pool_set_recovery",
            "modes_pool_recovery_stats", "modes_set_weak_preambles", "modes_get_weak_recovery_stats", "modes_weak_device",
            "modes_weak_fetch", "modes_resolver_run_weak", "modes_resolver_run_shards_weak", "modes_resolver_weak_stats",
-           "modes_pool_set_weak_preambles", "modes_pool_weak_stats", "modes_set_arrival", "modes_pool_set_arrival"]
+           "modes_pool_set_weak_preambles", "modes_pool_weak_stats", "modes_set_arrival", "modes_pool_set_arrival",
+           "modes_set_input_rate", "modes_resample_device"]
+
+INPUT_RATES = (2_000_000, 2_400_000)      # modes_set_input_rate
+
+
+def resampled_samples(n_input_bytes: int) -> int:
+    """2 MHz samples of a 2.4 MS/s stream of n_input_bytes bytes: N_out = ceil(5 n_in / 6) with
+    n_in = ceil(bytes / 2) (modes_set_input_rate)."""
+    n_in = (int(n_input_bytes) + 1) // 2
+    return (5 * n_in + 5) // 6
 
 
 def lib():
@@ -321,6 +331,9 @@ def lib():
         L.modes_resolver_weak_stats.argtypes = [C.c_void_p, C.POINTER(RecoveryStats)]
         L.modes_pool_set_weak_preambles.argtypes = [C.c_void_p, C.c_int]
         L.modes_pool_weak_stats.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(RecoveryStats)]
+        L.modes_set_input_rate.argtypes = [C.c_void_p, C.c_uint32]
+        L.modes_resample_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int64, C.c_int64, C.c_size_t,
+                                            C.c_int64, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -399,14 +412,20 @@ class Decoder:
     Message.recovered: recovery_stats().  weak_preambles=True (with recover=True) also searches the weak
     preambles the reference's preamble test rejects (modes_set_weak_preambles): Message.recovered = 2,
     weak_recovery_stats().  arrival=True measures every decoded frame's arrival time to a sixth of a
-    sample on the GPU (modes_set_arrival): Message.arrival, timestamp_12mhz(), beast()."""
+    sample on the GPU (modes_set_arrival): Message.arrival, timestamp_12mhz(), beast().
+    input_rate=2_400_000 takes 2.4 MS/s bytes (what dump1090-fa and readsb record) and resamples them
+    to 2 MHz on the GPU before the pipeline (modes_set_input_rate): the messages are exactly the 2 MHz
+    decoder's on the resampled bytes.  Message.sample_pos still counts 2 MHz samples, and
+    6 * sample_pos is the input time in 12 MHz ticks at either rate."""
 
     def __init__(self, signal: bool = False, levels: bool = False, recover: bool = False, weak_preambles: bool = False,
-                 arrival: bool = False, **cfg):
+                 arrival: bool = False, input_rate: int = 2_000_000, **cfg):
         self.cfg = make_config(**cfg)
         self._h = lib().modes_create(C.byref(self.cfg))
         if not self._h:
             raise RuntimeError("modes_create failed: " + lib().modes_last_error(None).decode())
+        if input_rate != 2_000_000:
+            self.set_input_rate(input_rate)
         if signal:
             self.set_signal(True)
         if arrival:
@@ -497,6 +516,12 @@ class Decoder:
     def set_signal(self, on: bool) -> None:
         """Measure the signal level for batches submitted from now on (modes_set_signal)."""
         self._check(lib().modes_set_signal(self._h, int(bool(on))))
+
+    def set_input_rate(self, hz: int) -> None:
+        """The sample rate of the stream that begins at the next reset (decode() resets): 2_000_000 or
+        2_400_000 (modes_set_input_rate); refused while a stream is in progress.  sample_pos counts 2 MHz
+        samples at either rate, and 6 * sample_pos is the input time in 12 MHz ticks."""
+        self._check(lib().modes_set_input_rate(self._h, int(hz)))
 
     def set_arrival(self, on: bool) -> None:
         """Measure the arrival time for batches submitted from now on (modes_set_arrival)."""
@@ -608,6 +633,18 @@ class Decoder:
         out = (Message * n)()
         self._check(lib().modes_decode_frames(self._h, buf, n, out))
         return [out[i] for i in range(n)]
+
+    def resample_device(self, d_in_ptr: int, in_bytes: int, in_first_sample: int, first_buffer: int, n_buffers: int,
+                        d_out_ptr: int, out_end: int = -1, want_carry: bool = True) -> bytes | None:
+        """2 MHz reference buffers first_buffer ... of a 2.4 MS/s stream, from in_bytes of its input (input
+        sample in_first_sample on) in device memory, into device memory at d_out_ptr (modes_resample_device).
+        Output samples at or past out_end are 127 (negative: no limit).  Returns the CARRY_BYTES 2 MHz
+        bytes before the first buffer (for detect_device), or None with want_carry=False (then nothing waits)."""
+        carry = (C.c_uint8 * CARRY_BYTES)() if want_carry else None
+        self._check(lib().modes_resample_device(self._h, C.c_void_p(d_in_ptr or None), int(in_bytes), int(in_first_sample),
+                                                int(first_buffer), int(n_buffers), int(out_end), C.c_void_p(d_out_ptr),
+                                                carry))
+        return bytes(carry) if want_carry else None
 
     def levels_device(self, d_iq_ptr: int, n_buffers: int, stride_bytes: int = 0) -> None:
         """Level records of n_buffers buffers in device memory, buffer k at d_iq_ptr + k * stride_bytes."""

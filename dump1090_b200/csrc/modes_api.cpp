@@ -14,6 +14,7 @@
 #include <string>
 #include <vector>
 #include "modes_internal.h"
+#include "modes_resample_core.cuh"
 
 using namespace modes;
 
@@ -68,6 +69,7 @@ struct Slot {
     cudaStream_t stream = nullptr;
     DevBuf<uint8_t> d_iq;
     DevBuf<uint8_t> d_halo;
+    DevBuf<uint8_t> d_in;             // 2.4 MS/s input: the input bytes the batch's resampling reads
     DevBuf<uint32_t> d_cand_v;       // its capacity is the slot's candidate capacity
     DevBuf<modes_candidate> d_records;
     DevBuf<modes_tile> d_tiles;
@@ -157,6 +159,17 @@ struct modes_ctx {
     uint8_t carry[MODES_CARRY_BYTES];
     int64_t buffers_done = 0;
     bool finished = false;
+    bool started = false;                 // modes_process or modes_finish since create / reset
+    // modes_set_input_rate: at 2.4 MS/s each batch is resampled to 2 MHz on the device (K9) from the
+    // stream's input bytes; the 2 MHz bytes never exist on the host.  hold keeps the stream bytes
+    // [hold0, in_total) that later batches read (the filter's history and a buffer not yet complete).
+    uint32_t input_rate = 2000000;
+    int64_t in_total = 0;
+    PinnedBuf<uint8_t> hold;
+    int64_t hold0 = 0;
+    // modes_resample_device: the carry block (device, pinned host copy)
+    DevBuf<uint8_t> d_rs_halo;
+    PinnedBuf<uint8_t> h_rs_halo;
     ResolveState rs;
     ResolveScratch *scratch = nullptr;
     MessageOut out;                       // modes_set_sink / modes_set_output
@@ -302,9 +315,11 @@ int gpu_resolve_ensure(modes_ctx *ctx, Slot &s, GpuResolve &g) {
     return 0;
 }
 
-// Queue one batch on the slot's stream: (optional H2D) + halo + scan + frame evaluation.
+// Queue one batch on the slot's stream: (optional H2D) + halo + scan + frame evaluation.  halo_on_device:
+// the slot's carry block is already queued on the stream (the resampler writes it), so carry476 is unused.
 int submit(modes_ctx *ctx, Slot &s, const uint8_t *host_iq, const void *d_iq, size_t n_buffers,
-           const uint8_t *carry476, modes_candidate *d_records_ext, uint32_t cap_ext, modes_tile *d_tiles_ext) {
+           const uint8_t *carry476, modes_candidate *d_records_ext, uint32_t cap_ext, modes_tile *d_tiles_ext,
+           bool halo_on_device = false) {
     const uint64_t n_samples = (uint64_t)n_buffers * kBufSamples;
     if (n_samples + kHaloSamples >= (1ull << 32)) return fail(ctx, "batch too large: %zu buffers", n_buffers);
     // caller-supplied record buffers: the slot's own position list must hold as many candidates
@@ -326,13 +341,15 @@ int submit(modes_ctx *ctx, Slot &s, const uint8_t *host_iq, const void *d_iq, si
         d_iq = s.d_iq.get();
     }
     if ((reinterpret_cast<uintptr_t>(d_iq) & 15) != 0) return fail(ctx, "device I/Q pointer must be 16-byte aligned");
-    const unsigned hi = s.halo_next++ % Slot::kHaloRing;
-    uint8_t *h_halo = s.h_halo.get() + (size_t)hi * kHaloAlloc;
-    CK(ctx, cudaEventSynchronize(s.halo_ev[hi]));                         // its previous copy (8 submits ago) has left the host
-    memset(h_halo, 127, kHaloAlloc);                                      // dump1090.c:344 no-signal
-    if (carry476) memcpy(h_halo + (kHaloBytes - MODES_CARRY_BYTES), carry476, MODES_CARRY_BYTES);
-    CK(ctx, cudaMemcpyAsync(s.d_halo.get(), h_halo, kHaloAlloc, cudaMemcpyHostToDevice, s.stream));
-    CK(ctx, cudaEventRecord(s.halo_ev[hi], s.stream));
+    if (!halo_on_device) {
+        const unsigned hi = s.halo_next++ % Slot::kHaloRing;
+        uint8_t *h_halo = s.h_halo.get() + (size_t)hi * kHaloAlloc;
+        CK(ctx, cudaEventSynchronize(s.halo_ev[hi]));                     // its previous copy (8 submits ago) has left the host
+        memset(h_halo, 127, kHaloAlloc);                                  // dump1090.c:344 no-signal
+        if (carry476) memcpy(h_halo + (kHaloBytes - MODES_CARRY_BYTES), carry476, MODES_CARRY_BYTES);
+        CK(ctx, cudaMemcpyAsync(s.d_halo.get(), h_halo, kHaloAlloc, cudaMemcpyHostToDevice, s.stream));
+        CK(ctx, cudaEventRecord(s.halo_ev[hi], s.stream));
+    }
     s.batch_iq = d_iq;
     s.n_buffers = n_buffers;
     s.own_outputs = d_records_ext == nullptr;
@@ -602,9 +619,65 @@ int collect_group(modes_ctx *ctx, int parity) {
     return 0;
 }
 
+// Where the batches of a run read their input.  2 MHz: the run's whole reference buffers at iq.
+// 2.4 MS/s (iq == nullptr): the stream's input bytes [hold0, call0) at hold and [call0, end) at call;
+// every later byte is no signal, and output samples at or past out_end are the EOF buffer's padding.
+struct Source {
+    const uint8_t *iq = nullptr;
+    const uint8_t *hold = nullptr;
+    int64_t hold0 = 0;
+    const uint8_t *call = nullptr;
+    int64_t call0 = 0, end = 0;
+    int64_t out_end = INT64_MAX;
+};
+
+// 2.4 MS/s: upload the input bytes the slot's batch (nb buffers from s.buffer_base, and the carry before
+// them) reads, straight from where they are, and resample them into the slot's body and carry block.
+int stage_resampled(modes_ctx *ctx, Slot &s, const Source &src, size_t nb) {
+    const int64_t o0 = s.buffer_base * (int64_t)kBufSamples;
+    const int64_t o1 = o0 + (int64_t)nb * kBufSamples;
+    int64_t lo = 2 * resample::in_lo(o0 - MODES_CARRY_BYTES / 2);
+    int64_t hi = 2 * resample::in_hi(o1 - 1);
+    if (lo < 0) lo = 0;
+    if (hi > src.end) hi = src.end;
+    if (hi < lo) hi = lo;
+    if (lo < src.hold0) return fail(ctx, "internal: input history starts at byte %lld, batch reads from %lld",
+                                    (long long)src.hold0, (long long)lo);
+    CK(ctx, s.d_iq.ensure((size_t)(o1 - o0) * 2));
+    CK(ctx, s.d_in.ensure((size_t)(hi - lo) + 16));
+    if (lo < src.call0) {
+        const int64_t n = (hi < src.call0 ? hi : src.call0) - lo;
+        if (n) CK(ctx, cudaMemcpyAsync(s.d_in.get(), src.hold + (lo - src.hold0), (size_t)n, cudaMemcpyHostToDevice, s.stream));
+    }
+    if (hi > src.call0) {
+        const int64_t from = lo > src.call0 ? lo : src.call0;
+        CK(ctx, cudaMemcpyAsync(s.d_in.get() + (from - lo), src.call + (from - src.call0), (size_t)(hi - from),
+                                cudaMemcpyHostToDevice, s.stream));
+    }
+    launch_resample(ResampleJob{s.d_in.get(), (uint64_t)(hi - lo), lo / 2, o0, (uint64_t)(o1 - o0), src.out_end,
+                                s.d_iq.get(), s.d_halo.get()},
+                    s.stream);
+    CK(ctx, cudaGetLastError());
+    ctx->launches++;
+    return 0;
+}
+
+// Queue the run's next nb buffers (from s.buffer_base) on slot s of context g, whose run ctx leads (g is
+// ctx itself, or one of its GPUs), and move src past them.
+int submit_next(modes_ctx *ctx, modes_ctx *g, Slot &s, Source &src, size_t nb) {
+    if (!src.iq) {
+        if (stage_resampled(g, s, src, nb)) return -1;
+        return submit(g, s, nullptr, s.d_iq.get(), nb, nullptr, nullptr, 0, nullptr, true);
+    }
+    if (submit(g, s, src.iq, nullptr, nb, ctx->carry, nullptr, 0, nullptr)) return -1;
+    memcpy(ctx->carry, src.iq + nb * MODES_BUFFER_BYTES - MODES_CARRY_BYTES, MODES_CARRY_BYTES);
+    src.iq += nb * MODES_BUFFER_BYTES;
+    return 0;
+}
+
 // Multi-GPU streaming decode: batches of whole buffers dealt round-robin to the GPUs, one group of
 // gpus.size() batches in flight per slot parity; group g-1 is resolved while group g uploads and runs.
-int run_buffers_multi(modes_ctx *ctx, const uint8_t *host_iq, size_t n_buffers) {
+int run_buffers_multi(modes_ctx *ctx, Source src, size_t n_buffers) {
     size_t max_b = (size_t)(ctx->cfg.max_batch_bytes / MODES_BUFFER_BYTES);
     if (max_b < 1) max_b = 1;
     int cur = 0;
@@ -619,10 +692,8 @@ int run_buffers_multi(modes_ctx *ctx, const uint8_t *host_iq, size_t n_buffers) 
             Slot &s = g->slot[cur];
             CK(ctx, cudaSetDevice(g->cfg.device));
             s.buffer_base = ctx->buffers_done;
-            if (submit(g, s, host_iq, nullptr, nb, ctx->carry, nullptr, 0, nullptr)) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
-            memcpy(ctx->carry, host_iq + nb * MODES_BUFFER_BYTES - MODES_CARRY_BYTES, MODES_CARRY_BYTES);
+            if (submit_next(ctx, g, s, src, nb)) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
             ctx->buffers_done += (int64_t)nb;
-            host_iq += nb * MODES_BUFFER_BYTES;
             n_buffers -= nb;
         }
         ctx->group_n[cur] = k;
@@ -634,9 +705,9 @@ int run_buffers_multi(modes_ctx *ctx, const uint8_t *host_iq, size_t n_buffers) 
     return cudaSetDevice(ctx->cfg.device) == cudaSuccess ? 0 : fail(ctx, "cudaSetDevice failed");
 }
 
-// Decode n_buffers whole reference buffers that sit in host memory.
-int run_buffers(modes_ctx *ctx, const uint8_t *host_iq, size_t n_buffers) {
-    if (!ctx->gpus.empty()) return run_buffers_multi(ctx, host_iq, n_buffers);
+// Decode the next n_buffers whole reference buffers of the stream from src.
+int run_buffers(modes_ctx *ctx, Source src, size_t n_buffers) {
+    if (!ctx->gpus.empty()) return run_buffers_multi(ctx, src, n_buffers);
     size_t max_b = (size_t)(ctx->cfg.max_batch_bytes / MODES_BUFFER_BYTES);
     if (max_b < 1) max_b = 1;
     int cur = 0;
@@ -649,10 +720,8 @@ int run_buffers(modes_ctx *ctx, const uint8_t *host_iq, size_t n_buffers) {
         Slot &s = ctx->slot[cur];
         if (collect(ctx, s)) return -1;                                  // slot may still hold batch b-2
         s.buffer_base = ctx->buffers_done;
-        if (submit(ctx, s, host_iq, nullptr, nb, ctx->carry, nullptr, 0, nullptr)) return -1;
-        memcpy(ctx->carry, host_iq + nb * MODES_BUFFER_BYTES - MODES_CARRY_BYTES, MODES_CARRY_BYTES);
+        if (submit_next(ctx, ctx, s, src, nb)) return -1;
         ctx->buffers_done += (int64_t)nb;
-        host_iq += nb * MODES_BUFFER_BYTES;
         n_buffers -= nb;
         cur ^= 1;
         if (collect(ctx, ctx->slot[cur])) return -1;                     // resolve batch b-1 while b runs
@@ -660,6 +729,64 @@ int run_buffers(modes_ctx *ctx, const uint8_t *host_iq, size_t n_buffers) {
     if (collect(ctx, ctx->slot[cur])) return -1;
     if (collect(ctx, ctx->slot[cur ^ 1])) return -1;
     return 0;
+}
+
+Source host_buffers(const uint8_t *iq) {
+    Source src;
+    src.iq = iq;
+    return src;
+}
+
+// 2.4 MS/s: the most the hold can need: the input of one reference buffer and of the carry before it,
+// with the filter's reach on both sides (a whole buffer's input would have run).
+constexpr size_t kHoldBytes = 2 * ((size_t)6 * (kBufSamples + MODES_CARRY_BYTES / 2) / 5 + 2 * resample::kTaps + 16);
+
+// 2.4 MS/s: run every whole buffer whose input (with the filter's lookahead) has arrived, reading the
+// hold and the caller's bytes where they are (run_buffers returns with every copy done), then keep in
+// the hold what later batches read.
+int process_resampled(modes_ctx *ctx, const uint8_t *iq, size_t nbytes) {
+    CK(ctx, ctx->hold.ensure(kHoldBytes));
+    const int64_t call0 = ctx->in_total;
+    ctx->in_total += (int64_t)nbytes;
+    const int64_t avail = ctx->in_total / 2;                               // whole input samples
+    const int64_t B = kBufSamples;
+    int64_t m = (5 * avail / 6) / B;                                        // buffers [0, m) are ready
+    while (m > ctx->buffers_done && resample::in_hi(m * B - 1) > avail) m--;
+    while (resample::in_hi((m + 1) * B - 1) <= avail) m++;
+    if (m > ctx->buffers_done) {
+        Source src;
+        src.hold = ctx->hold.get(); src.hold0 = ctx->hold0;
+        src.call = iq; src.call0 = call0; src.end = ctx->in_total;
+        if (run_buffers(ctx, src, (size_t)(m - ctx->buffers_done))) return -1;
+    }
+    int64_t keep = 2 * resample::in_lo(ctx->buffers_done * B - MODES_CARRY_BYTES / 2);
+    if (keep < ctx->hold0) keep = ctx->hold0;
+    if ((size_t)(ctx->in_total - keep) > ctx->hold.capacity())
+        return fail(ctx, "internal: 2.4 MS/s input history of %lld bytes", (long long)(ctx->in_total - keep));
+    uint8_t *h = ctx->hold.get();
+    if (keep < call0) {
+        memmove(h, h + (keep - ctx->hold0), (size_t)(call0 - keep));
+        memcpy(h + (call0 - keep), iq, nbytes);
+    } else {
+        memcpy(h, iq + (keep - call0), (size_t)(ctx->in_total - keep));
+    }
+    ctx->hold0 = keep;
+    return 0;
+}
+
+// 2.4 MS/s at the end of the stream: the output is N_out = ceil(5 n_in / 6) samples; the remaining whole
+// buffers and the EOF buffer (127 past N_out) run from the hold, the input 127-padded past its end.
+int finish_resampled(modes_ctx *ctx) {
+    const int64_t n_out = resample::n_out((ctx->in_total + 1) / 2);
+    ctx->eof_buffer = n_out / kBufSamples;                                  // its level record counts the real samples only
+    ctx->eof_samples = (uint32_t)(n_out % kBufSamples);
+    const int64_t last = ctx->eof_buffer + (ctx->cfg.drop_eof_buffer ? 0 : 1);
+    if (last <= ctx->buffers_done) return 0;
+    Source src;
+    src.hold = ctx->hold.get(); src.hold0 = ctx->hold0;
+    src.call0 = src.end = ctx->in_total;
+    src.out_end = n_out;
+    return run_buffers(ctx, src, (size_t)(last - ctx->buffers_done));
 }
 
 // One switch of the context and of its GPUs' contexts; each batch runs as the switches were at submit.
@@ -955,9 +1082,23 @@ int modes_reset(modes_ctx *ctx) {
     ctx->pending_len = 0;
     ctx->buffers_done = 0;
     ctx->finished = false;
+    ctx->started = false;
+    ctx->in_total = 0;
+    ctx->hold0 = 0;
     ctx->level_q.clear();
     ctx->eof_buffer = -1;
     memset(ctx->carry, 127, sizeof(ctx->carry));
+    return 0;
+}
+
+int modes_set_input_rate(modes_ctx *ctx, uint32_t hz) {
+    if (!ctx) return -1;
+    if (hz != 2000000 && hz != 2400000)
+        return fail(ctx, "modes_set_input_rate: %u samples/s is not supported (2000000 or 2400000)", hz);
+    if (ctx->started && !ctx->finished)
+        return fail(ctx, "modes_set_input_rate: a stream is in progress; call modes_finish or modes_reset first");
+    ctx->input_rate = hz;
+    for (modes_ctx *g : ctx->gpus) g->input_rate = hz;
     return 0;
 }
 
@@ -965,17 +1106,19 @@ int modes_process(modes_ctx *ctx, const uint8_t *iq, size_t nbytes) {
     if (!ctx) return -1;
     if (ctx->finished) return fail(ctx, "modes_process after modes_finish; call modes_reset first");
     CK(ctx, cudaSetDevice(ctx->cfg.device));
+    ctx->started = true;
+    if (ctx->input_rate == 2400000) return process_resampled(ctx, iq, nbytes);
     if (ctx->pending_len) {
         size_t take = MODES_BUFFER_BYTES - ctx->pending_len;
         if (take > nbytes) take = nbytes;
         memcpy(ctx->pending.get() + ctx->pending_len, iq, take);
         ctx->pending_len += take; iq += take; nbytes -= take;
         if (ctx->pending_len < MODES_BUFFER_BYTES) return 0;
-        if (run_buffers(ctx, ctx->pending.get(), 1)) return -1;
+        if (run_buffers(ctx, host_buffers(ctx->pending.get()), 1)) return -1;
         ctx->pending_len = 0;
     }
     size_t whole = nbytes / MODES_BUFFER_BYTES;
-    if (whole && run_buffers(ctx, iq, whole)) return -1;
+    if (whole && run_buffers(ctx, host_buffers(iq), whole)) return -1;
     iq += whole * MODES_BUFFER_BYTES; nbytes -= whole * MODES_BUFFER_BYTES;
     if (nbytes) { memcpy(ctx->pending.get(), iq, nbytes); ctx->pending_len = nbytes; }
     return 0;
@@ -986,6 +1129,8 @@ int modes_finish(modes_ctx *ctx) {
     if (ctx->finished) return 0;
     CK(ctx, cudaSetDevice(ctx->cfg.device));
     ctx->finished = true;
+    ctx->started = true;
+    if (ctx->input_rate == 2400000) return finish_resampled(ctx);
     // The read that hits EOF still hands a 127-padded buffer to the decoder (dump1090.c:496-510);
     // whether it is decoded is the reference's race, made a switch here.
     memset(ctx->pending.get() + ctx->pending_len, 127, MODES_BUFFER_BYTES - ctx->pending_len);
@@ -993,7 +1138,7 @@ int modes_finish(modes_ctx *ctx) {
     ctx->eof_samples = (uint32_t)((ctx->pending_len + 1) / 2);
     ctx->pending_len = 0;
     if (ctx->cfg.drop_eof_buffer) return 0;
-    return run_buffers(ctx, ctx->pending.get(), 1);
+    return run_buffers(ctx, host_buffers(ctx->pending.get()), 1);
 }
 
 int modes_get_stats(const modes_ctx *ctx, modes_stats *out) {
@@ -1040,6 +1185,33 @@ int modes_detect_host(modes_ctx *ctx, const uint8_t *iq, size_t n_buffers, const
     uint32_t cap = cand_capacity > 0xFFFFFFF0ull ? 0xFFFFFFF0u : (uint32_t)cand_capacity;
     return submit(ctx, ctx->detect, iq, nullptr, n_buffers, carry476,
                   static_cast<modes_candidate *>(d_candidates), cap, static_cast<modes_tile *>(d_tiles));
+}
+
+int modes_resample_device(modes_ctx *ctx, const void *d_in, size_t in_bytes, int64_t in_first_sample,
+                          int64_t first_buffer, size_t n_buffers, int64_t out_end, void *d_out, uint8_t *carry476) {
+    if (!ctx) return -1;
+    if (!d_out || !n_buffers) return fail(ctx, "modes_resample_device: empty output");
+    if (!d_in && in_bytes) return fail(ctx, "modes_resample_device: no input");
+    if (first_buffer < 0) return fail(ctx, "modes_resample_device: buffer index %lld", (long long)first_buffer);
+    if (((reinterpret_cast<uintptr_t>(d_in) | reinterpret_cast<uintptr_t>(d_out)) & 15) != 0)
+        return fail(ctx, "modes_resample_device: input and output must be 16-byte aligned");
+    CK(ctx, cudaSetDevice(ctx->cfg.device));
+    cudaStream_t st = ctx->detect.stream;
+    if (carry476) {
+        CK(ctx, ctx->d_rs_halo.ensure(kHaloAlloc));
+        CK(ctx, ctx->h_rs_halo.ensure(kHaloAlloc));
+    }
+    launch_resample(ResampleJob{static_cast<const uint8_t *>(d_in), in_bytes, in_first_sample, first_buffer * (int64_t)kBufSamples,
+                                (uint64_t)n_buffers * kBufSamples, out_end < 0 ? INT64_MAX : out_end,
+                                static_cast<uint8_t *>(d_out), carry476 ? ctx->d_rs_halo.get() : nullptr},
+                    st);
+    CK(ctx, cudaGetLastError());
+    ctx->launches++;
+    if (!carry476) return 0;
+    CK(ctx, cudaMemcpyAsync(ctx->h_rs_halo.get(), ctx->d_rs_halo.get(), kHaloAlloc, cudaMemcpyDeviceToHost, st));
+    CK(ctx, wait_stream(st));
+    memcpy(carry476, ctx->h_rs_halo.get() + (kHaloBytes - MODES_CARRY_BYTES), MODES_CARRY_BYTES);
+    return 0;
 }
 
 int modes_detect_wait(modes_ctx *ctx, uint64_t *n_candidates) {

@@ -85,6 +85,21 @@ void launch_levels(const uint8_t *d_iq, uint32_t n_buffers, uint64_t stride_byte
                    modes_level *out, int sm_count, cudaStream_t stream);
 static_assert(sizeof(modes_level) == 40 && offsetof(modes_level, sum_mag) == 16 && offsetof(modes_level, peak) == 32,
               "level record layout");
+// 2.4 MS/s input resampled to 2 MHz bytes (modes_resample.cu, arithmetic in modes_resample_core.cuh).
+// Output sample n (stream index, 2 MHz) reads the input samples around 1.2 n; the job holds the stream's
+// input bytes [2 in_first, 2 in_first + in_bytes) and every other input byte reads as 127.
+struct ResampleJob {
+    const uint8_t *in;           // 16-byte aligned
+    uint64_t       in_bytes;
+    int64_t        in_first;     // stream input sample of in[0]
+    int64_t        out_first;    // stream output sample of body[0]: a multiple of 8
+    uint64_t       out_samples;
+    int64_t        out_end;      // output samples at or past it are written as 127 (the EOF buffer's padding)
+    uint8_t       *body;         // 2 * out_samples bytes, 16-byte aligned
+    uint8_t       *halo;         // kHaloAlloc bytes laid out as a batch's carry block (the 238 samples before
+                                 // body[0] at kHaloBytes - MODES_CARRY_BYTES, 127 elsewhere), or nullptr
+};
+void launch_resample(const ResampleJob &j, cudaStream_t stream);
 // Recovery records (modes_recover.cu): writes out[k] for k < min(counters[0], capacity) from the
 // candidate records and the windows the scan and frame evaluation read.
 void launch_recover(const BatchView &in, const DeviceTables &tab, const ScanOutputs &scan, const modes_candidate *records,

@@ -132,6 +132,70 @@ def frame_envelope(frame: bytes, frac: float = 0.0) -> np.ndarray:
     return env
 
 
+def _rate_ratio(sample_rate: int) -> tuple[int, int]:
+    """sample_rate / 2 MHz as a reduced fraction (a, b): one 0.5 us half-bit slot is a / b samples."""
+    from math import gcd
+    g = gcd(int(sample_rate), 2_000_000)
+    return int(sample_rate) // g, 2_000_000 // g
+
+
+def _slot_edge(slot: int, frac: float, a: int, b: int) -> tuple[int, float]:
+    """The start of half-bit slot `slot` (counted in 0.5 us from the stream start) delayed by frac slots,
+    in samples at a / b samples per slot: (whole samples, fraction in [0, 1))."""
+    whole, rem = divmod(a * slot, b)
+    f = rem / b + (frac * a) / b
+    carry = int(np.floor(f))
+    return whole + carry, f - carry
+
+
+def frame_envelope_at(frame: bytes, pos: int, frac: float, sample_rate: int) -> tuple[int, np.ndarray]:
+    """Amplitude envelope (0..1) of preamble + frame arriving at 2 MHz position pos + frac, sampled at
+    sample_rate: each 0.5 us pulse is a rectangle, and each sample is the pulse's overlap with its sample
+    period, over the period.  Returns (index of the first sample, envelope from it).  At 2 MHz this is
+    frame_envelope(frame, frac) at sample pos, bit for bit."""
+    a, b = _rate_ratio(sample_rate)
+    nbits = len(frame) * 8
+    slots = [0, 2, 7, 9] + [16 + 2 * k + (0 if (frame[k >> 3] >> (7 - (k & 7))) & 1 else 1) for k in range(nbits)]
+    first, _ = _slot_edge(pos, frac, a, b)
+    last, _ = _slot_edge(pos + 16 + 2 * nbits + 1, frac, a, b)
+    env = np.zeros(last - first + 2, dtype=np.float64)
+    for p in sorted(slots):
+        ks, fs = _slot_edge(pos + p, frac, a, b)
+        ke, fe = _slot_edge(pos + p + 1, frac, a, b)
+        ks -= first
+        ke -= first
+        if ks == ke:
+            env[ks] += fe - fs
+            continue
+        env[ks] += 1.0 - fs
+        env[ks + 1: ke] += 1.0
+        env[ke] += fe
+    return first, env
+
+
+def synth_stream_at(nsamples: int, frames, sigma: float = 1.5, seed: int = 1, sample_rate: int = 2_000_000) -> np.ndarray:
+    """synth_stream at any sample rate: frames are (pos, frame_bytes, amplitude_lsb, carrier_phase_rad,
+    frac) with the arrival time pos + frac in 2 MHz samples (0.5 us), pulses per frame_envelope_at, and
+    the same noise per sample as synth_stream.  At 2 MHz it equals synth_stream bit for bit."""
+    i = noise(nsamples, sigma, seed * 2 + 11)
+    q = noise(nsamples, sigma, seed * 2 + 12)
+    for pos, frame, amp, phase, frac in frames:
+        start, env = frame_envelope_at(frame, pos, frac, sample_rate)
+        env = env * amp
+        if sample_rate == 2_000_000:                       # synth_stream's envelope length
+            env = env[: 16 + 2 * len(frame) * 8 + 1]
+        end = min(nsamples, start + len(env))
+        if start >= nsamples or end <= start:
+            continue
+        seg = env[: end - start]
+        i[start:end] += seg * np.cos(phase)
+        q[start:end] += seg * np.sin(phase)
+    out = np.empty(2 * nsamples, dtype=np.uint8)
+    out[0::2] = np.clip(np.rint(127.0 + i), 0, 255).astype(np.uint8)
+    out[1::2] = np.clip(np.rint(127.0 + q), 0, 255).astype(np.uint8)
+    return out
+
+
 def synth_stream(nsamples: int, frames, sigma: float = 1.5, seed: int = 1) -> np.ndarray:
     """Build a u8 interleaved I/Q stream of `nsamples` samples.
 
@@ -287,6 +351,26 @@ def fleet_at(snr_db: float, nframes: int, seed: int, n_aircraft: int = 20, amp: 
         frames.append((200 + k * period + rng.below(100), frame, amp, 2 * np.pi * rng.uniform(), 0.5 * rng.uniform()))
         truth.add(frame.hex())
     return synth_stream(200 + nframes * period + 400, frames, sigma=sigma, seed=seed), truth
+
+
+def fleet_at_rate(snr_db: float, nframes: int, seed: int, sample_rate: int = 2_400_000, n_aircraft: int = 20,
+                  amp: float = 20.0, period: int = 400):
+    """fleet_at sampled at sample_rate (2.4 MS/s: what dump1090-fa and readsb record): the same frames,
+    arrival times, amplitudes and carrier phases, over the same stretch of time, with the same noise per
+    sample.  Returns (stream, set of the frames' hex)."""
+    sigma = amp / (np.sqrt(2.0) * 10 ** (snr_db / 20.0))
+    rng = Counter(seed)
+    fleet = [0x400000 + rng.below(0x3FFFFF) for _ in range(n_aircraft)]
+    frames, truth = [], set()
+    for k in range(nframes):
+        aa = fleet[rng.below(n_aircraft)].to_bytes(3, "big")
+        me = [_me_ident, _me_airborne, _me_airborne, _me_velocity][rng.below(4)](rng)
+        frame = make_frame(17, 5, aa + me)
+        frames.append((200 + k * period + rng.below(100), frame, amp, 2 * np.pi * rng.uniform(), 0.5 * rng.uniform()))
+        truth.add(frame.hex())
+    a, b = _rate_ratio(sample_rate)
+    n = -(-(200 + nframes * period + 400) * a // b)
+    return synth_stream_at(n, frames, sigma=sigma, seed=seed, sample_rate=sample_rate), truth
 
 
 def tile_to(data: np.ndarray, nbytes: int) -> np.ndarray:

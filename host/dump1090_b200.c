@@ -27,6 +27,9 @@
  * (modes_config.gpu_resolve); it has no recovery rule, so it is refused together with --recover.
  * --recover-weak implies --recover and also searches weak preambles, positions the reference's
  * preamble test rejects (modes_set_weak_preambles); with --stats a second line goes to stderr.
+ * --sample-rate <hz> gives the rate of the file: 2000000 (the default) or 2400000, what dump1090-fa and
+ * readsb record (modes_set_input_rate: resampled to 2 MHz on the GPU, sample positions and Beast
+ * timestamps on the same 2 MHz / 12 MHz clocks).  It combines with every output mode and switch.
  * The live-radio, networking and interactive options are out of scope.
  */
 #include <math.h>
@@ -105,6 +108,7 @@ int main(int argc, char **argv) {
     modes_config cfg;
     const char *filename = NULL;
     size_t chunk = 16u << 20;
+    unsigned long sample_rate = 2000000;
     modes_default_config(&cfg);
     for (int j = 1; j < argc; j++) {
         int more = j + 1 < argc;
@@ -127,12 +131,17 @@ int main(int argc, char **argv) {
         else if (!strcmp(argv[j], "--device") && more) cfg.device = atoi(argv[++j]);
         else if (!strcmp(argv[j], "--gpus") && more) cfg.n_gpus = atoi(argv[++j]);
         else if (!strcmp(argv[j], "--chunk") && more) chunk = (size_t)strtoull(argv[++j], NULL, 10);
+        else if (!strcmp(argv[j], "--sample-rate") && more) sample_rate = strtoul(argv[++j], NULL, 10);
         else {
             fprintf(stderr, "Unknown or not enough arguments for option '%s'.\n", argv[j]);
             return 1;
         }
     }
     if (!filename) { fprintf(stderr, "--ifile <filename> is required (use '-' for stdin)\n"); return 1; }
+    if (sample_rate != 2000000 && sample_rate != 2400000) {
+        fprintf(stderr, "--sample-rate takes 2000000 or 2400000\n");
+        return 1;
+    }
     if (opt_beast && (opt_raw || opt_onlyaddr || opt_sbs || opt_json)) {
         fprintf(stderr, "--beast writes binary frames to stdout: it cannot be combined with --raw, --onlyaddr, --sbs or --aircraft-json\n");
         return 1;
@@ -155,6 +164,7 @@ int main(int argc, char **argv) {
         tracker = modes_tracker_create(cfg.check_crc);
         if (!tracker) { fprintf(stderr, "out of memory\n"); return 1; }
     }
+    if (modes_set_input_rate(ctx, (uint32_t)sample_rate)) { fprintf(stderr, "--sample-rate: %s\n", modes_last_error(ctx)); return 1; }
     if (opt_beast) modes_set_signal(ctx, 1);
     if (opt_arrival) modes_set_arrival(ctx, 1);
     if (opt_levels) modes_set_levels(ctx, 1);

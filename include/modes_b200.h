@@ -173,6 +173,29 @@ int  modes_finish(modes_ctx *ctx);
 int  modes_reset(modes_ctx *ctx);
 int  modes_get_stats(const modes_ctx *ctx, modes_stats *out);
 
+/* ---- 2.4 MS/s input ------------------------------------------------------ */
+/* The sample rate of the bytes modes_process takes: 2000000 (the default, what dump1090 reads) or
+ * 2400000 (what dump1090-fa and readsb record from RTL-SDR dongles); any other value is refused.  It is
+ * also refused between the first modes_process of a stream and modes_finish / modes_reset, and takes
+ * effect for the stream that begins at create or reset.  On an n_gpus > 1 context it reaches every GPU.
+ * The receiver pool stays at 2 MHz.
+ *
+ * At 2400000 every batch is first resampled to 2 MHz on the device by an exact 5:6 polyphase filter,
+ * and the whole pipeline (and every modes_set_* pass) runs on those bytes unchanged, so a 2.4 MS/s
+ * stream decodes to exactly what the 2 MHz decoder gives on the stream's resampled bytes:
+ *   input   UC8 I/Q, zero at 127; n_in = ceil(bytes / 2), a trailing odd byte is an I whose Q is 127,
+ *           and samples outside [0, n_in) read as (127, 127)
+ *   output  sample n = 5q + r (r = 0..4) with base input index b = 6q + r, for I and Q separately
+ *               y = clamp(127 + ((sum_k h[r][k] * (x[b + k - T/2 + 1] - 127) + 8192) >> 14), 0, 255)
+ *           (int32 sum, arithmetic shift); N_out = ceil(5 n_in / 6) output samples
+ *   taps    T = 6, signed 16-bit Q14, every branch summing to 16384: a Kaiser-windowed sinc (beta 5,
+ *           cutoff 1.1 MHz) sampled at input offsets k - T/2 + 1 - 0.2 r (modes_resample_core.cuh)
+ * The EOF buffer is 127 past N_out, as modes_finish pads a 2 MHz stream.  sample_pos counts 2 MHz
+ * samples; output sample n sits at input time 1.2 n exactly, so 6 * sample_pos is the input time in
+ * 12 MHz ticks and the Beast timestamps keep their meaning.  Level records describe the resampled
+ * bytes (their clipping count can be lower than the input's). */
+int  modes_set_input_rate(modes_ctx *ctx, uint32_t hz);
+
 /* ---- stage-level entry points (tests, bench, multi-GPU sharding) -------- */
 /* computeMagnitudeVector() alone (dump1090.c:1454-1469): nsamples I/Q pairs in
  * host memory -> nsamples u16 magnitudes in host memory, computed on the device. */
@@ -192,6 +215,19 @@ int  modes_detect_device(modes_ctx *ctx, const void *d_iq, size_t n_buffers, con
  * memory with one asynchronous copy on the same stream, then launches the kernels. */
 int  modes_detect_host(modes_ctx *ctx, const uint8_t *iq, size_t n_buffers, const uint8_t *carry476,
                        void *d_candidates, size_t cand_capacity, void *d_tiles);
+/* The resampling of modes_set_input_rate(2400000) over a span already in device memory, for a job that
+ * decodes its own shard of a 2.4 MS/s capture with modes_detect_device.  d_in: in_bytes bytes of the
+ * stream's input from input sample in_first_sample on (16-byte aligned); every other input byte reads as
+ * no signal (127), so the span must hold the input samples
+ *     [floor(6 n0 / 5) - 2, floor(6 (n1 - 1) / 5) + 4)   with n0 = MODES_BUFFER_SAMPLES * first_buffer - 238,
+ *                                                          n1 = MODES_BUFFER_SAMPLES * (first_buffer + n_buffers)
+ * that exist.  Writes the 2 MHz reference buffers first_buffer ... first_buffer + n_buffers - 1 to d_out
+ * (n_buffers * MODES_BUFFER_BYTES, 16-byte aligned); output samples at or past out_end are 127 (the
+ * EOF buffer: out_end = N_out; negative = no limit).  carry476 (host memory, or NULL): the
+ * MODES_CARRY_BYTES 2 MHz bytes before d_out, as modes_detect_device takes them; with it the call waits
+ * for them, without it it returns at once.  Runs on the context's stream. */
+int  modes_resample_device(modes_ctx *ctx, const void *d_in, size_t in_bytes, int64_t in_first_sample,
+                           int64_t first_buffer, size_t n_buffers, int64_t out_end, void *d_out, uint8_t *carry476);
 /* Wait for the last modes_detect_device; returns the candidate count. */
 int  modes_detect_wait(modes_ctx *ctx, uint64_t *n_candidates);
 /* Copy the last result to host memory (arrays sized by the caller from
