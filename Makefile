@@ -68,7 +68,7 @@ tests/_build/libeval_serial_host.so: tests/host_shim/eval_serial_host.cpp $(CSRC
 # test infrastructure: device harness over the product's own kernel objects (recovery and signal
 # passes on constructed corpora, and the exhaustive sweeps of the core headers' device build)
 DSHIM_OBJS := build/modes_recover.o build/modes_signal.o build/modes_levels.o build/modes_tables.o
-dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so tests/_build/libscan_eval_device.so
+dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so tests/_build/libscan_eval_device.so tests/_build/libresample_pool_device.so
 tests/_build/libkernels_device.so: tests/device_shim/kernels_device.cu $(DSHIM_OBJS) $(CSRC)/modes_internal.h $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_levels_core.cuh include/modes_b200.h
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/kernels_device.cu -o tests/_build/kernels_device.o
@@ -84,6 +84,11 @@ tests/_build/libscan_eval_device.so: tests/device_shim/scan_eval_device.cu $(SCA
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/scan_eval_device.cu -o tests/_build/scan_eval_device.o
 	$(NVCC) $(ARCH) -shared -o $@ tests/_build/scan_eval_device.o $(SCAN_EVAL_OBJS) -cudart static
+# the receiver pool's resampling and history launches on constructed jobs (tests/test_pool_input_rate.py)
+tests/_build/libresample_pool_device.so: tests/device_shim/resample_pool_device.cu build/modes_resample.o $(CSRC)/modes_internal.h include/modes_b200.h
+	@mkdir -p tests/_build
+	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/resample_pool_device.cu -o tests/_build/resample_pool_device.o
+	$(NVCC) $(ARCH) -shared -o $@ tests/_build/resample_pool_device.o build/modes_resample.o -cudart static
 
 clean:
 	rm -rf build tests/_build $(LIB) dump1090-b200

@@ -194,7 +194,7 @@ EXPORTS = ["modes_abi_version", "modes_default_config", "modes_create", "modes_d
            "modes_pool_recovery_stats", "modes_set_weak_preambles", "modes_get_weak_recovery_stats", "modes_weak_device",
            "modes_weak_fetch", "modes_resolver_run_weak", "modes_resolver_run_shards_weak", "modes_resolver_weak_stats",
            "modes_pool_set_weak_preambles", "modes_pool_weak_stats", "modes_set_arrival", "modes_pool_set_arrival",
-           "modes_set_input_rate", "modes_resample_device"]
+           "modes_set_input_rate", "modes_resample_device", "modes_pool_set_input_rate"]
 
 INPUT_RATES = (2_000_000, 2_400_000)      # modes_set_input_rate
 
@@ -332,6 +332,7 @@ def lib():
         L.modes_pool_set_weak_preambles.argtypes = [C.c_void_p, C.c_int]
         L.modes_pool_weak_stats.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(RecoveryStats)]
         L.modes_set_input_rate.argtypes = [C.c_void_p, C.c_uint32]
+        L.modes_pool_set_input_rate.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32]
         L.modes_resample_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int64, C.c_int64, C.c_size_t,
                                             C.c_int64, C.c_void_p, C.c_void_p]
         _lib = L
@@ -870,10 +871,14 @@ class ReceiverPool:
     batch.  Messages are collected per receiver (`take(receiver)`).  signal=True: as for Decoder.
     levels=True: level records of every receiver's buffers (`take_levels(receiver)`).
     recover=True: as for Decoder, with statistics per receiver (`recovery_stats(receiver)`).
-    weak_preambles=True: as for Decoder (`weak_recovery_stats(receiver)`).  arrival=True: as for Decoder."""
+    weak_preambles=True: as for Decoder (`weak_recovery_stats(receiver)`).  arrival=True: as for Decoder.
+    input_rate=2_400_000 sets every receiver to 2.4 MS/s at creation, set_input_rate(receiver, hz) one
+    receiver (modes_pool_set_input_rate): a buffer is still BUFFER_BYTES of the receiver's stream, and its
+    2 MHz buffers are decoded as their input completes (`buffers(receiver)` counts them)."""
 
     def __init__(self, n_receivers: int, max_batch: int = 0, signal: bool = False, levels: bool = False,
-                 recover: bool = False, weak_preambles: bool = False, arrival: bool = False, **cfg):
+                 recover: bool = False, weak_preambles: bool = False, arrival: bool = False,
+                 input_rate: int = 2_000_000, **cfg):
         self.cfg = make_config(**cfg)
         self.n = n_receivers
         self._h = lib().modes_pool_create(C.byref(self.cfg), n_receivers, max_batch)
@@ -889,6 +894,9 @@ class ReceiverPool:
             self.set_recovery(True)
         if weak_preambles:
             self.set_weak_preambles(True)
+        if input_rate != 2_000_000:
+            for r in range(n_receivers):
+                self.set_input_rate(r, input_rate)
         self.messages = [[] for _ in range(n_receivers)]
         self._fn = POOL_SINK_FN(self._on)
 
@@ -999,6 +1007,11 @@ class ReceiverPool:
 
     def buffers(self, receiver: int) -> int:
         return int(lib().modes_pool_buffers(self._h, receiver))
+
+    def set_input_rate(self, receiver: int, hz: int) -> None:
+        """The receiver's input sample rate, 2_000_000 or 2_400_000 (modes_pool_set_input_rate); refused
+        while it has a stream in progress (until reset(receiver), which keeps the rate)."""
+        self._check(lib().modes_pool_set_input_rate(self._h, int(receiver), int(hz)))
 
     def reset(self, receiver: int) -> None:
         lib().modes_pool_reset(self._h, receiver)

@@ -100,6 +100,30 @@ struct ResampleJob {
                                  // body[0] at kHaloBytes - MODES_CARRY_BYTES, 127 elsewhere), or nullptr
 };
 void launch_resample(const ResampleJob &j, cudaStream_t stream);
+// The receiver pool's 2.4 MS/s receivers (modes_pool.cpp): one launch for one job per pair of the pool's
+// batch.  A job's input is its receiver's stream bytes [hist0, call0) at hist (the receiver's device input
+// history) and [call0, call0 + MODES_BUFFER_BYTES) at stage (the call's bytes); every other input byte
+// reads as 127.  hist0 and call0 are multiples of 16, hist and stage 16-byte aligned.
+struct PoolResampleJob {
+    const uint8_t *hist;
+    const uint8_t *stage;
+    int64_t        hist0, call0;
+    int64_t        out_first;    // the 2 MHz buffer's first sample (a multiple of MODES_BUFFER_SAMPLES);
+                                 // negative: a 2 MHz receiver, stage is copied to data as it is
+    uint8_t       *pad_tail;     // MODES_CARRY_BYTES: samples out_first - 238 ... out_first - 1
+    uint8_t       *data;         // MODES_BUFFER_BYTES, 16-byte aligned: samples out_first ...
+};
+// The history step of the same receivers: their stream bytes [keep, call0 + MODES_BUFFER_BYTES), read as
+// a PoolResampleJob reads them, to out (the other half of the history; keep a multiple of 16).
+struct PoolHistoryJob {
+    const uint8_t *hist;
+    const uint8_t *stage;
+    int64_t        hist0, call0, keep;
+    uint8_t       *out;
+};
+// d_jobs: device memory; max_bytes: the most bytes one history job writes.
+void launch_resample_pool(const PoolResampleJob *d_jobs, uint32_t n_jobs, cudaStream_t stream);
+void launch_history_pool(const PoolHistoryJob *d_jobs, uint32_t n_jobs, uint64_t max_bytes, cudaStream_t stream);
 // Recovery records (modes_recover.cu): writes out[k] for k < min(counters[0], capacity) from the
 // candidate records and the windows the scan and frame evaluation read.
 void launch_recover(const BatchView &in, const DeviceTables &tab, const ScanOutputs &scan, const modes_candidate *records,

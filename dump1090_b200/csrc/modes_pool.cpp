@@ -21,6 +21,15 @@
 // The order-dependent half is the existing host resolver, one per receiver: the records of a data
 // buffer are re-based to that receiver's own stream position and replayed with its own address
 // cache.  Built on the public C ABI only (modes_detect_device / _fetch, modes_resolver_*).
+//
+// A receiver at 2.4 MS/s (modes_pool_set_input_rate) brings 131072 input samples per call, and its 2 MHz
+// buffers complete at their own pace (157286.4 input samples each): at most one per call, none in the
+// first and in about one call in six after it.  A call that names such a receiver uploads every buffer
+// once to a staging area; one launch (K9's pool form) then resamples the buffer each 2.4 MS/s receiver
+// completes into its pair (carry into the pad tail, buffer into the data buffer), reading the receiver's
+// device-resident input history and the staging area, and moves the 2 MHz receivers' buffers into
+// theirs; a second launch appends the call's bytes to each 2.4 MS/s receiver's history.  Only the
+// receivers that complete a buffer get a pair, so the scan and every pass after it see 2 MHz bytes only.
 #include <algorithm>
 #include <cstdarg>
 #include <cstdio>
@@ -36,19 +45,51 @@
 #include <cuda_runtime.h>
 #include "modes_b200.h"
 #include "modes_internal.h"
+#include "modes_resample_core.cuh"
 
 namespace {
 
 constexpr size_t kBuf = MODES_BUFFER_BYTES;
 constexpr int64_t kBufSamples = MODES_BUFFER_SAMPLES;
+constexpr int64_t kCarrySamples = MODES_CARRY_BYTES / 2;
+constexpr uint32_t kRate2M = 2000000, kRate24 = 2400000;
+// 2.4 MS/s: the most one half of a receiver's input history holds: the input of one 2 MHz buffer and of
+// the carry before it, with the filter's reach and 16-byte alignment (as modes_api.cpp's hold), plus one
+// call's bytes.
+constexpr size_t kHistBytes = 2 * ((size_t)6 * (kBufSamples + kCarrySamples) / 5 + 2 * modes::resample::kTaps + 16) + kBuf;
 
 struct Receiver {
     modes_resolver *res = nullptr;
     int64_t buffers = 0;                       // buffers of this receiver decoded so far
-    int64_t submitted = 0;                     // buffers of this receiver submitted so far
+    int64_t submitted = 0;                     // buffers of this receiver submitted so far (2 MHz buffers)
     uint8_t carry[MODES_CARRY_BYTES];
     modes::LevelQueue levels;
+    uint32_t rate = kRate2M;                   // modes_pool_set_input_rate
+    // 2.4 MS/s: input bytes of the stream so far, and its device input history: stream bytes
+    // [hist0, in_total) at hist[cur], hist0 a multiple of 16; the other half is where the next call's
+    // history step writes (no launch reads what it writes)
+    int64_t in_total = 0, hist0 = 0;
+    uint8_t *hist[2] = {nullptr, nullptr};
+    int cur = 0;
 };
+
+// 2.4 MS/s: what a call of one buffer's bytes does to receiver r: whether it completes the 2 MHz buffer
+// r.submitted (its last sample with the filter's lookahead has arrived; never more than one), and
+// the first stream byte later buffers read.
+struct RatePlan {
+    bool completes;
+    int64_t keep;
+};
+RatePlan rate_plan(const Receiver &r) {
+    const int64_t avail = (r.in_total + (int64_t)kBuf) / 2;
+    RatePlan pl;
+    pl.completes = modes::resample::in_hi((r.submitted + 1) * kBufSamples - 1) <= avail;
+    const int64_t next = r.submitted + (pl.completes ? 1 : 0);
+    int64_t keep = 2 * modes::resample::in_lo(next * kBufSamples - kCarrySamples);
+    keep = keep < 0 ? 0 : keep & ~(int64_t)15;
+    pl.keep = keep < r.hist0 ? r.hist0 : keep;
+    return pl;
+}
 
 // A few persistent helper threads: run(n, f) executes f(0..n-1), f(0) on the calling thread.
 class Crew {
@@ -119,6 +160,13 @@ struct modes_pool {
         std::vector<modes_level> level_out;
         modes::Features feat;                  // the switches as they were at submit
         bool busy = false;
+        // calls that name a 2.4 MS/s receiver: the call's buffers, the job arrays of the two launches
+        // (pinned and device: PoolResampleJob[max_batch], then PoolHistoryJob[max_batch]), and an event
+        // after the launches, which the other slot's next such call waits for (a receiver in both batches)
+        uint8_t *d_stage = nullptr;
+        void *h_jobs = nullptr, *d_jobs = nullptr;
+        cudaEvent_t rate_done = nullptr;
+        bool rate_recorded = false;
     } slot[2];
     unsigned submitted = 0, collected = 0;     // batches so far: slot = number & 1
     std::vector<modes_candidate> cands;
@@ -207,6 +255,131 @@ int ensure_device(modes_pool *p) {
     return 0;
 }
 
+constexpr size_t kJobBytes = sizeof(modes::PoolResampleJob) + sizeof(modes::PoolHistoryJob);
+
+// The device half of 2.4 MS/s receivers, made the first time a call names one.
+int ensure_rate_device(modes_pool *p, const uint32_t *receivers, size_t n) {
+    for (modes_pool::Slot &sl : p->slot) {
+        if (sl.d_stage) continue;
+        sl.d_stage = static_cast<uint8_t *>(modes_device_alloc(p->max_batch * kBuf));
+        sl.d_jobs = modes_device_alloc(p->max_batch * kJobBytes);
+        sl.h_jobs = modes_host_alloc(p->max_batch * kJobBytes);
+        if (!sl.d_stage || !sl.d_jobs || !sl.h_jobs) return fail(p, "out of memory for %zu receivers per batch", p->max_batch);
+        if (cudaEventCreateWithFlags(&sl.rate_done, cudaEventDisableTiming) != cudaSuccess)
+            return fail(p, "event creation failed: %s", cudaGetErrorString(cudaGetLastError()));
+    }
+    for (size_t i = 0; i < n; i++) {
+        Receiver &r = p->rx[receivers[i]];
+        if (r.rate == kRate2M || r.hist[0]) continue;
+        for (uint8_t *&h : r.hist) h = static_cast<uint8_t *>(modes_device_alloc(kHistBytes));
+        if (!r.hist[0] || !r.hist[1]) return fail(p, "out of memory for the input history of receiver %u", receivers[i]);
+    }
+    return 0;
+}
+
+// The callers' buffers to dst + i * pitch.  Buffers at a constant distance in host memory (one staging
+// block): one strided copy instead of n calls (2-3 us of host time each: at 256 receivers more than the
+// copy itself takes).
+int upload_buffers(modes_pool *p, cudaStream_t st, const uint8_t *const *iq, size_t n, uint8_t *dst, size_t pitch) {
+    bool strided = n > 1 && iq[1] > iq[0];
+    const size_t stride = strided ? (size_t)(iq[1] - iq[0]) : 0;
+    for (size_t i = 1; strided && i + 1 < n; i++) strided = iq[i + 1] > iq[i] && (size_t)(iq[i + 1] - iq[i]) == stride;
+    if (strided && stride >= kBuf && stride < ((size_t)1 << 30)) {
+        if (cudaMemcpy2DAsync(dst, pitch, iq[0], stride, kBuf, n, cudaMemcpyHostToDevice, st) != cudaSuccess)
+            return fail(p, "buffer upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+    } else {
+        for (size_t i = 0; i < n; i++)
+            if (cudaMemcpyAsync(dst + i * pitch, iq[i], kBuf, cudaMemcpyHostToDevice, st) != cudaSuccess)
+                return fail(p, "buffer upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+    }
+    return 0;
+}
+
+// The scan and the passes of the switches over the slot's n pairs, already in place.
+int detect_pairs(modes_pool *p, modes_pool::Slot &sl, size_t n) {
+    if (modes_detect_device(sl.ctx, sl.d_batch, 2 * n, nullptr, nullptr, 0, nullptr)) return fail(p, "%s", modes_last_error(sl.ctx));
+    sl.feat = p->feat;
+    sl.feat.weak &= sl.feat.recover;
+    if (sl.feat.recover && modes_recover_device(sl.ctx, nullptr, 0)) return fail(p, "%s", modes_last_error(sl.ctx));
+    // the data buffers only (every second buffer), like the level pass
+    if (sl.feat.weak && modes::weak_device_strided(sl.ctx, nullptr, nullptr, 0, 1, 2)) return fail(p, "%s", modes_last_error(sl.ctx));
+    // the data buffers only (every second buffer), on the same stream: no wait before the collect
+    if (sl.feat.levels && modes_levels_device(sl.ctx, sl.d_batch + kBuf, n, 2 * kBuf)) return fail(p, "%s", modes_last_error(sl.ctx));
+    return 0;
+}
+
+// A call that names a 2.4 MS/s receiver (the buffers are checked): every buffer to the staging area, the
+// pairs of the receivers that complete a buffer resampled / moved into place, the histories advanced.
+int submit_rated(modes_pool *p, modes_pool::Slot &sl, const uint32_t *receivers, const uint8_t *const *iq, size_t n) {
+    if (ensure_rate_device(p, receivers, n)) return -1;
+    cudaStream_t st = static_cast<cudaStream_t>(modes_stream(sl.ctx));
+    modes::PoolResampleJob *rj = static_cast<modes::PoolResampleJob *>(sl.h_jobs);
+    modes::PoolHistoryJob *hj = reinterpret_cast<modes::PoolHistoryJob *>(rj + p->max_batch);
+    size_t n_pairs = 0, n_hist = 0;
+    uint64_t hist_max = 0;
+    bool carries = false;
+    sl.ids.clear();
+    sl.buf_index.clear();
+    for (size_t i = 0; i < n; i++) {
+        const Receiver &r = p->rx[receivers[i]];
+        uint8_t *pad = sl.d_batch + 2 * n_pairs * kBuf;
+        const uint8_t *stage = sl.d_stage + i * kBuf;
+        if (r.rate == kRate2M) {
+            memcpy(sl.h_carry + n_pairs * MODES_CARRY_BYTES, r.carry, MODES_CARRY_BYTES);
+            rj[n_pairs++] = modes::PoolResampleJob{nullptr, stage, 0, 0, -1, nullptr, pad + kBuf};
+            sl.ids.push_back(receivers[i]);
+            sl.buf_index.push_back(r.submitted);
+            carries = true;
+            continue;
+        }
+        const RatePlan pl = rate_plan(r);
+        if (pl.completes) {
+            rj[n_pairs++] = modes::PoolResampleJob{r.hist[r.cur], stage, r.hist0, r.in_total, r.submitted * kBufSamples,
+                                                   pad + kBuf - MODES_CARRY_BYTES, pad + kBuf};
+            sl.ids.push_back(receivers[i]);
+            sl.buf_index.push_back(r.submitted);
+        }
+        const uint64_t bytes = (uint64_t)(r.in_total + (int64_t)kBuf - pl.keep);
+        if (bytes > kHistBytes)
+            return fail(p, "internal: 2.4 MS/s input history of %llu bytes for receiver %u", (unsigned long long)bytes, receivers[i]);
+        hj[n_hist++] = modes::PoolHistoryJob{r.hist[r.cur], stage, r.hist0, r.in_total, pl.keep, r.hist[r.cur ^ 1]};
+        if (bytes > hist_max) hist_max = bytes;
+    }
+    if (upload_buffers(p, st, iq, n, sl.d_stage, kBuf)) return -1;
+    // the 2 MHz receivers' carries as the 2 MHz path uploads them (the 2.4 MS/s pairs' tails are then
+    // overwritten by the resampler)
+    if (carries && cudaMemcpy2DAsync(sl.d_batch + kBuf - MODES_CARRY_BYTES, 2 * kBuf, sl.h_carry, MODES_CARRY_BYTES,
+                                     MODES_CARRY_BYTES, n_pairs, cudaMemcpyHostToDevice, st) != cudaSuccess)
+        return fail(p, "carry upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+    if (cudaMemcpyAsync(sl.d_jobs, sl.h_jobs, p->max_batch * kJobBytes, cudaMemcpyHostToDevice, st) != cudaSuccess)
+        return fail(p, "job upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+    // the other batch in flight may name the same receivers: its reads and its history step first
+    const modes_pool::Slot &other = p->slot[(p->submitted & 1) ^ 1];
+    if (other.rate_recorded && cudaStreamWaitEvent(st, other.rate_done, 0) != cudaSuccess)
+        return fail(p, "stream wait failed: %s", cudaGetErrorString(cudaGetLastError()));
+    const modes::PoolResampleJob *d_rj = static_cast<const modes::PoolResampleJob *>(sl.d_jobs);
+    modes::launch_resample_pool(d_rj, (uint32_t)n_pairs, st);
+    modes::launch_history_pool(reinterpret_cast<const modes::PoolHistoryJob *>(d_rj + p->max_batch), (uint32_t)n_hist, hist_max, st);
+    if (cudaGetLastError() != cudaSuccess || cudaEventRecord(sl.rate_done, st) != cudaSuccess)
+        return fail(p, "resampling launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+    sl.rate_recorded = true;
+    if (n_pairs && detect_pairs(p, sl, n_pairs)) return -1;
+    for (size_t i = 0; i < n; i++) {
+        Receiver &r = p->rx[receivers[i]];
+        if (r.rate == kRate2M) {
+            r.submitted++;
+            memcpy(r.carry, iq[i] + kBuf - MODES_CARRY_BYTES, MODES_CARRY_BYTES);     // dump1090.c:481
+            continue;
+        }
+        const RatePlan pl = rate_plan(r);
+        r.submitted += pl.completes ? 1 : 0;
+        r.in_total += (int64_t)kBuf;
+        r.hist0 = pl.keep;
+        r.cur ^= 1;
+    }
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -228,9 +401,15 @@ modes_pool *modes_pool_create(const modes_config *cfg, size_t n_receivers, size_
 void modes_pool_destroy(modes_pool *p) {
     if (!p) return;
     for (Receiver &r : p->rx) if (r.res) modes_resolver_destroy(r.res);
+    for (Receiver &r : p->rx)
+        for (uint8_t *h : r.hist) if (h) modes_device_free(h);
     for (modes_pool::Slot &sl : p->slot) {
         if (sl.d_batch) modes_device_free(sl.d_batch);
         if (sl.h_carry) modes_host_free(sl.h_carry);
+        if (sl.d_stage) modes_device_free(sl.d_stage);
+        if (sl.d_jobs) modes_device_free(sl.d_jobs);
+        if (sl.h_jobs) modes_host_free(sl.h_jobs);
+        if (sl.rate_done) cudaEventDestroy(sl.rate_done);
         if (sl.ctx) modes_destroy(sl.ctx);
     }
     delete p;
@@ -377,36 +556,26 @@ int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *c
     if (ensure_device(p)) return -1;
     modes_pool::Slot &sl = p->slot[p->submitted & 1];
     if (sl.busy) return fail(p, "two batches are in flight: modes_pool_collect first");
-    cudaStream_t st = static_cast<cudaStream_t>(modes_stream(sl.ctx));
-    // the carries into the tails of the pad buffers, the new buffers behind them
+    bool rated = false;
     for (size_t i = 0; i < n; i++) {
         if (!iq[i]) return fail(p, "receiver %u: no buffer", receivers[i]);
-        memcpy(sl.h_carry + i * MODES_CARRY_BYTES, p->rx[receivers[i]].carry, MODES_CARRY_BYTES);
+        rated |= p->rx[receivers[i]].rate != kRate2M;
     }
+    if (rated) {
+        if (submit_rated(p, sl, receivers, iq, n)) return -1;
+        sl.busy = true;
+        p->submitted++;
+        return 0;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(modes_stream(sl.ctx));
+    // the carries into the tails of the pad buffers, the new buffers behind them
+    for (size_t i = 0; i < n; i++)
+        memcpy(sl.h_carry + i * MODES_CARRY_BYTES, p->rx[receivers[i]].carry, MODES_CARRY_BYTES);
     if (cudaMemcpy2DAsync(sl.d_batch + kBuf - MODES_CARRY_BYTES, 2 * kBuf, sl.h_carry, MODES_CARRY_BYTES, MODES_CARRY_BYTES, n,
                           cudaMemcpyHostToDevice, st) != cudaSuccess)
         return fail(p, "carry upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-    // receivers' buffers at a constant distance in host memory (one staging block): one strided copy
-    // instead of n calls (2-3 us of host time each: at 256 receivers more than the copy itself takes)
-    bool strided = n > 1 && iq[1] > iq[0];
-    const size_t stride = strided ? (size_t)(iq[1] - iq[0]) : 0;
-    for (size_t i = 1; strided && i + 1 < n; i++) strided = iq[i + 1] > iq[i] && (size_t)(iq[i + 1] - iq[i]) == stride;
-    if (strided && stride >= kBuf && stride < ((size_t)1 << 30)) {
-        if (cudaMemcpy2DAsync(sl.d_batch + kBuf, 2 * kBuf, iq[0], stride, kBuf, n, cudaMemcpyHostToDevice, st) != cudaSuccess)
-            return fail(p, "buffer upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-    } else {
-        for (size_t i = 0; i < n; i++)
-            if (cudaMemcpyAsync(sl.d_batch + (2 * i + 1) * kBuf, iq[i], kBuf, cudaMemcpyHostToDevice, st) != cudaSuccess)
-                return fail(p, "buffer upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-    }
-    if (modes_detect_device(sl.ctx, sl.d_batch, 2 * n, nullptr, nullptr, 0, nullptr)) return fail(p, "%s", modes_last_error(sl.ctx));
-    sl.feat = p->feat;
-    sl.feat.weak &= sl.feat.recover;
-    if (sl.feat.recover && modes_recover_device(sl.ctx, nullptr, 0)) return fail(p, "%s", modes_last_error(sl.ctx));
-    // the data buffers only (every second buffer), like the level pass
-    if (sl.feat.weak && modes::weak_device_strided(sl.ctx, nullptr, nullptr, 0, 1, 2)) return fail(p, "%s", modes_last_error(sl.ctx));
-    // the data buffers only (every second buffer), on the same stream: no wait before the collect
-    if (sl.feat.levels && modes_levels_device(sl.ctx, sl.d_batch + kBuf, n, 2 * kBuf)) return fail(p, "%s", modes_last_error(sl.ctx));
+    if (upload_buffers(p, st, iq, n, sl.d_batch + kBuf, 2 * kBuf)) return -1;
+    if (detect_pairs(p, sl, n)) return -1;
     sl.buf_index.resize(n);
     for (size_t i = 0; i < n; i++) sl.buf_index[i] = p->rx[receivers[i]].submitted++;
     // what each receiver carries into its next buffer (dump1090.c:481)
@@ -422,6 +591,15 @@ int modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user) {
     if (!p) return -1;
     if (p->collected == p->submitted) return fail(p, "no batch in flight");
     modes_pool::Slot &sl = p->slot[p->collected & 1];
+    if (sl.ids.empty()) {
+        // a call in which no receiver completed a buffer: nothing was scanned; its copies done, the
+        // callers' buffers are free again
+        if (cudaStreamSynchronize(static_cast<cudaStream_t>(modes_stream(sl.ctx))) != cudaSuccess)
+            return fail(p, "%s", cudaGetErrorString(cudaGetLastError()));
+        sl.busy = false;
+        p->collected++;
+        return 0;
+    }
     uint64_t n_cand = 0;
     if (modes_detect_wait(sl.ctx, &n_cand)) return fail(p, "%s", modes_last_error(sl.ctx));
     const size_t n = sl.ids.size();
@@ -473,9 +651,23 @@ int modes_pool_reset(modes_pool *p, uint32_t receiver) {
     Receiver &r = p->rx[receiver];
     r.buffers = 0;
     r.submitted = 0;
+    r.in_total = 0;
+    r.hist0 = 0;
     r.levels.clear();
     memset(r.carry, 127, sizeof r.carry);
     return modes_resolver_reset(r.res);
+}
+
+int modes_pool_set_input_rate(modes_pool *p, uint32_t receiver, uint32_t hz) {
+    if (!p) return -1;
+    if (hz != kRate2M && hz != kRate24)
+        return fail(p, "modes_pool_set_input_rate: %u samples/s is not supported (2000000 or 2400000)", hz);
+    if (receiver >= p->rx.size()) return fail(p, "receiver %u out of range (%zu receivers)", receiver, p->rx.size());
+    Receiver &r = p->rx[receiver];
+    if (r.submitted || r.in_total)
+        return fail(p, "modes_pool_set_input_rate: receiver %u has a stream in progress; call modes_pool_reset first", receiver);
+    r.rate = hz;
+    return 0;
 }
 
 int modes_pool_set_output(modes_pool *p, modes_message *out, uint32_t *receiver_of, size_t capacity) {

@@ -21,6 +21,27 @@ constexpr int kTileOutBytes = 10 * kPeriods;
 constexpr int kTileInSamples = 6 * kPeriods + R::kPeriodIn;
 constexpr int kInWords = (2 * kTileInSamples + 15) / 16 + 1;     // + one word of alignment slack
 
+// The tile's periods q0 ... q0 + kPeriods - 1 from its input samples 6 q0 - kLead ... at x (staged in shared
+// memory) into s_out; output samples at or past out_end are no signal.
+__device__ __forceinline__ void tile_periods(const uint8_t *x_in, uint8_t *s_out, int64_t q0, int64_t out_end) {
+    for (int t = threadIdx.x; t < kPeriods; t += kThreads) {
+        const uint16_t *x = reinterpret_cast<const uint16_t *>(x_in + 12 * t);
+        int xi[R::kPeriodIn], xq[R::kPeriodIn];
+#pragma unroll
+        for (int k = 0; k < R::kPeriodIn; k++) {
+            const uint32_t v = x[k];
+            xi[k] = (int)(v & 0xff) - 127;
+            xq[k] = (int)(v >> 8) - 127;
+        }
+        uint32_t y[5];
+        R::period(xi, xq, y);
+        const int64_t n0 = 5 * (q0 + t);
+        uint16_t *o = reinterpret_cast<uint16_t *>(s_out + 10 * t);
+#pragma unroll
+        for (int r = 0; r < 5; r++) o[r] = (uint16_t)(n0 + r >= out_end ? 0x7f7fu : y[r]);
+    }
+}
+
 __global__ void __launch_bounds__(kThreads) resample_kernel(ResampleJob j, int64_t q_first) {
     __shared__ __align__(16) uint8_t s_in[kInWords * 16];
     __shared__ __align__(16) uint8_t s_out[kTileOutBytes];
@@ -55,22 +76,7 @@ __global__ void __launch_bounds__(kThreads) resample_kernel(ResampleJob j, int64
     }
     __syncthreads();
 
-    for (int t = threadIdx.x; t < kPeriods; t += kThreads) {
-        const uint16_t *x = reinterpret_cast<const uint16_t *>(s_in + sh + 12 * t);
-        int xi[R::kPeriodIn], xq[R::kPeriodIn];
-#pragma unroll
-        for (int k = 0; k < R::kPeriodIn; k++) {
-            const uint32_t v = x[k];
-            xi[k] = (int)(v & 0xff) - 127;
-            xq[k] = (int)(v >> 8) - 127;
-        }
-        uint32_t y[5];
-        R::period(xi, xq, y);
-        const int64_t n0 = 5 * (q0 + t);
-        uint16_t *o = reinterpret_cast<uint16_t *>(s_out + 10 * t);
-#pragma unroll
-        for (int r = 0; r < 5; r++) o[r] = (uint16_t)(n0 + r >= j.out_end ? 0x7f7fu : y[r]);
-    }
+    tile_periods(s_in + sh, s_out, q0, j.out_end);
     __syncthreads();
 
     // the body: tile and body bounds are multiples of 16 bytes apart
@@ -96,7 +102,86 @@ __global__ void __launch_bounds__(kThreads) resample_kernel(ResampleJob j, int64
     }
 }
 
+// ---- the receiver pool (modes_pool.cpp): one launch for the batch's jobs, grid (tile, job)
+
+constexpr int kCarrySamples = MODES_CARRY_BYTES / 2;
+constexpr int64_t kPoolOut = (int64_t)kBufSamples + kCarrySamples;           // samples a job writes
+// Tiles of a job: its periods [q_first, q_end), q_first rounded down to a multiple of 8, for any out_first.
+constexpr int kPoolTiles = (int)((kPoolOut / 5 + 2 + 8 + kPeriods - 1) / kPeriods);
+constexpr int kBufWords = MODES_BUFFER_BYTES / 16;
+
+// Stream byte p (a multiple of 16) of a job's input: the history [hist0, call0), the call [call0, + buffer),
+// no signal elsewhere.
+template <class Job>
+__device__ __forceinline__ uint4 job_word(const Job &j, int64_t p) {
+    if (p >= j.hist0 && p < j.call0) return __ldg(reinterpret_cast<const uint4 *>(j.hist + (p - j.hist0)));
+    if (p >= j.call0 && p < j.call0 + MODES_BUFFER_BYTES) return __ldg(reinterpret_cast<const uint4 *>(j.stage + (p - j.call0)));
+    return make_uint4(0x7f7f7f7fu, 0x7f7f7f7fu, 0x7f7f7f7fu, 0x7f7f7f7fu);
+}
+
+__global__ void __launch_bounds__(kThreads) resample_pool_kernel(const PoolResampleJob *jobs) {
+    __shared__ __align__(16) uint8_t s_in[kInWords * 16];
+    __shared__ __align__(16) uint8_t s_out[kTileOutBytes];
+    const PoolResampleJob j = jobs[blockIdx.y];
+    if (j.out_first < 0) {
+        // a 2 MHz receiver: its buffer moves from the staging area to its pair's data buffer as it is
+        constexpr int kPer = (kBufWords + kPoolTiles - 1) / kPoolTiles;
+        const int w1 = (int)blockIdx.x * kPer + kPer < kBufWords ? (int)blockIdx.x * kPer + kPer : kBufWords;
+        for (int w = (int)blockIdx.x * kPer + threadIdx.x; w < w1; w += kThreads)
+            reinterpret_cast<uint4 *>(j.data)[w] = __ldg(reinterpret_cast<const uint4 *>(j.stage) + w);
+        return;
+    }
+    const int64_t c0 = j.out_first - kCarrySamples;
+    const int64_t q0 = R::floor_div(R::floor_div(c0, 5), 8) * 8 + (int64_t)blockIdx.x * kPeriods;
+    if (5 * q0 >= j.out_first + (int64_t)kBufSamples) return;
+
+    // input samples 6 q0 - kLead ... of the tile, stream bytes from a0 (hist0 and call0 are multiples of 16)
+    const int64_t s0 = 2 * (6 * q0 - R::kLead);
+    const int64_t a0 = s0 & ~(int64_t)15;
+    for (int w = threadIdx.x; w < kInWords; w += kThreads)
+        *reinterpret_cast<uint4 *>(s_in + 16 * w) = job_word(j, a0 + 16 * (int64_t)w);
+    __syncthreads();
+    tile_periods(s_in + (int)(s0 - a0), s_out, q0, INT64_MAX);
+    __syncthreads();
+
+    // the data buffer: tile and buffer bounds are multiples of 16 bytes apart
+    const int64_t tb = 2 * (5 * q0 - j.out_first);
+    for (int w = threadIdx.x; w < kTileOutBytes / 16; w += kThreads) {
+        const int64_t p = tb + 16 * (int64_t)w;
+        if (p >= 0 && p + 16 <= (int64_t)MODES_BUFFER_BYTES)
+            *reinterpret_cast<uint4 *>(j.data + p) = *reinterpret_cast<const uint4 *>(s_out + 16 * w);
+    }
+    // the carry: samples out_first - 238 ... out_first - 1 into the tail of the pair's pad buffer, and
+    // nothing else of it (its other bytes stay no signal)
+    const int64_t lo = c0 > 5 * q0 ? c0 : 5 * q0;
+    const int64_t hi = j.out_first < 5 * q0 + 5 * kPeriods ? j.out_first : 5 * q0 + 5 * kPeriods;
+    for (int64_t n = lo + threadIdx.x; n < hi; n += kThreads)
+        reinterpret_cast<uint16_t *>(j.pad_tail)[n - c0] = reinterpret_cast<const uint16_t *>(s_out)[n - 5 * q0];
+}
+
+constexpr int kHistWordsPerThread = 4;
+constexpr int64_t kHistBlockBytes = 16 * kHistWordsPerThread * kThreads;
+
+__global__ void __launch_bounds__(kThreads) history_pool_kernel(const PoolHistoryJob *jobs) {
+    const PoolHistoryJob j = jobs[blockIdx.y];
+    const int64_t end = j.call0 + MODES_BUFFER_BYTES;
+#pragma unroll
+    for (int k = 0; k < kHistWordsPerThread; k++) {
+        const int64_t p = j.keep + (int64_t)blockIdx.x * kHistBlockBytes + 16 * (int64_t)(k * kThreads + threadIdx.x);
+        if (p < end) *reinterpret_cast<uint4 *>(j.out + (p - j.keep)) = job_word(j, p);
+    }
+}
+
 }  // namespace
+
+void launch_resample_pool(const PoolResampleJob *d_jobs, uint32_t n_jobs, cudaStream_t stream) {
+    if (n_jobs) resample_pool_kernel<<<dim3(kPoolTiles, n_jobs), kThreads, 0, stream>>>(d_jobs);
+}
+
+void launch_history_pool(const PoolHistoryJob *d_jobs, uint32_t n_jobs, uint64_t max_bytes, cudaStream_t stream) {
+    const unsigned blocks = (unsigned)((max_bytes + kHistBlockBytes - 1) / kHistBlockBytes);
+    if (n_jobs && blocks) history_pool_kernel<<<dim3(blocks, n_jobs), kThreads, 0, stream>>>(d_jobs);
+}
 
 void launch_resample(const ResampleJob &j, cudaStream_t stream) {
     const int64_t first = j.out_first - (j.halo ? MODES_CARRY_BYTES / 2 : 0);

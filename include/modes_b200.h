@@ -178,7 +178,7 @@ int  modes_get_stats(const modes_ctx *ctx, modes_stats *out);
  * 2400000 (what dump1090-fa and readsb record from RTL-SDR dongles); any other value is refused.  It is
  * also refused between the first modes_process of a stream and modes_finish / modes_reset, and takes
  * effect for the stream that begins at create or reset.  On an n_gpus > 1 context it reaches every GPU.
- * The receiver pool stays at 2 MHz.
+ * A receiver of the pool has its own rate: modes_pool_set_input_rate below.
  *
  * At 2400000 every batch is first resampled to 2 MHz on the device by an exact 5:6 polyphase filter,
  * and the whole pipeline (and every modes_set_* pass) runs on those bytes unchanged, so a 2.4 MS/s
@@ -195,6 +195,21 @@ int  modes_get_stats(const modes_ctx *ctx, modes_stats *out);
  * 12 MHz ticks and the Beast timestamps keep their meaning.  Level records describe the resampled
  * bytes (their clipping count can be lower than the input's). */
 int  modes_set_input_rate(modes_ctx *ctx, uint32_t hz);
+/* The same per receiver of a pool (modes_pool_* below): 2000000 (the default) or 2400000; refused for
+ * any other value, a receiver out of range, and while the receiver has a stream in progress (from the
+ * first modes_pool_submit / _ingest that names it until modes_pool_reset, which keeps the rate).  It
+ * touches no device.  A 2.4 MS/s receiver's iq[i] is still MODES_BUFFER_BYTES of its stream (131072
+ * input samples); a 2 MHz buffer of its resampled stream is decoded in the call whose input completes it
+ * (its last sample and the filter's 4-sample lookahead have arrived): at most one per call, none in the
+ * first call and in about one call in six after it.  A call in which no named receiver completes a buffer
+ * delivers nothing and is still collected.  modes_pool_buffers counts the 2 MHz buffers decoded, and the
+ * receiver's messages, sample_pos (2 MHz samples), statistics and level records (their buffer index a
+ * 2 MHz buffer's) equal those of the 2 MHz decode, without the EOF buffer, of the first
+ * modes_pool_buffers buffers of the receiver's resampled stream, with every switch.  The pool's device
+ * memory grows by a staging area (2 x 256 KiB per receiver of a batch) and about 1.1 MiB of input
+ * history per 2.4 MS/s receiver. */
+typedef struct modes_pool modes_pool;                /* the receiver pool: "many receivers on one GPU" below */
+int  modes_pool_set_input_rate(modes_pool *p, uint32_t receiver, uint32_t hz);
 
 /* ---- stage-level entry points (tests, bench, multi-GPU sharding) -------- */
 /* computeMagnitudeVector() alone (dump1090.c:1454-1469): nsamples I/Q pairs in
@@ -400,7 +415,6 @@ size_t modes_tile_count(size_t n_buffers);
  * receiver are delivered in its stream order with sample_pos counted in its own stream; receivers are
  * served in the order they are listed.  Every receiver's output equals a modes_ctx fed that receiver's
  * buffers alone. */
-typedef struct modes_pool modes_pool;
 typedef void (*modes_pool_sink_fn)(void *user, uint32_t receiver, const modes_message *mm);
 /* max_batch_receivers: most receivers one modes_pool_ingest call names (0: n_receivers); sizes the
  * resident batch (2 x 256 KiB per receiver).  No device is touched before the first modes_pool_ingest. */
@@ -420,7 +434,8 @@ int  modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *
 int  modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user);
 /* The host half alone, for candidate records produced elsewhere over a batch laid out as the pool lays
  * it out: buffer 2i = pad buffer of receivers[i] (no signal, last MODES_CARRY_BYTES = its carry), buffer
- * 2i+1 = its new buffer; candidates/tiles as modes_detect_fetch returns them for those 2n buffers. */
+ * 2i+1 = its new buffer; candidates/tiles as modes_detect_fetch returns them for those 2n buffers.  The
+ * buffers are 2 MHz buffers whatever the receivers' input rates. */
 int  modes_pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, const modes_candidate *candidates,
                         const modes_tile *tiles, modes_pool_sink_fn sink, void *user);
 /* Like modes_set_output: messages are ALSO written to a caller-owned array, all receivers' in delivery
