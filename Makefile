@@ -68,7 +68,7 @@ tests/_build/libeval_serial_host.so: tests/host_shim/eval_serial_host.cpp $(CSRC
 # test infrastructure: device harness over the product's own kernel objects (recovery and signal
 # passes on constructed corpora, and the exhaustive sweeps of the core headers' device build)
 DSHIM_OBJS := build/modes_recover.o build/modes_signal.o build/modes_levels.o build/modes_tables.o
-dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so tests/_build/libscan_eval_device.so tests/_build/libresample_pool_device.so
+dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so tests/_build/libscan_eval_device.so tests/_build/libresample_pool_device.so tests/_build/libresolve_device.so
 tests/_build/libkernels_device.so: tests/device_shim/kernels_device.cu $(DSHIM_OBJS) $(CSRC)/modes_internal.h $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_levels_core.cuh include/modes_b200.h
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/kernels_device.cu -o tests/_build/kernels_device.o
@@ -89,6 +89,11 @@ tests/_build/libresample_pool_device.so: tests/device_shim/resample_pool_device.
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/resample_pool_device.cu -o tests/_build/resample_pool_device.o
 	$(NVCC) $(ARCH) -shared -o $@ tests/_build/resample_pool_device.o build/modes_resample.o -cudart static
+# the device resolve with a chosen SM count, batch size and delivery capacity (tests/test_resolve_device.py)
+tests/_build/libresolve_device.so: tests/device_shim/resolve_device.cu build/modes_resolve_gpu.o $(CSRC)/modes_internal.h include/modes_b200.h
+	@mkdir -p tests/_build
+	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/resolve_device.cu -o tests/_build/resolve_device.o
+	$(NVCC) $(ARCH) -shared -o $@ tests/_build/resolve_device.o build/modes_resolve_gpu.o -cudart static
 
 clean:
 	rm -rf build tests/_build $(LIB) dump1090-b200

@@ -1448,6 +1448,15 @@ int modes_decode_frames(modes_ctx *ctx, const uint8_t *frames, size_t n, modes_m
         finish_message(ctx->rs, ctx->h_frame_evals[i], &out[i]);
         out[i].sample_pos = -1;
     }
+    if (ctx->cfg.gpu_resolve) {
+        // The device resolve reads the next batch's cache from d_cache[cache_cur], not from rs.icao: hand
+        // the frames' writes over.  No batch is in flight here (run_buffers collects both slots before
+        // modes_process / modes_finish return), so nothing else reads or writes the device cache.  Queued
+        // on the detect stream and waited for: the slot streams are non-blocking, so a copy on the legacy
+        // default stream would not be ordered before their next batch.
+        CK(ctx, cudaMemcpyAsync(ctx->d_cache[ctx->cache_cur].get(), ctx->rs.icao, sizeof(ctx->rs.icao), cudaMemcpyHostToDevice, st));
+        CK(ctx, wait_stream(st));
+    }
     return 0;
 }
 

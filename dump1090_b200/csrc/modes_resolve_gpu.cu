@@ -25,7 +25,8 @@
 // The host then only builds struct modesMessage fields from 40-byte deliveries (in parallel); the
 // 56-byte candidate records never leave the GPU (47 MB -> 17 MB per GiB of the dense capture).
 // Exactness is checked on the CPU for the algorithm (tests/test_resolve_core_host.py) and on the
-// GPU against the host resolver and the oracle (tests/test_gpu_resolve.py).
+// GPU against the host resolver and the oracle (tests/test_gpu_resolve.py), and kernel by kernel, at
+// any grid and batch size, through a device harness (tests/test_resolve_device.py).
 #include <cstdint>
 #include <cuda_runtime.h>
 #include "modes_internal.h"

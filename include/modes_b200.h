@@ -293,7 +293,9 @@ size_t modes_resolver_output_count(const modes_resolver *r);
 
 /* decodeModesMessage() on frame bytes (the reference's hex door,
  * decodeHexMessage dump1090.c:2472-2502): CRC, fix and field decode run on the
- * device + resolve path with the context's ICAO cache. */
+ * device + resolve path with the context's ICAO cache: the frames see every address the stream
+ * decoded so far, and the addresses they announce are seen by the stream's later batches, whether
+ * the host or the device (gpu_resolve) resolves them. */
 int  modes_decode_frame(modes_ctx *ctx, const uint8_t msg[14], modes_message *out);
 /* n frames of 14 bytes each in one launch (device staging is kept by the context); decoded in
  * order, as n calls of modes_decode_frame would. */
