@@ -11,11 +11,11 @@ OBJS      := build/modes_kernels.o build/modes_scan2.o build/modes_eval_fused.o 
 
 all: $(LIB) dump1090-b200
 
-build/%.o: $(CSRC)/%.cu $(CSRC)/modes_internal.h $(CSRC)/modes_eval_serial.cuh $(CSRC)/modes_scan_core.cuh $(CSRC)/modes_resolve_core.cuh $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_arrival_core.cuh $(CSRC)/modes_levels_core.cuh $(CSRC)/modes_recover_core.cuh $(CSRC)/modes_weak_core.cuh $(CSRC)/modes_resample_core.cuh include/modes_b200.h
+build/%.o: $(CSRC)/%.cu $(CSRC)/modes_internal.h $(CSRC)/modes_eval_serial.cuh $(CSRC)/modes_scan_core.cuh $(CSRC)/modes_resolve_core.cuh $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_arrival_core.cuh $(CSRC)/modes_levels_core.cuh $(CSRC)/modes_recover_core.cuh $(CSRC)/modes_weak_core.cuh $(CSRC)/modes_resample_core.cuh $(CSRC)/modes_input_core.cuh include/modes_b200.h
 	@mkdir -p build
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@
 
-build/%.o: $(CSRC)/%.cpp $(CSRC)/modes_internal.h include/modes_b200.h
+build/%.o: $(CSRC)/%.cpp $(CSRC)/modes_internal.h $(CSRC)/modes_input_core.cuh $(CSRC)/modes_resample_core.cuh include/modes_b200.h
 	@mkdir -p build
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 
@@ -30,7 +30,10 @@ oracle:
 	if [ -d /root/reference ]; then $(MAKE) -C oracle ref; fi
 
 # test infrastructure: host build of the per-candidate evaluation (logic checked against the oracle on CPU)
-shim: tests/_build/libeval_serial_host.so tests/_build/libscan_core_host.so tests/_build/libresolve_core_host.so tests/_build/libsignal_core_host.so tests/_build/liblevels_core_host.so tests/_build/librecover_core_host.so tests/_build/libweak_core_host.so tests/_build/libarrival_core_host.so tests/_build/libresample_core_host.so
+shim: tests/_build/libeval_serial_host.so tests/_build/libscan_core_host.so tests/_build/libresolve_core_host.so tests/_build/libsignal_core_host.so tests/_build/liblevels_core_host.so tests/_build/librecover_core_host.so tests/_build/libweak_core_host.so tests/_build/libarrival_core_host.so tests/_build/libresample_core_host.so tests/_build/libinput_core_host.so
+tests/_build/libinput_core_host.so: tests/host_shim/input_core_host.cpp $(CSRC)/modes_input_core.cuh
+	@mkdir -p tests/_build
+	g++ -O2 -std=c++17 -shared -fPIC -Wall -Wno-unknown-pragmas -x c++ -I$(CSRC) tests/host_shim/input_core_host.cpp -o $@
 tests/_build/libresample_core_host.so: tests/host_shim/resample_core_host.cpp $(CSRC)/modes_resample_core.cuh
 	@mkdir -p tests/_build
 	g++ -O2 -std=c++17 -shared -fPIC -Wall -Wno-unknown-pragmas -x c++ -I$(CSRC) tests/host_shim/resample_core_host.cpp -o $@
@@ -68,7 +71,7 @@ tests/_build/libeval_serial_host.so: tests/host_shim/eval_serial_host.cpp $(CSRC
 # test infrastructure: device harness over the product's own kernel objects (recovery and signal
 # passes on constructed corpora, and the exhaustive sweeps of the core headers' device build)
 DSHIM_OBJS := build/modes_recover.o build/modes_signal.o build/modes_levels.o build/modes_tables.o
-dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so tests/_build/libscan_eval_device.so tests/_build/libresample_pool_device.so tests/_build/libresolve_device.so
+dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so tests/_build/libscan_eval_device.so tests/_build/libresample_pool_device.so tests/_build/libresolve_device.so tests/_build/libinput_device.so
 tests/_build/libkernels_device.so: tests/device_shim/kernels_device.cu $(DSHIM_OBJS) $(CSRC)/modes_internal.h $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_levels_core.cuh include/modes_b200.h
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/kernels_device.cu -o tests/_build/kernels_device.o
@@ -89,6 +92,11 @@ tests/_build/libresample_pool_device.so: tests/device_shim/resample_pool_device.
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/resample_pool_device.cu -o tests/_build/resample_pool_device.o
 	$(NVCC) $(ARCH) -shared -o $@ tests/_build/resample_pool_device.o build/modes_resample.o -cudart static
+# the 16-bit input launches on chosen spans, and their timing (tests/test_input_format.py, scripts/input_format_time.py)
+tests/_build/libinput_device.so: tests/device_shim/input_device.cu build/modes_resample.o $(CSRC)/modes_internal.h include/modes_b200.h
+	@mkdir -p tests/_build
+	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/input_device.cu -o tests/_build/input_device.o
+	$(NVCC) $(ARCH) -shared -o $@ tests/_build/input_device.o build/modes_resample.o -cudart static
 # the device resolve with a chosen SM count, batch size and delivery capacity (tests/test_resolve_device.py)
 tests/_build/libresolve_device.so: tests/device_shim/resolve_device.cu build/modes_resolve_gpu.o $(CSRC)/modes_internal.h include/modes_b200.h
 	@mkdir -p tests/_build

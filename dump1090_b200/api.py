@@ -194,9 +194,10 @@ EXPORTS = ["modes_abi_version", "modes_default_config", "modes_create", "modes_d
            "modes_pool_recovery_stats", "modes_set_weak_preambles", "modes_get_weak_recovery_stats", "modes_weak_device",
            "modes_weak_fetch", "modes_resolver_run_weak", "modes_resolver_run_shards_weak", "modes_resolver_weak_stats",
            "modes_pool_set_weak_preambles", "modes_pool_weak_stats", "modes_set_arrival", "modes_pool_set_arrival",
-           "modes_set_input_rate", "modes_resample_device", "modes_pool_set_input_rate"]
+           "modes_set_input_rate", "modes_resample_device", "modes_pool_set_input_rate", "modes_set_input_format"]
 
 INPUT_RATES = (2_000_000, 2_400_000)      # modes_set_input_rate
+INPUT_FORMATS = {"uc8": 0, "sc16": 1, "sc16q11": 2}     # modes_set_input_format: MODES_INPUT_*
 
 
 def resampled_samples(n_input_bytes: int) -> int:
@@ -333,6 +334,7 @@ def lib():
         L.modes_pool_weak_stats.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(RecoveryStats)]
         L.modes_set_input_rate.argtypes = [C.c_void_p, C.c_uint32]
         L.modes_pool_set_input_rate.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32]
+        L.modes_set_input_format.argtypes = [C.c_void_p, C.c_uint32, C.c_int32]
         L.modes_resample_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int64, C.c_int64, C.c_size_t,
                                             C.c_int64, C.c_void_p, C.c_void_p]
         _lib = L
@@ -417,16 +419,23 @@ class Decoder:
     input_rate=2_400_000 takes 2.4 MS/s bytes (what dump1090-fa and readsb record) and resamples them
     to 2 MHz on the GPU before the pipeline (modes_set_input_rate): the messages are exactly the 2 MHz
     decoder's on the resampled bytes.  Message.sample_pos still counts 2 MHz samples, and
-    6 * sample_pos is the input time in 12 MHz ticks at either rate."""
+    6 * sample_pos is the input time in 12 MHz ticks at either rate.
+    input_format="sc16" or "sc16q11" takes signed 16-bit I/Q bytes (SoapySDR and Airspy-class tools,
+    bladeRF) and converts them to 8-bit I/Q on the GPU with input_shift (None: the format's default)
+    before the pipeline (modes_set_input_format): the messages are exactly the UC8 decoder's on the
+    converted bytes, at either input rate."""
 
     def __init__(self, signal: bool = False, levels: bool = False, recover: bool = False, weak_preambles: bool = False,
-                 arrival: bool = False, input_rate: int = 2_000_000, **cfg):
+                 arrival: bool = False, input_rate: int = 2_000_000, input_format: str = "uc8",
+                 input_shift: int | None = None, **cfg):
         self.cfg = make_config(**cfg)
         self._h = lib().modes_create(C.byref(self.cfg))
         if not self._h:
             raise RuntimeError("modes_create failed: " + lib().modes_last_error(None).decode())
         if input_rate != 2_000_000:
             self.set_input_rate(input_rate)
+        if input_format != "uc8" or input_shift is not None:
+            self.set_input_format(input_format, input_shift)
         if signal:
             self.set_signal(True)
         if arrival:
@@ -523,6 +532,15 @@ class Decoder:
         2_400_000 (modes_set_input_rate); refused while a stream is in progress.  sample_pos counts 2 MHz
         samples at either rate, and 6 * sample_pos is the input time in 12 MHz ticks."""
         self._check(lib().modes_set_input_rate(self._h, int(hz)))
+
+    def set_input_format(self, fmt: str, shift: int | None = None) -> None:
+        """The sample format of the stream that begins at the next reset: "uc8", "sc16" or "sc16q11"
+        (INPUT_FORMATS, modes_set_input_format), with the shift 0 ... 15 that converts 16-bit values to
+        8 bits (None: the format's default, 8 for sc16 and 4 for sc16q11); refused while a stream is in
+        progress."""
+        if fmt not in INPUT_FORMATS:
+            raise ValueError(f"input format {fmt!r} is not one of {sorted(INPUT_FORMATS)}")
+        self._check(lib().modes_set_input_format(self._h, INPUT_FORMATS[fmt], -1 if shift is None else int(shift)))
 
     def set_arrival(self, on: bool) -> None:
         """Measure the arrival time for batches submitted from now on (modes_set_arrival)."""

@@ -14,6 +14,7 @@
 #include <string>
 #include <vector>
 #include "modes_internal.h"
+#include "modes_input_core.cuh"
 #include "modes_resample_core.cuh"
 
 using namespace modes;
@@ -69,7 +70,7 @@ struct Slot {
     cudaStream_t stream = nullptr;
     DevBuf<uint8_t> d_iq;
     DevBuf<uint8_t> d_halo;
-    DevBuf<uint8_t> d_in;             // 2.4 MS/s input: the input bytes the batch's resampling reads
+    DevBuf<uint8_t> d_in;             // 2.4 MS/s or 16-bit input: the input bytes the batch is made from
     DevBuf<uint32_t> d_cand_v;       // its capacity is the slot's candidate capacity
     DevBuf<modes_candidate> d_records;
     DevBuf<modes_tile> d_tiles;
@@ -160,10 +161,13 @@ struct modes_ctx {
     int64_t buffers_done = 0;
     bool finished = false;
     bool started = false;                 // modes_process or modes_finish since create / reset
-    // modes_set_input_rate: at 2.4 MS/s each batch is resampled to 2 MHz on the device (K9) from the
-    // stream's input bytes; the 2 MHz bytes never exist on the host.  hold keeps the stream bytes
-    // [hold0, in_total) that later batches read (the filter's history and a buffer not yet complete).
+    // modes_set_input_rate / modes_set_input_format: at 2.4 MS/s, or in a 16-bit format, each batch's 2 MHz
+    // UC8 bytes are made on the device (K9 resamples, K10 converts) from the stream's input bytes; they
+    // never exist on the host.  hold keeps the stream bytes [hold0, in_total) that later batches read (the
+    // filter's history and a buffer not yet complete).  input_shift: the format's shift, default resolved.
     uint32_t input_rate = 2000000;
+    uint32_t input_format = input::kUC8;
+    int input_shift = 0;
     int64_t in_total = 0;
     PinnedBuf<uint8_t> hold;
     int64_t hold0 = 0;
@@ -619,9 +623,10 @@ int collect_group(modes_ctx *ctx, int parity) {
     return 0;
 }
 
-// Where the batches of a run read their input.  2 MHz: the run's whole reference buffers at iq.
-// 2.4 MS/s (iq == nullptr): the stream's input bytes [hold0, call0) at hold and [call0, end) at call;
-// every later byte is no signal, and output samples at or past out_end are the EOF buffer's padding.
+// Where the batches of a run read their input.  2 MHz UC8: the run's whole reference buffers at iq.
+// 2.4 MS/s or a 16-bit format (iq == nullptr): the stream's input bytes [hold0, call0) at hold and
+// [call0, end) at call; every later byte is no signal, and output samples at or past out_end are the EOF
+// buffer's padding.
 struct Source {
     const uint8_t *iq = nullptr;
     const uint8_t *hold = nullptr;
@@ -631,13 +636,28 @@ struct Source {
     int64_t out_end = INT64_MAX;
 };
 
-// 2.4 MS/s: upload the input bytes the slot's batch (nb buffers from s.buffer_base, and the carry before
-// them) reads, straight from where they are, and resample them into the slot's body and carry block.
-int stage_resampled(modes_ctx *ctx, Slot &s, const Source &src, size_t nb) {
+// The input paths through the hold: 2.4 MS/s (resampled, K9) or a 16-bit format (converted, K10; at
+// 2.4 MS/s converted, then resampled).
+bool held_input(const modes_ctx *ctx) { return ctx->input_rate == 2400000 || ctx->input_format != input::kUC8; }
+
+// The input samples [batch_in_lo(o0), batch_in_hi(o1)) that the 2 MHz output samples [o0, o1) of a batch
+// and its carry block read.  At 2 MHz output sample n reads input sample n, and the span starts with the
+// carry block's 240 samples, so that a 16-bit upload starts on a 16-byte boundary.
+int64_t batch_in_lo(const modes_ctx *ctx, int64_t o0) {
+    return ctx->input_rate == 2400000 ? resample::in_lo(o0 - MODES_CARRY_BYTES / 2) : o0 - kHaloSamples;
+}
+int64_t batch_in_hi(const modes_ctx *ctx, int64_t o1) {
+    return ctx->input_rate == 2400000 ? resample::in_hi(o1 - 1) : o1;
+}
+
+// Upload the input bytes the slot's batch (nb buffers from s.buffer_base, and the carry before them) reads,
+// straight from where they are, and make the slot's body and carry block from them on the device.
+int stage_held(modes_ctx *ctx, Slot &s, const Source &src, size_t nb) {
+    const int bps = input::sample_bytes(ctx->input_format);
     const int64_t o0 = s.buffer_base * (int64_t)kBufSamples;
     const int64_t o1 = o0 + (int64_t)nb * kBufSamples;
-    int64_t lo = 2 * resample::in_lo(o0 - MODES_CARRY_BYTES / 2);
-    int64_t hi = 2 * resample::in_hi(o1 - 1);
+    int64_t lo = bps * batch_in_lo(ctx, o0);
+    int64_t hi = bps * batch_in_hi(ctx, o1);
     if (lo < 0) lo = 0;
     if (hi > src.end) hi = src.end;
     if (hi < lo) hi = lo;
@@ -654,9 +674,11 @@ int stage_resampled(modes_ctx *ctx, Slot &s, const Source &src, size_t nb) {
         CK(ctx, cudaMemcpyAsync(s.d_in.get() + (from - lo), src.call + (from - src.call0), (size_t)(hi - from),
                                 cudaMemcpyHostToDevice, s.stream));
     }
-    launch_resample(ResampleJob{s.d_in.get(), (uint64_t)(hi - lo), lo / 2, o0, (uint64_t)(o1 - o0), src.out_end,
-                                s.d_iq.get(), s.d_halo.get()},
-                    s.stream);
+    const ResampleJob j{s.d_in.get(), (uint64_t)(hi - lo), lo / bps, o0, (uint64_t)(o1 - o0), src.out_end,
+                        s.d_iq.get(), s.d_halo.get()};
+    if (ctx->input_format == input::kUC8) launch_resample(j, s.stream);
+    else if (ctx->input_rate == 2400000) launch_resample_sc16(j, ctx->input_shift, s.stream);
+    else launch_convert_sc16(j, ctx->input_shift, s.stream);
     CK(ctx, cudaGetLastError());
     ctx->launches++;
     return 0;
@@ -666,7 +688,7 @@ int stage_resampled(modes_ctx *ctx, Slot &s, const Source &src, size_t nb) {
 // ctx itself, or one of its GPUs), and move src past them.
 int submit_next(modes_ctx *ctx, modes_ctx *g, Slot &s, Source &src, size_t nb) {
     if (!src.iq) {
-        if (stage_resampled(g, s, src, nb)) return -1;
+        if (stage_held(g, s, src, nb)) return -1;
         return submit(g, s, nullptr, s.d_iq.get(), nb, nullptr, nullptr, 0, nullptr, true);
     }
     if (submit(g, s, src.iq, nullptr, nb, ctx->carry, nullptr, 0, nullptr)) return -1;
@@ -737,32 +759,37 @@ Source host_buffers(const uint8_t *iq) {
     return src;
 }
 
-// 2.4 MS/s: the most the hold can need: the input of one reference buffer and of the carry before it,
-// with the filter's reach on both sides (a whole buffer's input would have run).
-constexpr size_t kHoldBytes = 2 * ((size_t)6 * (kBufSamples + MODES_CARRY_BYTES / 2) / 5 + 2 * resample::kTaps + 16);
+// The most the hold can need: the input of one reference buffer and of the carry before it, with the
+// filter's reach on both sides at 2.4 MS/s (a whole buffer's input would have run).
+size_t hold_bytes(const modes_ctx *ctx) {
+    const size_t reach = ctx->input_rate == 2400000
+                             ? (size_t)6 * (kBufSamples + MODES_CARRY_BYTES / 2) / 5 + 2 * resample::kTaps
+                             : (size_t)kBufSamples + kHaloSamples;
+    return (size_t)input::sample_bytes(ctx->input_format) * (reach + 16);
+}
 
-// 2.4 MS/s: run every whole buffer whose input (with the filter's lookahead) has arrived, reading the
+// Run every whole buffer whose input (at 2.4 MS/s with the filter's lookahead) has arrived, reading the
 // hold and the caller's bytes where they are (run_buffers returns with every copy done), then keep in
-// the hold what later batches read.
-int process_resampled(modes_ctx *ctx, const uint8_t *iq, size_t nbytes) {
-    CK(ctx, ctx->hold.ensure(kHoldBytes));
+// the hold what later batches read, a sample split across calls included.
+int process_held(modes_ctx *ctx, const uint8_t *iq, size_t nbytes) {
+    CK(ctx, ctx->hold.ensure(hold_bytes(ctx)));
     const int64_t call0 = ctx->in_total;
     ctx->in_total += (int64_t)nbytes;
-    const int64_t avail = ctx->in_total / 2;                               // whole input samples
+    const int64_t avail = ctx->in_total / input::sample_bytes(ctx->input_format);   // whole input samples
     const int64_t B = kBufSamples;
-    int64_t m = (5 * avail / 6) / B;                                        // buffers [0, m) are ready
-    while (m > ctx->buffers_done && resample::in_hi(m * B - 1) > avail) m--;
-    while (resample::in_hi((m + 1) * B - 1) <= avail) m++;
+    int64_t m = (ctx->input_rate == 2400000 ? 5 * avail / 6 : avail) / B;       // buffers [0, m) are ready
+    while (m > ctx->buffers_done && batch_in_hi(ctx, m * B) > avail) m--;
+    while (batch_in_hi(ctx, (m + 1) * B) <= avail) m++;
     if (m > ctx->buffers_done) {
         Source src;
         src.hold = ctx->hold.get(); src.hold0 = ctx->hold0;
         src.call = iq; src.call0 = call0; src.end = ctx->in_total;
         if (run_buffers(ctx, src, (size_t)(m - ctx->buffers_done))) return -1;
     }
-    int64_t keep = 2 * resample::in_lo(ctx->buffers_done * B - MODES_CARRY_BYTES / 2);
+    int64_t keep = input::sample_bytes(ctx->input_format) * batch_in_lo(ctx, ctx->buffers_done * B);
     if (keep < ctx->hold0) keep = ctx->hold0;
     if ((size_t)(ctx->in_total - keep) > ctx->hold.capacity())
-        return fail(ctx, "internal: 2.4 MS/s input history of %lld bytes", (long long)(ctx->in_total - keep));
+        return fail(ctx, "internal: input history of %lld bytes", (long long)(ctx->in_total - keep));
     uint8_t *h = ctx->hold.get();
     if (keep < call0) {
         memmove(h, h + (keep - ctx->hold0), (size_t)(call0 - keep));
@@ -774,10 +801,13 @@ int process_resampled(modes_ctx *ctx, const uint8_t *iq, size_t nbytes) {
     return 0;
 }
 
-// 2.4 MS/s at the end of the stream: the output is N_out = ceil(5 n_in / 6) samples; the remaining whole
-// buffers and the EOF buffer (127 past N_out) run from the hold, the input 127-padded past its end.
-int finish_resampled(modes_ctx *ctx) {
-    const int64_t n_out = resample::n_out((ctx->in_total + 1) / 2);
+// The end of a held stream: n_in input samples (UC8: ceil(bytes / 2), a trailing odd byte an I whose Q is
+// 127; 16-bit: floor(bytes / 4)) make N_out = n_in (2 MHz) or ceil(5 n_in / 6) (2.4 MS/s) output samples;
+// the remaining whole buffers and the EOF buffer (127 past N_out) run from the hold, the input 127-padded
+// past its end.
+int finish_held(modes_ctx *ctx) {
+    const int64_t n_in = ctx->input_format == input::kUC8 ? (ctx->in_total + 1) / 2 : ctx->in_total / 4;
+    const int64_t n_out = ctx->input_rate == 2400000 ? resample::n_out(n_in) : n_in;
     ctx->eof_buffer = n_out / kBufSamples;                                  // its level record counts the real samples only
     ctx->eof_samples = (uint32_t)(n_out % kBufSamples);
     const int64_t last = ctx->eof_buffer + (ctx->cfg.drop_eof_buffer ? 0 : 1);
@@ -1102,12 +1132,34 @@ int modes_set_input_rate(modes_ctx *ctx, uint32_t hz) {
     return 0;
 }
 
+int modes_set_input_format(modes_ctx *ctx, uint32_t format, int32_t shift) {
+    if (!ctx) return -1;
+    if (!input::known(format))
+        return fail(ctx, "modes_set_input_format: format %u is not supported (MODES_INPUT_UC8, MODES_INPUT_SC16 or "
+                         "MODES_INPUT_SC16Q11)", format);
+    if (shift > input::kMaxShift)
+        return fail(ctx, "modes_set_input_format: shift %d is not supported (0 to %d, or negative for the format's default)",
+                    (int)shift, input::kMaxShift);
+    if (format == input::kUC8 && shift > 0)
+        return fail(ctx, "modes_set_input_format: shift %d is not supported with UC8 (0, or negative)", (int)shift);
+    if (ctx->started && !ctx->finished)
+        return fail(ctx, "modes_set_input_format: a stream is in progress; call modes_finish or modes_reset first");
+    const int s = shift < 0 ? input::default_shift(format) : (int)shift;
+    ctx->input_format = format;
+    ctx->input_shift = s;
+    for (modes_ctx *g : ctx->gpus) {
+        g->input_format = format;
+        g->input_shift = s;
+    }
+    return 0;
+}
+
 int modes_process(modes_ctx *ctx, const uint8_t *iq, size_t nbytes) {
     if (!ctx) return -1;
     if (ctx->finished) return fail(ctx, "modes_process after modes_finish; call modes_reset first");
     CK(ctx, cudaSetDevice(ctx->cfg.device));
     ctx->started = true;
-    if (ctx->input_rate == 2400000) return process_resampled(ctx, iq, nbytes);
+    if (held_input(ctx)) return process_held(ctx, iq, nbytes);
     if (ctx->pending_len) {
         size_t take = MODES_BUFFER_BYTES - ctx->pending_len;
         if (take > nbytes) take = nbytes;
@@ -1130,7 +1182,7 @@ int modes_finish(modes_ctx *ctx) {
     CK(ctx, cudaSetDevice(ctx->cfg.device));
     ctx->finished = true;
     ctx->started = true;
-    if (ctx->input_rate == 2400000) return finish_resampled(ctx);
+    if (held_input(ctx)) return finish_held(ctx);
     // The read that hits EOF still hands a 127-padded buffer to the decoder (dump1090.c:496-510);
     // whether it is decoded is the reference's race, made a switch here.
     memset(ctx->pending.get() + ctx->pending_len, 127, MODES_BUFFER_BYTES - ctx->pending_len);

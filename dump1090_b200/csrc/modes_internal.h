@@ -85,7 +85,7 @@ void launch_levels(const uint8_t *d_iq, uint32_t n_buffers, uint64_t stride_byte
                    modes_level *out, int sm_count, cudaStream_t stream);
 static_assert(sizeof(modes_level) == 40 && offsetof(modes_level, sum_mag) == 16 && offsetof(modes_level, peak) == 32,
               "level record layout");
-// 2.4 MS/s input resampled to 2 MHz bytes (modes_resample.cu, arithmetic in modes_resample_core.cuh).
+// 2.4 MS/s UC8 input resampled to 2 MHz bytes (modes_resample.cu, arithmetic in modes_resample_core.cuh).
 // Output sample n (stream index, 2 MHz) reads the input samples around 1.2 n; the job holds the stream's
 // input bytes [2 in_first, 2 in_first + in_bytes) and every other input byte reads as 127.
 struct ResampleJob {
@@ -100,6 +100,12 @@ struct ResampleJob {
                                  // body[0] at kHaloBytes - MODES_CARRY_BYTES, 127 elsewhere), or nullptr
 };
 void launch_resample(const ResampleJob &j, cudaStream_t stream);
+// 16-bit input (modes_set_input_format, arithmetic in modes_input_core.cuh): the same job over int16 I/Q,
+// in[0] the first byte of input sample in_first (4 bytes a sample, a trailing partial sample not in the
+// span), converted with the shift and then resampled (K9, 2.4 MS/s) or converted only (K10, 2 MHz:
+// output sample n is input sample n; in_first a multiple of 4, so that its 16-byte loads are aligned).
+void launch_resample_sc16(const ResampleJob &j, int shift, cudaStream_t stream);
+void launch_convert_sc16(const ResampleJob &j, int shift, cudaStream_t stream);
 // The receiver pool's 2.4 MS/s receivers (modes_pool.cpp): one launch for one job per pair of the pool's
 // batch.  A job's input is its receiver's stream bytes [hist0, call0) at hist (the receiver's device input
 // history) and [call0, call0 + MODES_BUFFER_BYTES) at stage (the call's bytes); every other input byte

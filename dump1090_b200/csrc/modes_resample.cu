@@ -7,7 +7,14 @@
 // periods (the taps are immediates, no index arithmetic by 5 or 6), and the block writes the tile's
 // output with 16-byte stores.  Tiles start at a period index that is a multiple of 8 (80 output bytes),
 // so with the body starting at a multiple of 8 samples every body store is aligned.
+//
+// 16-bit input (modes_set_input_format, arithmetic in modes_input_core.cuh) is converted, then resampled:
+// at 2.4 MS/s K9's staging loader converts each int16 sample to its UC8 pair as it fills s_in, so the
+// filter sees exactly the bytes it would see on the converted stream; at 2 MHz K10 (convert_kernel)
+// converts the batch's span straight into its body and carry block.  UC8 keeps its own loader, chosen
+// at compile time.
 #include "modes_internal.h"
+#include "modes_input_core.cuh"
 #include "modes_resample_core.cuh"
 
 namespace modes {
@@ -42,38 +49,69 @@ __device__ __forceinline__ void tile_periods(const uint8_t *x_in, uint8_t *s_out
     }
 }
 
-__global__ void __launch_bounds__(kThreads) resample_kernel(ResampleJob j, int64_t q_first) {
+// Staging loaders: the 16 UC8 bytes of the tile's input at byte p of the converted stream relative to the
+// job's first input sample (p a multiple of 16); bytes outside the job's span are no signal.
+struct Uc8Input {
+    __device__ __forceinline__ uint4 word(const ResampleJob &j, int64_t p) const {
+        const int64_t in_bytes = (int64_t)j.in_bytes;
+        if (p >= 0 && p + 16 <= in_bytes) return __ldg(reinterpret_cast<const uint4 *>(j.in + p));
+        uint32_t b[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            uint32_t word = 0;
+#pragma unroll
+            for (int e = 0; e < 4; e++) {
+                const int64_t pe = p + 4 * k + e;
+                const uint32_t x = (pe >= 0 && pe < in_bytes) ? j.in[pe] : 127u;
+                word |= x << (8 * e);
+            }
+            b[k] = word;
+        }
+        return make_uint4(b[0], b[1], b[2], b[3]);
+    }
+};
+
+// SC16 / SC16Q11: the 8 samples of a word are 32 int16 bytes at 2 p; a sample is in the span when all 4
+// of its bytes are (the trailing partial sample is not).  A missing sample reads as (0, 0), which
+// converts to (127, 127) at every shift.
+struct Sc16Input {
+    int shift;
+    __device__ __forceinline__ uint4 word(const ResampleJob &j, int64_t p) const {
+        const int64_t b = 2 * p;
+        const int64_t in_bytes = (int64_t)(j.in_bytes & ~(uint64_t)3);
+        uint32_t w[8];
+        if (b >= 0 && b + 32 <= in_bytes) {
+            const uint4 lo = __ldg(reinterpret_cast<const uint4 *>(j.in + b));
+            const uint4 hi = __ldg(reinterpret_cast<const uint4 *>(j.in + b + 16));
+            w[0] = lo.x; w[1] = lo.y; w[2] = lo.z; w[3] = lo.w;
+            w[4] = hi.x; w[5] = hi.y; w[6] = hi.z; w[7] = hi.w;
+        } else {
+#pragma unroll
+            for (int k = 0; k < 8; k++) {
+                const int64_t e = b + 4 * k;
+                w[k] = (e >= 0 && e + 4 <= in_bytes) ? __ldg(reinterpret_cast<const uint32_t *>(j.in + e)) : 0u;
+            }
+        }
+        uint32_t o[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++)
+            o[k] = input::convert_pair(w[2 * k], shift) | input::convert_pair(w[2 * k + 1], shift) << 16;
+        return make_uint4(o[0], o[1], o[2], o[3]);
+    }
+};
+
+template <class Input>
+__device__ __forceinline__ void resample_tile(const ResampleJob &j, int64_t q_first, const Input &input) {
     __shared__ __align__(16) uint8_t s_in[kInWords * 16];
     __shared__ __align__(16) uint8_t s_out[kTileOutBytes];
     const int64_t q0 = q_first + (int64_t)blockIdx.x * kPeriods;
 
-    // input samples 6 q0 - kLead ... of the tile; bytes outside the job's span are no signal
+    // input samples 6 q0 - kLead ... of the tile
     const int64_t off = 2 * (6 * q0 - R::kLead - j.in_first);
     const int64_t a0 = off & ~(int64_t)15;
     const int sh = (int)(off - a0);
-    const int64_t in_bytes = (int64_t)j.in_bytes;
-    for (int w = threadIdx.x; w < kInWords; w += kThreads) {
-        const int64_t p = a0 + 16 * (int64_t)w;
-        uint4 v;
-        if (p >= 0 && p + 16 <= in_bytes) {
-            v = __ldg(reinterpret_cast<const uint4 *>(j.in + p));
-        } else {
-            uint32_t b[4];
-#pragma unroll
-            for (int k = 0; k < 4; k++) {
-                uint32_t word = 0;
-#pragma unroll
-                for (int e = 0; e < 4; e++) {
-                    const int64_t pe = p + 4 * k + e;
-                    const uint32_t x = (pe >= 0 && pe < in_bytes) ? j.in[pe] : 127u;
-                    word |= x << (8 * e);
-                }
-                b[k] = word;
-            }
-            v = make_uint4(b[0], b[1], b[2], b[3]);
-        }
-        *reinterpret_cast<uint4 *>(s_in + 16 * w) = v;
-    }
+    for (int w = threadIdx.x; w < kInWords; w += kThreads)
+        *reinterpret_cast<uint4 *>(s_in + 16 * w) = input.word(j, a0 + 16 * (int64_t)w);
     __syncthreads();
 
     tile_periods(s_in + sh, s_out, q0, j.out_end);
@@ -100,6 +138,36 @@ __global__ void __launch_bounds__(kThreads) resample_kernel(ResampleJob j, int64
             for (int b = threadIdx.x; b < kHaloAlloc; b += kThreads)
                 if (b < kHaloBytes - MODES_CARRY_BYTES || b >= kHaloBytes) j.halo[b] = 127;
     }
+}
+
+__global__ void __launch_bounds__(kThreads) resample_kernel(ResampleJob j, int64_t q_first) {
+    resample_tile(j, q_first, Uc8Input{});
+}
+
+__global__ void __launch_bounds__(kThreads) resample_sc16_kernel(ResampleJob j, int64_t q_first, int shift) {
+    resample_tile(j, q_first, Sc16Input{shift});
+}
+
+// K10: 2 MHz int16 input.  Output sample n is input sample n converted, so a thread converts a group of 8
+// samples (32 input bytes, two 16-byte loads) into one 16-byte store.  The groups start at g_first
+// (8 g_first = out_first, or out_first - 240 with the carry block) and cover the carry block's 240
+// samples (the first 2 no signal) and the body; block 0 also writes the block's trailing no-signal bytes.
+__global__ void __launch_bounds__(kThreads) convert_kernel(ResampleJob j, int64_t g_first, int64_t n_groups, int shift) {
+    if (j.halo && blockIdx.x == 0 && threadIdx.x < (kHaloAlloc - kHaloBytes) / 16)
+        reinterpret_cast<uint4 *>(j.halo + kHaloBytes)[threadIdx.x] = make_uint4(0x7f7f7f7fu, 0x7f7f7f7fu, 0x7f7f7f7fu, 0x7f7f7f7fu);
+    const int64_t g = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+    if (g >= n_groups) return;
+    const int64_t n0 = 8 * (g_first + g);
+    uint4 v = Sc16Input{shift}.word(j, 2 * (n0 - j.in_first));
+    const int64_t c0 = j.out_first - MODES_CARRY_BYTES / 2;
+    if (n0 + 8 > j.out_end || n0 < c0) {
+        uint16_t *x = reinterpret_cast<uint16_t *>(&v);
+#pragma unroll
+        for (int k = 0; k < 8; k++)
+            if (n0 + k >= j.out_end || n0 + k < c0) x[k] = 0x7f7fu;
+    }
+    uint8_t *dst = n0 >= j.out_first ? j.body + 2 * (n0 - j.out_first) : j.halo + 2 * (n0 - (j.out_first - kHaloSamples));
+    *reinterpret_cast<uint4 *>(dst) = v;
 }
 
 // ---- the receiver pool (modes_pool.cpp): one launch for the batch's jobs, grid (tile, job)
@@ -183,12 +251,33 @@ void launch_history_pool(const PoolHistoryJob *d_jobs, uint32_t n_jobs, uint64_t
     if (n_jobs && blocks) history_pool_kernel<<<dim3(blocks, n_jobs), kThreads, 0, stream>>>(d_jobs);
 }
 
-void launch_resample(const ResampleJob &j, cudaStream_t stream) {
+// K9's tiles for a job: the first period (a multiple of 8) and the number of tiles.
+void resample_grid(const ResampleJob &j, int64_t *q_first, unsigned *blocks) {
     const int64_t first = j.out_first - (j.halo ? MODES_CARRY_BYTES / 2 : 0);
-    const int64_t q_first = R::floor_div(R::floor_div(first, 5), 8) * 8;
+    *q_first = R::floor_div(R::floor_div(first, 5), 8) * 8;
     const int64_t q_end = R::floor_div(j.out_first + (int64_t)j.out_samples - 1, 5) + 1;
-    const int64_t blocks = (q_end - q_first + kPeriods - 1) / kPeriods;
-    resample_kernel<<<(unsigned)blocks, kThreads, 0, stream>>>(j, q_first);
+    *blocks = (unsigned)((q_end - *q_first + kPeriods - 1) / kPeriods);
+}
+
+void launch_resample(const ResampleJob &j, cudaStream_t stream) {
+    int64_t q_first;
+    unsigned blocks;
+    resample_grid(j, &q_first, &blocks);
+    resample_kernel<<<blocks, kThreads, 0, stream>>>(j, q_first);
+}
+
+void launch_resample_sc16(const ResampleJob &j, int shift, cudaStream_t stream) {
+    int64_t q_first;
+    unsigned blocks;
+    resample_grid(j, &q_first, &blocks);
+    resample_sc16_kernel<<<blocks, kThreads, 0, stream>>>(j, q_first, shift);
+}
+
+void launch_convert_sc16(const ResampleJob &j, int shift, cudaStream_t stream) {
+    const int64_t first = j.out_first - (j.halo ? kHaloSamples : 0);
+    const int64_t groups = (j.out_first + (int64_t)j.out_samples - first) / 8;
+    const int64_t blocks = (groups + kThreads - 1) / kThreads;
+    convert_kernel<<<(unsigned)blocks, kThreads, 0, stream>>>(j, first / 8, groups, shift);
 }
 
 }  // namespace modes

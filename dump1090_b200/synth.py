@@ -173,10 +173,13 @@ def frame_envelope_at(frame: bytes, pos: int, frac: float, sample_rate: int) -> 
     return first, env
 
 
-def synth_stream_at(nsamples: int, frames, sigma: float = 1.5, seed: int = 1, sample_rate: int = 2_000_000) -> np.ndarray:
+def synth_stream_at(nsamples: int, frames, sigma: float = 1.5, seed: int = 1, sample_rate: int = 2_000_000,
+                    dtype: str = "uc8", scale: float = 1.0) -> np.ndarray:
     """synth_stream at any sample rate: frames are (pos, frame_bytes, amplitude_lsb, carrier_phase_rad,
     frac) with the arrival time pos + frac in 2 MHz samples (0.5 us), pulses per frame_envelope_at, and
-    the same noise per sample as synth_stream.  At 2 MHz it equals synth_stream bit for bit."""
+    the same noise per sample as synth_stream.  At 2 MHz it equals synth_stream bit for bit.
+    dtype="sc16": the same signal as signed little-endian 16-bit I/Q bytes (4 a sample), scale int16
+    units to an 8-bit LSB (16 is SC16Q11's full scale, 256 SC16's), rounded and clamped to int16."""
     i = noise(nsamples, sigma, seed * 2 + 11)
     q = noise(nsamples, sigma, seed * 2 + 12)
     for pos, frame, amp, phase, frac in frames:
@@ -190,6 +193,13 @@ def synth_stream_at(nsamples: int, frames, sigma: float = 1.5, seed: int = 1, sa
         seg = env[: end - start]
         i[start:end] += seg * np.cos(phase)
         q[start:end] += seg * np.sin(phase)
+    if dtype == "sc16":
+        out16 = np.empty(2 * nsamples, dtype="<i2")
+        out16[0::2] = np.clip(np.rint(scale * i), -32768, 32767)
+        out16[1::2] = np.clip(np.rint(scale * q), -32768, 32767)
+        return out16.view(np.uint8)
+    if dtype != "uc8":
+        raise ValueError(f"dtype {dtype!r}: uc8 or sc16")
     out = np.empty(2 * nsamples, dtype=np.uint8)
     out[0::2] = np.clip(np.rint(127.0 + i), 0, 255).astype(np.uint8)
     out[1::2] = np.clip(np.rint(127.0 + q), 0, 255).astype(np.uint8)
@@ -354,10 +364,10 @@ def fleet_at(snr_db: float, nframes: int, seed: int, n_aircraft: int = 20, amp: 
 
 
 def fleet_at_rate(snr_db: float, nframes: int, seed: int, sample_rate: int = 2_400_000, n_aircraft: int = 20,
-                  amp: float = 20.0, period: int = 400):
+                  amp: float = 20.0, period: int = 400, dtype: str = "uc8", scale: float = 1.0):
     """fleet_at sampled at sample_rate (2.4 MS/s: what dump1090-fa and readsb record): the same frames,
     arrival times, amplitudes and carrier phases, over the same stretch of time, with the same noise per
-    sample.  Returns (stream, set of the frames' hex)."""
+    sample; dtype and scale as synth_stream_at.  Returns (stream, set of the frames' hex)."""
     sigma = amp / (np.sqrt(2.0) * 10 ** (snr_db / 20.0))
     rng = Counter(seed)
     fleet = [0x400000 + rng.below(0x3FFFFF) for _ in range(n_aircraft)]
@@ -370,7 +380,7 @@ def fleet_at_rate(snr_db: float, nframes: int, seed: int, sample_rate: int = 2_4
         truth.add(frame.hex())
     a, b = _rate_ratio(sample_rate)
     n = -(-(200 + nframes * period + 400) * a // b)
-    return synth_stream_at(n, frames, sigma=sigma, seed=seed, sample_rate=sample_rate), truth
+    return synth_stream_at(n, frames, sigma=sigma, seed=seed, sample_rate=sample_rate, dtype=dtype, scale=scale), truth
 
 
 def tile_to(data: np.ndarray, nbytes: int) -> np.ndarray:

@@ -1,7 +1,7 @@
 /* dump1090-b200 — C host for the H100 demodulator: the --ifile side of
  * dump1090's command line (dump1090.c:2849-3010) over the C ABI of
  * include/modes_b200.h.  Reads 8-bit unsigned I/Q at 2 MHz from a file (or '-'
- * for stdin), feeds it to the device library, prints what the reference prints.
+ * for stdin; --sample-rate and --iformat below for other captures), feeds it to the device library, prints what the reference prints.
  *
  * Supported options (same spelling and meaning as the reference):
  *   --ifile <file>  --raw  --onlyaddr  --no-fix  --no-crc-check  --aggressive  --stats
@@ -30,12 +30,18 @@
  * --sample-rate <hz> gives the rate of the file: 2000000 (the default) or 2400000, what dump1090-fa and
  * readsb record (modes_set_input_rate: resampled to 2 MHz on the GPU, sample positions and Beast
  * timestamps on the same 2 MHz / 12 MHz clocks).  It combines with every output mode and switch.
+ * --iformat UC8|SC16|SC16Q11 gives the sample format of the file, as dump1090-fa spells it: 8-bit
+ * unsigned (the default), or signed 16-bit I/Q (SoapySDR and Airspy-class tools; bladeRF's 12-bit values),
+ * converted to 8 bits on the GPU (modes_set_input_format).  --iformat-shift <0..15> replaces the
+ * format's default shift (SC16 8, SC16Q11 4; not with UC8): a smaller one for a quiet capture, checked
+ * with the clipping count of --levels.  Both combine with --sample-rate, every output mode and switch.
  * The live-radio, networking and interactive options are out of scope.
  */
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <strings.h>
 #include "modes_b200.h"
 
 static int opt_raw = 0, opt_onlyaddr = 0, opt_stats = 0, opt_check_crc = 1, opt_sbs = 0, opt_json = 0, opt_beast = 0;
@@ -109,6 +115,8 @@ int main(int argc, char **argv) {
     const char *filename = NULL;
     size_t chunk = 16u << 20;
     unsigned long sample_rate = 2000000;
+    const char *iformat = "UC8";
+    const char *iformat_shift = NULL;
     modes_default_config(&cfg);
     for (int j = 1; j < argc; j++) {
         int more = j + 1 < argc;
@@ -132,6 +140,8 @@ int main(int argc, char **argv) {
         else if (!strcmp(argv[j], "--gpus") && more) cfg.n_gpus = atoi(argv[++j]);
         else if (!strcmp(argv[j], "--chunk") && more) chunk = (size_t)strtoull(argv[++j], NULL, 10);
         else if (!strcmp(argv[j], "--sample-rate") && more) sample_rate = strtoul(argv[++j], NULL, 10);
+        else if (!strcmp(argv[j], "--iformat") && more) iformat = argv[++j];
+        else if (!strcmp(argv[j], "--iformat-shift") && more) iformat_shift = argv[++j];
         else {
             fprintf(stderr, "Unknown or not enough arguments for option '%s'.\n", argv[j]);
             return 1;
@@ -141,6 +151,28 @@ int main(int argc, char **argv) {
     if (sample_rate != 2000000 && sample_rate != 2400000) {
         fprintf(stderr, "--sample-rate takes 2000000 or 2400000\n");
         return 1;
+    }
+    uint32_t format;
+    if (!strcasecmp(iformat, "UC8")) format = MODES_INPUT_UC8;
+    else if (!strcasecmp(iformat, "SC16")) format = MODES_INPUT_SC16;
+    else if (!strcasecmp(iformat, "SC16Q11")) format = MODES_INPUT_SC16Q11;
+    else {
+        fprintf(stderr, "--iformat takes UC8, SC16 or SC16Q11\n");
+        return 1;
+    }
+    int32_t shift = -1;
+    if (iformat_shift) {
+        char *end;
+        const long v = strtol(iformat_shift, &end, 10);
+        if (!*iformat_shift || *end || v < 0 || v > 15) {
+            fprintf(stderr, "--iformat-shift takes a whole number from 0 to 15\n");
+            return 1;
+        }
+        if (format == MODES_INPUT_UC8) {
+            fprintf(stderr, "--iformat-shift needs --iformat SC16 or SC16Q11: UC8 input is not shifted\n");
+            return 1;
+        }
+        shift = (int32_t)v;
     }
     if (opt_beast && (opt_raw || opt_onlyaddr || opt_sbs || opt_json)) {
         fprintf(stderr, "--beast writes binary frames to stdout: it cannot be combined with --raw, --onlyaddr, --sbs or --aircraft-json\n");
@@ -165,6 +197,7 @@ int main(int argc, char **argv) {
         if (!tracker) { fprintf(stderr, "out of memory\n"); return 1; }
     }
     if (modes_set_input_rate(ctx, (uint32_t)sample_rate)) { fprintf(stderr, "--sample-rate: %s\n", modes_last_error(ctx)); return 1; }
+    if (modes_set_input_format(ctx, format, shift)) { fprintf(stderr, "--iformat: %s\n", modes_last_error(ctx)); return 1; }
     if (opt_beast) modes_set_signal(ctx, 1);
     if (opt_arrival) modes_set_arrival(ctx, 1);
     if (opt_levels) modes_set_levels(ctx, 1);

@@ -211,6 +211,32 @@ int  modes_set_input_rate(modes_ctx *ctx, uint32_t hz);
 typedef struct modes_pool modes_pool;                /* the receiver pool: "many receivers on one GPU" below */
 int  modes_pool_set_input_rate(modes_pool *p, uint32_t receiver, uint32_t hz);
 
+/* ---- 16-bit input ---------------------------------------------------------- */
+/* The sample format of the bytes modes_process takes, dump1090-fa's --iformat:
+ *   MODES_INPUT_UC8      unsigned 8-bit I/Q, zero at 127 (the default, what dump1090 reads)
+ *   MODES_INPUT_SC16     signed little-endian 16-bit I/Q (SoapySDR devices, Airspy-class tools)
+ *   MODES_INPUT_SC16Q11  the same with 12-bit values (bladeRF)
+ * shift: 0 ... 15, or negative for the format's default, which maps full scale to full scale: 8 for SC16,
+ * 4 for SC16Q11.  Refused: an unknown format, a shift above 15, a shift other than 0 or negative with
+ * UC8, and, as modes_set_input_rate, a call between the first modes_process of a stream and
+ * modes_finish / modes_reset.  It takes effect for the stream that begins at create or reset (which keeps
+ * it), reaches every GPU of an n_gpus > 1 context, and combines with either input rate.  The receiver
+ * pool takes UC8 only.
+ *
+ * A 16-bit stream is converted to UC8 on the device, then decoded as a UC8 stream at the input rate
+ * (at 2400000: converted, then resampled), so it decodes to exactly what the UC8 decoder gives on the
+ * converted bytes:
+ *   input   I, Q interleaved, 4 bytes a sample; n_in = floor(bytes / 4), 1-3 trailing bytes are ignored
+ *   output  for a value v (I or Q) and the shift s, in int32 with an arithmetic shift (round half up):
+ *               q = s ? (v + (1 << (s - 1))) >> s : v,   byte = clamp(127 + q, 0, 255)
+ * At 2 MHz the EOF buffer is 127 past n_in, as modes_finish pads a UC8 stream.  Level records describe
+ * the converted bytes, so their clipping count is the samples the shift saturated: a smaller shift
+ * resolves weaker signals and clips strong ones sooner. */
+#define MODES_INPUT_UC8      0u
+#define MODES_INPUT_SC16     1u
+#define MODES_INPUT_SC16Q11  2u
+int  modes_set_input_format(modes_ctx *ctx, uint32_t format, int32_t shift);
+
 /* ---- stage-level entry points (tests, bench, multi-GPU sharding) -------- */
 /* computeMagnitudeVector() alone (dump1090.c:1454-1469): nsamples I/Q pairs in
  * host memory -> nsamples u16 magnitudes in host memory, computed on the device. */
