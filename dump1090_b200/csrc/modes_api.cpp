@@ -74,17 +74,22 @@ struct Slot {
     DevBuf<uint32_t> d_cand_v;       // its capacity is the slot's candidate capacity
     DevBuf<modes_candidate> d_records;
     DevBuf<modes_tile> d_tiles;
-    DevBuf<uint32_t> d_counters;
-    // pinned carry blocks: a ring, because modes_detect_device/_host return without waiting and the
-    // next call must not rewrite a block whose host-to-device copy is still queued
-    static constexpr int kHaloRing = 8;
-    PinnedBuf<uint8_t> h_halo;       // kHaloRing x kHaloAlloc
-    cudaEvent_t halo_ev[kHaloRing] = {};
-    unsigned halo_next = 0;
-    PinnedBuf<uint32_t> h_counters;
+    // two counter sets (ScanOutputs), used in turn: `set` is the last batch's, and its scan zeroed the
+    // other one for the slot's next batch (whose scan runs after every pass that reads this batch's set)
+    DevBuf<uint32_t> d_counters;     // 2 x kCounterWords
+    unsigned set = 1;
+    uint32_t *counters() const { return d_counters.get() + kCounterWords * set; }
+    // the last batch's candidate count and overflow flag, written by its scan (mapped pinned memory)
+    uint32_t *h_counts = nullptr;
+    // the batch's carry block, passed to the scan by value (carry_on_host), or already on the device in
+    // d_halo (the resampler writes it there)
+    uint8_t carry[kHaloAlloc];
+    bool carry_on_host = false;
     PinnedBuf<modes_candidate> h_records;
     PinnedBuf<modes_tile> h_tiles;
-    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    // the batch's last operation on the stream (what wait_batch waits for); never timed, so that recording it
+    // costs the stream no timestamp
+    cudaEvent_t done = nullptr;
     // cfg.gpu_resolve: workspace of the device resolve (the storage behind a GpuResolve view)
     DevBuf<uint32_t> gr_start, gr_end, gr_written, gr_readfirst, gr_rerun, gr_n_deliv, gr_offsets, gr_flags;
     DevBuf<uint64_t> gr_stats;
@@ -261,18 +266,21 @@ uint32_t default_cand_capacity(uint64_t n_samples) {
 int slot_init(modes_ctx *ctx, Slot &s) {
     CK(ctx, cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
     CK(ctx, s.d_halo.ensure(kHaloAlloc));
-    CK(ctx, s.d_counters.ensure(4));
-    CK(ctx, s.h_halo.ensure((size_t)kHaloAlloc * Slot::kHaloRing));
-    for (auto &e : s.halo_ev) CK(ctx, cudaEventCreateWithFlags(&e, event_flags(false)));
-    CK(ctx, s.h_counters.ensure(4));
-    for (auto &e : s.ev) CK(ctx, cudaEventCreateWithFlags(&e, event_flags(true)));
+    CK(ctx, s.d_counters.ensure(2 * kCounterWords));
+    CK(ctx, cudaMemsetAsync(s.d_counters.get(), 0, 2 * kCounterWords * sizeof(uint32_t), s.stream));
+    CK(ctx, cudaStreamSynchronize(s.stream));
+    void *h = nullptr;
+    CK(ctx, cudaHostAlloc(&h, 2 * sizeof(uint32_t), cudaHostAllocMapped));
+    s.h_counts = static_cast<uint32_t *>(h);
+    s.h_counts[0] = s.h_counts[1] = 0;
+    CK(ctx, cudaEventCreateWithFlags(&s.done, event_flags(false)));
     return 0;
 }
 
 void slot_free(Slot &s) {
     if (s.stream) wait_stream(s.stream);
-    for (auto &e : s.ev) if (e) cudaEventDestroy(e);
-    for (auto &e : s.halo_ev) if (e) cudaEventDestroy(e);
+    if (s.done) cudaEventDestroy(s.done);
+    if (s.h_counts) cudaFreeHost(s.h_counts);
     if (s.stream) cudaStreamDestroy(s.stream);
     s = Slot();                       // releases its buffers: nothing queued uses them any more
 }
@@ -319,8 +327,8 @@ int gpu_resolve_ensure(modes_ctx *ctx, Slot &s, GpuResolve &g) {
     return 0;
 }
 
-// Queue one batch on the slot's stream: (optional H2D) + halo + scan + frame evaluation.  halo_on_device:
-// the slot's carry block is already queued on the stream (the resampler writes it), so carry476 is unused.
+// Queue one batch on the slot's stream: (optional H2D) + scan + frame evaluation.  halo_on_device: the
+// slot's carry block is already queued on the stream (the resampler writes it), so carry476 is unused.
 int submit(modes_ctx *ctx, Slot &s, const uint8_t *host_iq, const void *d_iq, size_t n_buffers,
            const uint8_t *carry476, modes_candidate *d_records_ext, uint32_t cap_ext, modes_tile *d_tiles_ext,
            bool halo_on_device = false) {
@@ -345,14 +353,10 @@ int submit(modes_ctx *ctx, Slot &s, const uint8_t *host_iq, const void *d_iq, si
         d_iq = s.d_iq.get();
     }
     if ((reinterpret_cast<uintptr_t>(d_iq) & 15) != 0) return fail(ctx, "device I/Q pointer must be 16-byte aligned");
-    if (!halo_on_device) {
-        const unsigned hi = s.halo_next++ % Slot::kHaloRing;
-        uint8_t *h_halo = s.h_halo.get() + (size_t)hi * kHaloAlloc;
-        CK(ctx, cudaEventSynchronize(s.halo_ev[hi]));                     // its previous copy (8 submits ago) has left the host
-        memset(h_halo, 127, kHaloAlloc);                                  // dump1090.c:344 no-signal
-        if (carry476) memcpy(h_halo + (kHaloBytes - MODES_CARRY_BYTES), carry476, MODES_CARRY_BYTES);
-        CK(ctx, cudaMemcpyAsync(s.d_halo.get(), h_halo, kHaloAlloc, cudaMemcpyHostToDevice, s.stream));
-        CK(ctx, cudaEventRecord(s.halo_ev[hi], s.stream));
+    s.carry_on_host = !halo_on_device;
+    if (s.carry_on_host) {
+        memset(s.carry, 127, kHaloAlloc);                                 // dump1090.c:344 no-signal
+        if (carry476) memcpy(s.carry + (kHaloBytes - MODES_CARRY_BYTES), carry476, MODES_CARRY_BYTES);
     }
     s.batch_iq = d_iq;
     s.n_buffers = n_buffers;
@@ -418,9 +422,11 @@ bool weak_overflowed(const Slot &s) {
 // The two kernels over the slot's staged batch (also used to repeat a batch that overflowed).
 int launch_batch(modes_ctx *ctx, Slot &s) {
     const uint64_t n_samples = (uint64_t)s.n_buffers * kBufSamples;
-    CK(ctx, cudaMemsetAsync(s.d_counters.get(), 0, 4 * sizeof(uint32_t), s.stream));
+    // a repeated batch takes the other set too: the first run's scan zeroed it
+    s.set ^= 1;
     BatchView in{static_cast<const uint8_t *>(s.batch_iq), s.d_halo.get(), n_samples};
-    ScanOutputs so{s.d_cand_v.get(), s.out_cap, s.out_tiles, s.d_counters.get()};
+    ScanOutputs so{s.d_cand_v.get(), s.out_cap, s.out_tiles, s.counters(),
+                   s.d_counters.get() + kCounterWords * (s.set ^ 1), s.h_counts};
 
     cudaEvent_t *pe = nullptr;
     if (ctx->cfg.profile) {
@@ -433,7 +439,7 @@ int launch_batch(modes_ctx *ctx, Slot &s) {
         ctx->prof_head++;
     }
     if (pe) CK(ctx, cudaEventRecord(pe[0], s.stream));
-    launch_scan(in, ctx->tab, so, ctx->sm_count, s.stream);
+    launch_scan(in, ctx->tab, so, ctx->sm_count, s.stream, s.carry_on_host ? s.carry : nullptr);
     if (pe) CK(ctx, cudaEventRecord(pe[1], s.stream));
     launch_eval(in, ctx->tab, so, s.out_records, ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->sm_count, s.stream);
     if (pe) CK(ctx, cudaEventRecord(pe[2], s.stream));
@@ -467,10 +473,9 @@ int launch_batch(modes_ctx *ctx, Slot &s) {
         CK(ctx, cudaMemcpyAsync(h + 4, g.stats_out, 8 * sizeof(uint64_t), cudaMemcpyDeviceToHost, s.stream));
         CK(ctx, cudaMemcpyAsync(h + 20, g.cache_out, 1024 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
     }
-    CK(ctx, cudaMemcpyAsync(s.h_counters.get(), s.d_counters.get(), 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
     if (f.levels)
         CK(ctx, cudaMemcpyAsync(s.h_levels.get(), s.d_levels.get(), s.n_buffers * sizeof(modes_level), cudaMemcpyDeviceToHost, s.stream));
-    CK(ctx, cudaEventRecord(s.ev[3], s.stream));
+    CK(ctx, cudaEventRecord(s.done, s.stream));
     s.busy = true;
     return 0;
 }
@@ -480,12 +485,12 @@ int launch_batch(modes_ctx *ctx, Slot &s) {
 // they are the slot's own; caller-supplied buffers cannot grow and report the overflow.
 int wait_batch(modes_ctx *ctx, Slot &s, uint64_t *n_out) {
     for (;;) {
-        CK(ctx, cudaEventSynchronize(s.ev[3]));
-        const bool cand_over = s.h_counters[1] || s.h_counters[0] > s.out_cap;
+        CK(ctx, cudaEventSynchronize(s.done));
+        const bool cand_over = s.h_counts[1] || s.h_counts[0] > s.out_cap;
         if (!cand_over && !weak_overflowed(s)) break;
         if (ctx->cfg.gpu_resolve && &s != &ctx->detect) break;           // reported by collect(): the device resolve ran on a truncated list
         if (cand_over) {
-            const uint32_t found = s.h_counters[0];
+            const uint32_t found = s.h_counts[0];
             if (!s.own_outputs)
                 return fail(ctx, "candidate capacity exceeded: %u found, room for %u", found, s.out_cap);
             s.want_cap = found + found / 8 + 1024;
@@ -496,7 +501,7 @@ int wait_batch(modes_ctx *ctx, Slot &s, uint64_t *n_out) {
         if (weak_overflowed(s)) s.want_weak_cap = s.h_weak_counters[1] + s.h_weak_counters[1] / 8 + 1024;
         if (launch_batch(ctx, s)) return -1;
     }
-    *n_out = s.h_counters[0];
+    *n_out = s.h_counts[0];
     return 0;
 }
 
@@ -551,11 +556,11 @@ int collect(modes_ctx *ctx, Slot &s) {
     const double t0 = dbg ? now_ms() : 0;
     if (wait_batch(ctx, s, &n)) return -1;
     s.busy = false;                                     // a repeated (overflowed) batch re-arms the flag
-    append_levels(ctx, s);                              // copied with the counters: on the host since ev[3]
+    append_levels(ctx, s);                              // copied with the counters: on the host since s.done
     const double t1 = dbg ? now_ms() : 0;
     if (ctx->cfg.gpu_resolve) {
         // the verdicts were taken on the device: fetch the deliveries, build the structs
-        if (s.h_counters[1] || s.h_counters[0] > s.out_cap) return fail(ctx, "gpu_resolve: candidate capacity exceeded (%u found)", s.h_counters[0]);
+        if (s.h_counts[1] || s.h_counts[0] > s.out_cap) return fail(ctx, "gpu_resolve: candidate capacity exceeded (%u found)", s.h_counts[0]);
         // internal check: the in-order fallback leaves every buffer's cache as the hand-over computes it
         if (s.h_gr_flags[0]) return fail(ctx, "gpu_resolve: internal error: address caches did not settle after the in-order replay");
         if (s.h_gr_flags[1]) return fail(ctx, "gpu_resolve: delivery capacity exceeded (%u messages)", s.h_gr_flags[2]);
@@ -1024,7 +1029,7 @@ int modes::weak_device_strided(modes_ctx *ctx, void *d_pos, void *d_rec, size_t 
     // a batch that wait_batch repeats (after a candidate or weak overflow) runs the passes again (launch_batch)
     BatchView in{static_cast<const uint8_t *>(s.batch_iq), s.d_halo.get(), (uint64_t)s.n_buffers * kBufSamples};
     if (launch_weak(ctx, s, in)) return -1;
-    CK(ctx, cudaEventRecord(s.ev[3], s.stream));           // wait_batch sees the weak count too
+    CK(ctx, cudaEventRecord(s.done, s.stream));            // wait_batch sees the weak count too
     return 0;
 }
 
@@ -1059,7 +1064,7 @@ int modes_recover_device(modes_ctx *ctx, void *d_out, size_t capacity) {
     s.rec_ext_cap = capacity > 0xFFFFFFF0ull ? 0xFFFFFFF0u : (uint32_t)capacity;
     // a batch that wait_batch repeats after an overflow runs the pass again (launch_batch)
     BatchView in{static_cast<const uint8_t *>(s.batch_iq), s.d_halo.get(), (uint64_t)s.n_buffers * kBufSamples};
-    ScanOutputs so{s.d_cand_v.get(), s.out_cap, s.out_tiles, s.d_counters.get()};
+    ScanOutputs so{s.d_cand_v.get(), s.out_cap, s.out_tiles, s.counters()};
     return launch_recovery(ctx, s, in, so);
 }
 
@@ -1572,7 +1577,7 @@ int modes_device_memset(void *dst_device, int value, size_t nbytes) {
 
 int modes_detect_publish_count(modes_ctx *ctx, void *dst) {
     if (!ctx || !dst) return -1;
-    CK(ctx, cudaMemcpyAsync(dst, ctx->detect.d_counters.get(), 4 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->detect.stream));
+    CK(ctx, cudaMemcpyAsync(dst, ctx->detect.counters(), 4 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->detect.stream));
     return 0;
 }
 

@@ -31,6 +31,8 @@
 //    measured slightly slower than whole windows (0.170 against 0.166 ms).
 #include <cstdint>
 #include <cstdlib>
+#include <mutex>
+#include <vector>
 #include <cuda_runtime.h>
 #include "modes_internal.h"
 #include "modes_eval_serial.cuh"
@@ -44,7 +46,12 @@ constexpr int kNibWords = 28 * 16;
 constexpr int kLutWords = serial::kIqLutEntries / 2;
 constexpr int kTableWords = 112 + kFixHashSlots + kNibWords + kLutWords;
 static_assert(serial::kIqLutStride == kLutIqStride && serial::kIqLutEntries % 8 == 0, "table geometry");
-static_assert(kTableWords % 2 == 0, "record staging uses 8-byte stores");
+static_assert(kTableWords % 4 == 0, "the table image is copied in 16-byte pieces");
+
+// The kernel's shared-memory tables as s_mem lays them out: bit syndromes, fix hash, nibble syndromes and
+// the (|I-127|, |Q-127|) magnitude table.  Built on the host once per device (table_image_ready); each CTA
+// copies it in behind its read of the candidate count instead of assembling it.
+__device__ __align__(16) uint32_t g_table_image[kTableWords];
 
 // kFirst = blocks of the walk (of 4) whose slots are staged first; the rest follows into the same
 // rows once every lane is through them.  4: the whole walk (113 slots) at once, 8 warps per SM
@@ -72,6 +79,10 @@ __device__ __forceinline__ uint32_t raw_sample(const BatchView &in, uint64_t v) 
 
 __device__ __forceinline__ void cp_async4(uint32_t dst_shared, const uint32_t *src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst_shared), "l"(src) : "memory");
+}
+
+__device__ __forceinline__ void cp_async16(uint32_t dst_shared, const uint32_t *src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst_shared), "l"(src) : "memory");
 }
 
 // One lane's atomic add.  For an atomic on a warp-uniform address in divergent code ptxas emits its
@@ -168,13 +179,9 @@ eval_fused_kernel(BatchView in, DeviceTables tab, const uint32_t *__restrict__ c
     uint32_t *s_syn = s_mem, *s_hash = s_syn + 112, *s_nib = s_hash + kFixHashSlots;
     uint16_t *s_lut = reinterpret_cast<uint16_t *>(s_nib + kNibWords);
     uint32_t *s_warp = s_nib + kNibWords + kLutWords;
-    for (int i = threadIdx.x; i < 112; i += G::kThreads) s_syn[i] = tab.bit_syn[i];
-    for (int i = threadIdx.x; i < kFixHashSlots; i += G::kThreads) s_hash[i] = tab.fix_hash[i];
-    for (int i = threadIdx.x; i < serial::kIqLutEntries / 8; i += G::kThreads)
-        reinterpret_cast<uint4 *>(s_lut)[i] = __ldg(reinterpret_cast<const uint4 *>(tab.lut_iq) + i);
-    __syncthreads();
-    for (int i = threadIdx.x; i < kNibWords; i += G::kThreads) s_nib[i] = serial::nibble_syndrome(s_syn, i >> 4, i & 15);
-    __syncthreads();
+    // the tables arrive while the candidate count is read
+    for (int i = threadIdx.x; i < kTableWords / 4; i += G::kThreads)
+        cp_async16((uint32_t)__cvta_generic_to_shared(s_mem + 4 * i), g_table_image + 4 * i);
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     uint32_t *rows = s_warp + warp * G::kWarpWords;
@@ -194,10 +201,14 @@ eval_fused_kernel(BatchView in, DeviceTables tab, const uint32_t *__restrict__ c
     // chunk i+2's positions are loaded and its preamble words copied.
     // (The counter values are used untouched until a chunk later: arithmetic on them right away
     // would wait for the atomic's round trip.)
+    // Chunk c holds candidates first(c) ..: the list is walked from its end, where the tiles the scan took
+    // last are, whose windows may still be in L2.
+    auto first = [&](uint32_t c) -> uint32_t { return (n_chunks - 1 - c) * 32; };
     auto positions = [&](uint32_t c) -> uint32_t {
         if (c >= n_chunks) return 0u;
-        const uint32_t nc = n_cand - c * 32 < 32u ? n_cand - c * 32 : 32u;   // idle lanes of the last chunk duplicate its last candidate
-        return cand_v[c * 32 + ((uint32_t)lane < nc ? lane : nc - 1)];
+        const uint32_t b = first(c);
+        const uint32_t nc = n_cand - b < 32u ? n_cand - b : 32u;   // idle lanes of the last chunk duplicate its last candidate
+        return cand_v[b + ((uint32_t)lane < nc ? lane : nc - 1)];
     };
     // Chunk c (positions v): preamble words -> preamble area.  Its windows are not prefetched into
     // L2: on an H100 (400 W) a prefetch of chunk i+2's windows (five lines per lane) made the kernel
@@ -218,6 +229,10 @@ eval_fused_kernel(BatchView in, DeviceTables tab, const uint32_t *__restrict__ c
     };
 
     uint32_t chunk = blockIdx.x * G::kWarps + warp;
+    // (waited for here, before any warp leaves: behind the candidate count's load, with the walk's
+    // code as it was when each CTA assembled the tables)
+    asm volatile("cp.async.wait_all;" ::: "memory");
+    __syncthreads();                                       // every thread's share of the tables has landed
     if (chunk >= n_chunks) return;
     uint32_t next1 = 0, next2_raw = 0;
     uint32_t *const hand_out = counters + 3 + lane * c_zero;
@@ -239,7 +254,7 @@ eval_fused_kernel(BatchView in, DeviceTables tab, const uint32_t *__restrict__ c
         const uint32_t next2 = total_warps + __shfl_sync(0xffffffffu, next2_raw, 0);
         if (lane == 0) next2_raw = atom_add(hand_out, 1u);
         const uint32_t v2 = positions(next2);              // used after the walk
-        const uint32_t base = chunk * 32;
+        const uint32_t base = first(chunk);
         const uint32_t n = n_cand - base < 32u ? n_cand - base : 32u;
         const uint32_t *row = rows + lane * G::kRow;
         fz::Walk W;
@@ -282,6 +297,29 @@ eval_fused_kernel(BatchView in, DeviceTables tab, const uint32_t *__restrict__ c
     }
 }
 
+// g_table_image on the current device, once per device and process (a context's first launch; no kernel
+// of the module reads the image before it).  The copy is queued on `stream` and waited for, so that the
+// first launch on any other stream is ordered behind it as well.
+void table_image_ready(cudaStream_t stream) {
+    static std::once_flag once[64];
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
+    std::call_once(once[dev], [stream] {
+        std::vector<uint32_t> img(kTableWords);
+        uint32_t *syn = img.data(), *hash = syn + 112, *nib = hash + kFixHashSlots;
+        build_bit_syndromes(syn);
+        build_fix_hash(syn, hash);                     // cannot fail: the context checked it at creation
+        for (int i = 0; i < kNibWords; i++) {          // serial::nibble_syndrome: frame nibble i >> 4, value i & 15
+            uint32_t x = 0;
+            for (int k = 0; k < 4; k++) x ^= (((i & 15) >> (3 - k)) & 1) ? syn[4 * (i >> 4) + k] : 0u;
+            nib[i] = x;
+        }
+        build_lut_iq(reinterpret_cast<uint16_t *>(nib + kNibWords));
+        cudaMemcpyToSymbolAsync(g_table_image, img.data(), sizeof(uint32_t) * kTableWords, 0, cudaMemcpyHostToDevice, stream);
+        cudaStreamSynchronize(stream);
+    });
+}
+
 template <int kFirst, int kWarpsPerSm>
 void launch_fused(const BatchView &in, const DeviceTables &tab, const ScanOutputs &scan, modes_candidate *records,
                   int fix_errors, int aggressive, int sm_count, cudaStream_t stream) {
@@ -293,6 +331,7 @@ void launch_fused(const BatchView &in, const DeviceTables &tab, const ScanOutput
         cudaFuncSetAttribute(eval_fused_kernel<kFirst, kWarpsPerSm>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::kSmemBytes);
         if (dev >= 0 && dev < 64) configured[dev] = true;
     }
+    table_image_ready(stream);
     eval_fused_kernel<kFirst, kWarpsPerSm><<<sm_count, G::kThreads, G::kSmemBytes, stream>>>(in, tab, scan.cand_v, scan.counters, scan.cand_capacity,
                                                                                records, fix_errors, aggressive, 1u, 0xffffffffu, (uint32_t)-16384, 0u);
 }

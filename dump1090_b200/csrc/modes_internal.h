@@ -49,11 +49,20 @@ struct BatchView {
     uint64_t       n_samples;    // N = n_buffers * 131072
 };
 
+// One batch's counters: [0] candidates found (may exceed capacity), [1] overflow flag, [2]/[3] scan tile /
+// eval chunk hand-out, [4] scan CTAs finished (only with host_counts).  The scan starts from a zeroed set.
+constexpr int kCounterWords = 8;
+
 struct ScanOutputs {
     uint32_t   *cand_v;          // virtual positions of candidates, tile by tile
     uint32_t    cand_capacity;
     modes_tile *tiles;           // [n_tiles]
-    uint32_t   *counters;        // [0] candidates found (may exceed capacity), [1] overflow flag, [2]/[3] scan tile / eval chunk hand-out
+    uint32_t   *counters;        // kCounterWords (the first four without host_counts)
+    // A context's slot alternates between two counter sets, so that no memset or copy sits between its
+    // batches: the scan zeroes next_counters (the set of the slot's next batch) and its last CTA writes
+    // counters[0..1] to host_counts (mapped pinned host memory).  nullptr: neither.
+    uint32_t   *next_counters = nullptr;
+    uint32_t   *host_counts = nullptr;
 };
 
 inline uint32_t tiles_for(uint64_t n_samples) {
@@ -61,8 +70,10 @@ inline uint32_t tiles_for(uint64_t n_samples) {
 }
 
 // Kernel launchers (launch_scan: modes_scan2.cu; the rest: modes_kernels.cu).  All asynchronous on `stream`.
+// carry_block: nullptr, the batch's carry block is in.halo (device); else kHaloAlloc host bytes that travel
+// as a kernel parameter, and the scan stores them to in.halo for the batch's later kernels.
 void launch_scan(const BatchView &in, const DeviceTables &tab, const ScanOutputs &out, int sm_count,
-                 cudaStream_t stream);
+                 cudaStream_t stream, const uint8_t *carry_block = nullptr);
 void launch_eval(const BatchView &in, const DeviceTables &tab, const ScanOutputs &scan,
                  modes_candidate *records, int fix_errors, int aggressive, int sm_count,
                  cudaStream_t stream);

@@ -61,11 +61,11 @@ __device__ __forceinline__ TileSrc tile_source(const BatchView &in, uint32_t g, 
 // "no signal" (127,127).  Only the first and the last tiles of a batch come here.
 // (Out-of-line helpers take plain values: a reference to a kernel-parameter struct or to a register
 // array would force a copy in local memory, read back through L1 in the hot path.)
+// The carry block may be the kernel's parameter: a generic load, not __ldg (global space only).
 __device__ __noinline__ uint4 load_vchunk(const uint8_t *body, const uint8_t *halo, uint64_t c, uint64_t n_vchunks) {
     if (c >= n_vchunks) return make_uint4(0x7f7f7f7fu, 0x7f7f7f7fu, 0x7f7f7f7fu, 0x7f7f7f7fu);
-    const uint4 *p = (c < kHaloSamples / 8) ? reinterpret_cast<const uint4 *>(halo) + c
-                                            : reinterpret_cast<const uint4 *>(body) + (c - kHaloSamples / 8);
-    return __ldg(p);
+    if (c < kHaloSamples / 8) return reinterpret_cast<const uint4 *>(halo)[c];
+    return __ldg(reinterpret_cast<const uint4 *>(body) + (c - kHaloSamples / 8));
 }
 
 // Row r of a tile: this lane's 64 bytes.  Loaded through L1 (no L1::no_allocate): the exact tests
@@ -222,11 +222,16 @@ __device__ __noinline__ void dense_tile(const uint8_t *body, const uint8_t *halo
     __syncwarp();
 }
 
+struct alignas(16) CarryBlock { uint8_t b[kHaloAlloc]; };
+
 // 12 warps per SM (3 per scheduler) at up to 168 registers: the kernel needs about 160 and then has no
 // spill.  On the H100 that is faster than 16 warps at the 128-register cap with a spill (DESIGN §6).
+// carry_in_param: the batch's carry block is `carry`, and CTA 0 stores it to batch.halo for the kernels
+// after this one; else it is read at batch.halo.
 __global__ void __launch_bounds__(32, 12)
-scan_kernel(BatchView in, const uint16_t *__restrict__ lutn, ScanOutputs out, uint32_t n_tiles, uint32_t one,
-             uint32_t minus_one, uint32_t c65536) {
+scan_kernel(BatchView batch, __grid_constant__ const CarryBlock carry, uint32_t carry_in_param,
+            const uint16_t *__restrict__ lutn, ScanOutputs out, uint32_t n_tiles, uint32_t one, uint32_t minus_one,
+            uint32_t c65536) {
     __shared__ __align__(16) uint32_t s_mask[kRows * 32];
     __shared__ __align__(16) uint2 s_entry[kEntryCap];                // non-empty flag words: {word, position of bit 0 | first survivor slot << 16}
     __shared__ __align__(16) uint16_t s_surv[kSurvivorCap];           // survivor positions, position order
@@ -234,6 +239,13 @@ scan_kernel(BatchView in, const uint16_t *__restrict__ lutn, ScanOutputs out, ui
     uint32_t pend_tile = 0xffffffffu, pend_base = 0, pend_total = 0, pend_buf = 0;
 
     const int lane = threadIdx.x;
+    const BatchView in{batch.body, carry_in_param ? carry.b : batch.halo, batch.n_samples};
+    if (blockIdx.x == 0) {
+        static_assert(kHaloAlloc == 32 * 16 && kCounterWords <= 32, "one 16-byte carry chunk and one counter per lane");
+        if (carry_in_param)
+            reinterpret_cast<uint4 *>(const_cast<uint8_t *>(batch.halo))[lane] = reinterpret_cast<const uint4 *>(carry.b)[lane];
+        if (out.next_counters && lane < kCounterWords) out.next_counters[lane] = 0u;
+    }
     const uint32_t lt_mask = (1u << lane) - 1u;
     const uint64_t n_vchunks = (in.n_samples + kHaloSamples) / 8;
     const uint64_t t_end = in.n_samples;
@@ -445,11 +457,23 @@ scan_kernel(BatchView in, const uint16_t *__restrict__ lutn, ScanOutputs out, ui
         if (lane == 0 && pend_total) pend_base = atomicAdd(&out.counters[0], pend_total);
         emit_tile(out, s_olist + kOutCap * pend_buf, pend_tile, pend_base, pend_total, lane);
     }
+    // The last CTA to finish hands the final count and overflow flag to the host (lane 0 made every
+    // write to counters[1]; counters[0] only ever changes by atomics).  No CTA waits for another.
+    if (out.host_counts && lane == 0) {
+        __threadfence();
+        if (atomicAdd(&out.counters[4], 1u) == gridDim.x - 1) {
+            const volatile uint32_t *c = out.counters;
+            out.host_counts[0] = c[0];
+            out.host_counts[1] = c[1];
+            __threadfence_system();
+        }
+    }
 }
 
 }  // namespace
 
-void launch_scan(const BatchView &in, const DeviceTables &tab, const ScanOutputs &out, int sm_count, cudaStream_t stream) {
+void launch_scan(const BatchView &in, const DeviceTables &tab, const ScanOutputs &out, int sm_count, cudaStream_t stream,
+                 const uint8_t *carry_block) {
     // occupancy is a property of the device the context lives on
     static int ctas_per_sm[64] = {};
     int dev = 0;
@@ -461,8 +485,10 @@ void launch_scan(const BatchView &in, const DeviceTables &tab, const ScanOutputs
     }
     const uint32_t n_tiles = tiles_for(in.n_samples);
     uint32_t grid = (uint32_t)(sm_count * ctas_per_sm[dev]);   // persistent single-warp CTAs, all resident
-    if (grid > n_tiles) grid = n_tiles;
-    scan_kernel<<<grid, 32, 0, stream>>>(in, tab.lutn, out, n_tiles, 1u, 0xffffffffu, 65536u);
+    if (grid > n_tiles) grid = n_tiles;                         // (so that every CTA has a tile and reaches the end)
+    CarryBlock carry = {};
+    if (carry_block) memcpy(carry.b, carry_block, kHaloAlloc);
+    scan_kernel<<<grid, 32, 0, stream>>>(in, carry, carry_block ? 1u : 0u, tab.lutn, out, n_tiles, 1u, 0xffffffffu, 65536u);
 }
 
 }  // namespace modes
