@@ -30,7 +30,10 @@ oracle:
 	if [ -d /root/reference ]; then $(MAKE) -C oracle ref; fi
 
 # test infrastructure: host build of the per-candidate evaluation (logic checked against the oracle on CPU)
-shim: tests/_build/libeval_serial_host.so tests/_build/libscan_core_host.so tests/_build/libresolve_core_host.so tests/_build/libsignal_core_host.so tests/_build/liblevels_core_host.so tests/_build/librecover_core_host.so tests/_build/libweak_core_host.so tests/_build/libarrival_core_host.so tests/_build/libresample_core_host.so tests/_build/libinput_core_host.so
+shim: tests/_build/libeval_serial_host.so tests/_build/libscan_core_host.so tests/_build/libresolve_core_host.so tests/_build/libsignal_core_host.so tests/_build/liblevels_core_host.so tests/_build/librecover_core_host.so tests/_build/libweak_core_host.so tests/_build/libarrival_core_host.so tests/_build/libresample_core_host.so tests/_build/libinput_core_host.so tests/_build/libpool_carry_host.so
+tests/_build/libpool_carry_host.so: tests/host_shim/pool_carry_host.cpp $(CSRC)/modes_input_core.cuh
+	@mkdir -p tests/_build
+	g++ -O2 -std=c++17 -shared -fPIC -Wall -Wno-unknown-pragmas -x c++ -I$(CSRC) tests/host_shim/pool_carry_host.cpp -o $@
 tests/_build/libinput_core_host.so: tests/host_shim/input_core_host.cpp $(CSRC)/modes_input_core.cuh
 	@mkdir -p tests/_build
 	g++ -O2 -std=c++17 -shared -fPIC -Wall -Wno-unknown-pragmas -x c++ -I$(CSRC) tests/host_shim/input_core_host.cpp -o $@
@@ -71,7 +74,7 @@ tests/_build/libeval_serial_host.so: tests/host_shim/eval_serial_host.cpp $(CSRC
 # test infrastructure: device harness over the product's own kernel objects (recovery and signal
 # passes on constructed corpora, and the exhaustive sweeps of the core headers' device build)
 DSHIM_OBJS := build/modes_recover.o build/modes_signal.o build/modes_levels.o build/modes_tables.o
-dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so tests/_build/libscan_eval_device.so tests/_build/libresample_pool_device.so tests/_build/libresolve_device.so tests/_build/libinput_device.so
+dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so tests/_build/libscan_eval_device.so tests/_build/libresample_pool_device.so tests/_build/libresolve_device.so tests/_build/libinput_device.so tests/_build/libconvert_pool_device.so
 tests/_build/libkernels_device.so: tests/device_shim/kernels_device.cu $(DSHIM_OBJS) $(CSRC)/modes_internal.h $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_levels_core.cuh include/modes_b200.h
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/kernels_device.cu -o tests/_build/kernels_device.o
@@ -92,6 +95,11 @@ tests/_build/libresample_pool_device.so: tests/device_shim/resample_pool_device.
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/resample_pool_device.cu -o tests/_build/resample_pool_device.o
 	$(NVCC) $(ARCH) -shared -o $@ tests/_build/resample_pool_device.o build/modes_resample.o -cudart static
+# the receiver pool's conversion launch on constructed jobs (tests/test_pool_input_format.py)
+tests/_build/libconvert_pool_device.so: tests/device_shim/convert_pool_device.cu build/modes_resample.o $(CSRC)/modes_internal.h include/modes_b200.h
+	@mkdir -p tests/_build
+	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/convert_pool_device.cu -o tests/_build/convert_pool_device.o
+	$(NVCC) $(ARCH) -shared -o $@ tests/_build/convert_pool_device.o build/modes_resample.o -cudart static
 # the 16-bit input launches on chosen spans, and their timing (tests/test_input_format.py, scripts/input_format_time.py)
 tests/_build/libinput_device.so: tests/device_shim/input_device.cu build/modes_resample.o $(CSRC)/modes_internal.h include/modes_b200.h
 	@mkdir -p tests/_build

@@ -194,7 +194,8 @@ EXPORTS = ["modes_abi_version", "modes_default_config", "modes_create", "modes_d
            "modes_pool_recovery_stats", "modes_set_weak_preambles", "modes_get_weak_recovery_stats", "modes_weak_device",
            "modes_weak_fetch", "modes_resolver_run_weak", "modes_resolver_run_shards_weak", "modes_resolver_weak_stats",
            "modes_pool_set_weak_preambles", "modes_pool_weak_stats", "modes_set_arrival", "modes_pool_set_arrival",
-           "modes_set_input_rate", "modes_resample_device", "modes_pool_set_input_rate", "modes_set_input_format"]
+           "modes_set_input_rate", "modes_resample_device", "modes_pool_set_input_rate", "modes_set_input_format",
+           "modes_pool_set_input_format"]
 
 INPUT_RATES = (2_000_000, 2_400_000)      # modes_set_input_rate
 INPUT_FORMATS = {"uc8": 0, "sc16": 1, "sc16q11": 2}     # modes_set_input_format: MODES_INPUT_*
@@ -335,6 +336,7 @@ def lib():
         L.modes_set_input_rate.argtypes = [C.c_void_p, C.c_uint32]
         L.modes_pool_set_input_rate.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32]
         L.modes_set_input_format.argtypes = [C.c_void_p, C.c_uint32, C.c_int32]
+        L.modes_pool_set_input_format.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_int32]
         L.modes_resample_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int64, C.c_int64, C.c_size_t,
                                             C.c_int64, C.c_void_p, C.c_void_p]
         _lib = L
@@ -892,13 +894,19 @@ class ReceiverPool:
     weak_preambles=True: as for Decoder (`weak_recovery_stats(receiver)`).  arrival=True: as for Decoder.
     input_rate=2_400_000 sets every receiver to 2.4 MS/s at creation, set_input_rate(receiver, hz) one
     receiver (modes_pool_set_input_rate): a buffer is still BUFFER_BYTES of the receiver's stream, and its
-    2 MHz buffers are decoded as their input completes (`buffers(receiver)` counts them)."""
+    2 MHz buffers are decoded as their input completes (`buffers(receiver)` counts them).
+    input_format="sc16" / "sc16q11" (and input_shift) sets every receiver's sample format at creation,
+    set_input_format(receiver, fmt, shift) one receiver (modes_pool_set_input_format).  A buffer is the
+    receiver's next BUFFER_SAMPLES samples as uint8 bytes: BUFFER_BYTES for a UC8 receiver, 2 * BUFFER_BYTES
+    of little-endian int16 I/Q for an SC16 or SC16Q11 one; everything delivered for a 16-bit receiver
+    equals what a UC8 receiver at its rate delivers on the converted bytes."""
 
     def __init__(self, n_receivers: int, max_batch: int = 0, signal: bool = False, levels: bool = False,
                  recover: bool = False, weak_preambles: bool = False, arrival: bool = False,
-                 input_rate: int = 2_000_000, **cfg):
+                 input_rate: int = 2_000_000, input_format: str = "uc8", input_shift: int | None = None, **cfg):
         self.cfg = make_config(**cfg)
         self.n = n_receivers
+        self._bytes = [BUFFER_BYTES] * n_receivers
         self._h = lib().modes_pool_create(C.byref(self.cfg), n_receivers, max_batch)
         if not self._h:
             raise RuntimeError("modes_pool_create failed")
@@ -915,6 +923,9 @@ class ReceiverPool:
         if input_rate != 2_000_000:
             for r in range(n_receivers):
                 self.set_input_rate(r, input_rate)
+        if input_format != "uc8" or input_shift is not None:
+            for r in range(n_receivers):
+                self.set_input_format(r, input_format, input_shift)
         self.messages = [[] for _ in range(n_receivers)]
         self._fn = POOL_SINK_FN(self._on)
 
@@ -925,11 +936,20 @@ class ReceiverPool:
         if rc:
             raise RuntimeError(lib().modes_pool_last_error(self._h).decode())
 
-    def ingest(self, receivers, buffers) -> None:
-        """buffers[i]: BUFFER_BYTES of uint8 I/Q (numpy) = the next buffer of receivers[i]."""
+    def _buffers(self, receivers, buffers):
+        """The ids and the buffers as uint8 arrays, each of its receiver's size; ValueError otherwise."""
         ids = np.ascontiguousarray(receivers, dtype=np.uint32)
         bufs = [np.ascontiguousarray(b, dtype=np.uint8) for b in buffers]
-        assert ids.size == len(bufs) and all(b.size == BUFFER_BYTES for b in bufs)
+        assert ids.size == len(bufs)
+        for r, b in zip(ids.tolist(), bufs):
+            want = self._bytes[r] if r < self.n else BUFFER_BYTES
+            if b.size != want:
+                raise ValueError(f"receiver {r}: a buffer of {b.size} bytes, its input format takes {want}")
+        return ids, bufs
+
+    def ingest(self, receivers, buffers) -> None:
+        """buffers[i]: the next buffer of receivers[i], uint8 bytes (numpy) of its format (class docstring)."""
+        ids, bufs = self._buffers(receivers, buffers)
         ptrs = (C.c_void_p * len(bufs))(*[b.ctypes.data for b in bufs])
         self._check(lib().modes_pool_ingest(self._h, _ptr(ids), ptrs, ids.size, self._fn, None))
 
@@ -940,9 +960,7 @@ class ReceiverPool:
 
     def submit(self, receivers, buffers) -> None:
         """Upload + kernels, no waiting; `buffers` are kept alive until the matching collect()."""
-        ids = np.ascontiguousarray(receivers, dtype=np.uint32)
-        bufs = [np.ascontiguousarray(b, dtype=np.uint8) for b in buffers]
-        assert ids.size == len(bufs) and all(b.size == BUFFER_BYTES for b in bufs)
+        ids, bufs = self._buffers(receivers, buffers)
         ptrs = (C.c_void_p * len(bufs))(*[b.ctypes.data for b in bufs])
         self._check(lib().modes_pool_submit(self._h, _ptr(ids), ptrs, ids.size))
         self._inflight = getattr(self, "_inflight", []) + [(ids, bufs)]
@@ -1030,6 +1048,16 @@ class ReceiverPool:
         """The receiver's input sample rate, 2_000_000 or 2_400_000 (modes_pool_set_input_rate); refused
         while it has a stream in progress (until reset(receiver), which keeps the rate)."""
         self._check(lib().modes_pool_set_input_rate(self._h, int(receiver), int(hz)))
+
+    def set_input_format(self, receiver: int, fmt: str, shift: int | None = None) -> None:
+        """The receiver's sample format, one of INPUT_FORMATS, and its shift (None: the format's default)
+        (modes_pool_set_input_format); refused while it has a stream in progress (until reset(receiver),
+        which keeps the format)."""
+        if fmt not in INPUT_FORMATS:
+            raise ValueError(f"input format {fmt!r} is not one of {sorted(INPUT_FORMATS)}")
+        self._check(lib().modes_pool_set_input_format(self._h, int(receiver), INPUT_FORMATS[fmt],
+                                                      -1 if shift is None else int(shift)))
+        self._bytes[receiver] = BUFFER_BYTES * (1 if fmt == "uc8" else 2)
 
     def reset(self, receiver: int) -> None:
         lib().modes_pool_reset(self._h, receiver)

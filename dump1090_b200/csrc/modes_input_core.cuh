@@ -47,5 +47,16 @@ MODES_INPUT_FN uint32_t convert_pair(uint32_t w, int s) {
     return convert((int)(int16_t)(w & 0xffffu), s) | convert((int)(int16_t)(w >> 16), s) << 8;
 }
 
+// n whole samples of 16-bit I/Q bytes at in (4 bytes a sample, little-endian) to their 2 n UC8 bytes at out,
+// on the host: the carry of a 2 MHz 16-bit receiver of the pool (modes_pool.cpp).
+inline void convert_samples(const uint8_t *in, int64_t n, int s, uint8_t *out) {
+    for (int64_t k = 0; k < n; k++) {
+        const uint8_t *x = in + 4 * k;
+        const uint32_t y = convert_pair((uint32_t)x[0] | (uint32_t)x[1] << 8 | (uint32_t)x[2] << 16 | (uint32_t)x[3] << 24, s);
+        out[2 * k] = (uint8_t)y;
+        out[2 * k + 1] = (uint8_t)(y >> 8);
+    }
+}
+
 }  // namespace input
 }  // namespace modes

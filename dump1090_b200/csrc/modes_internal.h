@@ -141,6 +141,16 @@ struct PoolHistoryJob {
 // d_jobs: device memory; max_bytes: the most bytes one history job writes.
 void launch_resample_pool(const PoolResampleJob *d_jobs, uint32_t n_jobs, cudaStream_t stream);
 void launch_history_pool(const PoolHistoryJob *d_jobs, uint32_t n_jobs, uint64_t max_bytes, cudaStream_t stream);
+// The receiver pool's 16-bit receivers (modes_pool_set_input_format): one launch for one job per such
+// receiver of the batch, ahead of the two above.  A job converts one whole buffer, MODES_BUFFER_SAMPLES
+// int16 I/Q samples at in (2 x MODES_BUFFER_BYTES bytes), to its MODES_BUFFER_BYTES UC8 bytes at out
+// (modes_input_core.cuh at the shift); in and out 16-byte aligned.
+struct PoolConvertJob {
+    const uint8_t *in;
+    uint8_t       *out;
+    int32_t        shift;
+};
+void launch_convert_pool(const PoolConvertJob *d_jobs, uint32_t n_jobs, cudaStream_t stream);
 // Recovery records (modes_recover.cu): writes out[k] for k < min(counters[0], capacity) from the
 // candidate records and the windows the scan and frame evaluation read.
 void launch_recover(const BatchView &in, const DeviceTables &tab, const ScanOutputs &scan, const modes_candidate *records,

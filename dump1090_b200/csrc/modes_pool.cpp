@@ -30,6 +30,12 @@
 // device-resident input history and the staging area, and moves the 2 MHz receivers' buffers into
 // theirs; a second launch appends the call's bytes to each 2.4 MS/s receiver's history.  Only the
 // receivers that complete a buffer get a pair, so the scan and every pass after it see 2 MHz bytes only.
+//
+// A 16-bit receiver (modes_pool_set_input_format) brings 131072 int16 I/Q samples per call, twice a UC8
+// buffer's bytes.  Its call also goes the staged way: the 16-bit buffers cross PCIe into a second staging
+// area, and one launch ahead of the others (K10's pool form) converts each to its UC8 buffer, straight into
+// the pair's data buffer at 2 MHz, into the receiver's slot of the UC8 staging area at 2.4 MS/s.  From there
+// on the receiver is a UC8 receiver at its rate; its carry (2 MHz) is converted on the host.
 #include <algorithm>
 #include <cstdarg>
 #include <cstdio>
@@ -45,6 +51,7 @@
 #include <cuda_runtime.h>
 #include "modes_b200.h"
 #include "modes_internal.h"
+#include "modes_input_core.cuh"
 #include "modes_resample_core.cuh"
 
 namespace {
@@ -65,6 +72,8 @@ struct Receiver {
     uint8_t carry[MODES_CARRY_BYTES];
     modes::LevelQueue levels;
     uint32_t rate = kRate2M;                   // modes_pool_set_input_rate
+    uint32_t format = modes::input::kUC8;      // modes_pool_set_input_format, the shift resolved
+    int shift = 0;
     // 2.4 MS/s: input bytes of the stream so far, and its device input history: stream bytes
     // [hist0, in_total) at hist[cur], hist0 a multiple of 16; the other half is where the next call's
     // history step writes (no launch reads what it writes)
@@ -167,6 +176,11 @@ struct modes_pool {
         void *h_jobs = nullptr, *d_jobs = nullptr;
         cudaEvent_t rate_done = nullptr;
         bool rate_recorded = false;
+        // calls that name a 16-bit receiver: their 16-bit buffers, and the conversion jobs (pinned and
+        // device: PoolConvertJob[max_batch])
+        uint8_t *d_stage16 = nullptr;
+        void *h_cjobs = nullptr, *d_cjobs = nullptr;
+        std::vector<const uint8_t *> iq8, iq16;   // the call's UC8 and 16-bit buffers, each group in call order
     } slot[2];
     unsigned submitted = 0, collected = 0;     // batches so far: slot = number & 1
     std::vector<modes_candidate> cands;
@@ -269,6 +283,17 @@ int ensure_rate_device(modes_pool *p, const uint32_t *receivers, size_t n) {
             return fail(p, "event creation failed: %s", cudaGetErrorString(cudaGetLastError()));
     }
     for (size_t i = 0; i < n; i++) {
+        if (p->rx[receivers[i]].format == modes::input::kUC8) continue;
+        for (modes_pool::Slot &sl : p->slot) {
+            if (sl.d_stage16) continue;
+            sl.d_stage16 = static_cast<uint8_t *>(modes_device_alloc(p->max_batch * 2 * kBuf));
+            sl.d_cjobs = modes_device_alloc(p->max_batch * sizeof(modes::PoolConvertJob));
+            sl.h_cjobs = modes_host_alloc(p->max_batch * sizeof(modes::PoolConvertJob));
+            if (!sl.d_stage16 || !sl.d_cjobs || !sl.h_cjobs) return fail(p, "out of memory for %zu receivers per batch", p->max_batch);
+        }
+        break;
+    }
+    for (size_t i = 0; i < n; i++) {
         Receiver &r = p->rx[receivers[i]];
         if (r.rate == kRate2M || r.hist[0]) continue;
         for (uint8_t *&h : r.hist) h = static_cast<uint8_t *>(modes_device_alloc(kHistBytes));
@@ -277,19 +302,20 @@ int ensure_rate_device(modes_pool *p, const uint32_t *receivers, size_t n) {
     return 0;
 }
 
-// The callers' buffers to dst + i * pitch.  Buffers at a constant distance in host memory (one staging
-// block): one strided copy instead of n calls (2-3 us of host time each: at 256 receivers more than the
-// copy itself takes).
-int upload_buffers(modes_pool *p, cudaStream_t st, const uint8_t *const *iq, size_t n, uint8_t *dst, size_t pitch) {
+// The callers' buffers of `bytes` bytes each to dst + i * pitch.  Buffers at a constant distance of at
+// least their size in host memory (one staging block): one strided copy instead of n calls (2-3 us of host
+// time each: at 256 receivers more than the copy itself takes).
+int upload_buffers(modes_pool *p, cudaStream_t st, const uint8_t *const *iq, size_t n, uint8_t *dst, size_t pitch,
+                   size_t bytes) {
     bool strided = n > 1 && iq[1] > iq[0];
     const size_t stride = strided ? (size_t)(iq[1] - iq[0]) : 0;
     for (size_t i = 1; strided && i + 1 < n; i++) strided = iq[i + 1] > iq[i] && (size_t)(iq[i + 1] - iq[i]) == stride;
-    if (strided && stride >= kBuf && stride < ((size_t)1 << 30)) {
-        if (cudaMemcpy2DAsync(dst, pitch, iq[0], stride, kBuf, n, cudaMemcpyHostToDevice, st) != cudaSuccess)
+    if (strided && stride >= bytes && stride < ((size_t)1 << 30)) {
+        if (cudaMemcpy2DAsync(dst, pitch, iq[0], stride, bytes, n, cudaMemcpyHostToDevice, st) != cudaSuccess)
             return fail(p, "buffer upload failed: %s", cudaGetErrorString(cudaGetLastError()));
     } else {
         for (size_t i = 0; i < n; i++)
-            if (cudaMemcpyAsync(dst + i * pitch, iq[i], kBuf, cudaMemcpyHostToDevice, st) != cudaSuccess)
+            if (cudaMemcpyAsync(dst + i * pitch, iq[i], bytes, cudaMemcpyHostToDevice, st) != cudaSuccess)
                 return fail(p, "buffer upload failed: %s", cudaGetErrorString(cudaGetLastError()));
     }
     return 0;
@@ -308,34 +334,49 @@ int detect_pairs(modes_pool *p, modes_pool::Slot &sl, size_t n) {
     return 0;
 }
 
-// A call that names a 2.4 MS/s receiver (the buffers are checked): every buffer to the staging area, the
-// pairs of the receivers that complete a buffer resampled / moved into place, the histories advanced.
+// A call that names a 2.4 MS/s or a 16-bit receiver (the buffers are checked): every UC8 buffer to the
+// staging area and every 16-bit buffer to the 16-bit one, the 16-bit buffers converted (into their pairs at
+// 2 MHz, into the staging area at 2.4 MS/s), the pairs of the receivers that complete a buffer resampled /
+// moved into place, the histories advanced.  Staging slots: the UC8 buffers in call order, then the 16-bit
+// 2.4 MS/s receivers'.
 int submit_rated(modes_pool *p, modes_pool::Slot &sl, const uint32_t *receivers, const uint8_t *const *iq, size_t n) {
     if (ensure_rate_device(p, receivers, n)) return -1;
     cudaStream_t st = static_cast<cudaStream_t>(modes_stream(sl.ctx));
     modes::PoolResampleJob *rj = static_cast<modes::PoolResampleJob *>(sl.h_jobs);
     modes::PoolHistoryJob *hj = reinterpret_cast<modes::PoolHistoryJob *>(rj + p->max_batch);
-    size_t n_pairs = 0, n_hist = 0;
+    modes::PoolConvertJob *cj = static_cast<modes::PoolConvertJob *>(sl.h_cjobs);
+    size_t n_pairs = 0, n_rj = 0, n_hist = 0, n_conv = 0;
     uint64_t hist_max = 0;
     bool carries = false;
+    std::vector<const uint8_t *> &iq8 = sl.iq8, &iq16 = sl.iq16;
+    iq8.clear();
+    iq16.clear();
+    for (size_t i = 0; i < n; i++) (p->rx[receivers[i]].format == modes::input::kUC8 ? iq8 : iq16).push_back(iq[i]);
+    size_t n_stage = iq8.size();
     sl.ids.clear();
     sl.buf_index.clear();
-    for (size_t i = 0; i < n; i++) {
+    for (size_t i = 0, k8 = 0; i < n; i++) {
         const Receiver &r = p->rx[receivers[i]];
+        const bool uc8 = r.format == modes::input::kUC8;
         uint8_t *pad = sl.d_batch + 2 * n_pairs * kBuf;
-        const uint8_t *stage = sl.d_stage + i * kBuf;
+        const uint8_t *in16 = uc8 ? nullptr : sl.d_stage16 + n_conv * 2 * kBuf;
         if (r.rate == kRate2M) {
             memcpy(sl.h_carry + n_pairs * MODES_CARRY_BYTES, r.carry, MODES_CARRY_BYTES);
-            rj[n_pairs++] = modes::PoolResampleJob{nullptr, stage, 0, 0, -1, nullptr, pad + kBuf};
+            if (uc8) rj[n_rj++] = modes::PoolResampleJob{nullptr, sl.d_stage + k8++ * kBuf, 0, 0, -1, nullptr, pad + kBuf};
+            else cj[n_conv++] = modes::PoolConvertJob{in16, pad + kBuf, r.shift};
+            n_pairs++;
             sl.ids.push_back(receivers[i]);
             sl.buf_index.push_back(r.submitted);
             carries = true;
             continue;
         }
+        uint8_t *stage = sl.d_stage + (uc8 ? k8++ : n_stage++) * kBuf;
+        if (!uc8) cj[n_conv++] = modes::PoolConvertJob{in16, stage, r.shift};
         const RatePlan pl = rate_plan(r);
         if (pl.completes) {
-            rj[n_pairs++] = modes::PoolResampleJob{r.hist[r.cur], stage, r.hist0, r.in_total, r.submitted * kBufSamples,
-                                                   pad + kBuf - MODES_CARRY_BYTES, pad + kBuf};
+            rj[n_rj++] = modes::PoolResampleJob{r.hist[r.cur], stage, r.hist0, r.in_total, r.submitted * kBufSamples,
+                                                pad + kBuf - MODES_CARRY_BYTES, pad + kBuf};
+            n_pairs++;
             sl.ids.push_back(receivers[i]);
             sl.buf_index.push_back(r.submitted);
         }
@@ -345,7 +386,8 @@ int submit_rated(modes_pool *p, modes_pool::Slot &sl, const uint32_t *receivers,
         hj[n_hist++] = modes::PoolHistoryJob{r.hist[r.cur], stage, r.hist0, r.in_total, pl.keep, r.hist[r.cur ^ 1]};
         if (bytes > hist_max) hist_max = bytes;
     }
-    if (upload_buffers(p, st, iq, n, sl.d_stage, kBuf)) return -1;
+    if (!iq8.empty() && upload_buffers(p, st, iq8.data(), iq8.size(), sl.d_stage, kBuf, kBuf)) return -1;
+    if (!iq16.empty() && upload_buffers(p, st, iq16.data(), iq16.size(), sl.d_stage16, 2 * kBuf, 2 * kBuf)) return -1;
     // the 2 MHz receivers' carries as the 2 MHz path uploads them (the 2.4 MS/s pairs' tails are then
     // overwritten by the resampler)
     if (carries && cudaMemcpy2DAsync(sl.d_batch + kBuf - MODES_CARRY_BYTES, 2 * kBuf, sl.h_carry, MODES_CARRY_BYTES,
@@ -353,12 +395,16 @@ int submit_rated(modes_pool *p, modes_pool::Slot &sl, const uint32_t *receivers,
         return fail(p, "carry upload failed: %s", cudaGetErrorString(cudaGetLastError()));
     if (cudaMemcpyAsync(sl.d_jobs, sl.h_jobs, p->max_batch * kJobBytes, cudaMemcpyHostToDevice, st) != cudaSuccess)
         return fail(p, "job upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+    if (n_conv && cudaMemcpyAsync(sl.d_cjobs, sl.h_cjobs, n_conv * sizeof(modes::PoolConvertJob), cudaMemcpyHostToDevice, st) != cudaSuccess)
+        return fail(p, "job upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+    // the conversion writes only this slot's pairs and staging area: it need not wait for the other slot
+    modes::launch_convert_pool(static_cast<const modes::PoolConvertJob *>(sl.d_cjobs), (uint32_t)n_conv, st);
     // the other batch in flight may name the same receivers: its reads and its history step first
     const modes_pool::Slot &other = p->slot[(p->submitted & 1) ^ 1];
     if (other.rate_recorded && cudaStreamWaitEvent(st, other.rate_done, 0) != cudaSuccess)
         return fail(p, "stream wait failed: %s", cudaGetErrorString(cudaGetLastError()));
     const modes::PoolResampleJob *d_rj = static_cast<const modes::PoolResampleJob *>(sl.d_jobs);
-    modes::launch_resample_pool(d_rj, (uint32_t)n_pairs, st);
+    modes::launch_resample_pool(d_rj, (uint32_t)n_rj, st);
     modes::launch_history_pool(reinterpret_cast<const modes::PoolHistoryJob *>(d_rj + p->max_batch), (uint32_t)n_hist, hist_max, st);
     if (cudaGetLastError() != cudaSuccess || cudaEventRecord(sl.rate_done, st) != cudaSuccess)
         return fail(p, "resampling launch failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -368,7 +414,8 @@ int submit_rated(modes_pool *p, modes_pool::Slot &sl, const uint32_t *receivers,
         Receiver &r = p->rx[receivers[i]];
         if (r.rate == kRate2M) {
             r.submitted++;
-            memcpy(r.carry, iq[i] + kBuf - MODES_CARRY_BYTES, MODES_CARRY_BYTES);     // dump1090.c:481
+            if (r.format == modes::input::kUC8) memcpy(r.carry, iq[i] + kBuf - MODES_CARRY_BYTES, MODES_CARRY_BYTES);     // dump1090.c:481
+            else modes::input::convert_samples(iq[i] + 2 * (kBuf - MODES_CARRY_BYTES), MODES_CARRY_BYTES / 2, r.shift, r.carry);
             continue;
         }
         const RatePlan pl = rate_plan(r);
@@ -410,6 +457,9 @@ void modes_pool_destroy(modes_pool *p) {
         if (sl.d_jobs) modes_device_free(sl.d_jobs);
         if (sl.h_jobs) modes_host_free(sl.h_jobs);
         if (sl.rate_done) cudaEventDestroy(sl.rate_done);
+        if (sl.d_stage16) modes_device_free(sl.d_stage16);
+        if (sl.d_cjobs) modes_device_free(sl.d_cjobs);
+        if (sl.h_cjobs) modes_host_free(sl.h_cjobs);
         if (sl.ctx) modes_destroy(sl.ctx);
     }
     delete p;
@@ -559,7 +609,7 @@ int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *c
     bool rated = false;
     for (size_t i = 0; i < n; i++) {
         if (!iq[i]) return fail(p, "receiver %u: no buffer", receivers[i]);
-        rated |= p->rx[receivers[i]].rate != kRate2M;
+        rated |= p->rx[receivers[i]].rate != kRate2M || p->rx[receivers[i]].format != modes::input::kUC8;
     }
     if (rated) {
         if (submit_rated(p, sl, receivers, iq, n)) return -1;
@@ -574,7 +624,7 @@ int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *c
     if (cudaMemcpy2DAsync(sl.d_batch + kBuf - MODES_CARRY_BYTES, 2 * kBuf, sl.h_carry, MODES_CARRY_BYTES, MODES_CARRY_BYTES, n,
                           cudaMemcpyHostToDevice, st) != cudaSuccess)
         return fail(p, "carry upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-    if (upload_buffers(p, st, iq, n, sl.d_batch + kBuf, 2 * kBuf)) return -1;
+    if (upload_buffers(p, st, iq, n, sl.d_batch + kBuf, 2 * kBuf, kBuf)) return -1;
     if (detect_pairs(p, sl, n)) return -1;
     sl.buf_index.resize(n);
     for (size_t i = 0; i < n; i++) sl.buf_index[i] = p->rx[receivers[i]].submitted++;
@@ -667,6 +717,26 @@ int modes_pool_set_input_rate(modes_pool *p, uint32_t receiver, uint32_t hz) {
     if (r.submitted || r.in_total)
         return fail(p, "modes_pool_set_input_rate: receiver %u has a stream in progress; call modes_pool_reset first", receiver);
     r.rate = hz;
+    return 0;
+}
+
+int modes_pool_set_input_format(modes_pool *p, uint32_t receiver, uint32_t format, int32_t shift) {
+    namespace input = modes::input;
+    if (!p) return -1;
+    if (!input::known(format))
+        return fail(p, "modes_pool_set_input_format: format %u is not supported (MODES_INPUT_UC8, MODES_INPUT_SC16 or "
+                       "MODES_INPUT_SC16Q11)", format);
+    if (shift > input::kMaxShift)
+        return fail(p, "modes_pool_set_input_format: shift %d is not supported (0 to %d, or negative for the format's default)",
+                    (int)shift, input::kMaxShift);
+    if (format == input::kUC8 && shift > 0)
+        return fail(p, "modes_pool_set_input_format: shift %d is not supported with UC8 (0, or negative)", (int)shift);
+    if (receiver >= p->rx.size()) return fail(p, "receiver %u out of range (%zu receivers)", receiver, p->rx.size());
+    Receiver &r = p->rx[receiver];
+    if (r.submitted || r.in_total)
+        return fail(p, "modes_pool_set_input_format: receiver %u has a stream in progress; call modes_pool_reset first", receiver);
+    r.format = format;
+    r.shift = shift < 0 ? input::default_shift(format) : (int)shift;
     return 0;
 }
 

@@ -12,7 +12,8 @@
 // at 2.4 MS/s K9's staging loader converts each int16 sample to its UC8 pair as it fills s_in, so the
 // filter sees exactly the bytes it would see on the converted stream; at 2 MHz K10 (convert_kernel)
 // converts the batch's span straight into its body and carry block.  UC8 keeps its own loader, chosen
-// at compile time.
+// at compile time.  The receiver pool's 16-bit receivers have K10's pool form (convert_pool_kernel): one
+// launch converts every 16-bit buffer of a call, ahead of the pool's resampling launches.
 #include "modes_internal.h"
 #include "modes_input_core.cuh"
 #include "modes_resample_core.cuh"
@@ -240,7 +241,30 @@ __global__ void __launch_bounds__(kThreads) history_pool_kernel(const PoolHistor
     }
 }
 
+// K10's pool form: job blockIdx.y's buffer, 8 samples a thread (two 16-byte loads, one 16-byte store) as
+// convert_kernel's whole groups; a pool buffer is always whole, so there is no span edge and no carry block.
+constexpr int kConvertGroups = MODES_BUFFER_SAMPLES / 8;
+constexpr int kConvertBlocks = kConvertGroups / kThreads;
+static_assert(kConvertBlocks * kThreads == kConvertGroups, "whole blocks of groups");
+
+__global__ void __launch_bounds__(kThreads) convert_pool_kernel(const PoolConvertJob *jobs) {
+    const PoolConvertJob j = jobs[blockIdx.y];
+    const int g = (int)blockIdx.x * kThreads + threadIdx.x;
+    const uint4 lo = __ldg(reinterpret_cast<const uint4 *>(j.in) + 2 * g);
+    const uint4 hi = __ldg(reinterpret_cast<const uint4 *>(j.in) + 2 * g + 1);
+    uint4 o;
+    o.x = input::convert_pair(lo.x, j.shift) | input::convert_pair(lo.y, j.shift) << 16;
+    o.y = input::convert_pair(lo.z, j.shift) | input::convert_pair(lo.w, j.shift) << 16;
+    o.z = input::convert_pair(hi.x, j.shift) | input::convert_pair(hi.y, j.shift) << 16;
+    o.w = input::convert_pair(hi.z, j.shift) | input::convert_pair(hi.w, j.shift) << 16;
+    reinterpret_cast<uint4 *>(j.out)[g] = o;
+}
+
 }  // namespace
+
+void launch_convert_pool(const PoolConvertJob *d_jobs, uint32_t n_jobs, cudaStream_t stream) {
+    if (n_jobs) convert_pool_kernel<<<dim3(kConvertBlocks, n_jobs), kThreads, 0, stream>>>(d_jobs);
+}
 
 void launch_resample_pool(const PoolResampleJob *d_jobs, uint32_t n_jobs, cudaStream_t stream) {
     if (n_jobs) resample_pool_kernel<<<dim3(kPoolTiles, n_jobs), kThreads, 0, stream>>>(d_jobs);

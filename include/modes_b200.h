@@ -220,8 +220,8 @@ int  modes_pool_set_input_rate(modes_pool *p, uint32_t receiver, uint32_t hz);
  * 4 for SC16Q11.  Refused: an unknown format, a shift above 15, a shift other than 0 or negative with
  * UC8, and, as modes_set_input_rate, a call between the first modes_process of a stream and
  * modes_finish / modes_reset.  It takes effect for the stream that begins at create or reset (which keeps
- * it), reaches every GPU of an n_gpus > 1 context, and combines with either input rate.  The receiver
- * pool takes UC8 only.
+ * it), reaches every GPU of an n_gpus > 1 context, and combines with either input rate.  A receiver of
+ * the pool has its own format: modes_pool_set_input_format below.
  *
  * A 16-bit stream is converted to UC8 on the device, then decoded as a UC8 stream at the input rate
  * (at 2400000: converted, then resampled), so it decodes to exactly what the UC8 decoder gives on the
@@ -236,6 +236,20 @@ int  modes_pool_set_input_rate(modes_pool *p, uint32_t receiver, uint32_t hz);
 #define MODES_INPUT_SC16     1u
 #define MODES_INPUT_SC16Q11  2u
 int  modes_set_input_format(modes_ctx *ctx, uint32_t format, int32_t shift);
+/* The same per receiver of a pool (modes_pool_* below), with the same formats and shifts; refused for
+ * what modes_set_input_format refuses, a receiver out of range, and, as modes_pool_set_input_rate, while
+ * the receiver has a stream in progress (from the first modes_pool_submit / _ingest that names it until
+ * modes_pool_reset, which keeps the format and the shift).  It touches no device and combines with either
+ * input rate, set in either order.  One call still brings MODES_BUFFER_SAMPLES samples of every receiver
+ * it names: iq[i] is MODES_BUFFER_BYTES bytes for a UC8 receiver and 2 x MODES_BUFFER_BYTES bytes of
+ * little-endian int16 I/Q for an SC16 or SC16Q11 one, so the pool's schedule is the same at either format.
+ * Everything the pool delivers for a 16-bit receiver (messages and their fields, sample_pos, statistics,
+ * level records, recovery and weak statistics, modes_pool_buffers) equals what it delivers for a UC8
+ * receiver at the same rate fed the converted bytes; level records describe the converted bytes.  A call
+ * that names a 16-bit receiver converts its buffers on the device; the pool's device memory grows by a
+ * staging area of 2 x 512 KiB per receiver of a batch (one per batch in flight), besides the 2 x 256 KiB
+ * one a call that names a 2.4 MS/s receiver also uses.  modes_pool_resolve stays UC8 at 2 MHz. */
+int  modes_pool_set_input_format(modes_pool *p, uint32_t receiver, uint32_t format, int32_t shift);
 
 /* ---- stage-level entry points (tests, bench, multi-GPU sharding) -------- */
 /* computeMagnitudeVector() alone (dump1090.c:1454-1469): nsamples I/Q pairs in
