@@ -195,17 +195,22 @@ EXPORTS = ["modes_abi_version", "modes_default_config", "modes_create", "modes_d
            "modes_weak_fetch", "modes_resolver_run_weak", "modes_resolver_run_shards_weak", "modes_resolver_weak_stats",
            "modes_pool_set_weak_preambles", "modes_pool_weak_stats", "modes_set_arrival", "modes_pool_set_arrival",
            "modes_set_input_rate", "modes_resample_device", "modes_pool_set_input_rate", "modes_set_input_format",
-           "modes_pool_set_input_format"]
+           "modes_pool_set_input_format", "modes_resample_device_at"]
 
-INPUT_RATES = (2_000_000, 2_400_000)      # modes_set_input_rate
+INPUT_RATES = (2_000_000, 2_400_000, 4_000_000, 6_000_000, 8_000_000, 10_000_000)      # modes_set_input_rate
 INPUT_FORMATS = {"uc8": 0, "sc16": 1, "sc16q11": 2}     # modes_set_input_format: MODES_INPUT_*
 
 
-def resampled_samples(n_input_bytes: int) -> int:
-    """2 MHz samples of a 2.4 MS/s stream of n_input_bytes bytes: N_out = ceil(5 n_in / 6) with
-    n_in = ceil(bytes / 2) (modes_set_input_rate)."""
+def resampled_samples(n_input_bytes: int, rate: int = 2_400_000) -> int:
+    """2 MHz samples of a UC8 stream of n_input_bytes bytes at `rate` (modes_set_input_rate), with
+    n_in = ceil(bytes / 2): N_out = ceil(5 n_in / 6) at 2.4 MS/s, ceil(n_in / M) at 2 M MS/s, n_in at 2 MHz."""
     n_in = (int(n_input_bytes) + 1) // 2
-    return (5 * n_in + 5) // 6
+    if rate == 2_400_000:
+        return (5 * n_in + 5) // 6
+    if rate not in INPUT_RATES:
+        raise ValueError(f"{rate} samples/s is not supported {INPUT_RATES}")
+    m = rate // 2_000_000
+    return -(-n_in // m)
 
 
 def lib():
@@ -339,6 +344,8 @@ def lib():
         L.modes_pool_set_input_format.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_int32]
         L.modes_resample_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int64, C.c_int64, C.c_size_t,
                                             C.c_int64, C.c_void_p, C.c_void_p]
+        L.modes_resample_device_at.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_int64, C.c_int64,
+                                               C.c_size_t, C.c_int64, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -421,7 +428,9 @@ class Decoder:
     input_rate=2_400_000 takes 2.4 MS/s bytes (what dump1090-fa and readsb record) and resamples them
     to 2 MHz on the GPU before the pipeline (modes_set_input_rate): the messages are exactly the 2 MHz
     decoder's on the resampled bytes.  Message.sample_pos still counts 2 MHz samples, and
-    6 * sample_pos is the input time in 12 MHz ticks at either rate.
+    6 * sample_pos is the input time in 12 MHz ticks at either rate.  input_rate=4_000_000, 6_000_000,
+    8_000_000 or 10_000_000 (what Airspy, SDRplay and USRP radios usually record) decimates by 2-5 on the GPU
+    instead, with the same contract on the decimated bytes.
     input_format="sc16" or "sc16q11" takes signed 16-bit I/Q bytes (SoapySDR and Airspy-class tools,
     bladeRF) and converts them to 8-bit I/Q on the GPU with input_shift (None: the format's default)
     before the pipeline (modes_set_input_format): the messages are exactly the UC8 decoder's on the
@@ -530,9 +539,9 @@ class Decoder:
         self._check(lib().modes_set_signal(self._h, int(bool(on))))
 
     def set_input_rate(self, hz: int) -> None:
-        """The sample rate of the stream that begins at the next reset (decode() resets): 2_000_000 or
-        2_400_000 (modes_set_input_rate); refused while a stream is in progress.  sample_pos counts 2 MHz
-        samples at either rate, and 6 * sample_pos is the input time in 12 MHz ticks."""
+        """The sample rate of the stream that begins at the next reset (decode() resets): one of INPUT_RATES
+        (modes_set_input_rate); refused while a stream is in progress.  sample_pos counts 2 MHz samples at
+        every rate, and 6 * sample_pos is the input time in 12 MHz ticks."""
         self._check(lib().modes_set_input_rate(self._h, int(hz)))
 
     def set_input_format(self, fmt: str, shift: int | None = None) -> None:
@@ -665,6 +674,16 @@ class Decoder:
         self._check(lib().modes_resample_device(self._h, C.c_void_p(d_in_ptr or None), int(in_bytes), int(in_first_sample),
                                                 int(first_buffer), int(n_buffers), int(out_end), C.c_void_p(d_out_ptr),
                                                 carry))
+        return bytes(carry) if want_carry else None
+
+    def resample_device_at(self, hz: int, d_in_ptr: int, in_bytes: int, in_first_sample: int, first_buffer: int,
+                           n_buffers: int, d_out_ptr: int, out_end: int = -1, want_carry: bool = True) -> bytes | None:
+        """resample_device at any of INPUT_RATES but 2 MHz (modes_resample_device_at): 2.4 MS/s resampled,
+        4-10 MS/s decimated, UC8 input."""
+        carry = (C.c_uint8 * CARRY_BYTES)() if want_carry else None
+        self._check(lib().modes_resample_device_at(self._h, int(hz), C.c_void_p(d_in_ptr or None), int(in_bytes),
+                                                   int(in_first_sample), int(first_buffer), int(n_buffers), int(out_end),
+                                                   C.c_void_p(d_out_ptr), carry))
         return bytes(carry) if want_carry else None
 
     def levels_device(self, d_iq_ptr: int, n_buffers: int, stride_bytes: int = 0) -> None:

@@ -166,11 +166,12 @@ struct modes_ctx {
     int64_t buffers_done = 0;
     bool finished = false;
     bool started = false;                 // modes_process or modes_finish since create / reset
-    // modes_set_input_rate / modes_set_input_format: at 2.4 MS/s, or in a 16-bit format, each batch's 2 MHz
-    // UC8 bytes are made on the device (K9 resamples, K10 converts) from the stream's input bytes; they
-    // never exist on the host.  hold keeps the stream bytes [hold0, in_total) that later batches read (the
-    // filter's history and a buffer not yet complete).  input_shift: the format's shift, default resolved.
-    uint32_t input_rate = 2000000;
+    // modes_set_input_rate / modes_set_input_format: at 2.4 MS/s or more, or in a 16-bit format, each batch's
+    // 2 MHz UC8 bytes are made on the device (K9 resamples, K11 decimates, K10 converts) from the stream's
+    // input bytes; they never exist on the host.  hold keeps the stream bytes [hold0, in_total) that later
+    // batches read (the filter's history and a buffer not yet complete).  input_shift: the format's shift,
+    // default resolved.
+    const InputRate *rate = find_input_rate(2000000);
     uint32_t input_format = input::kUC8;
     int input_shift = 0;
     int64_t in_total = 0;
@@ -641,19 +642,15 @@ struct Source {
     int64_t out_end = INT64_MAX;
 };
 
-// The input paths through the hold: 2.4 MS/s (resampled, K9) or a 16-bit format (converted, K10; at
-// 2.4 MS/s converted, then resampled).
-bool held_input(const modes_ctx *ctx) { return ctx->input_rate == 2400000 || ctx->input_format != input::kUC8; }
+// The input paths through the hold: any rate but 2 MHz (resampled, K9, or decimated, K11) or a 16-bit
+// format (converted, K10; at the other rates converted as the resampling or decimation loads it).
+bool held_input(const modes_ctx *ctx) { return ctx->rate->hz != 2000000 || ctx->input_format != input::kUC8; }
 
 // The input samples [batch_in_lo(o0), batch_in_hi(o1)) that the 2 MHz output samples [o0, o1) of a batch
-// and its carry block read.  At 2 MHz output sample n reads input sample n, and the span starts with the
-// carry block's 240 samples, so that a 16-bit upload starts on a 16-byte boundary.
-int64_t batch_in_lo(const modes_ctx *ctx, int64_t o0) {
-    return ctx->input_rate == 2400000 ? resample::in_lo(o0 - MODES_CARRY_BYTES / 2) : o0 - kHaloSamples;
-}
-int64_t batch_in_hi(const modes_ctx *ctx, int64_t o1) {
-    return ctx->input_rate == 2400000 ? resample::in_hi(o1 - 1) : o1;
-}
+// and its carry block read (at 2 MHz the carry block's 240 samples, so that a 16-bit upload starts on a
+// 16-byte boundary).
+int64_t batch_in_lo(const modes_ctx *ctx, int64_t o0) { return in_lo(*ctx->rate, o0 - ctx->rate->carry); }
+int64_t batch_in_hi(const modes_ctx *ctx, int64_t o1) { return in_hi(*ctx->rate, o1 - 1); }
 
 // Upload the input bytes the slot's batch (nb buffers from s.buffer_base, and the carry before them) reads,
 // straight from where they are, and make the slot's body and carry block from them on the device.
@@ -681,8 +678,10 @@ int stage_held(modes_ctx *ctx, Slot &s, const Source &src, size_t nb) {
     }
     const ResampleJob j{s.d_in.get(), (uint64_t)(hi - lo), lo / bps, o0, (uint64_t)(o1 - o0), src.out_end,
                         s.d_iq.get(), s.d_halo.get()};
-    if (ctx->input_format == input::kUC8) launch_resample(j, s.stream);
-    else if (ctx->input_rate == 2400000) launch_resample_sc16(j, ctx->input_shift, s.stream);
+    const int shift = ctx->input_format == input::kUC8 ? -1 : ctx->input_shift;
+    if (ctx->rate->m) launch_decimate(j, ctx->rate->m, shift, s.stream);
+    else if (ctx->input_format == input::kUC8) launch_resample(j, s.stream);
+    else if (ctx->rate->hz == 2400000) launch_resample_sc16(j, ctx->input_shift, s.stream);
     else launch_convert_sc16(j, ctx->input_shift, s.stream);
     CK(ctx, cudaGetLastError());
     ctx->launches++;
@@ -765,11 +764,10 @@ Source host_buffers(const uint8_t *iq) {
 }
 
 // The most the hold can need: the input of one reference buffer and of the carry before it, with the
-// filter's reach on both sides at 2.4 MS/s (a whole buffer's input would have run).
+// filter's reach on both sides where there is a filter (a whole buffer's input would have run).
 size_t hold_bytes(const modes_ctx *ctx) {
-    const size_t reach = ctx->input_rate == 2400000
-                             ? (size_t)6 * (kBufSamples + MODES_CARRY_BYTES / 2) / 5 + 2 * resample::kTaps
-                             : (size_t)kBufSamples + kHaloSamples;
+    const InputRate &r = *ctx->rate;
+    const size_t reach = (size_t)r.in * (kBufSamples + r.carry) / r.out + (r.taps > 1 ? 2 * r.taps : 0);
     return (size_t)input::sample_bytes(ctx->input_format) * (reach + 16);
 }
 
@@ -782,7 +780,7 @@ int process_held(modes_ctx *ctx, const uint8_t *iq, size_t nbytes) {
     ctx->in_total += (int64_t)nbytes;
     const int64_t avail = ctx->in_total / input::sample_bytes(ctx->input_format);   // whole input samples
     const int64_t B = kBufSamples;
-    int64_t m = (ctx->input_rate == 2400000 ? 5 * avail / 6 : avail) / B;       // buffers [0, m) are ready
+    int64_t m = ctx->rate->out * avail / ctx->rate->in / B;                    // buffers [0, m) are ready
     while (m > ctx->buffers_done && batch_in_hi(ctx, m * B) > avail) m--;
     while (batch_in_hi(ctx, (m + 1) * B) <= avail) m++;
     if (m > ctx->buffers_done) {
@@ -807,12 +805,13 @@ int process_held(modes_ctx *ctx, const uint8_t *iq, size_t nbytes) {
 }
 
 // The end of a held stream: n_in input samples (UC8: ceil(bytes / 2), a trailing odd byte an I whose Q is
-// 127; 16-bit: floor(bytes / 4)) make N_out = n_in (2 MHz) or ceil(5 n_in / 6) (2.4 MS/s) output samples;
+// 127; 16-bit: floor(bytes / 4)) make N_out = n_in (2 MHz), ceil(5 n_in / 6) (2.4 MS/s) or ceil(n_in / M)
+// (2 M MS/s) output samples;
 // the remaining whole buffers and the EOF buffer (127 past N_out) run from the hold, the input 127-padded
 // past its end.
 int finish_held(modes_ctx *ctx) {
     const int64_t n_in = ctx->input_format == input::kUC8 ? (ctx->in_total + 1) / 2 : ctx->in_total / 4;
-    const int64_t n_out = ctx->input_rate == 2400000 ? resample::n_out(n_in) : n_in;
+    const int64_t n_out = modes::n_out(*ctx->rate, n_in);
     ctx->eof_buffer = n_out / kBufSamples;                                  // its level record counts the real samples only
     ctx->eof_samples = (uint32_t)(n_out % kBufSamples);
     const int64_t last = ctx->eof_buffer + (ctx->cfg.drop_eof_buffer ? 0 : 1);
@@ -1128,12 +1127,14 @@ int modes_reset(modes_ctx *ctx) {
 
 int modes_set_input_rate(modes_ctx *ctx, uint32_t hz) {
     if (!ctx) return -1;
-    if (hz != 2000000 && hz != 2400000)
-        return fail(ctx, "modes_set_input_rate: %u samples/s is not supported (2000000 or 2400000)", hz);
+    const InputRate *r = find_input_rate(hz);
+    if (!r)
+        return fail(ctx, "modes_set_input_rate: %u samples/s is not supported (2000000, 2400000, 4000000, 6000000, "
+                         "8000000 or 10000000)", hz);
     if (ctx->started && !ctx->finished)
         return fail(ctx, "modes_set_input_rate: a stream is in progress; call modes_finish or modes_reset first");
-    ctx->input_rate = hz;
-    for (modes_ctx *g : ctx->gpus) g->input_rate = hz;
+    ctx->rate = r;
+    for (modes_ctx *g : ctx->gpus) g->rate = r;
     return 0;
 }
 
@@ -1246,7 +1247,17 @@ int modes_detect_host(modes_ctx *ctx, const uint8_t *iq, size_t n_buffers, const
 
 int modes_resample_device(modes_ctx *ctx, const void *d_in, size_t in_bytes, int64_t in_first_sample,
                           int64_t first_buffer, size_t n_buffers, int64_t out_end, void *d_out, uint8_t *carry476) {
+    return modes_resample_device_at(ctx, 2400000, d_in, in_bytes, in_first_sample, first_buffer, n_buffers, out_end,
+                                    d_out, carry476);
+}
+
+int modes_resample_device_at(modes_ctx *ctx, uint32_t hz, const void *d_in, size_t in_bytes, int64_t in_first_sample,
+                             int64_t first_buffer, size_t n_buffers, int64_t out_end, void *d_out, uint8_t *carry476) {
     if (!ctx) return -1;
+    const InputRate *r = find_input_rate(hz);
+    if (!r || hz == 2000000)
+        return fail(ctx, "modes_resample_device: %u samples/s is not supported (2400000, 4000000, 6000000, 8000000 or "
+                         "10000000)", hz);
     if (!d_out || !n_buffers) return fail(ctx, "modes_resample_device: empty output");
     if (!d_in && in_bytes) return fail(ctx, "modes_resample_device: no input");
     if (first_buffer < 0) return fail(ctx, "modes_resample_device: buffer index %lld", (long long)first_buffer);
@@ -1258,10 +1269,11 @@ int modes_resample_device(modes_ctx *ctx, const void *d_in, size_t in_bytes, int
         CK(ctx, ctx->d_rs_halo.ensure(kHaloAlloc));
         CK(ctx, ctx->h_rs_halo.ensure(kHaloAlloc));
     }
-    launch_resample(ResampleJob{static_cast<const uint8_t *>(d_in), in_bytes, in_first_sample, first_buffer * (int64_t)kBufSamples,
-                                (uint64_t)n_buffers * kBufSamples, out_end < 0 ? INT64_MAX : out_end,
-                                static_cast<uint8_t *>(d_out), carry476 ? ctx->d_rs_halo.get() : nullptr},
-                    st);
+    const ResampleJob j{static_cast<const uint8_t *>(d_in), in_bytes, in_first_sample, first_buffer * (int64_t)kBufSamples,
+                        (uint64_t)n_buffers * kBufSamples, out_end < 0 ? INT64_MAX : out_end,
+                        static_cast<uint8_t *>(d_out), carry476 ? ctx->d_rs_halo.get() : nullptr};
+    if (r->m) launch_decimate(j, r->m, -1, st);
+    else launch_resample(j, st);
     CK(ctx, cudaGetLastError());
     ctx->launches++;
     if (!carry476) return 0;

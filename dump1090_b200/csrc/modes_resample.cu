@@ -14,6 +14,9 @@
 // converts the batch's span straight into its body and carry block.  UC8 keeps its own loader, chosen
 // at compile time.  The receiver pool's 16-bit receivers have K10's pool form (convert_pool_kernel): one
 // launch converts every 16-bit buffer of a call, ahead of the pool's resampling launches.
+//
+// K11 (decimate_kernel): 4, 6, 8 and 10 MS/s input decimated by M = 2..5, in K10's groups of 8 output
+// samples, from either staging loader.
 #include "modes_internal.h"
 #include "modes_input_core.cuh"
 #include "modes_resample_core.cuh"
@@ -171,6 +174,52 @@ __global__ void __launch_bounds__(kThreads) convert_kernel(ResampleJob j, int64_
     *reinterpret_cast<uint4 *>(dst) = v;
 }
 
+// K11: 4, 6, 8 and 10 MS/s input decimated by M (modes_resample_core.cuh).  The groups are convert_kernel's:
+// a thread makes 8 output samples, one 16-byte store into the body or the carry block.  Its group_in(M)
+// input samples are consecutive, so it loads the 16-byte words of the (converted) stream that hold them with
+// the staging loaders, straight into registers, and aligns them there: the window starts sh bytes into its
+// first word, and sh is the same for every group of a launch (groups are 16 M bytes apart).  The taps are
+// immediates; neighbouring groups share at most two words, which L1 serves.
+template <int M, class Input>
+__global__ void __launch_bounds__(kThreads) decimate_kernel(ResampleJob j, int64_t g_first, int64_t n_groups, Input input) {
+    namespace D = decimate;
+    if (j.halo && blockIdx.x == 0 && threadIdx.x < (kHaloAlloc - kHaloBytes) / 16)
+        reinterpret_cast<uint4 *>(j.halo + kHaloBytes)[threadIdx.x] = make_uint4(0x7f7f7f7fu, 0x7f7f7f7fu, 0x7f7f7f7fu, 0x7f7f7f7fu);
+    const int64_t g = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+    if (g >= n_groups) return;
+    const int64_t n0 = 8 * (g_first + g);
+    const int64_t p = 2 * (M * n0 - D::extent(M) - j.in_first);     // the window's first byte
+    const int64_t a = p & ~(int64_t)15;
+    const int sh = (int)(p - a);
+    constexpr int kWords = (2 * D::group_in(M) + 14 + 15) / 16;       // 16-byte words holding the window at any sh
+    uint32_t w[4 * kWords + 4];
+#pragma unroll
+    for (int k = 0; k < kWords; k++) {
+        const uint4 v = input.word(j, a + 16 * k);
+        w[4 * k] = v.x; w[4 * k + 1] = v.y; w[4 * k + 2] = v.z; w[4 * k + 3] = v.w;
+    }
+#pragma unroll
+    for (int k = 4 * kWords; k < 4 * kWords + 4; k++) w[k] = 0;
+    // w[i] = window bytes 4i .. 4i + 3: shift down by sh (even, block-uniform) in three selects
+#pragma unroll
+    for (int i = 0; i < 4 * kWords + 2; i++) w[i] = (sh & 8) ? w[i + 2] : w[i];
+#pragma unroll
+    for (int i = 0; i < 4 * kWords + 3; i++) w[i] = (sh & 4) ? w[i + 1] : w[i];
+#pragma unroll
+    for (int i = 0; i < 4 * kWords + 3; i++) w[i] = (sh & 2) ? __funnelshift_r(w[i], w[i + 1], 16) : w[i];
+    uint4 v;
+    D::group<M>(w, reinterpret_cast<uint32_t *>(&v));
+    const int64_t c0 = j.out_first - MODES_CARRY_BYTES / 2;
+    if (n0 + 8 > j.out_end || n0 < c0) {
+        uint16_t *x = reinterpret_cast<uint16_t *>(&v);
+#pragma unroll
+        for (int k = 0; k < 8; k++)
+            if (n0 + k >= j.out_end || n0 + k < c0) x[k] = 0x7f7fu;
+    }
+    uint8_t *dst = n0 >= j.out_first ? j.body + 2 * (n0 - j.out_first) : j.halo + 2 * (n0 - (j.out_first - kHaloSamples));
+    *reinterpret_cast<uint4 *>(dst) = v;
+}
+
 // ---- the receiver pool (modes_pool.cpp): one launch for the batch's jobs, grid (tile, job)
 
 constexpr int kCarrySamples = MODES_CARRY_BYTES / 2;
@@ -302,6 +351,26 @@ void launch_convert_sc16(const ResampleJob &j, int shift, cudaStream_t stream) {
     const int64_t groups = (j.out_first + (int64_t)j.out_samples - first) / 8;
     const int64_t blocks = (groups + kThreads - 1) / kThreads;
     convert_kernel<<<(unsigned)blocks, kThreads, 0, stream>>>(j, first / 8, groups, shift);
+}
+
+namespace {
+template <int M>
+void launch_decimate_m(const ResampleJob &j, int64_t g_first, int64_t groups, int shift, cudaStream_t stream) {
+    const unsigned blocks = (unsigned)((groups + kThreads - 1) / kThreads);
+    if (shift < 0) decimate_kernel<M><<<blocks, kThreads, 0, stream>>>(j, g_first, groups, Uc8Input{});
+    else decimate_kernel<M><<<blocks, kThreads, 0, stream>>>(j, g_first, groups, Sc16Input{shift});
+}
+}  // namespace
+
+void launch_decimate(const ResampleJob &j, int m, int shift, cudaStream_t stream) {
+    const int64_t first = j.out_first - (j.halo ? kHaloSamples : 0);
+    const int64_t groups = (j.out_first + (int64_t)j.out_samples - first) / 8;
+    switch (m) {
+    case 2: launch_decimate_m<2>(j, first / 8, groups, shift, stream); break;
+    case 3: launch_decimate_m<3>(j, first / 8, groups, shift, stream); break;
+    case 4: launch_decimate_m<4>(j, first / 8, groups, shift, stream); break;
+    case 5: launch_decimate_m<5>(j, first / 8, groups, shift, stream); break;
+    }
 }
 
 }  // namespace modes

@@ -174,14 +174,21 @@ def frame_envelope_at(frame: bytes, pos: int, frac: float, sample_rate: int) -> 
 
 
 def synth_stream_at(nsamples: int, frames, sigma: float = 1.5, seed: int = 1, sample_rate: int = 2_000_000,
-                    dtype: str = "uc8", scale: float = 1.0) -> np.ndarray:
+                    dtype: str = "uc8", scale: float = 1.0, tone=None) -> np.ndarray:
     """synth_stream at any sample rate: frames are (pos, frame_bytes, amplitude_lsb, carrier_phase_rad,
     frac) with the arrival time pos + frac in 2 MHz samples (0.5 us), pulses per frame_envelope_at, and
     the same noise per sample as synth_stream.  At 2 MHz it equals synth_stream bit for bit.
     dtype="sc16": the same signal as signed little-endian 16-bit I/Q bytes (4 a sample), scale int16
-    units to an 8-bit LSB (16 is SC16Q11's full scale, 256 SC16's), rounded and clamped to int16."""
+    units to an 8-bit LSB (16 is SC16Q11's full scale, 256 SC16's), rounded and clamped to int16.
+    tone=(offset_hz, amplitude_lsb): a continuous carrier at that offset from the channel centre is added
+    (an out-of-band interferer where the offset is past 1 MHz); None, the default, adds nothing."""
     i = noise(nsamples, sigma, seed * 2 + 11)
     q = noise(nsamples, sigma, seed * 2 + 12)
+    if tone is not None:
+        offset_hz, tone_amp = tone
+        w = 2 * np.pi * (offset_hz / sample_rate) * np.arange(nsamples, dtype=np.float64)
+        i += tone_amp * np.cos(w)
+        q += tone_amp * np.sin(w)
     for pos, frame, amp, phase, frac in frames:
         start, env = frame_envelope_at(frame, pos, frac, sample_rate)
         env = env * amp
@@ -364,10 +371,10 @@ def fleet_at(snr_db: float, nframes: int, seed: int, n_aircraft: int = 20, amp: 
 
 
 def fleet_at_rate(snr_db: float, nframes: int, seed: int, sample_rate: int = 2_400_000, n_aircraft: int = 20,
-                  amp: float = 20.0, period: int = 400, dtype: str = "uc8", scale: float = 1.0):
+                  amp: float = 20.0, period: int = 400, dtype: str = "uc8", scale: float = 1.0, tone=None):
     """fleet_at sampled at sample_rate (2.4 MS/s: what dump1090-fa and readsb record): the same frames,
     arrival times, amplitudes and carrier phases, over the same stretch of time, with the same noise per
-    sample; dtype and scale as synth_stream_at.  Returns (stream, set of the frames' hex)."""
+    sample; dtype, scale and tone as synth_stream_at.  Returns (stream, set of the frames' hex)."""
     sigma = amp / (np.sqrt(2.0) * 10 ** (snr_db / 20.0))
     rng = Counter(seed)
     fleet = [0x400000 + rng.below(0x3FFFFF) for _ in range(n_aircraft)]
@@ -380,7 +387,8 @@ def fleet_at_rate(snr_db: float, nframes: int, seed: int, sample_rate: int = 2_4
         truth.add(frame.hex())
     a, b = _rate_ratio(sample_rate)
     n = -(-(200 + nframes * period + 400) * a // b)
-    return synth_stream_at(n, frames, sigma=sigma, seed=seed, sample_rate=sample_rate, dtype=dtype, scale=scale), truth
+    return synth_stream_at(n, frames, sigma=sigma, seed=seed, sample_rate=sample_rate, dtype=dtype, scale=scale,
+                           tone=tone), truth
 
 
 def tile_to(data: np.ndarray, nbytes: int) -> np.ndarray:

@@ -27,9 +27,11 @@
  * (modes_config.gpu_resolve); it has no recovery rule, so it is refused together with --recover.
  * --recover-weak implies --recover and also searches weak preambles, positions the reference's
  * preamble test rejects (modes_set_weak_preambles); with --stats a second line goes to stderr.
- * --sample-rate <hz> gives the rate of the file: 2000000 (the default) or 2400000, what dump1090-fa and
+ * --sample-rate <hz> gives the rate of the file: 2000000 (the default), 2400000, what dump1090-fa and
  * readsb record (modes_set_input_rate: resampled to 2 MHz on the GPU, sample positions and Beast
- * timestamps on the same 2 MHz / 12 MHz clocks).  It combines with every output mode and switch.
+ * timestamps on the same 2 MHz / 12 MHz clocks), or 4000000, 6000000, 8000000 or 10000000, what Airspy,
+ * SDRplay and USRP radios usually record (decimated to 2 MHz on the GPU, on the same clocks).  It
+ * combines with every output mode and switch.
  * --iformat UC8|SC16|SC16Q11 gives the sample format of the file, as dump1090-fa spells it: 8-bit
  * unsigned (the default), or signed 16-bit I/Q (SoapySDR and Airspy-class tools; bladeRF's 12-bit values),
  * converted to 8 bits on the GPU (modes_set_input_format).  --iformat-shift <0..15> replaces the
@@ -148,8 +150,9 @@ int main(int argc, char **argv) {
         }
     }
     if (!filename) { fprintf(stderr, "--ifile <filename> is required (use '-' for stdin)\n"); return 1; }
-    if (sample_rate != 2000000 && sample_rate != 2400000) {
-        fprintf(stderr, "--sample-rate takes 2000000 or 2400000\n");
+    if (sample_rate != 2000000 && sample_rate != 2400000 && sample_rate != 4000000 && sample_rate != 6000000 &&
+        sample_rate != 8000000 && sample_rate != 10000000) {
+        fprintf(stderr, "--sample-rate takes 2000000, 2400000, 4000000, 6000000, 8000000 or 10000000\n");
         return 1;
     }
     uint32_t format;

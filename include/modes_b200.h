@@ -52,7 +52,9 @@ typedef struct modes_config {
                                    stock binary does in most runs */
     int32_t device;             /* CUDA device ordinal, default 0 */
     int32_t profile;            /* 1: record per-kernel CUDA-event times (modes_get_kernel_times) */
-    uint64_t max_batch_bytes;   /* device staging per in-flight batch; 0 = 64 MiB */
+    uint64_t max_batch_bytes;   /* device staging per in-flight batch; 0 = 64 MiB.  It counts the batch's
+                                   2 MHz UC8 bytes: the input span a batch uploads at another rate or format
+                                   is up to 10 times that (10 MS/s SC16) */
     int32_t n_gpus;             /* 0 or 1: one GPU (`device`).  N > 1: the streaming decode (modes_process /
                                    modes_finish) deals its batches of whole reference buffers round-robin to N
                                    devices starting at `device` — one stream, one pinned-to-device copy and
@@ -173,9 +175,11 @@ int  modes_finish(modes_ctx *ctx);
 int  modes_reset(modes_ctx *ctx);
 int  modes_get_stats(const modes_ctx *ctx, modes_stats *out);
 
-/* ---- 2.4 MS/s input ------------------------------------------------------ */
-/* The sample rate of the bytes modes_process takes: 2000000 (the default, what dump1090 reads) or
- * 2400000 (what dump1090-fa and readsb record from RTL-SDR dongles); any other value is refused.  It is
+/* ---- 2.4, 4, 6, 8 and 10 MS/s input -------------------------------------- */
+/* The sample rate of the bytes modes_process takes: 2000000 (the default, what dump1090 reads),
+ * 2400000 (what dump1090-fa and readsb record from RTL-SDR dongles), or 4000000, 6000000, 8000000 and
+ * 10000000 (what Airspy, SDRplay, USRP and other 16-bit radios usually record); any other value is
+ * refused with a message that says "not supported".  It is
  * also refused between the first modes_process of a stream and modes_finish / modes_reset, and takes
  * effect for the stream that begins at create or reset.  On an n_gpus > 1 context it reaches every GPU.
  * A receiver of the pool has its own rate: modes_pool_set_input_rate below.
@@ -193,10 +197,21 @@ int  modes_get_stats(const modes_ctx *ctx, modes_stats *out);
  * The EOF buffer is 127 past N_out, as modes_finish pads a 2 MHz stream.  sample_pos counts 2 MHz
  * samples; output sample n sits at input time 1.2 n exactly, so 6 * sample_pos is the input time in
  * 12 MHz ticks and the Beast timestamps keep their meaning.  Level records describe the resampled
- * bytes (their clipping count can be lower than the input's). */
+ * bytes (their clipping count can be lower than the input's).
+ *
+ * At 2000000 M (M = 2, 3, 4, 5) every batch is first decimated to 2 MHz on the device by an exact
+ * integer filter, with the same consequences: the stream decodes to exactly what the 2 MHz decoder gives
+ * on its decimated bytes, for every input format:
+ *   output  sample n stands for input samples [M n, M n + M); for I and Q separately
+ *               y = clamp(127 + ((sum_{k<T} h_M[k] * (x[M n - E + k] - 127) + 8192) >> 14), 0, 255)
+ *           (int32 sum, arithmetic shift), T = M + 2E; N_out = ceil(n_in / M) output samples
+ *   taps    signed 16-bit Q14, symmetric about input M n + (M - 1) / 2, each table summing to 16384
+ *           (modes_resample_core.cuh has them)
+ * Output sample n starts at input sample M n exactly, so 6 * sample_pos stays the 12 MHz time.  Level
+ * records describe the decimated bytes. */
 int  modes_set_input_rate(modes_ctx *ctx, uint32_t hz);
-/* The same per receiver of a pool (modes_pool_* below): 2000000 (the default) or 2400000; refused for
- * any other value, a receiver out of range, and while the receiver has a stream in progress (from the
+/* The same per receiver of a pool (modes_pool_* below): 2000000 (the default) or 2400000; refused, with
+ * "not supported", for any other value (the decimated rates included), a receiver out of range, and while the receiver has a stream in progress (from the
  * first modes_pool_submit / _ingest that names it until modes_pool_reset, which keeps the rate).  It
  * touches no device.  A 2.4 MS/s receiver's iq[i] is still MODES_BUFFER_BYTES of its stream (131072
  * input samples); a 2 MHz buffer of its resampled stream is decoded in the call whose input completes it
@@ -283,6 +298,13 @@ int  modes_detect_host(modes_ctx *ctx, const uint8_t *iq, size_t n_buffers, cons
  * for them, without it it returns at once.  Runs on the context's stream. */
 int  modes_resample_device(modes_ctx *ctx, const void *d_in, size_t in_bytes, int64_t in_first_sample,
                            int64_t first_buffer, size_t n_buffers, int64_t out_end, void *d_out, uint8_t *carry476);
+/* modes_resample_device at any rate modes_set_input_rate takes other than 2000000 (the call above is this
+ * one at 2400000), UC8 input as there, the same arguments and the same behaviour.  At 2000000 M the span
+ * must hold the input samples [M n0 - E, M n1 + E) that exist, with n0 = MODES_BUFFER_SAMPLES *
+ * first_buffer - 240 and n1 as above (E: 2 for M = 2, 3 and 4; 3 for M = 5).  Any other rate is refused
+ * with "not supported". */
+int  modes_resample_device_at(modes_ctx *ctx, uint32_t hz, const void *d_in, size_t in_bytes, int64_t in_first_sample,
+                              int64_t first_buffer, size_t n_buffers, int64_t out_end, void *d_out, uint8_t *carry476);
 /* Wait for the last modes_detect_device; returns the candidate count. */
 int  modes_detect_wait(modes_ctx *ctx, uint64_t *n_candidates);
 /* Copy the last result to host memory (arrays sized by the caller from

@@ -1,7 +1,12 @@
 """Device time of the 2.4 MS/s input resampler (K9, modes_resample.cu), its DRAM floor, and the end-to-end
 streaming decode of a 2.4 MS/s capture against the 2 MHz GiB it resamples to.
 
-    python scripts/resample_time.py [--steps 20] [--reps 3]
+    python scripts/resample_time.py [--steps 20] [--reps 3] [--rate 2400000] [--format uc8] [--gib 1]
+
+--rate 4000000 ... 10000000 times the integer decimator (K11) instead, on a capture of random_traffic-style
+frames at that rate (tests/test_input_decimation.traffic_at); --format sc16 feeds it 16-bit input, whose
+kernel time comes from torch.profiler over a streaming decode of the capture (the stage-level entry takes
+UC8 only).  --gib: GiB of 2 MHz output (the input is M or 2 M times as large).
 
 - Kernel: modes_resample_device over 1 GiB of 2 MHz output (4096 reference buffers) from the 1.2 GiB of
   2.4 MS/s input it reads, timed with CUDA events; median, min and max over the steps.
@@ -41,7 +46,12 @@ def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--rate", type=int, default=2_400_000)
+    ap.add_argument("--format", default="uc8", choices=["uc8", "sc16"])
+    ap.add_argument("--gib", type=float, default=1.0)
     args = ap.parse_args()
+    if args.rate != 2_400_000:
+        return decimation(args)
     import numpy as np
     import torch
 
@@ -122,6 +132,118 @@ def main() -> None:
           f"copy at {copy_tbs:.2f} TB/s (read + write) -> {floor_ms:.4f} ms; kernel {kern / floor_ms:.2f}x the floor")
     for name, v in e2e.items():
         nbytes = h24.nbytes if name == "2.4 MS/s" else h20.nbytes
+        med = statistics.median(v)
+        print(f"end to end {name}: {spread(v)} for {nbytes / 2**30:.3f} GiB from pinned memory "
+              f"({nbytes / 1e9 / (med * 1e-3):.2f} GB/s of input); {counts[name]} messages")
+
+
+def decimation(args) -> None:
+    import numpy as np
+    import torch
+
+    import decimate_model as DM
+    import input_format_model as IF
+    from dump1090_b200 import api, synth
+    from test_input_decimation import traffic_at
+
+    m = DM.RATES[args.rate]
+    sc16 = args.format == "sc16"
+    bps = 4 if sc16 else 2
+    card = query("name,power.limit")
+    nbuf = int(args.gib * NBUF)
+    n_out = nbuf * B
+    n_in = m * n_out + 8
+    # the UC8 capture; a 16-bit one holds the same samples (input_format_model.to_sc16 at shift 8), so both
+    # decimate to the same 2 MHz bytes
+    seed = traffic_at(m, "uc8", 2_000_000 * m, 9)
+    cap = synth.tile_to(seed, 2 * n_in)
+    label = f"{args.rate / 1e6:g} MS/s {args.format.upper()}"
+    e, taps = DM.extent(DM.taps(m), m), DM.taps(m).size
+    read_bytes, write_bytes = bps * (m * (n_out + 240) + e), 2 * n_out + 480
+    d_in = torch.from_numpy(cap).cuda()
+    d_out = torch.empty(2 * n_out, dtype=torch.uint8, device="cuda")
+    dec = api.Decoder()
+    stream = torch.cuda.Stream()
+    torch.cuda.set_stream(stream)
+    dec.set_stream(stream.cuda_stream)
+    times = []
+    for k in range(args.steps + 3):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        dec.resample_device_at(args.rate, d_in.data_ptr(), d_in.numel(), 0, 0, nbuf, d_out.data_ptr(), want_carry=False)
+        b.record()
+        b.synchronize()
+        if k >= 3:
+            times.append(a.elapsed_time(b))
+    torch.cuda.synchronize()
+    got = d_out[: 2 * B].cpu().numpy()
+    assert np.array_equal(got, DM.decimate_range(cap[: 2 * (m * B + 8)], m, 0, B)), "kernel output differs from the model"
+    y = d_out.cpu().numpy()
+    dec.close()
+    del d_out
+    if sc16:
+        del d_in
+        cap = synth.tile_to(IF.to_sc16(seed, 8), 4 * n_in)
+        d_in = torch.from_numpy(cap).cuda()
+    dst = torch.empty_like(d_in)
+    rates = []
+    for k in range(6):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        dst.copy_(d_in)
+        b.record()
+        b.synchronize()
+        if k:
+            rates.append(2 * d_in.numel() / (a.elapsed_time(b) * 1e-3) / 1e12)
+    del dst, d_in
+    torch.cuda.empty_cache()
+    copy_tbs = statistics.median(rates)
+    floor_ms = (read_bytes + write_bytes) / (copy_tbs * 1e12) * 1e3
+
+    hm = api.PinnedBuffer(cap.size)
+    hm.array[:] = cap
+    h20 = api.PinnedBuffer(y.size)
+    h20.array[:] = y
+    decs = {label: api.Decoder(input_rate=args.rate, input_format=args.format), "2 MHz": api.Decoder()}
+    torch.cuda.set_stream(torch.cuda.default_stream())
+    if sc16:
+        # the kernel's device time from the profiler, over one streaming decode of the capture
+        from torch.profiler import ProfilerActivity, profile
+        times = []
+        dd = decs[label]
+        for k in range(min(args.steps, 5) + 1):
+            dd.reset()
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                dd.process_ptr(hm.ptr, hm.nbytes)
+                dd.finish()
+                torch.cuda.synchronize()
+            us = sum(ev.device_time_total for ev in prof.key_averages() if "decimate_kernel" in ev.key)
+            if k:
+                times.append(us / 1e3 * nbuf / (nbuf + 1))          # without the EOF buffer's share
+    kern = statistics.median(times)
+    e2e = {label: [], "2 MHz": []}
+    counts = {}
+    for dd in decs.values():
+        dd.set_output_array(1 << 21)
+    for rep in range(args.reps + 1):
+        for name, dd in decs.items():
+            buf = hm if name == label else h20
+            dd.reset()
+            dd.rearm_output()
+            t0 = time.perf_counter()
+            dd.process_ptr(buf.ptr, buf.nbytes)
+            dd.finish()
+            t = time.perf_counter() - t0
+            counts[name] = dd.output_count()
+            if rep:
+                e2e[name].append(t * 1e3)
+    print(f"card: {card}")
+    print(f"K11 decimate by {m} (T = {taps}), {nbuf} buffers ({2 * n_out / 2**30:.2f} GiB of 2 MHz output) from "
+          f"{cap.size / 2**30:.3f} GiB of {label} input: {spread(times)}; {kern / (2 * n_out / 2**30):.4f} ms per GiB of output")
+    print(f"DRAM floor: {read_bytes / 1e9:.4f} GB read + {write_bytes / 1e9:.4f} GB written over a device-to-device "
+          f"copy at {copy_tbs:.2f} TB/s (read + write) -> {floor_ms:.4f} ms; kernel {kern / floor_ms:.2f}x the floor")
+    for name, v in e2e.items():
+        nbytes = hm.nbytes if name == label else h20.nbytes
         med = statistics.median(v)
         print(f"end to end {name}: {spread(v)} for {nbytes / 2**30:.3f} GiB from pinned memory "
               f"({nbytes / 1e9 / (med * 1e-3):.2f} GB/s of input); {counts[name]} messages")
