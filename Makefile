@@ -30,7 +30,10 @@ oracle:
 	if [ -d /root/reference ]; then $(MAKE) -C oracle ref; fi
 
 # test infrastructure: host build of the per-candidate evaluation (logic checked against the oracle on CPU)
-shim: tests/_build/libeval_serial_host.so tests/_build/libscan_core_host.so tests/_build/libresolve_core_host.so tests/_build/libsignal_core_host.so tests/_build/liblevels_core_host.so tests/_build/librecover_core_host.so tests/_build/libweak_core_host.so tests/_build/libarrival_core_host.so tests/_build/libresample_core_host.so tests/_build/libinput_core_host.so tests/_build/libpool_carry_host.so tests/_build/libdecimate_core_host.so
+shim: tests/_build/libeval_serial_host.so tests/_build/libscan_core_host.so tests/_build/libresolve_core_host.so tests/_build/libsignal_core_host.so tests/_build/liblevels_core_host.so tests/_build/librecover_core_host.so tests/_build/libweak_core_host.so tests/_build/libarrival_core_host.so tests/_build/libresample_core_host.so tests/_build/libinput_core_host.so tests/_build/libpool_carry_host.so tests/_build/libdecimate_core_host.so tests/_build/libshift_core_host.so
+tests/_build/libshift_core_host.so: tests/host_shim/shift_core_host.cpp $(CSRC)/modes_resample_core.cuh $(CSRC)/modes_input_core.cuh
+	@mkdir -p tests/_build
+	g++ -O2 -std=c++17 -shared -fPIC -Wall -Wno-unknown-pragmas -x c++ -I$(CSRC) tests/host_shim/shift_core_host.cpp -o $@
 tests/_build/libdecimate_core_host.so: tests/host_shim/decimate_core_host.cpp $(CSRC)/modes_resample_core.cuh $(CSRC)/modes_input_core.cuh
 	@mkdir -p tests/_build
 	g++ -O2 -std=c++17 -shared -fPIC -Wall -Wno-unknown-pragmas -x c++ -I$(CSRC) tests/host_shim/decimate_core_host.cpp -o $@

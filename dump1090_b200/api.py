@@ -195,7 +195,8 @@ EXPORTS = ["modes_abi_version", "modes_default_config", "modes_create", "modes_d
            "modes_weak_fetch", "modes_resolver_run_weak", "modes_resolver_run_shards_weak", "modes_resolver_weak_stats",
            "modes_pool_set_weak_preambles", "modes_pool_weak_stats", "modes_set_arrival", "modes_pool_set_arrival",
            "modes_set_input_rate", "modes_resample_device", "modes_pool_set_input_rate", "modes_set_input_format",
-           "modes_pool_set_input_format", "modes_resample_device_at"]
+           "modes_pool_set_input_format", "modes_resample_device_at", "modes_set_input_offset",
+           "modes_resample_device_shift"]
 
 INPUT_RATES = (2_000_000, 2_400_000, 4_000_000, 6_000_000, 8_000_000, 10_000_000)      # modes_set_input_rate
 INPUT_FORMATS = {"uc8": 0, "sc16": 1, "sc16q11": 2}     # modes_set_input_format: MODES_INPUT_*
@@ -346,6 +347,9 @@ def lib():
                                             C.c_int64, C.c_void_p, C.c_void_p]
         L.modes_resample_device_at.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_int64, C.c_int64,
                                                C.c_size_t, C.c_int64, C.c_void_p, C.c_void_p]
+        L.modes_set_input_offset.argtypes = [C.c_void_p, C.c_int32]
+        L.modes_resample_device_shift.argtypes = [C.c_void_p, C.c_uint32, C.c_int32, C.c_void_p, C.c_size_t, C.c_int64,
+                                                  C.c_int64, C.c_size_t, C.c_int64, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -434,11 +438,15 @@ class Decoder:
     input_format="sc16" or "sc16q11" takes signed 16-bit I/Q bytes (SoapySDR and Airspy-class tools,
     bladeRF) and converts them to 8-bit I/Q on the GPU with input_shift (None: the format's default)
     before the pipeline (modes_set_input_format): the messages are exactly the UC8 decoder's on the
-    converted bytes, at either input rate."""
+    converted bytes, at either input rate.
+    input_offset=+2_000_000 (Hz) decodes a 4-10 MS/s capture whose radio was tuned 2 MHz below 1090 MHz,
+    as zero-IF radios are to keep their DC spike off the channel: the input is shifted back by that much on
+    the GPU as it is decimated (modes_set_input_offset, |offset| <= input_rate / 2 - 1 MHz); 0 changes
+    nothing."""
 
     def __init__(self, signal: bool = False, levels: bool = False, recover: bool = False, weak_preambles: bool = False,
                  arrival: bool = False, input_rate: int = 2_000_000, input_format: str = "uc8",
-                 input_shift: int | None = None, **cfg):
+                 input_shift: int | None = None, input_offset: int = 0, **cfg):
         self.cfg = make_config(**cfg)
         self._h = lib().modes_create(C.byref(self.cfg))
         if not self._h:
@@ -447,6 +455,8 @@ class Decoder:
             self.set_input_rate(input_rate)
         if input_format != "uc8" or input_shift is not None:
             self.set_input_format(input_format, input_shift)
+        if input_offset:
+            self.set_input_offset(input_offset)
         if signal:
             self.set_signal(True)
         if arrival:
@@ -543,6 +553,13 @@ class Decoder:
         (modes_set_input_rate); refused while a stream is in progress.  sample_pos counts 2 MHz samples at
         every rate, and 6 * sample_pos is the input time in 12 MHz ticks."""
         self._check(lib().modes_set_input_rate(self._h, int(hz)))
+
+    def set_input_offset(self, hz: int) -> None:
+        """Where 1090 MHz sits in the capture's baseband, in Hz (+2_000_000: the radio was tuned to 1088 MHz),
+        for the stream that begins at the next reset (modes_set_input_offset): 0, or at the decimated rates
+        |hz| <= input_rate / 2 - 1 MHz; refused while a stream is in progress.  set_input_rate refuses a rate
+        that cannot take the offset already set, so set it to 0 before changing to such a rate."""
+        self._check(lib().modes_set_input_offset(self._h, int(hz)))
 
     def set_input_format(self, fmt: str, shift: int | None = None) -> None:
         """The sample format of the stream that begins at the next reset: "uc8", "sc16" or "sc16q11"
@@ -684,6 +701,17 @@ class Decoder:
         self._check(lib().modes_resample_device_at(self._h, int(hz), C.c_void_p(d_in_ptr or None), int(in_bytes),
                                                    int(in_first_sample), int(first_buffer), int(n_buffers), int(out_end),
                                                    C.c_void_p(d_out_ptr), carry))
+        return bytes(carry) if want_carry else None
+
+    def resample_device_shift(self, hz: int, offset_hz: int, d_in_ptr: int, in_bytes: int, in_first_sample: int,
+                              first_buffer: int, n_buffers: int, d_out_ptr: int, out_end: int = -1,
+                              want_carry: bool = True) -> bytes | None:
+        """resample_device_at with the input first shifted by offset_hz (modes_resample_device_shift), the phase
+        from each sample's stream index; offset_hz 0 is resample_device_at exactly."""
+        carry = (C.c_uint8 * CARRY_BYTES)() if want_carry else None
+        self._check(lib().modes_resample_device_shift(self._h, int(hz), int(offset_hz), C.c_void_p(d_in_ptr or None),
+                                                      int(in_bytes), int(in_first_sample), int(first_buffer),
+                                                      int(n_buffers), int(out_end), C.c_void_p(d_out_ptr), carry))
         return bytes(carry) if want_carry else None
 
     def levels_device(self, d_iq_ptr: int, n_buffers: int, stride_bytes: int = 0) -> None:

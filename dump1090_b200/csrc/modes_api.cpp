@@ -174,6 +174,9 @@ struct modes_ctx {
     const InputRate *rate = find_input_rate(2000000);
     uint32_t input_format = input::kUC8;
     int input_shift = 0;
+    // modes_set_input_offset: where 1090 MHz sits in the capture's baseband (0 unless rate->m); K12 rotates
+    // the input by it as it decimates.  The pair (rate, input_offset) is always one the setters accept.
+    int32_t input_offset = 0;
     int64_t in_total = 0;
     PinnedBuf<uint8_t> hold;
     int64_t hold0 = 0;
@@ -679,7 +682,7 @@ int stage_held(modes_ctx *ctx, Slot &s, const Source &src, size_t nb) {
     const ResampleJob j{s.d_in.get(), (uint64_t)(hi - lo), lo / bps, o0, (uint64_t)(o1 - o0), src.out_end,
                         s.d_iq.get(), s.d_halo.get()};
     const int shift = ctx->input_format == input::kUC8 ? -1 : ctx->input_shift;
-    if (ctx->rate->m) launch_decimate(j, ctx->rate->m, shift, s.stream);
+    if (ctx->rate->m) launch_decimate(j, ctx->rate->m, shift, shift::step(ctx->input_offset, ctx->rate->hz), s.stream);
     else if (ctx->input_format == input::kUC8) launch_resample(j, s.stream);
     else if (ctx->rate->hz == 2400000) launch_resample_sc16(j, ctx->input_shift, s.stream);
     else launch_convert_sc16(j, ctx->input_shift, s.stream);
@@ -1131,10 +1134,26 @@ int modes_set_input_rate(modes_ctx *ctx, uint32_t hz) {
     if (!r)
         return fail(ctx, "modes_set_input_rate: %u samples/s is not supported (2000000, 2400000, 4000000, 6000000, "
                          "8000000 or 10000000)", hz);
+    if (!offset_fits(*r, ctx->input_offset))
+        return fail(ctx, "modes_set_input_rate: %u samples/s is not supported with the input offset of %d Hz (at most "
+                         "%d Hz); set the offset to 0 first", hz, (int)ctx->input_offset, (int)max_offset(*r));
     if (ctx->started && !ctx->finished)
         return fail(ctx, "modes_set_input_rate: a stream is in progress; call modes_finish or modes_reset first");
     ctx->rate = r;
     for (modes_ctx *g : ctx->gpus) g->rate = r;
+    return 0;
+}
+
+int modes_set_input_offset(modes_ctx *ctx, int32_t offset_hz) {
+    if (!ctx) return -1;
+    if (!offset_fits(*ctx->rate, offset_hz))
+        return fail(ctx, "modes_set_input_offset: %d Hz is not supported at %u samples/s (at most %d Hz; 4000000 to "
+                         "10000000 samples/s take fs / 2 - 1 MHz, the other rates only 0)",
+                    (int)offset_hz, ctx->rate->hz, (int)max_offset(*ctx->rate));
+    if (ctx->started && !ctx->finished)
+        return fail(ctx, "modes_set_input_offset: a stream is in progress; call modes_finish or modes_reset first");
+    ctx->input_offset = offset_hz;
+    for (modes_ctx *g : ctx->gpus) g->input_offset = offset_hz;
     return 0;
 }
 
@@ -1253,11 +1272,21 @@ int modes_resample_device(modes_ctx *ctx, const void *d_in, size_t in_bytes, int
 
 int modes_resample_device_at(modes_ctx *ctx, uint32_t hz, const void *d_in, size_t in_bytes, int64_t in_first_sample,
                              int64_t first_buffer, size_t n_buffers, int64_t out_end, void *d_out, uint8_t *carry476) {
+    return modes_resample_device_shift(ctx, hz, 0, d_in, in_bytes, in_first_sample, first_buffer, n_buffers, out_end,
+                                       d_out, carry476);
+}
+
+int modes_resample_device_shift(modes_ctx *ctx, uint32_t hz, int32_t offset_hz, const void *d_in, size_t in_bytes,
+                                int64_t in_first_sample, int64_t first_buffer, size_t n_buffers, int64_t out_end,
+                                void *d_out, uint8_t *carry476) {
     if (!ctx) return -1;
     const InputRate *r = find_input_rate(hz);
     if (!r || hz == 2000000)
         return fail(ctx, "modes_resample_device: %u samples/s is not supported (2400000, 4000000, 6000000, 8000000 or "
                          "10000000)", hz);
+    if (!offset_fits(*r, offset_hz))
+        return fail(ctx, "modes_resample_device: an input offset of %d Hz is not supported at %u samples/s (at most %d Hz)",
+                    (int)offset_hz, hz, (int)max_offset(*r));
     if (!d_out || !n_buffers) return fail(ctx, "modes_resample_device: empty output");
     if (!d_in && in_bytes) return fail(ctx, "modes_resample_device: no input");
     if (first_buffer < 0) return fail(ctx, "modes_resample_device: buffer index %lld", (long long)first_buffer);
@@ -1272,7 +1301,7 @@ int modes_resample_device_at(modes_ctx *ctx, uint32_t hz, const void *d_in, size
     const ResampleJob j{static_cast<const uint8_t *>(d_in), in_bytes, in_first_sample, first_buffer * (int64_t)kBufSamples,
                         (uint64_t)n_buffers * kBufSamples, out_end < 0 ? INT64_MAX : out_end,
                         static_cast<uint8_t *>(d_out), carry476 ? ctx->d_rs_halo.get() : nullptr};
-    if (r->m) launch_decimate(j, r->m, -1, st);
+    if (r->m) launch_decimate(j, r->m, -1, shift::step(offset_hz, hz), st);
     else launch_resample(j, st);
     CK(ctx, cudaGetLastError());
     ctx->launches++;

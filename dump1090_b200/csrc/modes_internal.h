@@ -118,8 +118,9 @@ void launch_resample(const ResampleJob &j, cudaStream_t stream);
 void launch_resample_sc16(const ResampleJob &j, int shift, cudaStream_t stream);
 void launch_convert_sc16(const ResampleJob &j, int shift, cudaStream_t stream);
 // 4, 6, 8 and 10 MS/s (K11): the same job decimated by m = 2..5, the input UC8 (shift < 0) or int16
-// converted with the shift; any in_first, out_first a multiple of 8.
-void launch_decimate(const ResampleJob &j, int m, int shift, cudaStream_t stream);
+// converted with the shift; any in_first, out_first a multiple of 8.  step != 0 (K12): each input sample
+// is first rotated by shift::step's phase at its stream index (modes_set_input_offset); step 0 is K11.
+void launch_decimate(const ResampleJob &j, int m, int shift, uint32_t step, cudaStream_t stream);
 // The receiver pool's 2.4 MS/s receivers (modes_pool.cpp): one launch for one job per pair of the pool's
 // batch.  A job's input is its receiver's stream bytes [hist0, call0) at hist (the receiver's device input
 // history) and [call0, call0 + MODES_BUFFER_BYTES) at stage (the call's bytes); every other input byte

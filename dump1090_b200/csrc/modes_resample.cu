@@ -16,7 +16,8 @@
 // launch converts every 16-bit buffer of a call, ahead of the pool's resampling launches.
 //
 // K11 (decimate_kernel): 4, 6, 8 and 10 MS/s input decimated by M = 2..5, in K10's groups of 8 output
-// samples, from either staging loader.
+// samples, from either staging loader.  K12 (its Shift form): the same with each input sample first
+// rotated by the capture's offset from 1090 MHz (modes_set_input_offset).
 #include "modes_internal.h"
 #include "modes_input_core.cuh"
 #include "modes_resample_core.cuh"
@@ -180,11 +181,28 @@ __global__ void __launch_bounds__(kThreads) convert_kernel(ResampleJob j, int64_
 // the staging loaders, straight into registers, and aligns them there: the window starts sh bytes into its
 // first word, and sh is the same for every group of a launch (groups are 16 M bytes apart).  The taps are
 // immediates; neighbouring groups share at most two words, which L1 serves.
-template <int M, class Input>
-__global__ void __launch_bounds__(kThreads) decimate_kernel(ResampleJob j, int64_t g_first, int64_t n_groups, Input input) {
+//
+// K12 (Shift): the same kernel for a capture tuned off 1090 MHz (modes_set_input_offset).  Each sample of the
+// window is rotated once, by the phase of its absolute stream index (so batches, shards and GPUs agree with
+// nothing carried between them), and the filter runs on the rotated values (shift::shift_group).  The 1024
+// rotations sit in shared memory, one word (C, S) each, written by each block from the header's C and S: a
+// warp's phases differ from thread to thread unless 8 M step is a multiple of 2^32, which __constant__ would
+// serialise.  One word per phase keeps a warp's gather to one wavefront when its phases fall in distinct
+// banks; 16-byte entries that also held (-S, C) and both constants cost 1.5-2x K11's time at such offsets on
+// an H100, and the same table read with __ldg from global memory no less (DESIGN §3 K12).  Shift = false is
+// K11 as it was: step is not read.
+template <int M, class Input, bool Shift>
+__global__ void __launch_bounds__(kThreads) decimate_kernel(ResampleJob j, int64_t g_first, int64_t n_groups, Input input,
+                                                            uint32_t step) {
     namespace D = decimate;
     if (j.halo && blockIdx.x == 0 && threadIdx.x < (kHaloAlloc - kHaloBytes) / 16)
         reinterpret_cast<uint4 *>(j.halo + kHaloBytes)[threadIdx.x] = make_uint4(0x7f7f7f7fu, 0x7f7f7f7fu, 0x7f7f7f7fu, 0x7f7f7f7fu);
+    __shared__ uint32_t s_rot[Shift ? shift::kPhases : 1];
+    if constexpr (Shift) {
+#pragma unroll
+        for (int k = threadIdx.x; k < shift::kPhases; k += kThreads) s_rot[k] = shift::rotation(shift::kCos[k], shift::kSin[k]);
+        __syncthreads();
+    }
     const int64_t g = (int64_t)blockIdx.x * kThreads + threadIdx.x;
     if (g >= n_groups) return;
     const int64_t n0 = 8 * (g_first + g);
@@ -208,7 +226,10 @@ __global__ void __launch_bounds__(kThreads) decimate_kernel(ResampleJob j, int64
 #pragma unroll
     for (int i = 0; i < 4 * kWords + 3; i++) w[i] = (sh & 2) ? __funnelshift_r(w[i], w[i + 1], 16) : w[i];
     uint4 v;
-    D::group<M>(w, reinterpret_cast<uint32_t *>(&v));
+    if constexpr (Shift)
+        shift::shift_group<M>(w, s_rot, (uint32_t)(M * n0 - D::extent(M)) * step, step, reinterpret_cast<uint32_t *>(&v));
+    else
+        D::group<M>(w, reinterpret_cast<uint32_t *>(&v));
     const int64_t c0 = j.out_first - MODES_CARRY_BYTES / 2;
     if (n0 + 8 > j.out_end || n0 < c0) {
         uint16_t *x = reinterpret_cast<uint16_t *>(&v);
@@ -354,22 +375,28 @@ void launch_convert_sc16(const ResampleJob &j, int shift, cudaStream_t stream) {
 }
 
 namespace {
-template <int M>
-void launch_decimate_m(const ResampleJob &j, int64_t g_first, int64_t groups, int shift, cudaStream_t stream) {
+template <int M, bool Shift>
+void launch_decimate_m(const ResampleJob &j, int64_t g_first, int64_t groups, int shift, uint32_t step, cudaStream_t stream) {
     const unsigned blocks = (unsigned)((groups + kThreads - 1) / kThreads);
-    if (shift < 0) decimate_kernel<M><<<blocks, kThreads, 0, stream>>>(j, g_first, groups, Uc8Input{});
-    else decimate_kernel<M><<<blocks, kThreads, 0, stream>>>(j, g_first, groups, Sc16Input{shift});
+    if (shift < 0) decimate_kernel<M, Uc8Input, Shift><<<blocks, kThreads, 0, stream>>>(j, g_first, groups, Uc8Input{}, step);
+    else decimate_kernel<M, Sc16Input, Shift><<<blocks, kThreads, 0, stream>>>(j, g_first, groups, Sc16Input{shift}, step);
+}
+
+template <int M>
+void launch_decimate_m(const ResampleJob &j, int64_t g_first, int64_t groups, int shift, uint32_t step, cudaStream_t stream) {
+    if (step) launch_decimate_m<M, true>(j, g_first, groups, shift, step, stream);
+    else launch_decimate_m<M, false>(j, g_first, groups, shift, 0, stream);
 }
 }  // namespace
 
-void launch_decimate(const ResampleJob &j, int m, int shift, cudaStream_t stream) {
+void launch_decimate(const ResampleJob &j, int m, int shift, uint32_t step, cudaStream_t stream) {
     const int64_t first = j.out_first - (j.halo ? kHaloSamples : 0);
     const int64_t groups = (j.out_first + (int64_t)j.out_samples - first) / 8;
     switch (m) {
-    case 2: launch_decimate_m<2>(j, first / 8, groups, shift, stream); break;
-    case 3: launch_decimate_m<3>(j, first / 8, groups, shift, stream); break;
-    case 4: launch_decimate_m<4>(j, first / 8, groups, shift, stream); break;
-    case 5: launch_decimate_m<5>(j, first / 8, groups, shift, stream); break;
+    case 2: launch_decimate_m<2>(j, first / 8, groups, shift, step, stream); break;
+    case 3: launch_decimate_m<3>(j, first / 8, groups, shift, step, stream); break;
+    case 4: launch_decimate_m<4>(j, first / 8, groups, shift, step, stream); break;
+    case 5: launch_decimate_m<5>(j, first / 8, groups, shift, step, stream); break;
     }
 }
 

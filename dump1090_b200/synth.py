@@ -174,14 +174,18 @@ def frame_envelope_at(frame: bytes, pos: int, frac: float, sample_rate: int) -> 
 
 
 def synth_stream_at(nsamples: int, frames, sigma: float = 1.5, seed: int = 1, sample_rate: int = 2_000_000,
-                    dtype: str = "uc8", scale: float = 1.0, tone=None) -> np.ndarray:
+                    dtype: str = "uc8", scale: float = 1.0, tone=None, carrier_hz: float = 0.0, dc=None) -> np.ndarray:
     """synth_stream at any sample rate: frames are (pos, frame_bytes, amplitude_lsb, carrier_phase_rad,
     frac) with the arrival time pos + frac in 2 MHz samples (0.5 us), pulses per frame_envelope_at, and
     the same noise per sample as synth_stream.  At 2 MHz it equals synth_stream bit for bit.
     dtype="sc16": the same signal as signed little-endian 16-bit I/Q bytes (4 a sample), scale int16
     units to an 8-bit LSB (16 is SC16Q11's full scale, 256 SC16's), rounded and clamped to int16.
     tone=(offset_hz, amplitude_lsb): a continuous carrier at that offset from the channel centre is added
-    (an out-of-band interferer where the offset is past 1 MHz); None, the default, adds nothing."""
+    (an out-of-band interferer where the offset is past 1 MHz); None, the default, adds nothing.
+    carrier_hz: the frames are sent at that offset from the baseband's 0 Hz (a radio tuned carrier_hz below
+    1090 MHz), their phase turning by 2 pi carrier_hz / sample_rate per sample of the stream; 0, the
+    default, leaves them as they were.  dc=(i, q): a constant (a zero-IF radio's DC spike, in 8-bit LSB)
+    added to every sample; None, the default, adds nothing."""
     i = noise(nsamples, sigma, seed * 2 + 11)
     q = noise(nsamples, sigma, seed * 2 + 12)
     if tone is not None:
@@ -198,8 +202,16 @@ def synth_stream_at(nsamples: int, frames, sigma: float = 1.5, seed: int = 1, sa
         if start >= nsamples or end <= start:
             continue
         seg = env[: end - start]
-        i[start:end] += seg * np.cos(phase)
-        q[start:end] += seg * np.sin(phase)
+        if carrier_hz:
+            ph = phase + 2 * np.pi * (carrier_hz / sample_rate) * np.arange(start, end, dtype=np.float64)
+            i[start:end] += seg * np.cos(ph)
+            q[start:end] += seg * np.sin(ph)
+        else:
+            i[start:end] += seg * np.cos(phase)
+            q[start:end] += seg * np.sin(phase)
+    if dc is not None:
+        i += dc[0]
+        q += dc[1]
     if dtype == "sc16":
         out16 = np.empty(2 * nsamples, dtype="<i2")
         out16[0::2] = np.clip(np.rint(scale * i), -32768, 32767)
@@ -371,10 +383,11 @@ def fleet_at(snr_db: float, nframes: int, seed: int, n_aircraft: int = 20, amp: 
 
 
 def fleet_at_rate(snr_db: float, nframes: int, seed: int, sample_rate: int = 2_400_000, n_aircraft: int = 20,
-                  amp: float = 20.0, period: int = 400, dtype: str = "uc8", scale: float = 1.0, tone=None):
+                  amp: float = 20.0, period: int = 400, dtype: str = "uc8", scale: float = 1.0, tone=None,
+                  carrier_hz: float = 0.0, dc=None):
     """fleet_at sampled at sample_rate (2.4 MS/s: what dump1090-fa and readsb record): the same frames,
     arrival times, amplitudes and carrier phases, over the same stretch of time, with the same noise per
-    sample; dtype, scale and tone as synth_stream_at.  Returns (stream, set of the frames' hex)."""
+    sample; dtype, scale, tone, carrier_hz and dc as synth_stream_at.  Returns (stream, set of the frames' hex)."""
     sigma = amp / (np.sqrt(2.0) * 10 ** (snr_db / 20.0))
     rng = Counter(seed)
     fleet = [0x400000 + rng.below(0x3FFFFF) for _ in range(n_aircraft)]
@@ -388,7 +401,7 @@ def fleet_at_rate(snr_db: float, nframes: int, seed: int, sample_rate: int = 2_4
     a, b = _rate_ratio(sample_rate)
     n = -(-(200 + nframes * period + 400) * a // b)
     return synth_stream_at(n, frames, sigma=sigma, seed=seed, sample_rate=sample_rate, dtype=dtype, scale=scale,
-                           tone=tone), truth
+                           tone=tone, carrier_hz=carrier_hz, dc=dc), truth
 
 
 def tile_to(data: np.ndarray, nbytes: int) -> np.ndarray:

@@ -37,6 +37,10 @@
  * converted to 8 bits on the GPU (modes_set_input_format).  --iformat-shift <0..15> replaces the
  * format's default shift (SC16 8, SC16Q11 4; not with UC8): a smaller one for a quiet capture, checked
  * with the clipping count of --levels.  Both combine with --sample-rate, every output mode and switch.
+ * --input-offset <hz> says where 1090 MHz sits in the file's baseband, for a radio tuned off the channel
+ * (+2000000: tuned to 1088 MHz, as zero-IF radios are to keep their DC spike away from it): the input is
+ * shifted back by that much on the GPU as it is decimated (modes_set_input_offset).  It needs
+ * --sample-rate 4000000 to 10000000, and |hz| at most half the rate less 1 MHz (1, 2, 3 or 4 MHz).
  * The live-radio, networking and interactive options are out of scope.
  */
 #include <math.h>
@@ -119,6 +123,7 @@ int main(int argc, char **argv) {
     unsigned long sample_rate = 2000000;
     const char *iformat = "UC8";
     const char *iformat_shift = NULL;
+    const char *input_offset = NULL;
     modes_default_config(&cfg);
     for (int j = 1; j < argc; j++) {
         int more = j + 1 < argc;
@@ -144,6 +149,7 @@ int main(int argc, char **argv) {
         else if (!strcmp(argv[j], "--sample-rate") && more) sample_rate = strtoul(argv[++j], NULL, 10);
         else if (!strcmp(argv[j], "--iformat") && more) iformat = argv[++j];
         else if (!strcmp(argv[j], "--iformat-shift") && more) iformat_shift = argv[++j];
+        else if (!strcmp(argv[j], "--input-offset") && more) input_offset = argv[++j];
         else {
             fprintf(stderr, "Unknown or not enough arguments for option '%s'.\n", argv[j]);
             return 1;
@@ -177,6 +183,20 @@ int main(int argc, char **argv) {
         }
         shift = (int32_t)v;
     }
+    int32_t offset_hz = 0;
+    if (input_offset) {
+        char *end;
+        const long v = strtol(input_offset, &end, 10);
+        if (!*input_offset || *end || v < -4000000 || v > 4000000) {
+            fprintf(stderr, "--input-offset takes a whole number of Hz from -4000000 to 4000000\n");
+            return 1;
+        }
+        if (v && sample_rate < 4000000) {
+            fprintf(stderr, "--input-offset needs --sample-rate 4000000, 6000000, 8000000 or 10000000\n");
+            return 1;
+        }
+        offset_hz = (int32_t)v;
+    }
     if (opt_beast && (opt_raw || opt_onlyaddr || opt_sbs || opt_json)) {
         fprintf(stderr, "--beast writes binary frames to stdout: it cannot be combined with --raw, --onlyaddr, --sbs or --aircraft-json\n");
         return 1;
@@ -201,6 +221,7 @@ int main(int argc, char **argv) {
     }
     if (modes_set_input_rate(ctx, (uint32_t)sample_rate)) { fprintf(stderr, "--sample-rate: %s\n", modes_last_error(ctx)); return 1; }
     if (modes_set_input_format(ctx, format, shift)) { fprintf(stderr, "--iformat: %s\n", modes_last_error(ctx)); return 1; }
+    if (modes_set_input_offset(ctx, offset_hz)) { fprintf(stderr, "--input-offset: %s\n", modes_last_error(ctx)); return 1; }
     if (opt_beast) modes_set_signal(ctx, 1);
     if (opt_arrival) modes_set_arrival(ctx, 1);
     if (opt_levels) modes_set_levels(ctx, 1);

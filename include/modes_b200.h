@@ -210,6 +210,28 @@ int  modes_get_stats(const modes_ctx *ctx, modes_stats *out);
  * Output sample n starts at input sample M n exactly, so 6 * sample_pos stays the 12 MHz time.  Level
  * records describe the decimated bytes. */
 int  modes_set_input_rate(modes_ctx *ctx, uint32_t hz);
+/* Where 1090 MHz sits in the capture's baseband, for a radio tuned off the channel (a zero-IF front end
+ * tuned 1-3 MHz away from its DC spike, or a recording centred elsewhere): +2000000 means the radio was
+ * tuned to 1088 MHz.  The decoder multiplies the input by e^{-j 2 pi offset_hz n / fs} before decimating.
+ * 0, the default, is always taken.  Another value is taken only at 4000000 to 10000000 samples/s, with
+ * |offset_hz| <= fs / 2 - 1 MHz (1, 2, 3 and 4 MHz at 4, 6, 8 and 10 MS/s); otherwise it is refused with
+ * "not supported", and modes_set_input_rate likewise refuses a rate whose range excludes the offset
+ * already set (so a caller who changes both sets the offset to 0 first).  Both setters are refused between
+ * the first modes_process of a stream and modes_finish / modes_reset; modes_reset keeps the offset, and on
+ * an n_gpus > 1 context it reaches every GPU.  Exactly, for input sample m counted from the stream's start
+ * (int16 input after its conversion), xi = I - 127 and xq = Q - 127 (0 outside the stream):
+ *   step    = round(offset_hz 2^32 / fs)                       (int64 arithmetic, stored as uint32)
+ *   theta_m = (m step) mod 2^32                                (m taken mod 2^32 first)
+ *   k_m     = ((theta_m + 2^21) >> 22) & 1023                  (the nearest of 1024 phases)
+ *   c, s    = C[k_m], S[k_m]  with C[k] = round(16384 cos(2 pi k / 1024)), S[k] = round(16384 sin(2 pi k / 1024))
+ *   u_i     = (xi c + xq s + 8192) >> 14,  u_q = (xq c - xi s + 8192) >> 14   (int32, arithmetic shift)
+ *   y       = clamp(127 + ((sum_{k<T} h_M[k] u[M n - E + k] + 8192) >> 14), 0, 255)   for I and Q separately
+ * with h_M, E and T the decimator's above (modes_resample_core.cuh has C and S).  The shift applied is
+ * step fs / 2^32 Hz, within 0.002 Hz of offset_hz.  N_out, the EOF buffer, sample_pos, 6 * sample_pos as the
+ * 12 MHz time and the arrival estimate keep their meaning: output n still starts at input sample M n.  At
+ * offset 0 the output is the decimator's, byte for byte.  The receiver pool has no offset (it does not
+ * take the decimated rates). */
+int  modes_set_input_offset(modes_ctx *ctx, int32_t offset_hz);
 /* The same per receiver of a pool (modes_pool_* below): 2000000 (the default) or 2400000; refused, with
  * "not supported", for any other value (the decimated rates included), a receiver out of range, and while the receiver has a stream in progress (from the
  * first modes_pool_submit / _ingest that names it until modes_pool_reset, which keeps the rate).  It
@@ -305,6 +327,13 @@ int  modes_resample_device(modes_ctx *ctx, const void *d_in, size_t in_bytes, in
  * with "not supported". */
 int  modes_resample_device_at(modes_ctx *ctx, uint32_t hz, const void *d_in, size_t in_bytes, int64_t in_first_sample,
                               int64_t first_buffer, size_t n_buffers, int64_t out_end, void *d_out, uint8_t *carry476);
+/* modes_resample_device_at with the input first rotated by offset_hz as modes_set_input_offset defines it,
+ * the phase taken from each sample's stream index in_first_sample + i (so spans of one stream agree wherever
+ * they are cut).  offset_hz 0 is modes_resample_device_at exactly; another offset is taken only at
+ * 4000000 to 10000000 with |offset_hz| <= hz / 2 - 1 MHz, and refused with "not supported" otherwise. */
+int  modes_resample_device_shift(modes_ctx *ctx, uint32_t hz, int32_t offset_hz, const void *d_in, size_t in_bytes,
+                                 int64_t in_first_sample, int64_t first_buffer, size_t n_buffers, int64_t out_end,
+                                 void *d_out, uint8_t *carry476);
 /* Wait for the last modes_detect_device; returns the candidate count. */
 int  modes_detect_wait(modes_ctx *ctx, uint64_t *n_candidates);
 /* Copy the last result to host memory (arrays sized by the caller from
