@@ -7,15 +7,15 @@ ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := $(ARCH) -O3 -lineinfo -std=c++17 -Iinclude -Xcompiler -fPIC,-Wall,-Wextra
 CSRC      := dump1090_b200/csrc
 LIB       := dump1090_b200/libmodes_b200.so
-OBJS      := build/modes_kernels.o build/modes_scan2.o build/modes_eval_fused.o build/modes_signal.o build/modes_levels.o build/modes_recover.o build/modes_weak.o build/modes_resample.o build/modes_resolve_gpu.o build/modes_api.o build/modes_resolve.o build/modes_tables.o build/modes_format.o build/modes_tracker.o build/modes_pool.o
+OBJS      := build/modes_kernels.o build/modes_scan2.o build/modes_eval_fused.o build/modes_signal.o build/modes_levels.o build/modes_spectrum.o build/modes_recover.o build/modes_weak.o build/modes_resample.o build/modes_resolve_gpu.o build/modes_api.o build/modes_resolve.o build/modes_tables.o build/modes_format.o build/modes_tracker.o build/modes_pool.o
 
 all: $(LIB) dump1090-b200
 
-build/%.o: $(CSRC)/%.cu $(CSRC)/modes_internal.h $(CSRC)/modes_eval_serial.cuh $(CSRC)/modes_scan_core.cuh $(CSRC)/modes_resolve_core.cuh $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_arrival_core.cuh $(CSRC)/modes_levels_core.cuh $(CSRC)/modes_recover_core.cuh $(CSRC)/modes_weak_core.cuh $(CSRC)/modes_resample_core.cuh $(CSRC)/modes_input_core.cuh include/modes_b200.h
+build/%.o: $(CSRC)/%.cu $(CSRC)/modes_internal.h $(CSRC)/modes_eval_serial.cuh $(CSRC)/modes_scan_core.cuh $(CSRC)/modes_resolve_core.cuh $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_arrival_core.cuh $(CSRC)/modes_levels_core.cuh $(CSRC)/modes_recover_core.cuh $(CSRC)/modes_weak_core.cuh $(CSRC)/modes_resample_core.cuh $(CSRC)/modes_input_core.cuh $(CSRC)/modes_spectrum_core.cuh $(CSRC)/modes_stage.cuh include/modes_b200.h
 	@mkdir -p build
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@
 
-build/%.o: $(CSRC)/%.cpp $(CSRC)/modes_internal.h $(CSRC)/modes_input_core.cuh $(CSRC)/modes_resample_core.cuh include/modes_b200.h
+build/%.o: $(CSRC)/%.cpp $(CSRC)/modes_internal.h $(CSRC)/modes_input_core.cuh $(CSRC)/modes_resample_core.cuh $(CSRC)/modes_spectrum_core.cuh include/modes_b200.h
 	@mkdir -p build
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 
@@ -30,7 +30,10 @@ oracle:
 	if [ -d /root/reference ]; then $(MAKE) -C oracle ref; fi
 
 # test infrastructure: host build of the per-candidate evaluation (logic checked against the oracle on CPU)
-shim: tests/_build/libeval_serial_host.so tests/_build/libscan_core_host.so tests/_build/libresolve_core_host.so tests/_build/libsignal_core_host.so tests/_build/liblevels_core_host.so tests/_build/librecover_core_host.so tests/_build/libweak_core_host.so tests/_build/libarrival_core_host.so tests/_build/libresample_core_host.so tests/_build/libinput_core_host.so tests/_build/libpool_carry_host.so tests/_build/libdecimate_core_host.so tests/_build/libshift_core_host.so
+shim: tests/_build/libeval_serial_host.so tests/_build/libscan_core_host.so tests/_build/libresolve_core_host.so tests/_build/libsignal_core_host.so tests/_build/liblevels_core_host.so tests/_build/librecover_core_host.so tests/_build/libweak_core_host.so tests/_build/libarrival_core_host.so tests/_build/libresample_core_host.so tests/_build/libinput_core_host.so tests/_build/libpool_carry_host.so tests/_build/libdecimate_core_host.so tests/_build/libshift_core_host.so tests/_build/libspectrum_core_host.so
+tests/_build/libspectrum_core_host.so: tests/host_shim/spectrum_core_host.cpp $(CSRC)/modes_spectrum_core.cuh $(CSRC)/modes_resample_core.cuh include/modes_b200.h
+	@mkdir -p tests/_build
+	g++ -O2 -std=c++17 -shared -fPIC -Wall -Wno-unknown-pragmas -x c++ -Iinclude -I$(CSRC) tests/host_shim/spectrum_core_host.cpp -o $@
 tests/_build/libshift_core_host.so: tests/host_shim/shift_core_host.cpp $(CSRC)/modes_resample_core.cuh $(CSRC)/modes_input_core.cuh
 	@mkdir -p tests/_build
 	g++ -O2 -std=c++17 -shared -fPIC -Wall -Wno-unknown-pragmas -x c++ -I$(CSRC) tests/host_shim/shift_core_host.cpp -o $@

@@ -169,6 +169,57 @@ def level_summary(records) -> dict:
         out["clipped_fraction"] = clipped / n
     return out
 
+SPECTRUM_BINS = 256                       # MODES_SPECTRUM_BINS
+# struct modes_spectrum: the input power spectrum of one reference buffer (modes_set_spectrum)
+SPECTRUM_DTYPE = np.dtype([("buffer", "<i8"), ("frames", "<u4"), ("pad", "<u4"), ("power", "<u8", (SPECTRUM_BINS,))])
+assert SPECTRUM_DTYPE.itemsize == 16 + 8 * SPECTRUM_BINS
+BAND_HZ = 2_000_000                       # the width spectrum_summary searches: the 2 MHz the decoder keeps
+
+
+def spectrum_summary(records, input_rate: int) -> dict:
+    """What spectrum records (SPECTRUM_DTYPE) of a stream at input_rate say, for an operator:
+        freq_hz[i]     = (i - 128) fs / 256, the centre of bin i (bin 128 is DC)
+        power_db[i]    = 10 log10(sum power[i] / sum frames), the mean power per frame (-inf where it is 0)
+        floor_db       = the median of the mean powers, with the DC bin and its two neighbours (the Hann
+                         window's main lobe around DC) replaced by the mean of bins 126 and 130
+        dc_excess_db   = 10 log10(mean DC power / mean of bins 126 and 130') (0 when both are 0): a zero-IF
+                         radio's DC spike over the spectrum next to it
+        band_offset_hz = the centre of the W = floor(256 * 2 MHz / fs) adjacent bins with the most power above
+                         the floor (sum of max(mean - floor, 0); bins 127-129 replaced as for the floor; the
+                         lowest such band on a tie): where the 2 MHz channel most likely sits, the offset
+                         modes_set_input_offset takes
+    The band search and the floor are exact integer arithmetic on the sums.  With no frames every derived
+    value is None."""
+    r = np.asarray(records, dtype=SPECTRUM_DTYPE)
+    fs = int(input_rate)
+    if fs not in INPUT_RATES:
+        raise ValueError(f"{fs} samples/s is not supported {INPUT_RATES}")
+    n = SPECTRUM_BINS
+    frames = int(r["frames"].astype(np.uint64).sum()) if r.size else 0
+    total = [sum(int(v) for v in r["power"][:, i]) for i in range(n)] if r.size else [0] * n
+    out = dict(buffers=int(r.size), frames=frames, freq_hz=(np.arange(n) - n // 2) * (fs / n), power_db=None,
+               floor_db=None, dc_excess_db=None, band_offset_hz=None)
+    if not frames:
+        return out
+    out["power_db"] = np.array([10.0 * math.log10(t / frames) if t else -math.inf for t in total])
+    dc, nb = 2 * total[n // 2], total[n // 2 - 2] + total[n // 2 + 2]
+    out["dc_excess_db"] = 0.0 if dc == nb else math.inf if not nb else -math.inf if not dc else 10.0 * math.log10(dc / nb)
+    t2 = [2 * t for t in total]                                         # twice the sums: the DC notch exact
+    t2[n // 2 - 1: n // 2 + 2] = [nb] * 3
+    srt = sorted(t2)
+    floor4 = srt[n // 2 - 1] + srt[n // 2]                              # 4 x the median sum
+    out["floor_db"] = 10.0 * math.log10(floor4 / 4 / frames) if floor4 else -math.inf
+    above = [max(2 * t - floor4, 0) for t in t2]
+    w = n * BAND_HZ // fs
+    best, at = -1, 0
+    for i0 in range(n - w + 1):
+        score = sum(above[i0: i0 + w])
+        if score > best:
+            best, at = score, i0
+    out["band_offset_hz"] = (at + (w - 1) / 2 - n // 2) * fs / n
+    return out
+
+
 _lib = None
 
 # every symbol include/modes_b200.h declares
@@ -196,7 +247,8 @@ EXPORTS = ["modes_abi_version", "modes_default_config", "modes_create", "modes_d
            "modes_pool_set_weak_preambles", "modes_pool_weak_stats", "modes_set_arrival", "modes_pool_set_arrival",
            "modes_set_input_rate", "modes_resample_device", "modes_pool_set_input_rate", "modes_set_input_format",
            "modes_pool_set_input_format", "modes_resample_device_at", "modes_set_input_offset",
-           "modes_resample_device_shift"]
+           "modes_resample_device_shift", "modes_set_spectrum", "modes_take_spectra", "modes_pool_set_spectrum",
+           "modes_pool_take_spectra"]
 
 INPUT_RATES = (2_000_000, 2_400_000, 4_000_000, 6_000_000, 8_000_000, 10_000_000)      # modes_set_input_rate
 INPUT_FORMATS = {"uc8": 0, "sc16": 1, "sc16q11": 2}     # modes_set_input_format: MODES_INPUT_*
@@ -317,6 +369,12 @@ def lib():
         L.modes_pool_set_levels.argtypes = [C.c_void_p, C.c_int]
         L.modes_pool_take_levels.restype = C.c_size_t
         L.modes_pool_take_levels.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t]
+        L.modes_set_spectrum.argtypes = [C.c_void_p, C.c_int]
+        L.modes_take_spectra.restype = C.c_size_t
+        L.modes_take_spectra.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+        L.modes_pool_set_spectrum.argtypes = [C.c_void_p, C.c_int]
+        L.modes_pool_take_spectra.restype = C.c_size_t
+        L.modes_pool_take_spectra.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t]
         L.modes_set_recovery.argtypes = [C.c_void_p, C.c_int]
         L.modes_get_recovery_stats.argtypes = [C.c_void_p, C.POINTER(RecoveryStats)]
         L.modes_recover_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
@@ -442,11 +500,13 @@ class Decoder:
     input_offset=+2_000_000 (Hz) decodes a 4-10 MS/s capture whose radio was tuned 2 MHz below 1090 MHz,
     as zero-IF radios are to keep their DC spike off the channel: the input is shifted back by that much on
     the GPU as it is decimated (modes_set_input_offset, |offset| <= input_rate / 2 - 1 MHz); 0 changes
-    nothing."""
+    nothing.
+    spectrum=True measures every decoded buffer's input power spectrum on the GPU, before resampling,
+    decimation and the offset (modes_set_spectrum): take_spectra(), spectrum_summary()."""
 
     def __init__(self, signal: bool = False, levels: bool = False, recover: bool = False, weak_preambles: bool = False,
                  arrival: bool = False, input_rate: int = 2_000_000, input_format: str = "uc8",
-                 input_shift: int | None = None, input_offset: int = 0, **cfg):
+                 input_shift: int | None = None, input_offset: int = 0, spectrum: bool = False, **cfg):
         self.cfg = make_config(**cfg)
         self._h = lib().modes_create(C.byref(self.cfg))
         if not self._h:
@@ -463,6 +523,8 @@ class Decoder:
             self.set_arrival(True)
         if levels:
             self.set_levels(True)
+        if spectrum:
+            self.set_spectrum(True)
         if recover:
             self.set_recovery(True)
         if weak_preambles:
@@ -602,6 +664,17 @@ class Decoder:
         n = int(lib().modes_take_levels(self._h, None, 0))
         out = np.zeros(n, dtype=LEVEL_DTYPE)
         got = int(lib().modes_take_levels(self._h, _ptr(out), n)) if n else 0
+        return out[:got]
+
+    def set_spectrum(self, on: bool) -> None:
+        """Measure the buffers' input spectra for batches submitted from now on (modes_set_spectrum)."""
+        self._check(lib().modes_set_spectrum(self._h, int(bool(on))))
+
+    def take_spectra(self) -> np.ndarray:
+        """The queued spectrum records (SPECTRUM_DTYPE), oldest first, in stream order; the queue is emptied."""
+        n = int(lib().modes_take_spectra(self._h, None, 0))
+        out = np.zeros(n, dtype=SPECTRUM_DTYPE)
+        got = int(lib().modes_take_spectra(self._h, _ptr(out), n)) if n else 0
         return out[:got]
 
     def set_stream(self, cuda_stream: int) -> None:
@@ -937,6 +1010,7 @@ class ReceiverPool:
     statistics each, as one dump1090 process keeps per receiver), one buffer of each decoded per
     batch.  Messages are collected per receiver (`take(receiver)`).  signal=True: as for Decoder.
     levels=True: level records of every receiver's buffers (`take_levels(receiver)`).
+    spectrum=True: input spectrum records of every receiver's buffers (`take_spectra(receiver)`).
     recover=True: as for Decoder, with statistics per receiver (`recovery_stats(receiver)`).
     weak_preambles=True: as for Decoder (`weak_recovery_stats(receiver)`).  arrival=True: as for Decoder.
     input_rate=2_400_000 sets every receiver to 2.4 MS/s at creation, set_input_rate(receiver, hz) one
@@ -950,7 +1024,8 @@ class ReceiverPool:
 
     def __init__(self, n_receivers: int, max_batch: int = 0, signal: bool = False, levels: bool = False,
                  recover: bool = False, weak_preambles: bool = False, arrival: bool = False,
-                 input_rate: int = 2_000_000, input_format: str = "uc8", input_shift: int | None = None, **cfg):
+                 input_rate: int = 2_000_000, input_format: str = "uc8", input_shift: int | None = None,
+                 spectrum: bool = False, **cfg):
         self.cfg = make_config(**cfg)
         self.n = n_receivers
         self._bytes = [BUFFER_BYTES] * n_receivers
@@ -963,6 +1038,8 @@ class ReceiverPool:
             self.set_arrival(True)
         if levels:
             self.set_levels(True)
+        if spectrum:
+            self.set_spectrum(True)
         if recover:
             self.set_recovery(True)
         if weak_preambles:
@@ -1086,6 +1163,17 @@ class ReceiverPool:
         n = int(lib().modes_pool_take_levels(self._h, receiver, None, 0))
         out = np.zeros(n, dtype=LEVEL_DTYPE)
         got = int(lib().modes_pool_take_levels(self._h, receiver, _ptr(out), n)) if n else 0
+        return out[:got]
+
+    def set_spectrum(self, on: bool) -> None:
+        """Measure the input spectra of batches submitted from now on (modes_pool_set_spectrum)."""
+        self._check(lib().modes_pool_set_spectrum(self._h, int(bool(on))))
+
+    def take_spectra(self, receiver: int) -> np.ndarray:
+        """The receiver's queued spectrum records (SPECTRUM_DTYPE), its own buffer indices, oldest first."""
+        n = int(lib().modes_pool_take_spectra(self._h, receiver, None, 0))
+        out = np.zeros(n, dtype=SPECTRUM_DTYPE)
+        got = int(lib().modes_pool_take_spectra(self._h, receiver, _ptr(out), n)) if n else 0
         return out[:got]
 
     def buffers(self, receiver: int) -> int:

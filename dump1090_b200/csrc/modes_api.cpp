@@ -99,6 +99,12 @@ struct Slot {
     // modes_set_levels: one record per buffer of the batch (device, and its pinned host copy)
     DevBuf<modes_level> d_levels;
     PinnedBuf<modes_level> h_levels;
+    // modes_set_spectrum: one record per buffer of the batch (device, pinned host copy), and the input span
+    // the batch was made from (spec_shift < 0: UC8, else int16 with that shift)
+    DevBuf<modes_spectrum> d_spectra;
+    PinnedBuf<modes_spectrum> h_spectra;
+    ResampleJob spec_in{};
+    int spec_shift = -1;
     // modes_set_recovery / modes_recover_device: one record per candidate (device, and its pinned host copy)
     DevBuf<modes_recovered> d_recovered;
     PinnedBuf<modes_recovered> h_recovered;
@@ -193,6 +199,7 @@ struct modes_ctx {
     // soft-decision recovery of weak DF17/18 frames; weak: recovery at weak preambles too
     Features feat;
     LevelQueue level_q;
+    SpectrumQueue spectrum_q;
     int64_t eof_buffer = -1;              // modes_finish: stream index of the EOF buffer and its real samples
     uint32_t eof_samples = 0;
     // modes_levels_device: the records of the last call (device, pinned host copy)
@@ -313,6 +320,12 @@ void append_levels(modes_ctx *ctx, const Slot &s) {
     }
 }
 
+// Queue the spectrum records of the slot's finished batch (the kernel wrote their stream buffer indices).
+void append_spectra(modes_ctx *ctx, const Slot &s) {
+    if (!s.feat.spectrum) return;
+    for (size_t k = 0; k < s.n_buffers; k++) ctx->spectrum_q.push(s.h_spectra[k]);
+}
+
 // The device resolve's view of the slot's workspace, grown for its current batch.
 int gpu_resolve_ensure(modes_ctx *ctx, Slot &s, GpuResolve &g) {
     const size_t nb = s.n_buffers;
@@ -343,6 +356,7 @@ int submit(modes_ctx *ctx, Slot &s, const uint8_t *host_iq, const void *d_iq, si
     if (slot_ensure(ctx, s, n_samples, host_iq != nullptr, d_records_ext == nullptr)) return -1;
     s.feat = ctx->feat;
     s.feat.levels &= &s != &ctx->detect;
+    s.feat.spectrum &= &s != &ctx->detect;
     s.feat.recover &= &s != &ctx->detect;                 // the stage level asks with modes_recover_device
     s.rec_ext = nullptr; s.rec_ext_cap = 0;
     s.feat.weak &= s.feat.recover;                        // the stage level asks with modes_weak_device
@@ -351,6 +365,10 @@ int submit(modes_ctx *ctx, Slot &s, const uint8_t *host_iq, const void *d_iq, si
     if (s.feat.levels) {                                  // the slot's previous batch is collected: no copy is queued
         CK(ctx, s.d_levels.ensure(n_buffers));
         CK(ctx, s.h_levels.ensure(n_buffers));
+    }
+    if (s.feat.spectrum) {
+        CK(ctx, s.d_spectra.ensure(n_buffers));
+        CK(ctx, s.h_spectra.ensure(n_buffers));
     }
     if (host_iq) {
         CK(ctx, cudaMemcpyAsync(s.d_iq.get(), host_iq, n_samples * 2, cudaMemcpyHostToDevice, s.stream));
@@ -454,8 +472,14 @@ int launch_batch(modes_ctx *ctx, Slot &s) {
     // batch writes the same records
     if (f.levels)
         launch_levels(in.body, (uint32_t)s.n_buffers, MODES_BUFFER_BYTES, ctx->tab, s.d_levels.get(), ctx->sm_count, s.stream);
+    // the input the buffers stand for, where the batch was made from; the records start from zero
+    if (f.spectrum) {
+        CK(ctx, cudaMemsetAsync(s.d_spectra.get(), 0, s.n_buffers * sizeof(modes_spectrum), s.stream));
+        launch_spectrum(s.spec_in, s.spec_shift, ctx->rate->out, ctx->rate->in, s.buffer_base, (uint32_t)s.n_buffers,
+                        s.d_spectra.get(), s.stream);
+    }
     CK(ctx, cudaGetLastError());
-    ctx->launches += (f.signal || f.arrival ? 3 : 2) + (f.levels ? 1 : 0);
+    ctx->launches += (f.signal || f.arrival ? 3 : 2) + (f.levels ? 1 : 0) + (f.spectrum ? 1 : 0);
     if (f.recover && launch_recovery(ctx, s, in, so)) return -1;
     if (f.weak && launch_weak(ctx, s, in)) return -1;
     if (ctx->cfg.gpu_resolve && s.own_outputs && &s != &ctx->detect) {
@@ -479,6 +503,9 @@ int launch_batch(modes_ctx *ctx, Slot &s) {
     }
     if (f.levels)
         CK(ctx, cudaMemcpyAsync(s.h_levels.get(), s.d_levels.get(), s.n_buffers * sizeof(modes_level), cudaMemcpyDeviceToHost, s.stream));
+    if (f.spectrum)
+        CK(ctx, cudaMemcpyAsync(s.h_spectra.get(), s.d_spectra.get(), s.n_buffers * sizeof(modes_spectrum), cudaMemcpyDeviceToHost,
+                                s.stream));
     CK(ctx, cudaEventRecord(s.done, s.stream));
     s.busy = true;
     return 0;
@@ -561,6 +588,7 @@ int collect(modes_ctx *ctx, Slot &s) {
     if (wait_batch(ctx, s, &n)) return -1;
     s.busy = false;                                     // a repeated (overflowed) batch re-arms the flag
     append_levels(ctx, s);                              // copied with the counters: on the host since s.done
+    append_spectra(ctx, s);
     const double t1 = dbg ? now_ms() : 0;
     if (ctx->cfg.gpu_resolve) {
         // the verdicts were taken on the device: fetch the deliveries, build the structs
@@ -612,6 +640,7 @@ int collect_group(modes_ctx *ctx, int parity) {
         if (wait_batch(g, s, &nc)) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
         s.busy = false;
         append_levels(ctx, s);                          // groups and GPUs in stream order
+        append_spectra(ctx, s);
         ShardView v;
         if (fetch_async(g, s, nc, v)) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
         cands[k] = v.cands; tiles[k] = v.tiles; n_tiles[k] = v.n_tiles; base[k] = v.buffer_base;
@@ -682,6 +711,8 @@ int stage_held(modes_ctx *ctx, Slot &s, const Source &src, size_t nb) {
     const ResampleJob j{s.d_in.get(), (uint64_t)(hi - lo), lo / bps, o0, (uint64_t)(o1 - o0), src.out_end,
                         s.d_iq.get(), s.d_halo.get()};
     const int shift = ctx->input_format == input::kUC8 ? -1 : ctx->input_shift;
+    s.spec_in = j;
+    s.spec_shift = shift;
     if (ctx->rate->m) launch_decimate(j, ctx->rate->m, shift, shift::step(ctx->input_offset, ctx->rate->hz), s.stream);
     else if (ctx->input_format == input::kUC8) launch_resample(j, s.stream);
     else if (ctx->rate->hz == 2400000) launch_resample_sc16(j, ctx->input_shift, s.stream);
@@ -698,6 +729,13 @@ int submit_next(modes_ctx *ctx, modes_ctx *g, Slot &s, Source &src, size_t nb) {
         if (stage_held(g, s, src, nb)) return -1;
         return submit(g, s, nullptr, s.d_iq.get(), nb, nullptr, nullptr, 0, nullptr, true);
     }
+    // the batch bytes, uploaded to d_iq, are the input: the span of its own buffers
+    CK(g, s.d_iq.ensure((size_t)nb * MODES_BUFFER_BYTES));
+    s.spec_in = ResampleJob{};
+    s.spec_in.in = s.d_iq.get();
+    s.spec_in.in_bytes = (uint64_t)nb * MODES_BUFFER_BYTES;
+    s.spec_in.in_first = s.buffer_base * (int64_t)kBufSamples;
+    s.spec_shift = -1;
     if (submit(g, s, src.iq, nullptr, nb, ctx->carry, nullptr, 0, nullptr)) return -1;
     memcpy(ctx->carry, src.iq + nb * MODES_BUFFER_BYTES - MODES_CARRY_BYTES, MODES_CARRY_BYTES);
     src.iq += nb * MODES_BUFFER_BYTES;
@@ -950,6 +988,10 @@ int modes_set_levels(modes_ctx *ctx, int on) { return set_feature(ctx, &Features
 
 size_t modes_take_levels(modes_ctx *ctx, modes_level *out, size_t cap) { return ctx ? ctx->level_q.take(out, cap) : 0; }
 
+int modes_set_spectrum(modes_ctx *ctx, int on) { return set_feature(ctx, &Features::spectrum, on); }
+
+size_t modes_take_spectra(modes_ctx *ctx, modes_spectrum *out, size_t cap) { return ctx ? ctx->spectrum_q.take(out, cap) : 0; }
+
 int modes_levels_device(modes_ctx *ctx, const void *d_iq, size_t n_buffers, size_t stride_bytes) {
     if (!ctx) return -1;
     if (!d_iq || !n_buffers) return fail(ctx, "modes_levels_device: empty input");
@@ -1123,6 +1165,7 @@ int modes_reset(modes_ctx *ctx) {
     ctx->in_total = 0;
     ctx->hold0 = 0;
     ctx->level_q.clear();
+    ctx->spectrum_q.clear();
     ctx->eof_buffer = -1;
     memset(ctx->carry, 127, sizeof(ctx->carry));
     return 0;

@@ -155,6 +155,29 @@ struct PoolConvertJob {
     int32_t        shift;
 };
 void launch_convert_pool(const PoolConvertJob *d_jobs, uint32_t n_jobs, cudaStream_t stream);
+// The input spectrum pass (modes_spectrum.cu, K13; arithmetic in modes_spectrum_core.cuh): out[k] = the record of
+// reference buffer first_buffer + k, k < n_buffers, of a stream at the ratio out : in (InputRate) whose input
+// span the job holds (in, in_bytes, in_first: as launch_decimate reads them, UC8 with shift < 0, else int16
+// converted with the shift).  The records must be zero: each block adds its frames' power into its buffer's.
+void launch_spectrum(const ResampleJob &j, int shift, int out, int in, int64_t first_buffer, uint32_t n_buffers,
+                     modes_spectrum *records, cudaStream_t stream);
+// The receiver pool's form: one job per pair of a batch, record k from job k.  A job's input is read as a
+// PoolResampleJob's ([hist0, call0) at hist, [call0, call0 + MODES_BUFFER_BYTES) at stage, UC8 stream bytes):
+// its buffer's frames of `frames` start at stream sample `first`.  A 2 MHz receiver's job has hist0 = call0 =
+// 2 first and stage = its pair's data buffer.  max_frames: the most frames of a job.
+struct PoolSpectrumJob {
+    const uint8_t *hist;
+    const uint8_t *stage;
+    int64_t        hist0, call0;
+    int64_t        buffer;       // the receiver's own buffer index
+    int64_t        first;
+    uint32_t       frames;
+    uint32_t       pad;
+};
+void launch_spectrum_pool(const PoolSpectrumJob *d_jobs, uint32_t n_jobs, uint32_t max_frames, modes_spectrum *records,
+                          cudaStream_t stream);
+static_assert(sizeof(modes_spectrum) == 16 + 8 * MODES_SPECTRUM_BINS && offsetof(modes_spectrum, power) == 16,
+              "spectrum record layout");
 // Recovery records (modes_recover.cu): writes out[k] for k < min(counters[0], capacity) from the
 // candidate records and the windows the scan and frame evaluation read.
 void launch_recover(const BatchView &in, const DeviceTables &tab, const ScanOutputs &scan, const modes_candidate *records,
@@ -280,19 +303,20 @@ void add_recovery_stats(modes_recovery_stats &to, const modes_recovery_stats &fr
 
 // ---- host glue shared by the context (modes_api.cpp) and the receiver pool (modes_pool.cpp) ----
 // The optional measurements and searches of a decode (modes_set_* / modes_pool_set_*).
-struct Features { bool signal = false, arrival = false, levels = false, recover = false, weak = false; };
+struct Features { bool signal = false, arrival = false, levels = false, recover = false, weak = false, spectrum = false; };
 
-// Level records not taken yet, oldest first.
-class LevelQueue {
+// Level or spectrum records not taken yet, oldest first.
+template <typename T>
+class RecordQueue {
 public:
-    void push(const modes_level &r) { q_.push_back(r); }
+    void push(const T &r) { q_.push_back(r); }
     void clear() { q_.clear(); head_ = 0; }
     // Moves up to cap of the oldest records to out; out == nullptr: how many are queued.
-    size_t take(modes_level *out, size_t cap) {
+    size_t take(T *out, size_t cap) {
         const size_t queued = q_.size() - head_;
         if (!out) return queued;
         const size_t n = cap < queued ? cap : queued;
-        if (n) memcpy(out, q_.data() + head_, n * sizeof(modes_level));
+        if (n) memcpy(out, q_.data() + head_, n * sizeof(T));
         head_ += n;
         if (head_ == q_.size()) clear();
         else if (head_ >= 4096 && 2 * head_ >= q_.size()) {   // compact when the taken records are half the queue
@@ -302,8 +326,10 @@ public:
         return n;
     }
 private:
-    std::vector<modes_level> q_;
+    std::vector<T> q_;
     size_t head_ = 0;
 };
+using LevelQueue = RecordQueue<modes_level>;
+using SpectrumQueue = RecordQueue<modes_spectrum>;
 
 }  // namespace modes

@@ -53,6 +53,7 @@
 #include "modes_internal.h"
 #include "modes_input_core.cuh"
 #include "modes_resample_core.cuh"
+#include "modes_spectrum_core.cuh"
 
 namespace {
 
@@ -71,6 +72,7 @@ struct Receiver {
     int64_t submitted = 0;                     // buffers of this receiver submitted so far (2 MHz buffers)
     uint8_t carry[MODES_CARRY_BYTES];
     modes::LevelQueue levels;
+    modes::SpectrumQueue spectra;
     uint32_t rate = kRate2M;                   // modes_pool_set_input_rate
     uint32_t format = modes::input::kUC8;      // modes_pool_set_input_format, the shift resolved
     int shift = 0;
@@ -181,6 +183,10 @@ struct modes_pool {
         uint8_t *d_stage16 = nullptr;
         void *h_cjobs = nullptr, *d_cjobs = nullptr;
         std::vector<const uint8_t *> iq8, iq16;   // the call's UC8 and 16-bit buffers, each group in call order
+        // with spectra: one job and one record per pair (pinned and device), made the first time the switch is on
+        modes::PoolSpectrumJob *h_sjobs = nullptr;
+        void *d_sjobs = nullptr;
+        modes_spectrum *h_spectra = nullptr, *d_spectra = nullptr;
     } slot[2];
     unsigned submitted = 0, collected = 0;     // batches so far: slot = number & 1
     std::vector<modes_candidate> cands;
@@ -321,6 +327,46 @@ int upload_buffers(modes_pool *p, cudaStream_t st, const uint8_t *const *iq, siz
     return 0;
 }
 
+// The device half of the spectrum pass, made the first time a batch measures spectra.
+int ensure_spectrum_device(modes_pool *p) {
+    for (modes_pool::Slot &sl : p->slot) {
+        if (sl.h_sjobs) continue;
+        sl.h_sjobs = static_cast<modes::PoolSpectrumJob *>(modes_host_alloc(p->max_batch * sizeof(modes::PoolSpectrumJob)));
+        sl.d_sjobs = modes_device_alloc(p->max_batch * sizeof(modes::PoolSpectrumJob));
+        sl.h_spectra = static_cast<modes_spectrum *>(modes_host_alloc(p->max_batch * sizeof(modes_spectrum)));
+        sl.d_spectra = static_cast<modes_spectrum *>(modes_device_alloc(p->max_batch * sizeof(modes_spectrum)));
+        if (!sl.h_sjobs || !sl.d_sjobs || !sl.h_spectra || !sl.d_spectra)
+            return fail(p, "out of memory for %zu receivers per batch", p->max_batch);
+    }
+    return 0;
+}
+
+// A pair's spectrum job: receiver buffer `buffer` of a stream at 2 MHz (its bytes, data, in the pair) or 2.4 MS/s
+// (read from the history and the call's staging area as the resampling job reads it).
+modes::PoolSpectrumJob spectrum_job(const Receiver &r, int64_t buffer, const uint8_t *data, const uint8_t *stage) {
+    namespace SP = modes::spectrum;
+    if (r.rate == kRate2M)
+        return modes::PoolSpectrumJob{nullptr, data, 2 * buffer * kBufSamples, 2 * buffer * kBufSamples, buffer,
+                                      buffer * kBufSamples, SP::frames(1, 1, buffer), 0};
+    return modes::PoolSpectrumJob{r.hist[r.cur], stage, r.hist0, r.in_total, buffer, SP::first_sample(5, 6, buffer),
+                                  SP::frames(5, 6, buffer), 0};
+}
+
+// The spectrum launch over the slot's n pairs (their jobs at sl.h_sjobs), the records zeroed first and copied
+// back behind it, all on the slot's stream.
+int launch_pool_spectra(modes_pool *p, modes_pool::Slot &sl, cudaStream_t st, size_t n) {
+    uint32_t most = 0;
+    for (size_t i = 0; i < n; i++) most = sl.h_sjobs[i].frames > most ? sl.h_sjobs[i].frames : most;
+    if (cudaMemcpyAsync(sl.d_sjobs, sl.h_sjobs, n * sizeof(modes::PoolSpectrumJob), cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemsetAsync(sl.d_spectra, 0, n * sizeof(modes_spectrum), st) != cudaSuccess)
+        return fail(p, "spectrum job upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+    modes::launch_spectrum_pool(static_cast<const modes::PoolSpectrumJob *>(sl.d_sjobs), (uint32_t)n, most, sl.d_spectra, st);
+    if (cudaGetLastError() != cudaSuccess ||
+        cudaMemcpyAsync(sl.h_spectra, sl.d_spectra, n * sizeof(modes_spectrum), cudaMemcpyDeviceToHost, st) != cudaSuccess)
+        return fail(p, "spectrum launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+    return 0;
+}
+
 // The scan and the passes of the switches over the slot's n pairs, already in place.
 int detect_pairs(modes_pool *p, modes_pool::Slot &sl, size_t n) {
     if (modes_detect_device(sl.ctx, sl.d_batch, 2 * n, nullptr, nullptr, 0, nullptr)) return fail(p, "%s", modes_last_error(sl.ctx));
@@ -355,6 +401,8 @@ int submit_rated(modes_pool *p, modes_pool::Slot &sl, const uint32_t *receivers,
     size_t n_stage = iq8.size();
     sl.ids.clear();
     sl.buf_index.clear();
+    const bool spectra = p->feat.spectrum;
+    if (spectra && ensure_spectrum_device(p)) return -1;
     for (size_t i = 0, k8 = 0; i < n; i++) {
         const Receiver &r = p->rx[receivers[i]];
         const bool uc8 = r.format == modes::input::kUC8;
@@ -364,6 +412,7 @@ int submit_rated(modes_pool *p, modes_pool::Slot &sl, const uint32_t *receivers,
             memcpy(sl.h_carry + n_pairs * MODES_CARRY_BYTES, r.carry, MODES_CARRY_BYTES);
             if (uc8) rj[n_rj++] = modes::PoolResampleJob{nullptr, sl.d_stage + k8++ * kBuf, 0, 0, -1, nullptr, pad + kBuf};
             else cj[n_conv++] = modes::PoolConvertJob{in16, pad + kBuf, r.shift};
+            if (spectra) sl.h_sjobs[n_pairs] = spectrum_job(r, r.submitted, pad + kBuf, nullptr);
             n_pairs++;
             sl.ids.push_back(receivers[i]);
             sl.buf_index.push_back(r.submitted);
@@ -376,6 +425,7 @@ int submit_rated(modes_pool *p, modes_pool::Slot &sl, const uint32_t *receivers,
         if (pl.completes) {
             rj[n_rj++] = modes::PoolResampleJob{r.hist[r.cur], stage, r.hist0, r.in_total, r.submitted * kBufSamples,
                                                 pad + kBuf - MODES_CARRY_BYTES, pad + kBuf};
+            if (spectra) sl.h_sjobs[n_pairs] = spectrum_job(r, r.submitted, nullptr, stage);
             n_pairs++;
             sl.ids.push_back(receivers[i]);
             sl.buf_index.push_back(r.submitted);
@@ -406,6 +456,9 @@ int submit_rated(modes_pool *p, modes_pool::Slot &sl, const uint32_t *receivers,
     const modes::PoolResampleJob *d_rj = static_cast<const modes::PoolResampleJob *>(sl.d_jobs);
     modes::launch_resample_pool(d_rj, (uint32_t)n_rj, st);
     modes::launch_history_pool(reinterpret_cast<const modes::PoolHistoryJob *>(d_rj + p->max_batch), (uint32_t)n_hist, hist_max, st);
+    // the spectra read the histories too: before rate_done, after which the other slot's history step may
+    // overwrite them
+    if (spectra && n_pairs && launch_pool_spectra(p, sl, st, n_pairs)) return -1;
     if (cudaGetLastError() != cudaSuccess || cudaEventRecord(sl.rate_done, st) != cudaSuccess)
         return fail(p, "resampling launch failed: %s", cudaGetErrorString(cudaGetLastError()));
     sl.rate_recorded = true;
@@ -460,6 +513,10 @@ void modes_pool_destroy(modes_pool *p) {
         if (sl.d_stage16) modes_device_free(sl.d_stage16);
         if (sl.d_cjobs) modes_device_free(sl.d_cjobs);
         if (sl.h_cjobs) modes_host_free(sl.h_cjobs);
+        if (sl.h_sjobs) modes_host_free(sl.h_sjobs);
+        if (sl.d_sjobs) modes_device_free(sl.d_sjobs);
+        if (sl.h_spectra) modes_host_free(sl.h_spectra);
+        if (sl.d_spectra) modes_device_free(sl.d_spectra);
         if (sl.ctx) modes_destroy(sl.ctx);
     }
     delete p;
@@ -626,6 +683,15 @@ int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *c
         return fail(p, "carry upload failed: %s", cudaGetErrorString(cudaGetLastError()));
     if (upload_buffers(p, st, iq, n, sl.d_batch + kBuf, 2 * kBuf, kBuf)) return -1;
     if (detect_pairs(p, sl, n)) return -1;
+    // the pairs' data buffers, on the same stream after the scan
+    if (sl.feat.spectrum) {
+        if (ensure_spectrum_device(p)) return -1;
+        for (size_t i = 0; i < n; i++) {
+            const Receiver &r = p->rx[receivers[i]];
+            sl.h_sjobs[i] = spectrum_job(r, r.submitted, sl.d_batch + (2 * i + 1) * kBuf, nullptr);
+        }
+        if (launch_pool_spectra(p, sl, st, n)) return -1;
+    }
     sl.buf_index.resize(n);
     for (size_t i = 0; i < n; i++) sl.buf_index[i] = p->rx[receivers[i]].submitted++;
     // what each receiver carries into its next buffer (dump1090.c:481)
@@ -676,6 +742,11 @@ int modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user) {
             p->rx[sl.ids[i]].levels.push(r);
         }
     }
+    if (sl.feat.spectrum) {
+        if (cudaStreamSynchronize(static_cast<cudaStream_t>(modes_stream(sl.ctx))) != cudaSuccess)
+            return fail(p, "%s", cudaGetErrorString(cudaGetLastError()));
+        for (size_t i = 0; i < n; i++) p->rx[sl.ids[i]].spectra.push(sl.h_spectra[i]);
+    }
     sl.busy = false;
     p->collected++;
     return pool_resolve(p, sl.ids.data(), n, p->cands.data(), sl.feat.recover ? p->recovered.data() : nullptr, sl.feat.signal,
@@ -704,6 +775,7 @@ int modes_pool_reset(modes_pool *p, uint32_t receiver) {
     r.in_total = 0;
     r.hist0 = 0;
     r.levels.clear();
+    r.spectra.clear();
     memset(r.carry, 127, sizeof r.carry);
     return modes_resolver_reset(r.res);
 }
@@ -771,6 +843,13 @@ int modes_pool_set_levels(modes_pool *p, int on) { return set_feature(p, &modes:
 size_t modes_pool_take_levels(modes_pool *p, uint32_t receiver, modes_level *out, size_t cap) {
     if (!p || receiver >= p->rx.size()) return 0;
     return p->rx[receiver].levels.take(out, cap);
+}
+
+int modes_pool_set_spectrum(modes_pool *p, int on) { return set_feature(p, &modes::Features::spectrum, on); }
+
+size_t modes_pool_take_spectra(modes_pool *p, uint32_t receiver, modes_spectrum *out, size_t cap) {
+    if (!p || receiver >= p->rx.size()) return 0;
+    return p->rx[receiver].spectra.take(out, cap);
 }
 
 int64_t modes_pool_buffers(const modes_pool *p, uint32_t receiver) {

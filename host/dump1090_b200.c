@@ -41,6 +41,12 @@
  * (+2000000: tuned to 1088 MHz, as zero-IF radios are to keep their DC spike away from it): the input is
  * shifted back by that much on the GPU as it is decimated (modes_set_input_offset).  It needs
  * --sample-rate 4000000 to 10000000, and |hz| at most half the rate less 1 MHz (1, 2, 3 or 4 MHz).
+ * --spectrum measures every decoded buffer's input power spectrum on the GPU (modes_set_spectrum), before
+ * resampling, decimation and the offset, and prints one summary line on stderr at the end, as --levels
+ * does: the noise floor, the DC bin's excess over bins 126 and 130 (a zero-IF radio's spike) and the centre of
+ * the 2 MHz band with the most power above the floor (where the channel most likely sits: the value for
+ * --input-offset).  It combines with every --sample-rate, --iformat and --input-offset and leaves stdout
+ * as it is.
  * The live-radio, networking and interactive options are out of scope.
  */
 #include <math.h>
@@ -51,7 +57,7 @@
 #include "modes_b200.h"
 
 static int opt_raw = 0, opt_onlyaddr = 0, opt_stats = 0, opt_check_crc = 1, opt_sbs = 0, opt_json = 0, opt_beast = 0;
-static int opt_levels = 0, opt_recover = 0, opt_weak = 0, opt_arrival = 0;
+static int opt_levels = 0, opt_recover = 0, opt_weak = 0, opt_arrival = 0, opt_spectrum = 0;
 static modes_tracker *tracker = NULL;
 
 /* --levels: totals over the records taken so far */
@@ -78,6 +84,51 @@ static void print_levels(void) {
     const double peak = lv.peak ? 20.0 * log10(lv.peak / 65535.0) : -INFINITY;
     fprintf(stderr, "noise %.2f dBFS, peak %.2f dBFS, clipped %llu (%.6f)\n", noise, peak, lv.clipped,
             (double)lv.clipped / (double)lv.samples);
+}
+
+/* --spectrum: per-bin totals over the records taken so far (spectrum_summary in dump1090_b200/api.py is the
+ * same computation; the floor and the band search are exact on the integer sums) */
+static struct { long long buffers; unsigned long long frames; unsigned __int128 power[MODES_SPECTRUM_BINS]; } sp;
+
+static void take_spectra(modes_ctx *ctx) {
+    static modes_spectrum r[64];
+    size_t n;
+    while ((n = modes_take_spectra(ctx, r, 64)) > 0)
+        for (size_t i = 0; i < n; i++) {
+            sp.buffers++;
+            sp.frames += r[i].frames;
+            for (int k = 0; k < MODES_SPECTRUM_BINS; k++) sp.power[k] += r[i].power[k];
+        }
+}
+
+static int cmp_u128(const void *a, const void *b) {
+    const unsigned __int128 x = *(const unsigned __int128 *)a, y = *(const unsigned __int128 *)b;
+    return x < y ? -1 : x > y;
+}
+
+static void print_spectrum(unsigned long fs) {
+    enum { N = MODES_SPECTRUM_BINS };
+    fprintf(stderr, "spectrum: %lld buffers, %llu frames, ", sp.buffers, sp.frames);
+    if (!sp.frames) { fprintf(stderr, "floor n/a\n"); return; }
+    const unsigned __int128 dc = 2 * sp.power[N / 2], nb = sp.power[N / 2 - 2] + sp.power[N / 2 + 2];
+    const double dc_db = dc == nb ? 0.0 : !nb ? INFINITY : !dc ? -INFINITY : 10.0 * log10((double)dc / (double)nb);
+    unsigned __int128 t2[N], srt[N];
+    for (int i = 0; i < N; i++) t2[i] = 2 * sp.power[i];
+    t2[N / 2 - 1] = t2[N / 2] = t2[N / 2 + 1] = nb;          /* DC and the window's main lobe around it */
+    memcpy(srt, t2, sizeof(srt));
+    qsort(srt, N, sizeof(srt[0]), cmp_u128);
+    const unsigned __int128 floor4 = srt[N / 2 - 1] + srt[N / 2];
+    const double floor_db = floor4 ? 10.0 * log10((double)floor4 / 4.0 / (double)sp.frames) : -INFINITY;
+    const int w = (int)((unsigned long long)N * 2000000ull / fs);
+    unsigned __int128 best = 0;
+    int at = -1;
+    for (int i0 = 0; i0 + w <= N; i0++) {
+        unsigned __int128 score = 0;
+        for (int i = i0; i < i0 + w; i++) score += 2 * t2[i] > floor4 ? 2 * t2[i] - floor4 : 0;
+        if (at < 0 || score > best) { best = score; at = i0; }
+    }
+    fprintf(stderr, "floor %.2f dB, DC %+.2f dB over its neighbours, strongest 2 MHz band at %+.0f Hz\n", floor_db, dc_db,
+            (at + (w - 1) / 2.0 - N / 2) * (double)fs / N);
 }
 
 /* Message sink: the --raw / --onlyaddr forms of displayModesMessage
@@ -140,6 +191,7 @@ int main(int argc, char **argv) {
         else if (!strcmp(argv[j], "--beast")) opt_beast = 1;
         else if (!strcmp(argv[j], "--arrival")) opt_arrival = 1;
         else if (!strcmp(argv[j], "--levels")) opt_levels = 1;
+        else if (!strcmp(argv[j], "--spectrum")) opt_spectrum = 1;
         else if (!strcmp(argv[j], "--recover")) opt_recover = 1;
         else if (!strcmp(argv[j], "--recover-weak")) opt_recover = opt_weak = 1;
         else if (!strcmp(argv[j], "--gpu-resolve")) cfg.gpu_resolve = 1;
@@ -225,6 +277,7 @@ int main(int argc, char **argv) {
     if (opt_beast) modes_set_signal(ctx, 1);
     if (opt_arrival) modes_set_arrival(ctx, 1);
     if (opt_levels) modes_set_levels(ctx, 1);
+    if (opt_spectrum) modes_set_spectrum(ctx, 1);
     if (opt_recover && modes_set_recovery(ctx, 1)) { fprintf(stderr, "--recover: %s\n", modes_last_error(ctx)); return 1; }
     if (opt_weak && modes_set_weak_preambles(ctx, 1)) { fprintf(stderr, "--recover-weak: %s\n", modes_last_error(ctx)); return 1; }
     modes_set_sink(ctx, on_message, NULL);
@@ -234,9 +287,11 @@ int main(int argc, char **argv) {
     while ((n = fread(buf, 1, chunk, f)) > 0) {
         if (modes_process(ctx, buf, n)) { fprintf(stderr, "modes_process: %s\n", modes_last_error(ctx)); return 1; }
         if (opt_levels) take_levels(ctx);
+        if (opt_spectrum) take_spectra(ctx);
     }
     if (modes_finish(ctx)) { fprintf(stderr, "modes_finish: %s\n", modes_last_error(ctx)); return 1; }
     if (opt_levels) { take_levels(ctx); print_levels(); }
+    if (opt_spectrum) { take_spectra(ctx); print_spectrum(sample_rate); }
     if (opt_stats) {                                        /* dump1090.c:2993-3006 */
         modes_stats st;
         modes_get_stats(ctx, &st);

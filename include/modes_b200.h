@@ -323,7 +323,7 @@ int  modes_resample_device(modes_ctx *ctx, const void *d_in, size_t in_bytes, in
 /* modes_resample_device at any rate modes_set_input_rate takes other than 2000000 (the call above is this
  * one at 2400000), UC8 input as there, the same arguments and the same behaviour.  At 2000000 M the span
  * must hold the input samples [M n0 - E, M n1 + E) that exist, with n0 = MODES_BUFFER_SAMPLES *
- * first_buffer - 240 and n1 as above (E: 2 for M = 2, 3 and 4; 3 for M = 5).  Any other rate is refused
+ * first_buffer - 240 and n1 as above (E: 2 for M = 2, 4 and 5; 1 for M = 3).  Any other rate is refused
  * with "not supported". */
 int  modes_resample_device_at(modes_ctx *ctx, uint32_t hz, const void *d_in, size_t in_bytes, int64_t in_first_sample,
                               int64_t first_buffer, size_t n_buffers, int64_t out_end, void *d_out, uint8_t *carry476);
@@ -628,6 +628,46 @@ int    modes_levels_fetch(modes_ctx *ctx, modes_level *out);
  * order; modes_pool_reset clears the receiver's queue.  Same take convention as above. */
 int    modes_pool_set_levels(modes_pool *p, int on);
 size_t modes_pool_take_levels(modes_pool *p, uint32_t receiver, modes_level *out, size_t cap);
+
+/* ---- input spectrum: where in frequency each buffer's input energy is --------------------------
+ * The frequency-domain sibling of the levels above: where 1090 MHz sits in a capture (the offset to pass
+ * modes_set_input_offset), where a zero-IF radio's DC spike is, whether an interferer or an image sits on
+ * the channel, whether a 16-bit shift throws away the weak end.  One record per reference buffer decoded,
+ * measured on the input it stands for, before resampling, decimation and the input offset; it changes no
+ * message.  Exactly, in integers (modes_spectrum_core.cuh has the arithmetic):
+ *   span     buffer b (2 MHz samples [b B, (b + 1) B), B = MODES_BUFFER_SAMPLES) stands for the input samples
+ *            [s_b, s_{b+1}), s_b = floor(in b B / out) at the rate's ratio out : in (1:1 at 2000000, 5:6 at
+ *            2400000, 1:M at 2000000 M); its F = floor((s_{b+1} - s_b) / 256) whole frames of 256 input
+ *            samples start at s_b (F = 512, 614 and 512 M); the remainder is not measured
+ *   sample   xi = I - 127, xq = Q - 127 of the UC8 bytes, a 16-bit stream's converted bytes (so a shift that
+ *            clips or loses the weak end shows); samples past the stream's end are 0; no input offset
+ *   window   v = (x w[n] + 8192) >> 14 (int32, arithmetic shift), w[n] = (16384 - C[4 n]) >> 1, a Q14 Hann
+ *   FFT      radix-2 decimation in time over the bit-reversed frame, int32, no scaling; the butterfly of
+ *            stage s = 0..7 (half = 2^s) on a = X[i], b = X[i + half] with k = (i mod half) 2^(7-s),
+ *            c = C[4 k], s = S[4 k]:  t_re = (b_re c + b_im s + 8192) >> 14, t_im = (b_im c - b_re s + 8192) >> 14,
+ *            X[i] = a + t, X[i + half] = a - t  (C, S: the 1024-phase tables of modes_set_input_offset)
+ *   power    X_re^2 + X_im^2 as uint32 (|X| < 46400, so it fits), summed over the F frames in uint64
+ *   record   power[i] = the sum of FFT bin (i + 128) mod 256: natural frequency order, bin i at
+ *            (i - 128) fs / 256 Hz, bin 128 at DC
+ * Off by default.  When it is on, every batch the streaming decode submits afterwards runs one more kernel
+ * (one more launch per batch), on the same stream after the scan, over the input bytes already in HBM; the
+ * records are queued as level records are: in stream order, one per buffer decoded (the EOF buffer's too,
+ * unless drop_eof_buffer drops it), merged in stream order on an n_gpus > 1 context, dropped by modes_reset.
+ * Same take convention as modes_take_levels.  Returns 0 / -1 (NULL handle). */
+#define MODES_SPECTRUM_BINS 256
+typedef struct modes_spectrum {
+    int64_t  buffer;            /* stream index of the buffer (in a pool: the receiver's own buffer index) */
+    uint32_t frames;            /* F */
+    uint32_t pad;
+    uint64_t power[MODES_SPECTRUM_BINS];
+} modes_spectrum;
+int    modes_set_spectrum(modes_ctx *ctx, int on);
+size_t modes_take_spectra(modes_ctx *ctx, modes_spectrum *out, size_t cap);
+/* The pool measures every buffer a receiver decodes while the switch is on, on the receiver's own input
+ * (a 16-bit receiver's converted bytes), and queues its records under its own buffer index; its records
+ * equal the single-stream decoder's for the receiver's stream.  modes_pool_reset clears the receiver's queue. */
+int    modes_pool_set_spectrum(modes_pool *p, int on);
+size_t modes_pool_take_spectra(modes_pool *p, uint32_t receiver, modes_spectrum *out, size_t cap);
 
 /* ---- soft-decision recovery of weak DF17/DF18 frames of known aircraft -------------------------
  * Many weak frames pass the preamble test and fail the CRC because a few bits whose two half-bit
