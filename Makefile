@@ -83,7 +83,7 @@ tests/_build/libeval_serial_host.so: tests/host_shim/eval_serial_host.cpp $(CSRC
 # test infrastructure: device harness over the product's own kernel objects (recovery and signal
 # passes on constructed corpora, and the exhaustive sweeps of the core headers' device build)
 DSHIM_OBJS := build/modes_recover.o build/modes_signal.o build/modes_levels.o build/modes_tables.o
-dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so tests/_build/libscan_eval_device.so tests/_build/libresample_pool_device.so tests/_build/libresolve_device.so tests/_build/libinput_device.so tests/_build/libconvert_pool_device.so
+dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so tests/_build/libscan_eval_device.so tests/_build/libresample_pool_device.so tests/_build/libresolve_device.so tests/_build/libinput_device.so tests/_build/libconvert_pool_device.so tests/_build/librate_spectrum_device.so
 tests/_build/libkernels_device.so: tests/device_shim/kernels_device.cu $(DSHIM_OBJS) $(CSRC)/modes_internal.h $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_levels_core.cuh include/modes_b200.h
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/kernels_device.cu -o tests/_build/kernels_device.o
@@ -114,6 +114,12 @@ tests/_build/libinput_device.so: tests/device_shim/input_device.cu build/modes_r
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/input_device.cu -o tests/_build/input_device.o
 	$(NVCC) $(ARCH) -shared -o $@ tests/_build/input_device.o build/modes_resample.o -cudart static
+# the decimator, its frequency shift and the spectrum pass on chosen spans and pool jobs (tests/test_rate_kernels.py)
+RATE_SPECTRUM_OBJS := build/modes_resample.o build/modes_spectrum.o
+tests/_build/librate_spectrum_device.so: tests/device_shim/rate_spectrum_device.cu $(RATE_SPECTRUM_OBJS) $(CSRC)/modes_internal.h $(CSRC)/modes_resample_core.cuh $(CSRC)/modes_spectrum_core.cuh include/modes_b200.h
+	@mkdir -p tests/_build
+	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/rate_spectrum_device.cu -o tests/_build/rate_spectrum_device.o
+	$(NVCC) $(ARCH) -shared -o $@ tests/_build/rate_spectrum_device.o $(RATE_SPECTRUM_OBJS) -cudart static
 # the device resolve with a chosen SM count, batch size and delivery capacity (tests/test_resolve_device.py)
 tests/_build/libresolve_device.so: tests/device_shim/resolve_device.cu build/modes_resolve_gpu.o $(CSRC)/modes_internal.h include/modes_b200.h
 	@mkdir -p tests/_build
