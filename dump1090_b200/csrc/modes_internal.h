@@ -302,6 +302,44 @@ int finish_message(ResolveState &st, const modes_frame_eval &p, modes_message *o
 void add_recovery_stats(modes_recovery_stats &to, const modes_recovery_stats &from);
 
 // ---- host glue shared by the context (modes_api.cpp) and the receiver pool (modes_pool.cpp) ----
+// An owning, grow-only array of T in device memory (DevBuf) or pinned host memory (PinnedBuf).
+// ensure(n) replaces the array with one of exactly n elements when n exceeds its capacity, without
+// keeping the contents; the caller chooses n, so each growth policy stays where the array is used.
+template <typename T, bool Pinned>
+class CudaBuf {
+public:
+    CudaBuf() = default;
+    CudaBuf(CudaBuf &&o) noexcept : p_(o.p_), cap_(o.cap_) { o.p_ = nullptr; o.cap_ = 0; }
+    CudaBuf &operator=(CudaBuf &&o) noexcept {
+        if (this != &o) { release(); p_ = o.p_; cap_ = o.cap_; o.p_ = nullptr; o.cap_ = 0; }
+        return *this;
+    }
+    ~CudaBuf() { release(); }
+    cudaError_t ensure(size_t n) {
+        if (n <= cap_) return cudaSuccess;
+        release();
+        void *p = nullptr;
+        const cudaError_t e = Pinned ? cudaMallocHost(&p, n * sizeof(T)) : cudaMalloc(&p, n * sizeof(T));
+        if (e != cudaSuccess) return e;
+        p_ = static_cast<T *>(p);
+        cap_ = n;
+        return cudaSuccess;
+    }
+    T *get() const { return p_; }
+    T &operator[](size_t i) const { return p_[i]; }
+    size_t capacity() const { return cap_; }
+private:
+    void release() {
+        if (p_) { if (Pinned) cudaFreeHost(p_); else cudaFree(p_); }
+        p_ = nullptr;
+        cap_ = 0;
+    }
+    T *p_ = nullptr;
+    size_t cap_ = 0;
+};
+template <typename T> using DevBuf = CudaBuf<T, false>;
+template <typename T> using PinnedBuf = CudaBuf<T, true>;
+
 // The optional measurements and searches of a decode (modes_set_* / modes_pool_set_*).
 struct Features { bool signal = false, arrival = false, levels = false, recover = false, weak = false, spectrum = false; };
 

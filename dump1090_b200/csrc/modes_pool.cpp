@@ -80,7 +80,7 @@ struct Receiver {
     // [hist0, in_total) at hist[cur], hist0 a multiple of 16; the other half is where the next call's
     // history step writes (no launch reads what it writes)
     int64_t in_total = 0, hist0 = 0;
-    uint8_t *hist[2] = {nullptr, nullptr};
+    modes::DevBuf<uint8_t> hist[2];            // kHistBytes each, made on the receiver's first 2.4 MS/s call
     int cur = 0;
 };
 
@@ -101,6 +101,26 @@ RatePlan rate_plan(const Receiver &r) {
     pl.keep = keep < r.hist0 ? r.hist0 : keep;
     return pl;
 }
+
+// The job arrays of a slot's resampling and history launches (pinned or device): PoolResampleJob[n], then
+// PoolHistoryJob[n], in one allocation, so that one copy uploads both.
+template <bool Pinned>
+class RateJobs {
+public:
+    cudaError_t ensure(size_t n) {
+        const cudaError_t e = mem_.ensure(n * (sizeof(modes::PoolResampleJob) + sizeof(modes::PoolHistoryJob)));
+        if (e == cudaSuccess) n_ = n;
+        return e;
+    }
+    modes::PoolResampleJob *resample() const { return reinterpret_cast<modes::PoolResampleJob *>(mem_.get()); }
+    modes::PoolHistoryJob *history() const {
+        return reinterpret_cast<modes::PoolHistoryJob *>(mem_.get() + n_ * sizeof(modes::PoolResampleJob));
+    }
+    size_t bytes() const { return n_ * (sizeof(modes::PoolResampleJob) + sizeof(modes::PoolHistoryJob)); }
+private:
+    modes::CudaBuf<uint8_t, Pinned> mem_;
+    size_t n_ = 0;
+};
 
 // A few persistent helper threads: run(n, f) executes f(0..n-1), f(0) on the calling thread.
 class Crew {
@@ -161,32 +181,35 @@ struct modes_pool {
     modes::Features feat;
     std::string err;
     // device half (created on the first modes_pool_submit / _ingest): two batches may be in flight, so
-    // that one is uploaded and scanned while the one before it is resolved on the host
+    // that one is uploaded and scanned while the one before it is resolved on the host.  Each buffer is
+    // made the first time a call needs it and released after the slot context, which drains the stream.
     struct Slot {
         modes_ctx *ctx = nullptr;
-        uint8_t *d_batch = nullptr;            // [2 * max_batch] buffers: pad, data, pad, data, ...
-        uint8_t *h_carry = nullptr;            // pinned [max_batch][MODES_CARRY_BYTES]
+        modes::DevBuf<uint8_t> d_batch;        // [2 * max_batch] buffers: pad, data, pad, data, ...
+        modes::PinnedBuf<uint8_t> h_carry;     // [max_batch][MODES_CARRY_BYTES]
         std::vector<uint32_t> ids;             // the receivers of the batch in flight
         std::vector<int64_t> buf_index;        // with levels: each one's own index of its buffer
         std::vector<modes_level> level_out;
         modes::Features feat;                  // the switches as they were at submit
         bool busy = false;
-        // calls that name a 2.4 MS/s receiver: the call's buffers, the job arrays of the two launches
-        // (pinned and device: PoolResampleJob[max_batch], then PoolHistoryJob[max_batch]), and an event
-        // after the launches, which the other slot's next such call waits for (a receiver in both batches)
-        uint8_t *d_stage = nullptr;
-        void *h_jobs = nullptr, *d_jobs = nullptr;
+        // staged calls (a 2.4 MS/s or a 16-bit receiver): the call's UC8 buffers [max_batch], the jobs of
+        // the resampling and history launches (pinned and device), and an event after the launches, which
+        // the other slot's next staged call waits for (a receiver in both batches)
+        modes::DevBuf<uint8_t> d_stage;
+        RateJobs<true> h_jobs;
+        RateJobs<false> d_jobs;
         cudaEvent_t rate_done = nullptr;
         bool rate_recorded = false;
-        // calls that name a 16-bit receiver: their 16-bit buffers, and the conversion jobs (pinned and
-        // device: PoolConvertJob[max_batch])
-        uint8_t *d_stage16 = nullptr;
-        void *h_cjobs = nullptr, *d_cjobs = nullptr;
+        // calls that name a 16-bit receiver: their 16-bit buffers [max_batch], and the conversion jobs
+        modes::DevBuf<uint8_t> d_stage16;
+        modes::PinnedBuf<modes::PoolConvertJob> h_cjobs;
+        modes::DevBuf<modes::PoolConvertJob> d_cjobs;
         std::vector<const uint8_t *> iq8, iq16;   // the call's UC8 and 16-bit buffers, each group in call order
-        // with spectra: one job and one record per pair (pinned and device), made the first time the switch is on
-        modes::PoolSpectrumJob *h_sjobs = nullptr;
-        void *d_sjobs = nullptr;
-        modes_spectrum *h_spectra = nullptr, *d_spectra = nullptr;
+        // with spectra: one job and one record per pair
+        modes::PinnedBuf<modes::PoolSpectrumJob> h_sjobs;
+        modes::DevBuf<modes::PoolSpectrumJob> d_sjobs;
+        modes::PinnedBuf<modes_spectrum> h_spectra;
+        modes::DevBuf<modes_spectrum> d_spectra;
     } slot[2];
     unsigned submitted = 0, collected = 0;     // batches so far: slot = number & 1
     std::vector<modes_candidate> cands;
@@ -258,52 +281,32 @@ int set_feature(modes_pool *p, bool modes::Features::*f, int on) {
     return 0;
 }
 
+// A buffer of the pool could not be made: its error is cleared, so that a later call can try again.
+int out_of_memory(modes_pool *p) {
+    cudaGetLastError();
+    return fail(p, "out of memory for %zu receivers per batch", p->max_batch);
+}
+
+// The slot contexts that are missing and the batches' buffers, with the pool's device current.
 int ensure_device(modes_pool *p) {
-    if (p->slot[0].ctx) return 0;
+    if (cudaSetDevice(p->cfg.device) != cudaSuccess) return fail(p, "cudaSetDevice failed: %s", cudaGetErrorString(cudaGetLastError()));
     modes_config c = p->cfg;
     c.n_gpus = 1; c.gpu_resolve = 0;
     const size_t bytes = 2 * p->max_batch * kBuf;
     for (modes_pool::Slot &sl : p->slot) {
-        sl.ctx = modes_create(&c);
-        if (!sl.ctx) return fail(p, "%s", modes_last_error(nullptr));
-        share_features(p, sl.ctx);
-        sl.d_batch = static_cast<uint8_t *>(modes_device_alloc(bytes));
-        sl.h_carry = static_cast<uint8_t *>(modes_host_alloc(p->max_batch * MODES_CARRY_BYTES));
-        if (!sl.d_batch || !sl.h_carry) return fail(p, "out of memory for %zu receivers per batch", p->max_batch);
-        if (modes_device_memset(sl.d_batch, 127, bytes)) return fail(p, "device memset failed");      // dump1090.c:344 no signal
-    }
-    return 0;
-}
-
-constexpr size_t kJobBytes = sizeof(modes::PoolResampleJob) + sizeof(modes::PoolHistoryJob);
-
-// The device half of 2.4 MS/s receivers, made the first time a call names one.
-int ensure_rate_device(modes_pool *p, const uint32_t *receivers, size_t n) {
-    for (modes_pool::Slot &sl : p->slot) {
-        if (sl.d_stage) continue;
-        sl.d_stage = static_cast<uint8_t *>(modes_device_alloc(p->max_batch * kBuf));
-        sl.d_jobs = modes_device_alloc(p->max_batch * kJobBytes);
-        sl.h_jobs = modes_host_alloc(p->max_batch * kJobBytes);
-        if (!sl.d_stage || !sl.d_jobs || !sl.h_jobs) return fail(p, "out of memory for %zu receivers per batch", p->max_batch);
-        if (cudaEventCreateWithFlags(&sl.rate_done, cudaEventDisableTiming) != cudaSuccess)
-            return fail(p, "event creation failed: %s", cudaGetErrorString(cudaGetLastError()));
-    }
-    for (size_t i = 0; i < n; i++) {
-        if (p->rx[receivers[i]].format == modes::input::kUC8) continue;
-        for (modes_pool::Slot &sl : p->slot) {
-            if (sl.d_stage16) continue;
-            sl.d_stage16 = static_cast<uint8_t *>(modes_device_alloc(p->max_batch * 2 * kBuf));
-            sl.d_cjobs = modes_device_alloc(p->max_batch * sizeof(modes::PoolConvertJob));
-            sl.h_cjobs = modes_host_alloc(p->max_batch * sizeof(modes::PoolConvertJob));
-            if (!sl.d_stage16 || !sl.d_cjobs || !sl.h_cjobs) return fail(p, "out of memory for %zu receivers per batch", p->max_batch);
+        if (!sl.ctx) {
+            sl.ctx = modes_create(&c);
+            if (!sl.ctx) return fail(p, "%s", modes_last_error(nullptr));
+            share_features(p, sl.ctx);
         }
-        break;
-    }
-    for (size_t i = 0; i < n; i++) {
-        Receiver &r = p->rx[receivers[i]];
-        if (r.rate == kRate2M || r.hist[0]) continue;
-        for (uint8_t *&h : r.hist) h = static_cast<uint8_t *>(modes_device_alloc(kHistBytes));
-        if (!r.hist[0] || !r.hist[1]) return fail(p, "out of memory for the input history of receiver %u", receivers[i]);
+        if (sl.d_batch.capacity() < bytes) {
+            if (sl.d_batch.ensure(bytes)) return out_of_memory(p);
+            if (modes_device_memset(sl.d_batch.get(), 127, bytes)) {    // dump1090.c:344 no signal
+                sl.d_batch = modes::DevBuf<uint8_t>();                  // made again with its fill by the next call
+                return fail(p, "device memset failed");
+            }
+        }
+        if (sl.h_carry.ensure(p->max_batch * MODES_CARRY_BYTES)) return out_of_memory(p);
     }
     return 0;
 }
@@ -327,17 +330,11 @@ int upload_buffers(modes_pool *p, cudaStream_t st, const uint8_t *const *iq, siz
     return 0;
 }
 
-// The device half of the spectrum pass, made the first time a batch measures spectra.
-int ensure_spectrum_device(modes_pool *p) {
-    for (modes_pool::Slot &sl : p->slot) {
-        if (sl.h_sjobs) continue;
-        sl.h_sjobs = static_cast<modes::PoolSpectrumJob *>(modes_host_alloc(p->max_batch * sizeof(modes::PoolSpectrumJob)));
-        sl.d_sjobs = modes_device_alloc(p->max_batch * sizeof(modes::PoolSpectrumJob));
-        sl.h_spectra = static_cast<modes_spectrum *>(modes_host_alloc(p->max_batch * sizeof(modes_spectrum)));
-        sl.d_spectra = static_cast<modes_spectrum *>(modes_device_alloc(p->max_batch * sizeof(modes_spectrum)));
-        if (!sl.h_sjobs || !sl.d_sjobs || !sl.h_spectra || !sl.d_spectra)
-            return fail(p, "out of memory for %zu receivers per batch", p->max_batch);
-    }
+// The carries of the slot's first n pairs, gathered in h_carry, into the tails of their pad buffers.
+int upload_carries(modes_pool *p, modes_pool::Slot &sl, cudaStream_t st, size_t n) {
+    if (cudaMemcpy2DAsync(sl.d_batch.get() + kBuf - MODES_CARRY_BYTES, 2 * kBuf, sl.h_carry.get(), MODES_CARRY_BYTES,
+                          MODES_CARRY_BYTES, n, cudaMemcpyHostToDevice, st) != cudaSuccess)
+        return fail(p, "carry upload failed: %s", cudaGetErrorString(cudaGetLastError()));
     return 0;
 }
 
@@ -348,7 +345,7 @@ modes::PoolSpectrumJob spectrum_job(const Receiver &r, int64_t buffer, const uin
     if (r.rate == kRate2M)
         return modes::PoolSpectrumJob{nullptr, data, 2 * buffer * kBufSamples, 2 * buffer * kBufSamples, buffer,
                                       buffer * kBufSamples, SP::frames(1, 1, buffer), 0};
-    return modes::PoolSpectrumJob{r.hist[r.cur], stage, r.hist0, r.in_total, buffer, SP::first_sample(5, 6, buffer),
+    return modes::PoolSpectrumJob{r.hist[r.cur].get(), stage, r.hist0, r.in_total, buffer, SP::first_sample(5, 6, buffer),
                                   SP::frames(5, 6, buffer), 0};
 }
 
@@ -357,126 +354,26 @@ modes::PoolSpectrumJob spectrum_job(const Receiver &r, int64_t buffer, const uin
 int launch_pool_spectra(modes_pool *p, modes_pool::Slot &sl, cudaStream_t st, size_t n) {
     uint32_t most = 0;
     for (size_t i = 0; i < n; i++) most = sl.h_sjobs[i].frames > most ? sl.h_sjobs[i].frames : most;
-    if (cudaMemcpyAsync(sl.d_sjobs, sl.h_sjobs, n * sizeof(modes::PoolSpectrumJob), cudaMemcpyHostToDevice, st) != cudaSuccess ||
-        cudaMemsetAsync(sl.d_spectra, 0, n * sizeof(modes_spectrum), st) != cudaSuccess)
+    if (cudaMemcpyAsync(sl.d_sjobs.get(), sl.h_sjobs.get(), n * sizeof(modes::PoolSpectrumJob), cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemsetAsync(sl.d_spectra.get(), 0, n * sizeof(modes_spectrum), st) != cudaSuccess)
         return fail(p, "spectrum job upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-    modes::launch_spectrum_pool(static_cast<const modes::PoolSpectrumJob *>(sl.d_sjobs), (uint32_t)n, most, sl.d_spectra, st);
+    modes::launch_spectrum_pool(sl.d_sjobs.get(), (uint32_t)n, most, sl.d_spectra.get(), st);
     if (cudaGetLastError() != cudaSuccess ||
-        cudaMemcpyAsync(sl.h_spectra, sl.d_spectra, n * sizeof(modes_spectrum), cudaMemcpyDeviceToHost, st) != cudaSuccess)
+        cudaMemcpyAsync(sl.h_spectra.get(), sl.d_spectra.get(), n * sizeof(modes_spectrum), cudaMemcpyDeviceToHost, st) != cudaSuccess)
         return fail(p, "spectrum launch failed: %s", cudaGetErrorString(cudaGetLastError()));
     return 0;
 }
 
 // The scan and the passes of the switches over the slot's n pairs, already in place.
 int detect_pairs(modes_pool *p, modes_pool::Slot &sl, size_t n) {
-    if (modes_detect_device(sl.ctx, sl.d_batch, 2 * n, nullptr, nullptr, 0, nullptr)) return fail(p, "%s", modes_last_error(sl.ctx));
+    if (modes_detect_device(sl.ctx, sl.d_batch.get(), 2 * n, nullptr, nullptr, 0, nullptr)) return fail(p, "%s", modes_last_error(sl.ctx));
     sl.feat = p->feat;
     sl.feat.weak &= sl.feat.recover;
     if (sl.feat.recover && modes_recover_device(sl.ctx, nullptr, 0)) return fail(p, "%s", modes_last_error(sl.ctx));
     // the data buffers only (every second buffer), like the level pass
     if (sl.feat.weak && modes::weak_device_strided(sl.ctx, nullptr, nullptr, 0, 1, 2)) return fail(p, "%s", modes_last_error(sl.ctx));
     // the data buffers only (every second buffer), on the same stream: no wait before the collect
-    if (sl.feat.levels && modes_levels_device(sl.ctx, sl.d_batch + kBuf, n, 2 * kBuf)) return fail(p, "%s", modes_last_error(sl.ctx));
-    return 0;
-}
-
-// A call that names a 2.4 MS/s or a 16-bit receiver (the buffers are checked): every UC8 buffer to the
-// staging area and every 16-bit buffer to the 16-bit one, the 16-bit buffers converted (into their pairs at
-// 2 MHz, into the staging area at 2.4 MS/s), the pairs of the receivers that complete a buffer resampled /
-// moved into place, the histories advanced.  Staging slots: the UC8 buffers in call order, then the 16-bit
-// 2.4 MS/s receivers'.
-int submit_rated(modes_pool *p, modes_pool::Slot &sl, const uint32_t *receivers, const uint8_t *const *iq, size_t n) {
-    if (ensure_rate_device(p, receivers, n)) return -1;
-    cudaStream_t st = static_cast<cudaStream_t>(modes_stream(sl.ctx));
-    modes::PoolResampleJob *rj = static_cast<modes::PoolResampleJob *>(sl.h_jobs);
-    modes::PoolHistoryJob *hj = reinterpret_cast<modes::PoolHistoryJob *>(rj + p->max_batch);
-    modes::PoolConvertJob *cj = static_cast<modes::PoolConvertJob *>(sl.h_cjobs);
-    size_t n_pairs = 0, n_rj = 0, n_hist = 0, n_conv = 0;
-    uint64_t hist_max = 0;
-    bool carries = false;
-    std::vector<const uint8_t *> &iq8 = sl.iq8, &iq16 = sl.iq16;
-    iq8.clear();
-    iq16.clear();
-    for (size_t i = 0; i < n; i++) (p->rx[receivers[i]].format == modes::input::kUC8 ? iq8 : iq16).push_back(iq[i]);
-    size_t n_stage = iq8.size();
-    sl.ids.clear();
-    sl.buf_index.clear();
-    const bool spectra = p->feat.spectrum;
-    if (spectra && ensure_spectrum_device(p)) return -1;
-    for (size_t i = 0, k8 = 0; i < n; i++) {
-        const Receiver &r = p->rx[receivers[i]];
-        const bool uc8 = r.format == modes::input::kUC8;
-        uint8_t *pad = sl.d_batch + 2 * n_pairs * kBuf;
-        const uint8_t *in16 = uc8 ? nullptr : sl.d_stage16 + n_conv * 2 * kBuf;
-        if (r.rate == kRate2M) {
-            memcpy(sl.h_carry + n_pairs * MODES_CARRY_BYTES, r.carry, MODES_CARRY_BYTES);
-            if (uc8) rj[n_rj++] = modes::PoolResampleJob{nullptr, sl.d_stage + k8++ * kBuf, 0, 0, -1, nullptr, pad + kBuf};
-            else cj[n_conv++] = modes::PoolConvertJob{in16, pad + kBuf, r.shift};
-            if (spectra) sl.h_sjobs[n_pairs] = spectrum_job(r, r.submitted, pad + kBuf, nullptr);
-            n_pairs++;
-            sl.ids.push_back(receivers[i]);
-            sl.buf_index.push_back(r.submitted);
-            carries = true;
-            continue;
-        }
-        uint8_t *stage = sl.d_stage + (uc8 ? k8++ : n_stage++) * kBuf;
-        if (!uc8) cj[n_conv++] = modes::PoolConvertJob{in16, stage, r.shift};
-        const RatePlan pl = rate_plan(r);
-        if (pl.completes) {
-            rj[n_rj++] = modes::PoolResampleJob{r.hist[r.cur], stage, r.hist0, r.in_total, r.submitted * kBufSamples,
-                                                pad + kBuf - MODES_CARRY_BYTES, pad + kBuf};
-            if (spectra) sl.h_sjobs[n_pairs] = spectrum_job(r, r.submitted, nullptr, stage);
-            n_pairs++;
-            sl.ids.push_back(receivers[i]);
-            sl.buf_index.push_back(r.submitted);
-        }
-        const uint64_t bytes = (uint64_t)(r.in_total + (int64_t)kBuf - pl.keep);
-        if (bytes > kHistBytes)
-            return fail(p, "internal: 2.4 MS/s input history of %llu bytes for receiver %u", (unsigned long long)bytes, receivers[i]);
-        hj[n_hist++] = modes::PoolHistoryJob{r.hist[r.cur], stage, r.hist0, r.in_total, pl.keep, r.hist[r.cur ^ 1]};
-        if (bytes > hist_max) hist_max = bytes;
-    }
-    if (!iq8.empty() && upload_buffers(p, st, iq8.data(), iq8.size(), sl.d_stage, kBuf, kBuf)) return -1;
-    if (!iq16.empty() && upload_buffers(p, st, iq16.data(), iq16.size(), sl.d_stage16, 2 * kBuf, 2 * kBuf)) return -1;
-    // the 2 MHz receivers' carries as the 2 MHz path uploads them (the 2.4 MS/s pairs' tails are then
-    // overwritten by the resampler)
-    if (carries && cudaMemcpy2DAsync(sl.d_batch + kBuf - MODES_CARRY_BYTES, 2 * kBuf, sl.h_carry, MODES_CARRY_BYTES,
-                                     MODES_CARRY_BYTES, n_pairs, cudaMemcpyHostToDevice, st) != cudaSuccess)
-        return fail(p, "carry upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-    if (cudaMemcpyAsync(sl.d_jobs, sl.h_jobs, p->max_batch * kJobBytes, cudaMemcpyHostToDevice, st) != cudaSuccess)
-        return fail(p, "job upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-    if (n_conv && cudaMemcpyAsync(sl.d_cjobs, sl.h_cjobs, n_conv * sizeof(modes::PoolConvertJob), cudaMemcpyHostToDevice, st) != cudaSuccess)
-        return fail(p, "job upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-    // the conversion writes only this slot's pairs and staging area: it need not wait for the other slot
-    modes::launch_convert_pool(static_cast<const modes::PoolConvertJob *>(sl.d_cjobs), (uint32_t)n_conv, st);
-    // the other batch in flight may name the same receivers: its reads and its history step first
-    const modes_pool::Slot &other = p->slot[(p->submitted & 1) ^ 1];
-    if (other.rate_recorded && cudaStreamWaitEvent(st, other.rate_done, 0) != cudaSuccess)
-        return fail(p, "stream wait failed: %s", cudaGetErrorString(cudaGetLastError()));
-    const modes::PoolResampleJob *d_rj = static_cast<const modes::PoolResampleJob *>(sl.d_jobs);
-    modes::launch_resample_pool(d_rj, (uint32_t)n_rj, st);
-    modes::launch_history_pool(reinterpret_cast<const modes::PoolHistoryJob *>(d_rj + p->max_batch), (uint32_t)n_hist, hist_max, st);
-    // the spectra read the histories too: before rate_done, after which the other slot's history step may
-    // overwrite them
-    if (spectra && n_pairs && launch_pool_spectra(p, sl, st, n_pairs)) return -1;
-    if (cudaGetLastError() != cudaSuccess || cudaEventRecord(sl.rate_done, st) != cudaSuccess)
-        return fail(p, "resampling launch failed: %s", cudaGetErrorString(cudaGetLastError()));
-    sl.rate_recorded = true;
-    if (n_pairs && detect_pairs(p, sl, n_pairs)) return -1;
-    for (size_t i = 0; i < n; i++) {
-        Receiver &r = p->rx[receivers[i]];
-        if (r.rate == kRate2M) {
-            r.submitted++;
-            if (r.format == modes::input::kUC8) memcpy(r.carry, iq[i] + kBuf - MODES_CARRY_BYTES, MODES_CARRY_BYTES);     // dump1090.c:481
-            else modes::input::convert_samples(iq[i] + 2 * (kBuf - MODES_CARRY_BYTES), MODES_CARRY_BYTES / 2, r.shift, r.carry);
-            continue;
-        }
-        const RatePlan pl = rate_plan(r);
-        r.submitted += pl.completes ? 1 : 0;
-        r.in_total += (int64_t)kBuf;
-        r.hist0 = pl.keep;
-        r.cur ^= 1;
-    }
+    if (sl.feat.levels && modes_levels_device(sl.ctx, sl.d_batch.get() + kBuf, n, 2 * kBuf)) return fail(p, "%s", modes_last_error(sl.ctx));
     return 0;
 }
 
@@ -501,25 +398,11 @@ modes_pool *modes_pool_create(const modes_config *cfg, size_t n_receivers, size_
 void modes_pool_destroy(modes_pool *p) {
     if (!p) return;
     for (Receiver &r : p->rx) if (r.res) modes_resolver_destroy(r.res);
-    for (Receiver &r : p->rx)
-        for (uint8_t *h : r.hist) if (h) modes_device_free(h);
     for (modes_pool::Slot &sl : p->slot) {
-        if (sl.d_batch) modes_device_free(sl.d_batch);
-        if (sl.h_carry) modes_host_free(sl.h_carry);
-        if (sl.d_stage) modes_device_free(sl.d_stage);
-        if (sl.d_jobs) modes_device_free(sl.d_jobs);
-        if (sl.h_jobs) modes_host_free(sl.h_jobs);
         if (sl.rate_done) cudaEventDestroy(sl.rate_done);
-        if (sl.d_stage16) modes_device_free(sl.d_stage16);
-        if (sl.d_cjobs) modes_device_free(sl.d_cjobs);
-        if (sl.h_cjobs) modes_host_free(sl.h_cjobs);
-        if (sl.h_sjobs) modes_host_free(sl.h_sjobs);
-        if (sl.d_sjobs) modes_device_free(sl.d_sjobs);
-        if (sl.h_spectra) modes_host_free(sl.h_spectra);
-        if (sl.d_spectra) modes_device_free(sl.d_spectra);
-        if (sl.ctx) modes_destroy(sl.ctx);
+        if (sl.ctx) modes_destroy(sl.ctx);     // waits for the slot's stream
     }
-    delete p;
+    delete p;                                  // and with it the buffers, which nothing queued uses any more
 }
 
 const char *modes_pool_last_error(const modes_pool *p) { return p ? p->err.c_str() : "no pool"; }
@@ -655,7 +538,15 @@ int modes_pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, const
     return pool_resolve(p, receivers, n, candidates, nullptr, false, tiles, sink, user);
 }
 
+// One buffer of each listed receiver.  A receiver gets a pair when it decodes a buffer in this call: a 2 MHz
+// receiver always, a 2.4 MS/s one when the call completes one.  A call that names only 2 MHz UC8 receivers
+// uploads its buffers straight into the pairs' data buffers.  Any other call is staged: every UC8 buffer
+// goes to the staging area and every 16-bit buffer to the 16-bit one; launches then convert the 16-bit
+// buffers (into their pairs at 2 MHz, into the staging area at 2.4 MS/s), resample the completing
+// receivers / move the 2 MHz ones into their pairs, and advance the histories.  Staging slots: the UC8
+// buffers in call order, then the 16-bit 2.4 MS/s receivers'.
 int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *const *iq, size_t n) {
+    namespace input = modes::input;
     if (!p) return -1;
     if (check_ids(p, receivers, n)) return -1;
     if (!n) return fail(p, "an empty batch");
@@ -663,41 +554,119 @@ int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *c
     if (ensure_device(p)) return -1;
     modes_pool::Slot &sl = p->slot[p->submitted & 1];
     if (sl.busy) return fail(p, "two batches are in flight: modes_pool_collect first");
-    bool rated = false;
+    bool staged = false, wide = false;
     for (size_t i = 0; i < n; i++) {
         if (!iq[i]) return fail(p, "receiver %u: no buffer", receivers[i]);
-        rated |= p->rx[receivers[i]].rate != kRate2M || p->rx[receivers[i]].format != modes::input::kUC8;
+        const Receiver &r = p->rx[receivers[i]];
+        wide |= r.format != input::kUC8;
+        staged |= wide || r.rate != kRate2M;
     }
-    if (rated) {
-        if (submit_rated(p, sl, receivers, iq, n)) return -1;
-        sl.busy = true;
-        p->submitted++;
-        return 0;
-    }
-    cudaStream_t st = static_cast<cudaStream_t>(modes_stream(sl.ctx));
-    // the carries into the tails of the pad buffers, the new buffers behind them
-    for (size_t i = 0; i < n; i++)
-        memcpy(sl.h_carry + i * MODES_CARRY_BYTES, p->rx[receivers[i]].carry, MODES_CARRY_BYTES);
-    if (cudaMemcpy2DAsync(sl.d_batch + kBuf - MODES_CARRY_BYTES, 2 * kBuf, sl.h_carry, MODES_CARRY_BYTES, MODES_CARRY_BYTES, n,
-                          cudaMemcpyHostToDevice, st) != cudaSuccess)
-        return fail(p, "carry upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-    if (upload_buffers(p, st, iq, n, sl.d_batch + kBuf, 2 * kBuf, kBuf)) return -1;
-    if (detect_pairs(p, sl, n)) return -1;
-    // the pairs' data buffers, on the same stream after the scan
-    if (sl.feat.spectrum) {
-        if (ensure_spectrum_device(p)) return -1;
-        for (size_t i = 0; i < n; i++) {
-            const Receiver &r = p->rx[receivers[i]];
-            sl.h_sjobs[i] = spectrum_job(r, r.submitted, sl.d_batch + (2 * i + 1) * kBuf, nullptr);
+    const size_t mb = p->max_batch;
+    const bool spectra = p->feat.spectrum;
+    if (staged && (sl.d_stage.ensure(mb * kBuf) || sl.h_jobs.ensure(mb) || sl.d_jobs.ensure(mb))) return out_of_memory(p);
+    if (wide && (sl.d_stage16.ensure(mb * 2 * kBuf) || sl.h_cjobs.ensure(mb) || sl.d_cjobs.ensure(mb))) return out_of_memory(p);
+    if (spectra && (sl.h_sjobs.ensure(mb) || sl.d_sjobs.ensure(mb) || sl.h_spectra.ensure(mb) || sl.d_spectra.ensure(mb)))
+        return out_of_memory(p);
+    if (staged && !sl.rate_done && cudaEventCreateWithFlags(&sl.rate_done, cudaEventDisableTiming) != cudaSuccess)
+        return fail(p, "event creation failed: %s", cudaGetErrorString(cudaGetLastError()));
+
+    modes::PoolResampleJob *rj = sl.h_jobs.resample();
+    modes::PoolHistoryJob *hj = sl.h_jobs.history();
+    size_t n_pairs = 0, n_rj = 0, n_hist = 0, n_conv = 0;
+    uint64_t hist_max = 0;
+    bool carries = false;
+    sl.iq8.clear();
+    sl.iq16.clear();
+    for (size_t i = 0; i < n; i++) (p->rx[receivers[i]].format == input::kUC8 ? sl.iq8 : sl.iq16).push_back(iq[i]);
+    size_t n_stage = sl.iq8.size();
+    sl.ids.clear();
+    sl.buf_index.clear();
+    for (size_t i = 0, k8 = 0; i < n; i++) {
+        Receiver &r = p->rx[receivers[i]];
+        const bool uc8 = r.format == input::kUC8;
+        uint8_t *data = sl.d_batch.get() + (2 * n_pairs + 1) * kBuf;    // the data buffer of its pair, if it gets one
+        // staged: where its call's UC8 bytes are staged (none for a 16-bit 2 MHz receiver, converted into its pair)
+        uint8_t *stage = staged && (uc8 || r.rate != kRate2M) ? sl.d_stage.get() + (uc8 ? k8++ : n_stage++) * kBuf : nullptr;
+        if (!uc8) {
+            sl.h_cjobs[n_conv] = modes::PoolConvertJob{sl.d_stage16.get() + n_conv * 2 * kBuf, stage ? stage : data, r.shift};
+            n_conv++;
         }
-        if (launch_pool_spectra(p, sl, st, n)) return -1;
+        bool pair = true;
+        if (r.rate == kRate2M) {
+            memcpy(sl.h_carry.get() + n_pairs * MODES_CARRY_BYTES, r.carry, MODES_CARRY_BYTES);
+            carries = true;
+            if (stage) rj[n_rj++] = modes::PoolResampleJob{nullptr, stage, 0, 0, -1, nullptr, data};
+        } else {
+            for (modes::DevBuf<uint8_t> &h : r.hist)
+                if (h.ensure(kHistBytes)) {
+                    cudaGetLastError();
+                    return fail(p, "out of memory for the input history of receiver %u", receivers[i]);
+                }
+            const RatePlan pl = rate_plan(r);
+            pair = pl.completes;
+            if (pair)
+                rj[n_rj++] = modes::PoolResampleJob{r.hist[r.cur].get(), stage, r.hist0, r.in_total, r.submitted * kBufSamples,
+                                                    data - MODES_CARRY_BYTES, data};
+            const uint64_t bytes = (uint64_t)(r.in_total + (int64_t)kBuf - pl.keep);
+            if (bytes > kHistBytes)
+                return fail(p, "internal: 2.4 MS/s input history of %llu bytes for receiver %u", (unsigned long long)bytes, receivers[i]);
+            hj[n_hist++] = modes::PoolHistoryJob{r.hist[r.cur].get(), stage, r.hist0, r.in_total, pl.keep, r.hist[r.cur ^ 1].get()};
+            if (bytes > hist_max) hist_max = bytes;
+        }
+        if (!pair) continue;
+        if (spectra) sl.h_sjobs[n_pairs] = spectrum_job(r, r.submitted, data, stage);
+        n_pairs++;
+        sl.ids.push_back(receivers[i]);
+        sl.buf_index.push_back(r.submitted);
     }
-    sl.buf_index.resize(n);
-    for (size_t i = 0; i < n; i++) sl.buf_index[i] = p->rx[receivers[i]].submitted++;
-    // what each receiver carries into its next buffer (dump1090.c:481)
-    for (size_t i = 0; i < n; i++)
-        memcpy(p->rx[receivers[i]].carry, iq[i] + kBuf - MODES_CARRY_BYTES, MODES_CARRY_BYTES);
-    sl.ids.assign(receivers, receivers + n);
+
+    cudaStream_t st = static_cast<cudaStream_t>(modes_stream(sl.ctx));
+    if (!staged) {
+        if (upload_carries(p, sl, st, n_pairs) || upload_buffers(p, st, iq, n, sl.d_batch.get() + kBuf, 2 * kBuf, kBuf)) return -1;
+    } else {
+        if (!sl.iq8.empty() && upload_buffers(p, st, sl.iq8.data(), sl.iq8.size(), sl.d_stage.get(), kBuf, kBuf)) return -1;
+        if (!sl.iq16.empty() && upload_buffers(p, st, sl.iq16.data(), sl.iq16.size(), sl.d_stage16.get(), 2 * kBuf, 2 * kBuf))
+            return -1;
+        // the 2.4 MS/s pairs' tails are then overwritten by the resampler
+        if (carries && upload_carries(p, sl, st, n_pairs)) return -1;
+        if (cudaMemcpyAsync(sl.d_jobs.resample(), rj, sl.h_jobs.bytes(), cudaMemcpyHostToDevice, st) != cudaSuccess ||
+            (n_conv && cudaMemcpyAsync(sl.d_cjobs.get(), sl.h_cjobs.get(), n_conv * sizeof(modes::PoolConvertJob),
+                                       cudaMemcpyHostToDevice, st) != cudaSuccess))
+            return fail(p, "job upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+        // the conversion writes only this slot's pairs and staging area: it need not wait for the other slot
+        modes::launch_convert_pool(sl.d_cjobs.get(), (uint32_t)n_conv, st);
+        // the other batch in flight may name the same receivers: its reads and its history step first
+        const modes_pool::Slot &other = p->slot[(p->submitted & 1) ^ 1];
+        if (other.rate_recorded && cudaStreamWaitEvent(st, other.rate_done, 0) != cudaSuccess)
+            return fail(p, "stream wait failed: %s", cudaGetErrorString(cudaGetLastError()));
+        modes::launch_resample_pool(sl.d_jobs.resample(), (uint32_t)n_rj, st);
+        modes::launch_history_pool(sl.d_jobs.history(), (uint32_t)n_hist, hist_max, st);
+    }
+    // the spectra read the histories too: before rate_done, after which the other slot's history step may
+    // overwrite them
+    if (spectra && n_pairs && launch_pool_spectra(p, sl, st, n_pairs)) return -1;
+    if (staged) {
+        if (cudaGetLastError() != cudaSuccess || cudaEventRecord(sl.rate_done, st) != cudaSuccess)
+            return fail(p, "resampling launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+        sl.rate_recorded = true;
+    }
+    if (n_pairs && detect_pairs(p, sl, n_pairs)) return -1;
+
+    for (size_t i = 0; i < n; i++) {
+        Receiver &r = p->rx[receivers[i]];
+        if (r.rate == kRate2M) {
+            r.submitted++;
+            // what it carries into its next buffer (dump1090.c:481)
+            if (r.format == input::kUC8) memcpy(r.carry, iq[i] + kBuf - MODES_CARRY_BYTES, MODES_CARRY_BYTES);
+            else input::convert_samples(iq[i] + 2 * (kBuf - MODES_CARRY_BYTES), MODES_CARRY_BYTES / 2, r.shift, r.carry);
+            continue;
+        }
+        const RatePlan pl = rate_plan(r);
+        r.submitted += pl.completes ? 1 : 0;
+        r.in_total += (int64_t)kBuf;
+        r.hist0 = pl.keep;
+        r.cur ^= 1;
+    }
     sl.busy = true;
     p->submitted++;
     return 0;
