@@ -248,7 +248,7 @@ EXPORTS = ["modes_abi_version", "modes_default_config", "modes_create", "modes_d
            "modes_set_input_rate", "modes_resample_device", "modes_pool_set_input_rate", "modes_set_input_format",
            "modes_pool_set_input_format", "modes_resample_device_at", "modes_set_input_offset",
            "modes_resample_device_shift", "modes_set_spectrum", "modes_take_spectra", "modes_pool_set_spectrum",
-           "modes_pool_take_spectra"]
+           "modes_pool_take_spectra", "modes_process_device"]
 
 INPUT_RATES = (2_000_000, 2_400_000, 4_000_000, 6_000_000, 8_000_000, 10_000_000)      # modes_set_input_rate
 INPUT_FORMATS = {"uc8": 0, "sc16": 1, "sc16q11": 2}     # modes_set_input_format: MODES_INPUT_*
@@ -280,6 +280,7 @@ def lib():
         L.modes_last_error.argtypes = [C.c_void_p]
         L.modes_set_sink.argtypes = [C.c_void_p, SINK_FN, C.c_void_p]
         L.modes_process.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+        L.modes_process_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
         L.modes_finish.argtypes = [C.c_void_p]
         L.modes_reset.argtypes = [C.c_void_p]
         L.modes_get_stats.argtypes = [C.c_void_p, C.POINTER(Stats)]
@@ -443,6 +444,17 @@ def _ptr(a: np.ndarray):
     return a.ctypes.data_as(C.c_void_p)
 
 
+def _is_cuda_tensor(x) -> bool:
+    """A torch tensor in GPU memory (checked without importing torch: numpy and bytes have no is_cuda)."""
+    return getattr(x, "is_cuda", False) is True
+
+
+def _sync_stream(t) -> None:
+    """Wait for the work queued on the tensor's current stream, which may still be writing it."""
+    import torch
+    torch.cuda.current_stream(t.device).synchronize()
+
+
 class _Collector:
     """A sink that copies every delivered message."""
 
@@ -502,7 +514,10 @@ class Decoder:
     the GPU as it is decimated (modes_set_input_offset, |offset| <= input_rate / 2 - 1 MHz); 0 changes
     nothing.
     spectrum=True measures every decoded buffer's input power spectrum on the GPU, before resampling,
-    decimation and the offset (modes_set_spectrum): take_spectra(), spectrum_summary()."""
+    decimation and the offset (modes_set_spectrum): take_spectra(), spectrum_summary().
+    process() and decode() also take a CUDA torch tensor of any dtype on the decoder's device, read as its
+    raw bytes (e.g. int16 SC16 I/Q), and decode it where it is (modes_process_device): the output is what
+    the same bytes give from host memory, without their two trips across PCIe."""
 
     def __init__(self, signal: bool = False, levels: bool = False, recover: bool = False, weak_preambles: bool = False,
                  arrival: bool = False, input_rate: int = 2_000_000, input_format: str = "uc8",
@@ -556,12 +571,30 @@ class Decoder:
 
     # -- streaming path (the --ifile main loop)
     def process(self, data) -> None:
+        if _is_cuda_tensor(data):
+            t = self._device_bytes(data)
+            self.process_device_ptr(t.data_ptr(), t.numel() * t.element_size())
+            return
         a = np.ascontiguousarray(data, dtype=np.uint8) if not isinstance(data, (bytes, bytearray)) \
             else np.frombuffer(data, dtype=np.uint8)
         self._check(lib().modes_process(self._h, _ptr(a), a.size))
 
     def process_ptr(self, ptr: int, nbytes: int) -> None:
         self._check(lib().modes_process(self._h, C.c_void_p(ptr), nbytes))
+
+    def process_device_ptr(self, ptr: int, nbytes: int) -> None:
+        """modes_process_device: nbytes of the stream at a device address of the decoder's device, fully
+        written before the call and no longer read after it."""
+        self._check(lib().modes_process_device(self._h, C.c_void_p(ptr), nbytes))
+
+    def _device_bytes(self, t):
+        """The CUDA tensor as a contiguous tensor on this decoder's device, its writers finished."""
+        if t.device.index != self.cfg.device:
+            raise ValueError(f"the tensor is on {t.device}, the decoder on cuda:{self.cfg.device}")
+        if not t.is_contiguous():
+            t = t.contiguous()
+        _sync_stream(t)
+        return t
 
     def finish(self) -> None:
         self._check(lib().modes_finish(self._h))
@@ -575,8 +608,17 @@ class Decoder:
         return out
 
     def decode(self, data, chunk: int | None = None) -> list:
-        """Decode a whole stream like `dump1090 --ifile`: returns the message list."""
+        """Decode a whole stream like `dump1090 --ifile`: returns the message list.  A CUDA tensor is
+        decoded in device memory, in calls of `chunk` bytes."""
         self.reset()
+        if _is_cuda_tensor(data):
+            t = self._device_bytes(data)
+            ptr, n = t.data_ptr(), t.numel() * t.element_size()
+            step = chunk or max(n, 1)
+            for off in range(0, max(n, 1), step):
+                self.process_device_ptr(ptr + off, min(step, n - off))
+            self.finish()
+            return self.take_messages()
         a = np.frombuffer(data, dtype=np.uint8) if isinstance(data, (bytes, bytearray)) else \
             np.ascontiguousarray(data, dtype=np.uint8)
         if chunk:

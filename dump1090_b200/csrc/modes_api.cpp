@@ -131,6 +131,14 @@ struct modes_ctx {
     PinnedBuf<uint8_t> pending;       // one reference buffer
     size_t pending_len = 0;
     uint8_t carry[MODES_CARRY_BYTES];
+    // which memory the stream is fed from (modes_process or modes_process_device), fixed by its first call
+    enum class Feed { none, host, device } feed = Feed::none;
+    // a device-fed stream's twins of pending, carry and hold, on cfg.device: created by its first call.  The
+    // hold lives in two halves used in turn, so that keeping its tail never copies a range onto itself.
+    DevBuf<uint8_t> d_pending;
+    DevBuf<uint8_t> d_carry;
+    DevBuf<uint8_t> d_hold[2];
+    int hold_cur = 0;
     int64_t buffers_done = 0;
     bool finished = false;
     bool started = false;                 // modes_process or modes_finish since create / reset
@@ -623,12 +631,15 @@ int collect_group(modes_ctx *ctx, int parity) {
     return 0;
 }
 
-// Where the batches of a run read their input.  2 MHz UC8: the run's whole reference buffers at iq.
+// Where the batches of a run read their input, host memory or (device) the leading context's device memory.
+// 2 MHz UC8: the run's whole reference buffers at iq.
 // 2.4 MS/s or a 16-bit format (iq == nullptr): the stream's input bytes [hold0, call0) at hold and
 // [call0, end) at call; every later byte is no signal, and output samples at or past out_end are the EOF
 // buffer's padding.
 struct Source {
     const uint8_t *iq = nullptr;
+    const uint8_t *carry = nullptr;   // device: the stream's 476 bytes before iq (host: the context's carry)
+    bool device = false;              // every pointer is device memory of the context's device
     const uint8_t *hold = nullptr;
     int64_t hold0 = 0;
     const uint8_t *call = nullptr;
@@ -647,8 +658,10 @@ int64_t batch_in_lo(const modes_ctx *ctx, int64_t o0) { return in_lo(*ctx->rate,
 int64_t batch_in_hi(const modes_ctx *ctx, int64_t o1) { return in_hi(*ctx->rate, o1 - 1); }
 
 // Upload the input bytes the slot's batch (nb buffers from s.buffer_base, and the carry before them) reads,
-// straight from where they are, and make the slot's body and carry block from them on the device.
+// straight from where they are (a device source: to this GPU's slot, from the leading context's device), and
+// make the slot's body and carry block from them on the device.
 int stage_held(modes_ctx *ctx, Slot &s, const Source &src, size_t nb) {
+    const cudaMemcpyKind kind = src.device ? cudaMemcpyDefault : cudaMemcpyHostToDevice;
     const int bps = input::sample_bytes(ctx->input_format);
     const int64_t o0 = s.buffer_base * (int64_t)kBufSamples;
     const int64_t o1 = o0 + (int64_t)nb * kBufSamples;
@@ -663,12 +676,12 @@ int stage_held(modes_ctx *ctx, Slot &s, const Source &src, size_t nb) {
     CK(ctx, s.d_in.ensure((size_t)(hi - lo) + 16));
     if (lo < src.call0) {
         const int64_t n = (hi < src.call0 ? hi : src.call0) - lo;
-        if (n) CK(ctx, cudaMemcpyAsync(s.d_in.get(), src.hold + (lo - src.hold0), (size_t)n, cudaMemcpyHostToDevice, s.stream));
+        if (n) CK(ctx, cudaMemcpyAsync(s.d_in.get(), src.hold + (lo - src.hold0), (size_t)n, kind, s.stream));
     }
     if (hi > src.call0) {
         const int64_t from = lo > src.call0 ? lo : src.call0;
-        CK(ctx, cudaMemcpyAsync(s.d_in.get() + (from - lo), src.call + (from - src.call0), (size_t)(hi - from),
-                                cudaMemcpyHostToDevice, s.stream));
+        CK(ctx, cudaMemcpyAsync(s.d_in.get() + (from - lo), src.call + (from - src.call0), (size_t)(hi - from), kind,
+                                s.stream));
     }
     const ResampleJob j{s.d_in.get(), (uint64_t)(hi - lo), lo / bps, o0, (uint64_t)(o1 - o0), src.out_end,
                         s.d_iq.get(), s.d_halo.get()};
@@ -698,8 +711,19 @@ int submit_next(modes_ctx *ctx, modes_ctx *g, Slot &s, Source &src, size_t nb) {
     s.spec_in.in_bytes = (uint64_t)nb * MODES_BUFFER_BYTES;
     s.spec_in.in_first = s.buffer_base * (int64_t)kBufSamples;
     s.spec_shift = -1;
-    if (submit(g, s, src.iq, nullptr, nb, ctx->carry, nullptr, 0, nullptr)) return -1;
-    memcpy(ctx->carry, src.iq + nb * MODES_BUFFER_BYTES - MODES_CARRY_BYTES, MODES_CARRY_BYTES);
+    if (src.device) {
+        // copied to the slot (its 16-byte alignment is the kernels'), the carry block built beside it: the
+        // stream's bytes never pass through the host
+        CK(g, cudaMemcpyAsync(s.d_iq.get(), src.iq, (size_t)nb * MODES_BUFFER_BYTES, cudaMemcpyDefault, s.stream));
+        CK(g, cudaMemsetAsync(s.d_halo.get(), 127, kHaloAlloc, s.stream));                  // dump1090.c:344 no-signal
+        CK(g, cudaMemcpyAsync(s.d_halo.get() + (kHaloBytes - MODES_CARRY_BYTES), src.carry, MODES_CARRY_BYTES,
+                              cudaMemcpyDefault, s.stream));
+        if (submit(g, s, nullptr, s.d_iq.get(), nb, nullptr, nullptr, 0, nullptr, true)) return -1;
+        src.carry = src.iq + nb * MODES_BUFFER_BYTES - MODES_CARRY_BYTES;
+    } else {
+        if (submit(g, s, src.iq, nullptr, nb, ctx->carry, nullptr, 0, nullptr)) return -1;
+        memcpy(ctx->carry, src.iq + nb * MODES_BUFFER_BYTES - MODES_CARRY_BYTES, MODES_CARRY_BYTES);
+    }
     src.iq += nb * MODES_BUFFER_BYTES;
     return 0;
 }
@@ -766,6 +790,20 @@ Source host_buffers(const uint8_t *iq) {
     return src;
 }
 
+Source device_buffers(const uint8_t *iq, const uint8_t *carry) {
+    Source src;
+    src.iq = iq;
+    src.carry = carry;
+    src.device = true;
+    return src;
+}
+
+// A device-fed stream's own copies (pending, carry, hold) are queued on slot 0's stream and waited for
+// before anything reads them: a multi-GPU run's first batch reads them from another device's stream.
+cudaError_t copy_on_device(modes_ctx *ctx, void *dst, const void *src, size_t n) {
+    return n ? cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToDevice, ctx->slot[0].stream) : cudaSuccess;
+}
+
 // The most the hold can need: the input of one reference buffer and of the carry before it, with the
 // filter's reach on both sides where there is a filter (a whole buffer's input would have run).
 size_t hold_bytes(const modes_ctx *ctx) {
@@ -778,7 +816,9 @@ size_t hold_bytes(const modes_ctx *ctx) {
 // hold and the caller's bytes where they are (run_buffers returns with every copy done), then keep in
 // the hold what later batches read, a sample split across calls included.
 int process_held(modes_ctx *ctx, const uint8_t *iq, size_t nbytes) {
-    CK(ctx, ctx->hold.ensure(hold_bytes(ctx)));
+    const bool dev = ctx->feed == modes_ctx::Feed::device;
+    if (dev) for (auto &h : ctx->d_hold) CK(ctx, h.ensure(hold_bytes(ctx)));
+    else CK(ctx, ctx->hold.ensure(hold_bytes(ctx)));
     const int64_t call0 = ctx->in_total;
     ctx->in_total += (int64_t)nbytes;
     const int64_t avail = ctx->in_total / input::sample_bytes(ctx->input_format);   // whole input samples
@@ -788,14 +828,30 @@ int process_held(modes_ctx *ctx, const uint8_t *iq, size_t nbytes) {
     while (batch_in_hi(ctx, (m + 1) * B) <= avail) m++;
     if (m > ctx->buffers_done) {
         Source src;
-        src.hold = ctx->hold.get(); src.hold0 = ctx->hold0;
+        src.hold = dev ? ctx->d_hold[ctx->hold_cur].get() : ctx->hold.get(); src.hold0 = ctx->hold0;
         src.call = iq; src.call0 = call0; src.end = ctx->in_total;
+        src.device = dev;
         if (run_buffers(ctx, src, (size_t)(m - ctx->buffers_done))) return -1;
     }
     int64_t keep = input::sample_bytes(ctx->input_format) * batch_in_lo(ctx, ctx->buffers_done * B);
     if (keep < ctx->hold0) keep = ctx->hold0;
-    if ((size_t)(ctx->in_total - keep) > ctx->hold.capacity())
+    if ((size_t)(ctx->in_total - keep) > (dev ? ctx->d_hold[0].capacity() : ctx->hold.capacity()))
         return fail(ctx, "internal: input history of %lld bytes", (long long)(ctx->in_total - keep));
+    if (dev) {
+        // into the other half: what it keeps of the hold, then of the call
+        const uint8_t *old = ctx->d_hold[ctx->hold_cur].get();
+        uint8_t *h = ctx->d_hold[ctx->hold_cur ^ 1].get();
+        if (keep < call0) {
+            CK(ctx, copy_on_device(ctx, h, old + (keep - ctx->hold0), (size_t)(call0 - keep)));
+            CK(ctx, copy_on_device(ctx, h + (call0 - keep), iq, nbytes));
+        } else {
+            CK(ctx, copy_on_device(ctx, h, iq + (keep - call0), (size_t)(ctx->in_total - keep)));
+        }
+        CK(ctx, wait_stream(ctx->slot[0].stream));
+        ctx->hold_cur ^= 1;
+        ctx->hold0 = keep;
+        return 0;
+    }
     uint8_t *h = ctx->hold.get();
     if (keep < call0) {
         memmove(h, h + (keep - ctx->hold0), (size_t)(call0 - keep));
@@ -820,7 +876,8 @@ int finish_held(modes_ctx *ctx) {
     const int64_t last = ctx->eof_buffer + (ctx->cfg.drop_eof_buffer ? 0 : 1);
     if (last <= ctx->buffers_done) return 0;
     Source src;
-    src.hold = ctx->hold.get(); src.hold0 = ctx->hold0;
+    src.device = ctx->feed == modes_ctx::Feed::device;
+    src.hold = src.device ? ctx->d_hold[ctx->hold_cur].get() : ctx->hold.get(); src.hold0 = ctx->hold0;
     src.call0 = src.end = ctx->in_total;
     src.out_end = n_out;
     return run_buffers(ctx, src, (size_t)(last - ctx->buffers_done));
@@ -1124,6 +1181,7 @@ int modes_reset(modes_ctx *ctx) {
     ctx->buffers_done = 0;
     ctx->finished = false;
     ctx->started = false;
+    ctx->feed = modes_ctx::Feed::none;
     ctx->in_total = 0;
     ctx->hold0 = 0;
     ctx->level_q.clear();
@@ -1187,8 +1245,11 @@ int modes_set_input_format(modes_ctx *ctx, uint32_t format, int32_t shift) {
 int modes_process(modes_ctx *ctx, const uint8_t *iq, size_t nbytes) {
     if (!ctx) return -1;
     if (ctx->finished) return fail(ctx, "modes_process after modes_finish; call modes_reset first");
+    if (ctx->feed == modes_ctx::Feed::device)
+        return fail(ctx, "modes_process: a stream fed from device memory is in progress; call modes_finish or modes_reset first");
     CK(ctx, cudaSetDevice(ctx->cfg.device));
     ctx->started = true;
+    ctx->feed = modes_ctx::Feed::host;
     if (held_input(ctx)) return process_held(ctx, iq, nbytes);
     if (ctx->pending_len) {
         size_t take = MODES_BUFFER_BYTES - ctx->pending_len;
@@ -1215,12 +1276,88 @@ int modes_finish(modes_ctx *ctx) {
     if (held_input(ctx)) return finish_held(ctx);
     // The read that hits EOF still hands a 127-padded buffer to the decoder (dump1090.c:496-510);
     // whether it is decoded is the reference's race, made a switch here.
-    memset(ctx->pending.get() + ctx->pending_len, 127, MODES_BUFFER_BYTES - ctx->pending_len);
+    const bool dev = ctx->feed == modes_ctx::Feed::device;
+    if (dev) {
+        if (modes_device_memset(ctx->d_pending.get() + ctx->pending_len, 127, MODES_BUFFER_BYTES - ctx->pending_len))
+            return fail(ctx, "modes_finish: padding the EOF buffer failed: %s", cudaGetErrorString(cudaGetLastError()));
+    } else {
+        memset(ctx->pending.get() + ctx->pending_len, 127, MODES_BUFFER_BYTES - ctx->pending_len);
+    }
     ctx->eof_buffer = ctx->buffers_done;                 // its level record counts the real samples only
     ctx->eof_samples = (uint32_t)((ctx->pending_len + 1) / 2);
     ctx->pending_len = 0;
     if (ctx->cfg.drop_eof_buffer) return 0;
-    return run_buffers(ctx, host_buffers(ctx->pending.get()), 1);
+    return run_buffers(ctx, dev ? device_buffers(ctx->d_pending.get(), ctx->d_carry.get()) : host_buffers(ctx->pending.get()), 1);
+}
+
+// modes_process_device's refusal of memory that is not the context's device memory, naming what it is.
+static int check_device_input(modes_ctx *ctx, const void *p) {
+    cudaPointerAttributes a;
+    const cudaError_t e = cudaPointerGetAttributes(&a, p);
+    if (e != cudaSuccess) {
+        (void)cudaGetLastError();
+        return fail(ctx, "modes_process_device: cudaPointerGetAttributes failed: %s", cudaGetErrorString(e));
+    }
+    const char *what = nullptr;
+    switch (a.type) {
+    case cudaMemoryTypeDevice:
+        if (a.device == ctx->cfg.device) return 0;
+        return fail(ctx, "modes_process_device: the bytes are in memory of device %d, not of the context's device %d",
+                    a.device, ctx->cfg.device);
+    case cudaMemoryTypeManaged: what = "managed memory"; break;
+    case cudaMemoryTypeHost: what = "pinned host memory"; break;
+    default: what = "host memory"; break;
+    }
+    return fail(ctx, "modes_process_device: the bytes are in %s, not in memory of the context's device %d (use modes_process)",
+                what, ctx->cfg.device);
+}
+
+int modes_process_device(modes_ctx *ctx, const void *d_iq, size_t nbytes) {
+    if (!ctx) return -1;
+    if (ctx->finished) return fail(ctx, "modes_process_device after modes_finish; call modes_reset first");
+    if (!d_iq && nbytes) return fail(ctx, "modes_process_device: null pointer with %zu bytes", nbytes);
+    if (ctx->feed == modes_ctx::Feed::host)
+        return fail(ctx, "modes_process_device: a stream fed from host memory is in progress; call modes_finish or "
+                         "modes_reset first");
+    CK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (d_iq && check_device_input(ctx, d_iq)) return -1;
+    const bool first = ctx->feed == modes_ctx::Feed::none;
+    ctx->started = true;
+    ctx->feed = modes_ctx::Feed::device;
+    const uint8_t *iq = static_cast<const uint8_t *>(d_iq);
+    if (held_input(ctx)) return process_held(ctx, iq, nbytes);
+    CK(ctx, ctx->d_pending.ensure(MODES_BUFFER_BYTES));
+    CK(ctx, ctx->d_carry.ensure(MODES_CARRY_BYTES));
+    const cudaStream_t st = ctx->slot[0].stream;
+    if (first) CK(ctx, cudaMemsetAsync(ctx->d_carry.get(), 127, MODES_CARRY_BYTES, st));
+    // as modes_process, with the pending buffer and the carry on the device: the carry of a run's first batch
+    // is d_carry or the pending buffer's tail, of every later one the caller's bytes before it
+    const uint8_t *carry = ctx->d_carry.get();
+    if (ctx->pending_len) {
+        size_t take = MODES_BUFFER_BYTES - ctx->pending_len;
+        if (take > nbytes) take = nbytes;
+        CK(ctx, copy_on_device(ctx, ctx->d_pending.get() + ctx->pending_len, iq, take));
+        ctx->pending_len += take; iq += take; nbytes -= take;
+        CK(ctx, wait_stream(st));
+        if (ctx->pending_len < MODES_BUFFER_BYTES) return 0;
+        if (run_buffers(ctx, device_buffers(ctx->d_pending.get(), carry), 1)) return -1;
+        carry = ctx->d_pending.get() + MODES_BUFFER_BYTES - MODES_CARRY_BYTES;
+        ctx->pending_len = 0;
+    } else if (first) {
+        CK(ctx, wait_stream(st));
+    }
+    const size_t whole = nbytes / MODES_BUFFER_BYTES;
+    if (whole) {
+        if (run_buffers(ctx, device_buffers(iq, carry), whole)) return -1;
+        carry = iq + whole * MODES_BUFFER_BYTES - MODES_CARRY_BYTES;
+    }
+    iq += whole * MODES_BUFFER_BYTES; nbytes -= whole * MODES_BUFFER_BYTES;
+    // the next call's carry, then its partial buffer (on one stream: in that order)
+    if (carry != ctx->d_carry.get()) CK(ctx, copy_on_device(ctx, ctx->d_carry.get(), carry, MODES_CARRY_BYTES));
+    CK(ctx, copy_on_device(ctx, ctx->d_pending.get(), iq, nbytes));
+    ctx->pending_len = nbytes;
+    CK(ctx, wait_stream(st));
+    return 0;
 }
 
 int modes_get_stats(const modes_ctx *ctx, modes_stats *out) {

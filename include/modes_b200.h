@@ -169,6 +169,24 @@ size_t modes_output_count(const modes_ctx *ctx);
 /* Feed the next `nbytes` of the u8 I/Q stream (host memory, pinned or not).
  * Whole reference buffers are decoded as they complete.  0 = ok, <0 = error. */
 int  modes_process(modes_ctx *ctx, const uint8_t *iq, size_t nbytes);
+/* modes_process for bytes in device memory of the context's device (cfg.device): a CUDA SDR front end, a
+ * torch pipeline or a capture read into GPU memory feeds the decoder without a copy through the host.
+ *   Same output: a sequence of calls, then modes_finish, gives exactly what modes_process gives on the same
+ *     bytes in the same call sizes: messages and every field, sample_pos, statistics, level, spectrum,
+ *     recovery and weak records, signal and arrival codes, both drop_eof_buffer outcomes; at every input
+ *     rate, format, offset and modes_set_* switch, with gpu_resolve and with n_gpus > 1 (whose other GPUs
+ *     receive their batches from cfg.device's memory, peer to peer where the driver allows).
+ *   Any pointer alignment and any byte count, odd counts and calls that split a buffer or a sample included.
+ *   The bytes must be fully written before the call: it does not order itself after the caller's streams.
+ *     When it returns, the decoder no longer reads d_iq, as modes_process returns with every copy done.
+ *   One kind of memory per stream: from its first call until modes_finish / modes_reset a stream is fed
+ *     either by modes_process or by modes_process_device; the other is refused with "in progress".
+ *     modes_finish ends either.
+ *   Refused: d_iq NULL with nbytes > 0, and memory that cudaPointerGetAttributes does not report as device
+ *     memory of cfg.device (host, pinned, managed, or another device's), with a message naming it.
+ * The stream's partial buffer, carry and input history then live on the device too; a stream fed from the
+ * host allocates none of them. */
+int  modes_process_device(modes_ctx *ctx, const void *d_iq, size_t nbytes);
 /* End of stream: 127-pad and decode (or drop) the EOF buffer (dump1090.c:496-507). */
 int  modes_finish(modes_ctx *ctx);
 /* Forget stream position, carry, ICAO cache and statistics (a new --ifile run). */
