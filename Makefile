@@ -11,11 +11,11 @@ OBJS      := build/modes_kernels.o build/modes_scan2.o build/modes_eval_fused.o 
 
 all: $(LIB) dump1090-b200
 
-build/%.o: $(CSRC)/%.cu $(CSRC)/modes_internal.h $(CSRC)/modes_eval_serial.cuh $(CSRC)/modes_scan_core.cuh $(CSRC)/modes_resolve_core.cuh $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_arrival_core.cuh $(CSRC)/modes_levels_core.cuh $(CSRC)/modes_recover_core.cuh $(CSRC)/modes_weak_core.cuh $(CSRC)/modes_resample_core.cuh $(CSRC)/modes_input_core.cuh $(CSRC)/modes_spectrum_core.cuh $(CSRC)/modes_stage.cuh include/modes_b200.h
+build/%.o: $(CSRC)/%.cu $(CSRC)/modes_internal.h $(CSRC)/modes_eval_serial.cuh $(CSRC)/modes_scan_core.cuh $(CSRC)/modes_resolve_core.cuh $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_arrival_core.cuh $(CSRC)/modes_carrier_core.cuh $(CSRC)/modes_levels_core.cuh $(CSRC)/modes_recover_core.cuh $(CSRC)/modes_weak_core.cuh $(CSRC)/modes_resample_core.cuh $(CSRC)/modes_input_core.cuh $(CSRC)/modes_spectrum_core.cuh $(CSRC)/modes_stage.cuh include/modes_b200.h
 	@mkdir -p build
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@
 
-build/%.o: $(CSRC)/%.cpp $(CSRC)/modes_internal.h $(CSRC)/modes_input_core.cuh $(CSRC)/modes_resample_core.cuh $(CSRC)/modes_spectrum_core.cuh include/modes_b200.h
+build/%.o: $(CSRC)/%.cpp $(CSRC)/modes_internal.h $(CSRC)/modes_carrier_core.cuh $(CSRC)/modes_input_core.cuh $(CSRC)/modes_resample_core.cuh $(CSRC)/modes_spectrum_core.cuh include/modes_b200.h
 	@mkdir -p build
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 
@@ -30,7 +30,10 @@ oracle:
 	if [ -d /root/reference ]; then $(MAKE) -C oracle ref; fi
 
 # test infrastructure: host build of the per-candidate evaluation (logic checked against the oracle on CPU)
-shim: tests/_build/libeval_serial_host.so tests/_build/libscan_core_host.so tests/_build/libresolve_core_host.so tests/_build/libsignal_core_host.so tests/_build/liblevels_core_host.so tests/_build/librecover_core_host.so tests/_build/libweak_core_host.so tests/_build/libarrival_core_host.so tests/_build/libresample_core_host.so tests/_build/libinput_core_host.so tests/_build/libpool_carry_host.so tests/_build/libdecimate_core_host.so tests/_build/libshift_core_host.so tests/_build/libspectrum_core_host.so
+shim: tests/_build/libeval_serial_host.so tests/_build/libscan_core_host.so tests/_build/libresolve_core_host.so tests/_build/libsignal_core_host.so tests/_build/liblevels_core_host.so tests/_build/librecover_core_host.so tests/_build/libweak_core_host.so tests/_build/libarrival_core_host.so tests/_build/libresample_core_host.so tests/_build/libinput_core_host.so tests/_build/libpool_carry_host.so tests/_build/libdecimate_core_host.so tests/_build/libshift_core_host.so tests/_build/libspectrum_core_host.so tests/_build/libcarrier_core_host.so
+tests/_build/libcarrier_core_host.so: tests/host_shim/carrier_core_host.cpp $(CSRC)/modes_carrier_core.cuh $(CSRC)/modes_arrival_core.cuh
+	@mkdir -p tests/_build
+	g++ -O2 -std=c++17 -shared -fPIC -Wall -Wno-unknown-pragmas -x c++ -I$(CSRC) tests/host_shim/carrier_core_host.cpp -o $@
 tests/_build/libspectrum_core_host.so: tests/host_shim/spectrum_core_host.cpp $(CSRC)/modes_spectrum_core.cuh $(CSRC)/modes_resample_core.cuh include/modes_b200.h
 	@mkdir -p tests/_build
 	g++ -O2 -std=c++17 -shared -fPIC -Wall -Wno-unknown-pragmas -x c++ -Iinclude -I$(CSRC) tests/host_shim/spectrum_core_host.cpp -o $@
@@ -83,7 +86,7 @@ tests/_build/libeval_serial_host.so: tests/host_shim/eval_serial_host.cpp $(CSRC
 # test infrastructure: device harness over the product's own kernel objects (recovery and signal
 # passes on constructed corpora, and the exhaustive sweeps of the core headers' device build)
 DSHIM_OBJS := build/modes_recover.o build/modes_signal.o build/modes_levels.o build/modes_tables.o
-dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so tests/_build/libscan_eval_device.so tests/_build/libresample_pool_device.so tests/_build/libresolve_device.so tests/_build/libinput_device.so tests/_build/libconvert_pool_device.so tests/_build/librate_spectrum_device.so
+dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so tests/_build/libscan_eval_device.so tests/_build/libresample_pool_device.so tests/_build/libresolve_device.so tests/_build/libinput_device.so tests/_build/libconvert_pool_device.so tests/_build/librate_spectrum_device.so tests/_build/libcarrier_device.so
 tests/_build/libkernels_device.so: tests/device_shim/kernels_device.cu $(DSHIM_OBJS) $(CSRC)/modes_internal.h $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_levels_core.cuh include/modes_b200.h
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/kernels_device.cu -o tests/_build/kernels_device.o
@@ -93,6 +96,11 @@ tests/_build/libarrival_device.so: tests/device_shim/arrival_device.cu build/mod
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/arrival_device.cu -o tests/_build/arrival_device.o
 	$(NVCC) $(ARCH) -shared -o $@ tests/_build/arrival_device.o build/modes_signal.o build/modes_tables.o -cudart static
+# the carrier measurement of the signal pass on constructed corpora (tests/test_carrier.py)
+tests/_build/libcarrier_device.so: tests/device_shim/carrier_device.cu build/modes_signal.o build/modes_tables.o $(CSRC)/modes_internal.h include/modes_b200.h
+	@mkdir -p tests/_build
+	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/carrier_device.cu -o tests/_build/carrier_device.o
+	$(NVCC) $(ARCH) -shared -o $@ tests/_build/carrier_device.o build/modes_signal.o build/modes_tables.o -cudart static
 # the scan, frame-evaluation and weak-preamble kernels with a chosen SM count (tests/test_persistent_kernels.py)
 SCAN_EVAL_OBJS := build/modes_scan2.o build/modes_eval_fused.o build/modes_kernels.o build/modes_weak.o build/modes_tables.o
 tests/_build/libscan_eval_device.so: tests/device_shim/scan_eval_device.cu $(SCAN_EVAL_OBJS) $(CSRC)/modes_internal.h include/modes_b200.h

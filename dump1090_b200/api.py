@@ -81,6 +81,19 @@ class Message(C.Structure):
         ticks = 6 * int(self.sample_pos) + (int(self.arrival) - 8 if self.arrival else 0)
         return 0 if ticks < 0 else ticks % (1 << 48)
 
+    @property
+    def carrier_code(self) -> int:
+        """modes_message.carrier (bytes 106-107, the end of pad1): 0 = not measured, otherwise
+        16384 + round(f / 100 Hz) for the frame's carrier f relative to the centre of the 2 MHz bytes
+        (modes_set_carrier)."""
+        return C.c_int16.from_address(C.addressof(self) + CARRIER_OFFSET).value
+
+    def carrier_hz(self):
+        """The frame's carrier frequency in Hz above the centre of the 2 MHz bytes the scan read (a
+        multiple of 100 Hz within +-500 kHz), or None when it was not measured."""
+        code = self.carrier_code
+        return None if code == 0 else (code - CARRIER_CODE_ZERO) * CARRIER_STEP_HZ
+
     def beast(self) -> bytes:
         """The Beast binary frame of this message (modes_format_beast); its timestamp is
         timestamp_12mhz()."""
@@ -92,6 +105,12 @@ class Message(C.Structure):
         m = Message()
         C.memmove(C.byref(m), C.byref(self), C.sizeof(Message))
         return m
+
+
+CARRIER_OFFSET = 106                      # offsetof(modes_message, carrier): the last two bytes of pad1
+CARRIER_CODE_ZERO = 16384                 # the carrier code of 0 Hz
+CARRIER_STEP_HZ = 100                     # Hz per carrier code
+assert C.sizeof(Message) == 200 and Message.pad1.offset == CARRIER_OFFSET - 1
 
 
 class FrameEval(C.Structure):
@@ -220,6 +239,31 @@ def spectrum_summary(records, input_rate: int) -> dict:
     return out
 
 
+def carrier_summary(messages) -> dict:
+    """What the carrier frequencies of delivered messages (Message.carrier_hz(), modes_set_carrier) say
+    about a receiver: the messages measured, the aircraft measured (distinct addresses aa1..aa3 among
+    them), each aircraft's median offset in Hz (`per_aircraft`, keyed by the 24-bit address), and the
+    receiver's estimate: the median over aircraft of their medians, in Hz (`receiver_hz`) and in ppm of
+    1090 MHz (`receiver_ppm`; positive: frames arrive above the centre of the receiver's 2 MHz bytes, so
+    its tuning is low).  Transponders scatter around 1090 MHz, so one aircraft says little; the median over
+    many is the receiver's own offset.  With no measured message the estimates are None."""
+    by_addr: dict[int, list[float]] = {}
+    n = 0
+    for m in messages:
+        hz = m.carrier_hz()
+        if hz is None:
+            continue
+        n += 1
+        addr = (int(m.aa1) << 16) | (int(m.aa2) << 8) | int(m.aa3)
+        by_addr.setdefault(addr, []).append(hz)
+    per = {a: float(np.median(v)) for a, v in sorted(by_addr.items())}
+    out = dict(messages=n, aircraft=len(per), per_aircraft=per, receiver_hz=None, receiver_ppm=None)
+    if per:
+        out["receiver_hz"] = float(np.median(list(per.values())))
+        out["receiver_ppm"] = out["receiver_hz"] / 1090.0
+    return out
+
+
 _lib = None
 
 # every symbol include/modes_b200.h declares
@@ -248,7 +292,7 @@ EXPORTS = ["modes_abi_version", "modes_default_config", "modes_create", "modes_d
            "modes_set_input_rate", "modes_resample_device", "modes_pool_set_input_rate", "modes_set_input_format",
            "modes_pool_set_input_format", "modes_resample_device_at", "modes_set_input_offset",
            "modes_resample_device_shift", "modes_set_spectrum", "modes_take_spectra", "modes_pool_set_spectrum",
-           "modes_pool_take_spectra", "modes_process_device"]
+           "modes_pool_take_spectra", "modes_process_device", "modes_set_carrier", "modes_pool_set_carrier"]
 
 INPUT_RATES = (2_000_000, 2_400_000, 4_000_000, 6_000_000, 8_000_000, 10_000_000)      # modes_set_input_rate
 INPUT_FORMATS = {"uc8": 0, "sc16": 1, "sc16q11": 2}     # modes_set_input_format: MODES_INPUT_*
@@ -360,6 +404,8 @@ def lib():
         L.modes_pool_set_signal.argtypes = [C.c_void_p, C.c_int]
         L.modes_set_arrival.argtypes = [C.c_void_p, C.c_int]
         L.modes_pool_set_arrival.argtypes = [C.c_void_p, C.c_int]
+        L.modes_set_carrier.argtypes = [C.c_void_p, C.c_int]
+        L.modes_pool_set_carrier.argtypes = [C.c_void_p, C.c_int]
         L.modes_format_beast.restype = C.c_size_t
         L.modes_format_beast.argtypes = [C.POINTER(Message), C.c_void_p, C.c_size_t]
         L.modes_set_levels.argtypes = [C.c_void_p, C.c_int]
@@ -515,13 +561,17 @@ class Decoder:
     nothing.
     spectrum=True measures every decoded buffer's input power spectrum on the GPU, before resampling,
     decimation and the offset (modes_set_spectrum): take_spectra(), spectrum_summary().
+    carrier=True measures every decoded frame's carrier frequency relative to the centre of the 2 MHz bytes
+    on the GPU (modes_set_carrier): Message.carrier_code, carrier_hz(), carrier_summary().  It cannot be
+    combined with gpu_resolve.
     process() and decode() also take a CUDA torch tensor of any dtype on the decoder's device, read as its
     raw bytes (e.g. int16 SC16 I/Q), and decode it where it is (modes_process_device): the output is what
     the same bytes give from host memory, without their two trips across PCIe."""
 
     def __init__(self, signal: bool = False, levels: bool = False, recover: bool = False, weak_preambles: bool = False,
                  arrival: bool = False, input_rate: int = 2_000_000, input_format: str = "uc8",
-                 input_shift: int | None = None, input_offset: int = 0, spectrum: bool = False, **cfg):
+                 input_shift: int | None = None, input_offset: int = 0, spectrum: bool = False, carrier: bool = False,
+                 **cfg):
         self.cfg = make_config(**cfg)
         self._h = lib().modes_create(C.byref(self.cfg))
         if not self._h:
@@ -540,6 +590,8 @@ class Decoder:
             self.set_levels(True)
         if spectrum:
             self.set_spectrum(True)
+        if carrier:
+            self.set_carrier(True)
         if recover:
             self.set_recovery(True)
         if weak_preambles:
@@ -677,6 +729,10 @@ class Decoder:
     def set_arrival(self, on: bool) -> None:
         """Measure the arrival time for batches submitted from now on (modes_set_arrival)."""
         self._check(lib().modes_set_arrival(self._h, int(bool(on))))
+
+    def set_carrier(self, on: bool) -> None:
+        """Measure the carrier frequency for batches submitted from now on (modes_set_carrier)."""
+        self._check(lib().modes_set_carrier(self._h, int(bool(on))))
 
     def set_levels(self, on: bool) -> None:
         """Measure the buffers' levels for batches submitted from now on (modes_set_levels)."""
@@ -1054,7 +1110,8 @@ class ReceiverPool:
     levels=True: level records of every receiver's buffers (`take_levels(receiver)`).
     spectrum=True: input spectrum records of every receiver's buffers (`take_spectra(receiver)`).
     recover=True: as for Decoder, with statistics per receiver (`recovery_stats(receiver)`).
-    weak_preambles=True: as for Decoder (`weak_recovery_stats(receiver)`).  arrival=True: as for Decoder.
+    weak_preambles=True: as for Decoder (`weak_recovery_stats(receiver)`).  arrival=True, carrier=True: as
+    for Decoder.
     input_rate=2_400_000 sets every receiver to 2.4 MS/s at creation, set_input_rate(receiver, hz) one
     receiver (modes_pool_set_input_rate): a buffer is still BUFFER_BYTES of the receiver's stream, and its
     2 MHz buffers are decoded as their input completes (`buffers(receiver)` counts them).
@@ -1067,7 +1124,7 @@ class ReceiverPool:
     def __init__(self, n_receivers: int, max_batch: int = 0, signal: bool = False, levels: bool = False,
                  recover: bool = False, weak_preambles: bool = False, arrival: bool = False,
                  input_rate: int = 2_000_000, input_format: str = "uc8", input_shift: int | None = None,
-                 spectrum: bool = False, **cfg):
+                 spectrum: bool = False, carrier: bool = False, **cfg):
         self.cfg = make_config(**cfg)
         self.n = n_receivers
         self._bytes = [BUFFER_BYTES] * n_receivers
@@ -1082,6 +1139,8 @@ class ReceiverPool:
             self.set_levels(True)
         if spectrum:
             self.set_spectrum(True)
+        if carrier:
+            self.set_carrier(True)
         if recover:
             self.set_recovery(True)
         if weak_preambles:
@@ -1177,6 +1236,10 @@ class ReceiverPool:
     def set_arrival(self, on: bool) -> None:
         """Measure the arrival time for batches submitted from now on (modes_pool_set_arrival)."""
         self._check(lib().modes_pool_set_arrival(self._h, int(bool(on))))
+
+    def set_carrier(self, on: bool) -> None:
+        """Measure the carrier frequency for batches submitted from now on (modes_pool_set_carrier)."""
+        self._check(lib().modes_pool_set_carrier(self._h, int(bool(on))))
 
     def set_levels(self, on: bool) -> None:
         """Measure the levels of batches submitted from now on (modes_pool_set_levels)."""

@@ -70,6 +70,9 @@ struct Slot {
     // modes_set_recovery / modes_recover_device: one record per candidate (device, and its pinned host copy)
     DevBuf<modes_recovered> d_recovered;
     PinnedBuf<modes_recovered> h_recovered;
+    // modes_set_carrier: one record per candidate (device, and its pinned host copy)
+    DevBuf<modes_carrier> d_carrier;
+    PinnedBuf<modes_carrier> h_carrier;
     // modes_set_weak_preambles / modes_weak_device: the weak positions and their records (device), the
     // scan's unordered scratch list (its capacity is the slot's weak capacity), its per-tile words
     // (source, count and destination of every tile's block) and counters, and pinned host copies
@@ -437,7 +440,9 @@ int launch_batch(modes_ctx *ctx, Slot &s) {
     if (pe) CK(ctx, cudaEventRecord(pe[2], s.stream));
     // after pe[2]: the kernel times keep their meaning; before the device resolve, which copies the field
     const Features &f = s.feat;
-    if (f.signal || f.arrival) launch_signal(in, ctx->tab, so, s.out_records, ctx->sm_count, s.stream, f.signal, f.arrival);
+    if (f.carrier) CK(ctx, s.d_carrier.ensure(s.out_cap));
+    if (f.signal || f.arrival || f.carrier)
+        launch_signal(in, ctx->tab, so, s.out_records, ctx->sm_count, s.stream, f.signal, f.arrival, f.carrier ? s.d_carrier.get() : nullptr);
     // the buffers' own bytes (the body, not the carry block); one writer per record, so a repeated
     // batch writes the same records
     if (f.levels)
@@ -449,7 +454,7 @@ int launch_batch(modes_ctx *ctx, Slot &s) {
                         s.d_spectra.get(), s.stream);
     }
     CK(ctx, cudaGetLastError());
-    ctx->launches += (f.signal || f.arrival ? 3 : 2) + (f.levels ? 1 : 0) + (f.spectrum ? 1 : 0);
+    ctx->launches += (f.signal || f.arrival || f.carrier ? 3 : 2) + (f.levels ? 1 : 0) + (f.spectrum ? 1 : 0);
     if (f.recover && launch_recovery(ctx, s, in, so)) return -1;
     if (f.weak && launch_weak(ctx, s, in)) return -1;
     if (ctx->cfg.gpu_resolve && s.own_outputs && &s != &ctx->detect) {
@@ -514,6 +519,7 @@ struct ShardView {
     int64_t buffer_base = 0;
     const modes_recovered *recovered = nullptr;   // the batch ran no recovery: nullptr
     WeakList weak;
+    const modes_carrier *carrier = nullptr;       // the batch measured no carrier: nullptr
 };
 
 // Queue the copies of the slot's finished batch (n candidate records) to pinned memory on its
@@ -538,8 +544,13 @@ int fetch_async(modes_ctx *ctx, Slot &s, uint64_t n, ShardView &v) {
         }
         wl = WeakList{s.h_weak_pos.get(), s.h_weak_rec.get(), nw};
     }
+    if (s.feat.carrier) {
+        CK(ctx, ensure_spare(s.h_carrier, n));
+        if (n) CK(ctx, cudaMemcpyAsync(s.h_carrier.get(), s.d_carrier.get(), n * sizeof(modes_carrier), cudaMemcpyDeviceToHost, s.stream));
+    }
     CK(ctx, cudaMemcpyAsync(s.h_tiles.get(), s.out_tiles, nt * sizeof(modes_tile), cudaMemcpyDeviceToHost, s.stream));
-    v = ShardView{s.h_records.get(), s.h_tiles.get(), nt, s.buffer_base, s.feat.recover ? s.h_recovered.get() : nullptr, wl};
+    v = ShardView{s.h_records.get(), s.h_tiles.get(), nt, s.buffer_base, s.feat.recover ? s.h_recovered.get() : nullptr, wl,
+                  s.feat.carrier ? s.h_carrier.get() : nullptr};
     return 0;
 }
 
@@ -582,7 +593,8 @@ int collect(modes_ctx *ctx, Slot &s) {
     CK(ctx, wait_stream(s.stream));
     const double t2 = dbg ? now_ms() : 0;
     ResolveConfig rc{ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->cfg.check_crc, s.feat.signal ? 1 : 0};
-    resolve_candidates(ctx->rs, rc, v.cands, v.tiles, v.n_tiles, v.buffer_base, ctx->out, ctx->scratch, v.recovered, v.weak);
+    resolve_candidates(ctx->rs, rc, v.cands, v.tiles, v.n_tiles, v.buffer_base, ctx->out, ctx->scratch, v.recovered, v.weak,
+                       v.carrier);
     if (dbg) fprintf(stderr, "[collect] %zu buffers, %llu cands: wait %.3f ms, d2h %.3f ms, resolve %.3f ms (t=%.3f)\n",
                      s.n_buffers, (unsigned long long)n, t1 - t0, t2 - t1, now_ms() - t2, now_ms());
     return 0;
@@ -600,7 +612,8 @@ int collect_group(modes_ctx *ctx, int parity) {
     std::vector<int64_t> base(n);
     std::vector<const modes_recovered *> recovered(n, nullptr);
     std::vector<WeakList> weak(n);
-    bool any_recover = false, signal = false;
+    std::vector<const modes_carrier *> carrier(n, nullptr);
+    bool any_recover = false, signal = false, any_carrier = false;
     for (size_t k = 0; k < n; k++) {
         modes_ctx *g = ctx->gpus[k];
         Slot &s = g->slot[parity];
@@ -614,8 +627,9 @@ int collect_group(modes_ctx *ctx, int parity) {
         ShardView v;
         if (fetch_async(g, s, nc, v)) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
         cands[k] = v.cands; tiles[k] = v.tiles; n_tiles[k] = v.n_tiles; base[k] = v.buffer_base;
-        recovered[k] = v.recovered; weak[k] = v.weak;
+        recovered[k] = v.recovered; weak[k] = v.weak; carrier[k] = v.carrier;
         any_recover |= s.feat.recover;
+        any_carrier |= s.feat.carrier;
         signal = s.feat.signal;
     }
     for (size_t k = 0; k < n; k++) {
@@ -626,8 +640,11 @@ int collect_group(modes_ctx *ctx, int parity) {
     if (any_recover)   // the switch is the same on every GPU of a group: all or none of the shards have records
         for (size_t k = 0; k < n; k++)
             if (!recovered[k]) return fail(ctx, "internal: recovery records missing for GPU %d", ctx->gpus[k]->cfg.device);
+    if (any_carrier)   // likewise
+        for (size_t k = 0; k < n; k++)
+            if (!carrier[k]) return fail(ctx, "internal: carrier records missing for GPU %d", ctx->gpus[k]->cfg.device);
     resolve_shards(ctx->rs, rc, n, cands.data(), tiles.data(), n_tiles.data(), base.data(), ctx->out, ctx->scratch,
-                   any_recover ? recovered.data() : nullptr, weak.data());
+                   any_recover ? recovered.data() : nullptr, weak.data(), any_carrier ? carrier.data() : nullptr);
     return 0;
 }
 
@@ -1005,6 +1022,12 @@ int modes_set_arrival(modes_ctx *ctx, int on) { return set_feature(ctx, &Feature
 
 int modes_set_levels(modes_ctx *ctx, int on) { return set_feature(ctx, &Features::levels, on); }
 
+int modes_set_carrier(modes_ctx *ctx, int on) {
+    // the device resolve's 40-byte delivery records have no room for the carrier
+    if (ctx && on && ctx->cfg.gpu_resolve) return fail(ctx, "modes_set_carrier: carrier measurement cannot be combined with gpu_resolve");
+    return set_feature(ctx, &Features::carrier, on);
+}
+
 size_t modes_take_levels(modes_ctx *ctx, modes_level *out, size_t cap) { return ctx ? ctx->level_q.take(out, cap) : 0; }
 
 int modes_set_spectrum(modes_ctx *ctx, int on) { return set_feature(ctx, &Features::spectrum, on); }
@@ -1130,6 +1153,23 @@ int modes_recover_device(modes_ctx *ctx, void *d_out, size_t capacity) {
     ScanOutputs so{s.d_cand_v.get(), s.out_cap, s.out_tiles, s.counters()};
     return launch_recovery(ctx, s, in, so);
 }
+
+}  // extern "C"
+
+int modes::carrier_fetch(modes_ctx *ctx, modes_carrier *out) {
+    if (!ctx) return -1;
+    Slot &s = ctx->detect;
+    if (!s.feat.carrier) return fail(ctx, "carrier records without modes_set_carrier");
+    if (!out) return fail(ctx, "carrier records: no output array");
+    CK(ctx, cudaSetDevice(ctx->cfg.device));
+    uint64_t n = 0;
+    if (wait_batch(ctx, s, &n)) return -1;
+    if (n) CK(ctx, cudaMemcpyAsync(out, s.d_carrier.get(), n * sizeof(modes_carrier), cudaMemcpyDeviceToHost, s.stream));
+    CK(ctx, wait_stream(s.stream));
+    return 0;
+}
+
+extern "C" {
 
 int modes_recover_fetch(modes_ctx *ctx, modes_recovered *out) {
     if (!ctx) return -1;
@@ -1490,7 +1530,14 @@ struct modes_resolver {
     ResolveState rs; ResolveConfig rc; MessageOut out; ResolveScratch *scratch = nullptr;
     ResolveState tentative;             // end state of the last modes_resolver_run_tentative
     bool has_tentative = false;
+    const modes_carrier *carrier = nullptr;   // the next modes_resolver_run_weak's carrier records (modes::resolver_set_carrier)
 };
+
+}  // extern "C"
+
+void modes::resolver_set_carrier(modes_resolver *r, const modes_carrier *carrier) { if (r) r->carrier = carrier; }
+
+extern "C" {
 
 modes_resolver *modes_resolver_create(const modes_config *cfg) {
     modes_resolver *r = new (std::nothrow) modes_resolver();
@@ -1547,8 +1594,10 @@ int modes_resolver_run_weak(modes_resolver *r, const modes_candidate *candidates
     for (size_t k = 1; k < n_weak; k++)
         if (weak_t[k] <= weak_t[k - 1]) return -1;                   // stream order, each position once
     r->out.sink = sink; r->out.user = user;
+    const modes_carrier *carrier = r->carrier;
+    r->carrier = nullptr;
     resolve_candidates(r->rs, r->rc, candidates, tiles, n_tiles, buffer_base, r->out, r->scratch, recovered,
-                       WeakList{weak_t, weak_rec, n_weak});
+                       WeakList{weak_t, weak_rec, n_weak}, carrier);
     return 0;
 }
 

@@ -85,11 +85,14 @@ void launch_magnitude(const uint8_t *d_iq, uint16_t *d_mag, uint64_t n_samples, 
 // CRC / fix on raw frame bytes (hex door): n frames of 14 bytes -> n modes_frame_eval.
 void launch_eval_frames(const uint8_t *d_frames, modes_frame_eval *d_out, uint32_t n, const DeviceTables &tab,
                         int fix_errors, int aggressive, cudaStream_t stream);
-// Signal level and arrival code of every decoded attempt (modes_signal.cu): writes pass[k].signal
-// (signal) and bits 4-7 of pass[k].flags (arrival) of the first min(counters[0], cand_capacity)
-// records over the same windows the scan and frame evaluation read.  Launches nothing when both are off.
+// Signal level, arrival code and carrier record of every decoded attempt (modes_signal.cu): writes
+// pass[k].signal (signal), bits 4-7 of pass[k].flags (arrival) and carrier[i] (carrier != nullptr: the
+// record of every candidate i with a decoded attempt) of the first min(counters[0], cand_capacity)
+// records over the same windows the scan and frame evaluation read.  Launches nothing when all are off.
 void launch_signal(const BatchView &in, const DeviceTables &tab, const ScanOutputs &scan, modes_candidate *records,
-                   int sm_count, cudaStream_t stream, bool signal = true, bool arrival = false);
+                   int sm_count, cudaStream_t stream, bool signal = true, bool arrival = false,
+                   modes_carrier *carrier = nullptr);
+static_assert(sizeof(modes_carrier) == 16, "carrier record layout");
 // Levels of n_buffers whole buffers at d_iq + k * stride_bytes (modes_levels.cu): writes out[k],
 // k < n_buffers, with buffer = k and n_samples = kBufSamples.
 void launch_levels(const uint8_t *d_iq, uint32_t n_buffers, uint64_t stride_bytes, const DeviceTables &tab,
@@ -205,13 +208,20 @@ void launch_weak_scan(const BatchView &in, const DeviceTables &tab, const WeakOu
 // search as launch_recover's).
 void launch_recover_weak(const BatchView &in, const DeviceTables &tab, const uint32_t *count, uint32_t capacity,
                          uint32_t scratch_cap, const uint32_t *pos, modes_recovered *out, int sm_count, cudaStream_t stream);
+// The carrier records of the last modes_detect_device batch (the receiver pool's slot contexts measure
+// them with modes_set_carrier): one per candidate, as many as modes_detect_fetch copies.
+int carrier_fetch(modes_ctx *ctx, modes_carrier *out);
+// The carrier records of the candidates of the resolver's next modes_resolver_run_weak call (nullptr: not
+// measured); the call clears them.
+void resolver_set_carrier(modes_resolver *r, const modes_carrier *carrier);
 // modes_weak_device over the buffers first_buffer + i * buffer_step of the last batch only (the
 // receiver pool: its data buffers, never its pad buffers); modes_weak_device is (0, 1).
 int weak_device_strided(modes_ctx *ctx, void *d_pos, void *d_rec, size_t capacity, uint32_t first_buffer, uint32_t buffer_step);
 static_assert(sizeof(modes_recovered) == 20 && offsetof(modes_recovered, status) == 14 && offsetof(modes_recovered, signal) == 16,
               "recovery record layout");
 static_assert(offsetof(modes_message, recovered) == 14 && offsetof(modes_message, arrival) == 15 &&
-              offsetof(modes_message, msgbits) == 16, "message layout");
+              offsetof(modes_message, msgbits) == 16 && offsetof(modes_message, carrier) == 106 &&
+              offsetof(modes_message, ew_dir) == 108 && sizeof(modes_message) == 200, "message layout");
 
 // The record layouts are ABI: the signal field took the two bytes every evaluation kernel already wrote as zero.
 static_assert(sizeof(modes_frame_eval) == 24 && offsetof(modes_frame_eval, signal) == 18 && offsetof(modes_frame_eval, crc) == 20,
@@ -282,14 +292,16 @@ void scratch_destroy(ResolveScratch *s);
 struct WeakList { const uint32_t *t = nullptr; const modes_recovered *rec = nullptr; size_t n = 0; };
 
 // recovered: one record per candidate (modes_recover.cu), or nullptr with recovery off; weak: the
-// weak positions merged into the walk (only with recovered)
+// weak positions merged into the walk (only with recovered); carrier: one carrier record per candidate
+// (modes_signal.cu), or nullptr with carrier measurement off
 void resolve_candidates(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands,
                         const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, MessageOut &out,
-                        ResolveScratch *scratch, const modes_recovered *recovered = nullptr, const WeakList &weak = WeakList());
+                        ResolveScratch *scratch, const modes_recovered *recovered = nullptr, const WeakList &weak = WeakList(),
+                        const modes_carrier *carrier = nullptr);
 void resolve_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards, const modes_candidate *const *cands,
                     const modes_tile *const *tiles, const size_t *n_tiles, const int64_t *buffer_base,
                     MessageOut &out, ResolveScratch *scratch, const modes_recovered *const *recovered = nullptr,
-                    const WeakList *weak = nullptr);
+                    const WeakList *weak = nullptr, const modes_carrier *const *carrier = nullptr);
 // A shard resolved from a GUESSED address cache (one rank / one GPU thread of a sharded decode):
 // verdicts only, deliveries held back in the scratch until the guess is verified.
 void resolve_tentative(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands, const modes_tile *tiles,
@@ -341,7 +353,7 @@ template <typename T> using DevBuf = CudaBuf<T, false>;
 template <typename T> using PinnedBuf = CudaBuf<T, true>;
 
 // The optional measurements and searches of a decode (modes_set_* / modes_pool_set_*).
-struct Features { bool signal = false, arrival = false, levels = false, recover = false, weak = false, spectrum = false; };
+struct Features { bool signal = false, arrival = false, levels = false, recover = false, weak = false, spectrum = false, carrier = false; };
 
 // Level or spectrum records not taken yet, oldest first.
 template <typename T>

@@ -176,7 +176,7 @@ struct modes_pool {
     modes_config cfg;
     std::vector<Receiver> rx;
     size_t max_batch = 0;
-    // signal and arrival are measured by the slot contexts' own passes and reach them at once;
+    // signal, arrival and carrier are measured by the slot contexts' own passes and reach them at once;
     // recovery, weak preambles and levels are run by the pool per batch, as they were at submit
     modes::Features feat;
     std::string err;
@@ -214,6 +214,7 @@ struct modes_pool {
     unsigned submitted = 0, collected = 0;     // batches so far: slot = number & 1
     std::vector<modes_candidate> cands;
     std::vector<modes_recovered> recovered;    // with recovery: one record per candidate
+    std::vector<modes_carrier> carrier;        // with carrier measurement: one record per candidate
     std::vector<uint32_t> weak_t;              // with weak preambles: the batch's weak positions and records
     std::vector<modes_recovered> weak_rec;
     std::vector<modes_tile> tiles;
@@ -221,6 +222,7 @@ struct modes_pool {
     struct Block {
         std::vector<modes_candidate> local;    // one receiver's records, re-based to its buffer
         std::vector<modes_recovered> local_rec;   // and their recovery records
+        std::vector<modes_carrier> local_car;     // and their carrier records
         std::vector<uint32_t> local_wt;        // the receiver's weak positions, re-based, and their records
         std::vector<modes_recovered> local_wrec;
         std::vector<modes_tile> local_tiles;
@@ -270,6 +272,7 @@ size_t pool_threads() {
 void share_features(const modes_pool *p, modes_ctx *ctx) {
     modes_set_signal(ctx, p->feat.signal);
     modes_set_arrival(ctx, p->feat.arrival);
+    modes_set_carrier(ctx, p->feat.carrier);
 }
 
 // One switch of the pool.
@@ -408,11 +411,12 @@ void modes_pool_destroy(modes_pool *p) {
 const char *modes_pool_last_error(const modes_pool *p) { return p ? p->err.c_str() : "no pool"; }
 
 // The per-receiver resolve; recovered: the batch's recovery records (nullptr: off), whose signal the
-// messages carry only when the batch measured signals; weak_t / weak_rec / n_weak: its weak positions.
+// messages carry only when the batch measured signals; weak_t / weak_rec / n_weak: its weak positions;
+// carrier: the batch's carrier records (nullptr: off).
 static int pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, const modes_candidate *candidates,
                         const modes_recovered *recovered, bool signal, const modes_tile *tiles, modes_pool_sink_fn sink,
                         void *user, const uint32_t *weak_t = nullptr, const modes_recovered *weak_rec = nullptr,
-                        size_t n_weak = 0) {
+                        size_t n_weak = 0, const modes_carrier *carrier = nullptr) {
     if (!p) return -1;
     if (check_ids(p, receivers, n)) return -1;
     if (!n) return 0;
@@ -456,6 +460,7 @@ static int pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, cons
             tile_range(i, g0, g1);
             bl.local.clear();
             bl.local_rec.clear();
+            bl.local_car.clear();
             for (modes_tile &lt : bl.local_tiles) { lt.offset = 0; lt.count = 0; }
             for (size_t g = g0; g <= g1; g++) {
                 const modes_candidate *c = candidates + tiles[g].offset;
@@ -472,6 +477,7 @@ static int pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, cons
                         if (!signal) rc.signal = 0;
                         bl.local_rec.push_back(rc);
                     }
+                    if (carrier) bl.local_car.push_back(carrier[tiles[g].offset + k]);
                 }
             }
             uint32_t off = 0;
@@ -485,6 +491,7 @@ static int pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, cons
                 bl.local_wrec.push_back(rc);
             }
             modes_resolver_set_output(r.res, bl.msgs.data() + used, room - used);
+            modes::resolver_set_carrier(r.res, carrier ? bl.local_car.data() : nullptr);
             if (modes_resolver_run_weak(r.res, bl.local.data(), recovered ? bl.local_rec.data() : nullptr, bl.local_tiles.data(),
                                         n_local, r.buffers, bl.local_wt.data(), bl.local_wrec.data(), bl.local_wt.size(),
                                         nullptr, nullptr)) {
@@ -695,6 +702,10 @@ int modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user) {
         p->recovered.resize(n_cand ? n_cand : 1);
         if (modes_recover_fetch(sl.ctx, p->recovered.data())) return fail(p, "%s", modes_last_error(sl.ctx));
     }
+    if (sl.feat.carrier) {
+        p->carrier.resize(n_cand ? n_cand : 1);
+        if (modes::carrier_fetch(sl.ctx, p->carrier.data())) return fail(p, "%s", modes_last_error(sl.ctx));
+    }
     uint64_t n_weak = 0;
     if (sl.feat.weak) {
         if (modes_weak_fetch(sl.ctx, nullptr, nullptr, &n_weak)) return fail(p, "%s", modes_last_error(sl.ctx));
@@ -719,7 +730,8 @@ int modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user) {
     sl.busy = false;
     p->collected++;
     return pool_resolve(p, sl.ids.data(), n, p->cands.data(), sl.feat.recover ? p->recovered.data() : nullptr, sl.feat.signal,
-                        p->tiles.data(), sink, user, p->weak_t.data(), p->weak_rec.data(), (size_t)n_weak);
+                        p->tiles.data(), sink, user, p->weak_t.data(), p->weak_rec.data(), (size_t)n_weak,
+                        sl.feat.carrier ? p->carrier.data() : nullptr);
 }
 
 int modes_pool_ingest(modes_pool *p, const uint32_t *receivers, const uint8_t *const *iq, size_t n,
@@ -790,6 +802,8 @@ int modes_pool_set_output(modes_pool *p, modes_message *out, uint32_t *receiver_
 size_t modes_pool_output_count(const modes_pool *p) { return p ? p->out_count : 0; }
 
 int modes_pool_set_arrival(modes_pool *p, int on) { return set_feature(p, &modes::Features::arrival, on); }
+
+int modes_pool_set_carrier(modes_pool *p, int on) { return set_feature(p, &modes::Features::carrier, on); }
 
 int modes_pool_set_signal(modes_pool *p, int on) { return set_feature(p, &modes::Features::signal, on); }
 

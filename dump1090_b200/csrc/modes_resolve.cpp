@@ -27,6 +27,7 @@
 #include <sched.h>
 #include <vector>
 #include "modes_internal.h"
+#include "modes_carrier_core.cuh"
 
 namespace modes {
 
@@ -200,6 +201,7 @@ struct Delivery {
     uint32_t iid, ap_addr;
     uint8_t crcok, phase_corrected;
     uint8_t recovered;           // eval is a recovery record's frame (1: at a candidate, 2: at a weak preamble): crc 0, nfixed = its flips
+    int16_t carrier;             // the attempt's carrier code (0: not measured)
 };
 
 static inline void materialise(const Delivery &d, modes_message *mm) {
@@ -207,6 +209,7 @@ static inline void materialise(const Delivery &d, modes_message *mm) {
     mm->sample_pos = d.sample_pos;
     mm->phase_corrected = d.phase_corrected;
     if (d.recovered) { mm->recovered = d.recovered; mm->errorbit = -1; }
+    mm->carrier = d.carrier;
 }
 
 // Cores this process may actually keep busy: the CPUs it is allowed on, cut down to the CPU-time
@@ -296,10 +299,11 @@ class BuildPool {
     uint64_t gen_ = 0;
 };
 
-// One evaluated attempt, as detectModeS handles it after the delta gate.
+// One evaluated attempt, as detectModeS handles it after the delta gate; car: the candidate's carrier
+// record (nullptr: not measured), k: which of its attempts this is.
 // Returns true when the message is good (the scan skips past it).
 static inline bool attempt(ResolveState &st, const ResolveConfig &cfg, const modes_frame_eval &p, bool retry,
-                           int64_t sample_pos, std::vector<Delivery> &deliveries) {
+                           int64_t sample_pos, std::vector<Delivery> &deliveries, const modes_carrier *car, int k) {
     if (!(p.flags & MODES_EVAL_DECODED)) return false;
     uint32_t iid, ap;
     const int crcok = judge(st, p, &iid, &ap);
@@ -309,7 +313,8 @@ static inline bool attempt(ResolveState &st, const ResolveConfig &cfg, const mod
         else { st.stats[4]++; st.stats[5]++; st.stats[6]++; }
     }
     if (cfg.check_crc == 0 || crcok)                       // dump1090.c:1803; :1772-1773
-        deliveries.push_back(Delivery{p, sample_pos, iid, ap, (uint8_t)crcok, (uint8_t)(crcok && retry), (uint8_t)0});
+        deliveries.push_back(Delivery{p, sample_pos, iid, ap, (uint8_t)crcok, (uint8_t)(crcok && retry), (uint8_t)0,
+                                      car ? carrier::code_of(car->re[k], car->im[k]) : (int16_t)0});
     return crcok != 0;
 }
 
@@ -361,7 +366,7 @@ static inline void recovery_step(ResolveState &st, const ResolveConfig &cfg, con
     pend.end = j + kRecoveredSpan;
     pend.stats = &stats;
     st.next_j_recovered = j + kRecoveredSpan;
-    deliveries.push_back(Delivery{e, pos, 0u, 0u, (uint8_t)1, (uint8_t)0, marker});
+    deliveries.push_back(Delivery{e, pos, 0u, 0u, (uint8_t)1, (uint8_t)0, marker, (int16_t)0});
     stats.delivered++;
 }
 
@@ -392,11 +397,11 @@ static inline void weak_steps(ResolveState &st, const ResolveConfig &cfg, WeakCu
 // numbers as in the records: t >> 17); the walk ends at the first candidate of buffer b_hi or later
 // (records are in stream order).  The whole array: 0, UINT32_MAX.  kRecover: apply the recovery rules
 // with `rec` and merge the weak positions `weak` (may be nullptr) into the walk (the walk without
-// them has no trace of them).
+// them has no trace of them).  car: the carrier records of the candidates (nullptr: not measured).
 template <bool kRecover>
 static void walk_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands, const modes_tile *tiles,
                        size_t n_tiles, int64_t buffer_base, std::vector<Delivery> &deliveries, uint32_t b_lo, uint32_t b_hi,
-                       const modes_recovered *rec, const WeakList *weak) {
+                       const modes_recovered *rec, const WeakList *weak, const modes_carrier *car) {
     RecoveryPending pend;
     WeakCursor wc;
     const bool merge = kRecover && weak && weak->n;
@@ -436,9 +441,10 @@ static void walk_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_c
             const int64_t pos = buffer * (int64_t)kBufSamples + j - MODES_CARRY_SAMPLES;
             bool good = false;
             const modes_frame_eval &p1 = c->pass[0];
+            const modes_carrier *ck = car ? car + k0 + k : nullptr;
             if (p1.flags & MODES_EVAL_GATE_OK) {           // dump1090.c:1723-1726
                 const uint32_t skip = (uint32_t)(8 + bits_by_type(p1.msgtype)) * 2 + 1;
-                if (attempt(st, cfg, p1, false, pos, deliveries)) {
+                if (attempt(st, cfg, p1, false, pos, deliveries, ck, 0)) {
                     st.next_j = j + skip;
                     good = true;
                 } else {
@@ -446,7 +452,7 @@ static void walk_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_c
                     const modes_frame_eval &p2 = c->pass[1];
                     if (p2.flags & MODES_EVAL_GATE_OK) {
                         const uint32_t skip2 = (uint32_t)(8 + bits_by_type(p2.msgtype)) * 2 + 1;
-                        if (attempt(st, cfg, p2, true, pos, deliveries)) { st.next_j = j + skip2; good = true; }
+                        if (attempt(st, cfg, p2, true, pos, deliveries, ck, 1)) { st.next_j = j + skip2; good = true; }
                     }
                 }
             }
@@ -460,9 +466,9 @@ static void walk_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_c
 static void judge_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands, const modes_tile *tiles,
                         size_t n_tiles, int64_t buffer_base, std::vector<Delivery> &deliveries,
                         uint32_t b_lo = 0, uint32_t b_hi = UINT32_MAX, const modes_recovered *rec = nullptr,
-                        const WeakList *weak = nullptr) {
-    if (rec) walk_tiles<true>(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, b_lo, b_hi, rec, weak);
-    else walk_tiles<false>(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, b_lo, b_hi, nullptr, nullptr);
+                        const WeakList *weak = nullptr, const modes_carrier *car = nullptr) {
+    if (rec) walk_tiles<true>(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, b_lo, b_hi, rec, weak, car);
+    else walk_tiles<false>(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, b_lo, b_hi, nullptr, nullptr, car);
 }
 
 // Build the delivered structs: in place and in parallel for array output, then the callback
@@ -534,6 +540,7 @@ struct Part {
     bool first_of_shard;         // the tail pass for a shard's first part walks the previous SHARD's array
     const modes_recovered *rec;  // the array's recovery records, or nullptr
     const WeakList *weak;        // the array's weak positions, or nullptr
+    const modes_carrier *car;    // the array's carrier records, or nullptr
 };
 struct PartRun { ResolveState start, end; std::vector<Delivery> deliveries; };
 struct ResolveScratch {
@@ -567,8 +574,9 @@ static size_t parts_for(size_t n_tiles) {
 // read from the records themselves: the buffer after the one the first candidate at or behind tile
 // k * n_tiles / want lies in (tiles do not line up with buffers; records are in stream order).
 static void cut_parts(const modes_candidate *cands, const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, size_t want,
-                      std::vector<Part> &parts, const modes_recovered *rec = nullptr, const WeakList *weak = nullptr) {
-    Part p{cands, tiles, n_tiles, 0, 0, UINT32_MAX, buffer_base, true, rec, weak};
+                      std::vector<Part> &parts, const modes_recovered *rec = nullptr, const WeakList *weak = nullptr,
+                      const modes_carrier *car = nullptr) {
+    Part p{cands, tiles, n_tiles, 0, 0, UINT32_MAX, buffer_base, true, rec, weak, car};
     for (size_t k = 1; k < want; k++) {
         size_t ti = k * n_tiles / want;
         while (ti < n_tiles && tiles[ti].count == 0) ti++;
@@ -604,7 +612,7 @@ static int judge_parts(ResolveState &st, const ResolveConfig &cfg, const std::ve
         r.end = r.start;
         r.deliveries.clear();
         judge_tiles(r.end, cfg, p.cands, p.tiles + p.tile_lo, p.n_tiles - p.tile_lo, p.buffer_base, r.deliveries, p.b_lo, p.b_hi,
-                    p.rec, p.weak);
+                    p.rec, p.weak, p.car);
     };
     int rounds = 0;
     size_t done = 0;                                       // parts [0, done) are final
@@ -673,7 +681,8 @@ static PartRun *runs_for(ResolveScratch *scratch, size_t n) {
 
 void resolve_candidates(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands,
                         const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, MessageOut &out,
-                        ResolveScratch *scratch, const modes_recovered *recovered, const WeakList &weak) {
+                        ResolveScratch *scratch, const modes_recovered *recovered, const WeakList &weak,
+                        const modes_carrier *carrier) {
     const bool timing = std::getenv("MODES_RESOLVE_TIMING") != nullptr;
     auto now = [] { return std::chrono::steady_clock::now(); };
     auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) {
@@ -684,14 +693,14 @@ void resolve_candidates(ResolveState &st, const ResolveConfig &cfg, const modes_
     if (want <= 1) {
         std::vector<Delivery> &deliveries = scratch->deliveries;
         deliveries.clear();
-        judge_tiles(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, 0, UINT32_MAX, recovered, &weak);
+        judge_tiles(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, 0, UINT32_MAX, recovered, &weak, carrier);
         const auto t1 = now();
         deliver(deliveries, out);
         if (timing) std::fprintf(stderr, "resolve_candidates: %zu tiles, verdicts %.2f ms, structs %.2f ms\n", n_tiles, ms(t0, t1), ms(t1, now()));
         return;
     }
     std::vector<Part> parts;
-    cut_parts(cands, tiles, n_tiles, buffer_base, want, parts, recovered, &weak);
+    cut_parts(cands, tiles, n_tiles, buffer_base, want, parts, recovered, &weak, carrier);
     PartRun *runs = runs_for(scratch, parts.size());
     const int rounds = judge_parts(st, cfg, parts, runs);
     const auto t1 = now();
@@ -730,7 +739,8 @@ void resolve_commit(MessageOut &out, ResolveScratch *scratch) {
 // is a part, long shards are cut once more (see judge_parts).
 void resolve_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards, const modes_candidate *const *cands,
                     const modes_tile *const *tiles, const size_t *n_tiles, const int64_t *buffer_base,
-                    MessageOut &out, ResolveScratch *scratch, const modes_recovered *const *recovered, const WeakList *weak) {
+                    MessageOut &out, ResolveScratch *scratch, const modes_recovered *const *recovered, const WeakList *weak,
+                    const modes_carrier *const *carrier) {
     const bool timing = std::getenv("MODES_RESOLVE_TIMING") != nullptr;
     auto now = [] { return std::chrono::steady_clock::now(); };
     auto t_start = now();
@@ -742,7 +752,7 @@ void resolve_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards,
         const size_t share = threads_left / (n_shards - k) > 0 ? threads_left / (n_shards - k) : 1;
         if (want > share) want = share;
         cut_parts(cands[k], tiles[k], n_tiles[k], buffer_base[k], want, parts, recovered ? recovered[k] : nullptr,
-                  recovered && weak ? weak + k : nullptr);
+                  recovered && weak ? weak + k : nullptr, carrier ? carrier[k] : nullptr);
         threads_left = threads_left > want ? threads_left - want : 0;
     }
     PartRun *runs = runs_for(scratch, parts.size());

@@ -1,13 +1,14 @@
-// modes_signal.cu — the signal-level pass (modes_set_signal) and the arrival-time pass
-// (modes_set_arrival): for every decoded attempt of every candidate record, the RMS pulse magnitude
-// of its frame (modes_signal_core.cuh), written into the record's pass[k].signal, and its arrival
-// code (modes_arrival_core.cuh), written into bits 4-7 of pass[k].flags.
+// modes_signal.cu — the signal-level pass (modes_set_signal), the arrival-time pass (modes_set_arrival)
+// and the carrier pass (modes_set_carrier): for every decoded attempt of every candidate record, the RMS
+// pulse magnitude of its frame (modes_signal_core.cuh), written into the record's pass[k].signal, its
+// arrival code (modes_arrival_core.cuh), written into bits 4-7 of pass[k].flags, and its carrier record
+// (modes_carrier_core.cuh), written into a separate array beside the records.
 //
 // It runs after frame evaluation, on the same stream and over the same virtual sample array
 // (BatchView: carry block + body) while the batch is still in HBM, whichever evaluation kernel
-// produced the records.  It is a separate kernel so that, with both features off, nothing about the
-// default kernels changes.  One instantiation serves each combination of the two switches, so with
-// both on the window is read once.
+// produced the records.  It is a separate kernel so that, with the features off, nothing about the
+// default kernels changes.  One instantiation serves each combination of the three switches, so with
+// several on the window is read once.
 //
 // Shape: a warp takes 32 consecutive records, one lane each, and reads their flags and positions
 // (one load per lane); records with no decoded attempt cost nothing more.  The decoded ones are then
@@ -18,12 +19,15 @@
 // even when they differ in length.  For the arrival time lanes 0-15 also hold the preamble's samples
 // 0-15, lane 16 sample 16+2*56 and lane 17 sample 16+2*112 (the sample after a frame's last bit);
 // each attempt's bits, read from its record, give the sample classes as mask words, and the warp
-// reduces four class sums per attempt.
+// reduces four class sums per attempt.  For the carrier lanes 0 and 1 also hold the preamble pairs
+// (samples 0, 2 and 7, 9); each attempt's bits pick every lane's pulse samples, the pulse of the next
+// bit comes from the next lane (one shuffle per word), and the warp reduces two sums per attempt.
 #include <cstdint>
 #include <cuda_runtime.h>
 #include "modes_internal.h"
 #include "modes_signal_core.cuh"
 #include "modes_arrival_core.cuh"
+#include "modes_carrier_core.cuh"
 
 namespace modes {
 
@@ -83,10 +87,44 @@ __device__ __forceinline__ uint32_t arrival_code(const uint32_t *rw, uint32_t b,
     return arrival::code_of(S, n);
 }
 
-template <bool kSignal, bool kArrival>
+// The preamble pair of lane 0 (samples 0 and 2) or lane 1 (samples 7 and 9) as one word, earlier sample in
+// the low half; no signal on the other lanes and for a record without a decoded attempt.
+__device__ __forceinline__ uint32_t carrier_preamble(const BatchView &in, uint32_t t, int lane, uint32_t nb) {
+    if (nb == 0 || lane > 1) return 0x7f7f7f7fu;
+    const uint32_t s = lane ? 7u : 0u;
+    return signal::raw_sample16(in, t + 2u + s) | (signal::raw_sample16(in, t + 4u + s) << 16);
+}
+
+// The carrier sums (re, im) of one decoded attempt of b bits whose first frame word is record word `w`:
+// pair[r] = the lane's bit pairs (see load_pairs), pre = its preamble pair (carrier_preamble).  Every lane
+// returns the sums.
+__device__ __forceinline__ void carrier_sums(const uint32_t *rw, uint32_t b, const uint32_t pair[4], uint32_t pre, int lane,
+                                             int32_t &re, int32_t &im) {
+    uint32_t mw[4], B[4], P[4];
+#pragma unroll
+    for (int q = 0; q < 4; q++) mw[q] = rw[q];
+    arrival::bit_words(mw, b, B);
+#pragma unroll
+    for (int r = 0; r < 4; r++) P[r] = carrier::pulse_of(pair[r], (B[r] >> lane) & 1u);
+    re = 0; im = 0;
+    carrier::add_pair(pre & 0xffffu, pre >> 16, re, im);                 // 0 on lanes without a preamble pair
+#pragma unroll
+    for (int r = 0; r < 4; r++) {
+        // the pulse of bit 32r + lane + 1: lane l reads lane l+1's, lane 31 lane 0's of the next word
+        const uint32_t next = __shfl_sync(0xffffffffu, lane == 0 ? (r < 3 ? P[r + 1] : 0x7f7fu) : P[r], (lane + 1) & 31);
+        if ((carrier::equal_next(B, r, b) >> lane) & 1u) carrier::add_pair(P[r], next, re, im);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        re += __shfl_xor_sync(0xffffffffu, re, o);
+        im += __shfl_xor_sync(0xffffffffu, im, o);
+    }
+}
+
+template <bool kSignal, bool kArrival, bool kCarrier>
 __global__ void __launch_bounds__(kSignalThreads)
 signal_kernel(BatchView in, const uint16_t *__restrict__ lutn, const uint32_t *counters, uint32_t cand_capacity,
-              modes_candidate *records) {
+              modes_candidate *records, modes_carrier *carrier) {
     const int lane = threadIdx.x & 31;
     uint32_t n = counters[0];
     if (n > cand_capacity) n = cand_capacity;
@@ -103,17 +141,18 @@ signal_kernel(BatchView in, const uint16_t *__restrict__ lutn, const uint32_t *c
         int c = __ffs(todo) - 1;
         todo &= todo - 1;
         uint32_t cw0 = __shfl_sync(0xffffffffu, w0, c), cw1 = __shfl_sync(0xffffffffu, w1, c);
-        uint32_t cur[4], cur_pre = 0;
+        uint32_t cur[4], cur_pre = 0, cur_cpre = 0;
         {
             // virtual index of the candidate's m[j] is t + 2; its first bit's pair is 16 samples later
             const uint32_t ct = __shfl_sync(0xffffffffu, t, c);
             load_pairs(in, ct + 18u, bits_needed(cw0, cw1), lane, cur);
             if (kArrival) cur_pre = edge_sample(in, ct, lane, bits_needed(cw0, cw1));
+            if (kCarrier) cur_cpre = carrier_preamble(in, ct, lane, bits_needed(cw0, cw1));
         }
         for (;;) {
             const bool more = todo != 0;
             int c2 = 0;
-            uint32_t nw0 = 0, nw1 = 0, nxt[4], nxt_pre = 0;
+            uint32_t nw0 = 0, nw1 = 0, nxt[4], nxt_pre = 0, nxt_cpre = 0;
             if (more) {
                 c2 = __ffs(todo) - 1;
                 todo &= todo - 1;
@@ -121,6 +160,7 @@ signal_kernel(BatchView in, const uint16_t *__restrict__ lutn, const uint32_t *c
                 const uint32_t nt = __shfl_sync(0xffffffffu, t, c2);
                 load_pairs(in, nt + 18u, bits_needed(nw0, nw1), lane, nxt);
                 if (kArrival) nxt_pre = edge_sample(in, nt, lane, bits_needed(nw0, nw1));
+                if (kCarrier) nxt_cpre = carrier_preamble(in, nt, lane, bits_needed(nw0, nw1));
             }
             if (kSignal) {
                 uint64_t q56 = 0, q112 = 0;                               // bits < 56 / bits 56..111
@@ -160,24 +200,45 @@ signal_kernel(BatchView in, const uint16_t *__restrict__ lutn, const uint32_t *c
                         (uint8_t)(((cw >> 24) & 0x0fu) | (code << MODES_EVAL_ARRIVAL_SHIFT));
                 }
             }
+            if (kCarrier) {
+                const uint32_t *rw = reinterpret_cast<const uint32_t *>(records + base + c);
+                int32_t re[2] = {0, 0}, im[2] = {0, 0};
+#pragma unroll
+                for (int k = 0; k < 2; k++) {
+                    const uint32_t nb = bits_needed(k ? cw1 : cw0, 0);
+                    if (nb) carrier_sums(rw + 2 + 6 * k, nb, cur, cur_cpre, lane, re[k], im[k]);   // warp-uniform
+                }
+                if (lane == 0) reinterpret_cast<int4 *>(carrier)[base + c] = make_int4(re[0], re[1], im[0], im[1]);
+            }
             if (!more) break;
             c = c2; cw0 = nw0; cw1 = nw1;
 #pragma unroll
             for (int r = 0; r < 4; r++) cur[r] = nxt[r];
             cur_pre = nxt_pre;
+            cur_cpre = nxt_cpre;
         }
     }
 }
 
 void launch_signal(const BatchView &in, const DeviceTables &tab, const ScanOutputs &scan, modes_candidate *records,
-                   int sm_count, cudaStream_t stream, bool signal, bool arrival) {
+                   int sm_count, cudaStream_t stream, bool signal, bool arrival, modes_carrier *carrier) {
     const dim3 grid(sm_count * kSignalBlocksPerSm), block(kSignalThreads);
-    if (signal && arrival)
-        signal_kernel<true, true><<<grid, block, 0, stream>>>(in, tab.lutn, scan.counters, scan.cand_capacity, records);
+    const uint32_t cap = scan.cand_capacity;
+    if (carrier) {
+        if (signal && arrival)
+            signal_kernel<true, true, true><<<grid, block, 0, stream>>>(in, tab.lutn, scan.counters, cap, records, carrier);
+        else if (arrival)
+            signal_kernel<false, true, true><<<grid, block, 0, stream>>>(in, tab.lutn, scan.counters, cap, records, carrier);
+        else if (signal)
+            signal_kernel<true, false, true><<<grid, block, 0, stream>>>(in, tab.lutn, scan.counters, cap, records, carrier);
+        else
+            signal_kernel<false, false, true><<<grid, block, 0, stream>>>(in, tab.lutn, scan.counters, cap, records, carrier);
+    } else if (signal && arrival)
+        signal_kernel<true, true, false><<<grid, block, 0, stream>>>(in, tab.lutn, scan.counters, cap, records, nullptr);
     else if (arrival)
-        signal_kernel<false, true><<<grid, block, 0, stream>>>(in, tab.lutn, scan.counters, scan.cand_capacity, records);
+        signal_kernel<false, true, false><<<grid, block, 0, stream>>>(in, tab.lutn, scan.counters, cap, records, nullptr);
     else if (signal)
-        signal_kernel<true, false><<<grid, block, 0, stream>>>(in, tab.lutn, scan.counters, scan.cand_capacity, records);
+        signal_kernel<true, false, false><<<grid, block, 0, stream>>>(in, tab.lutn, scan.counters, cap, records, nullptr);
 }
 
 }  // namespace modes

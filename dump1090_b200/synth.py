@@ -184,8 +184,10 @@ def synth_stream_at(nsamples: int, frames, sigma: float = 1.5, seed: int = 1, sa
     (an out-of-band interferer where the offset is past 1 MHz); None, the default, adds nothing.
     carrier_hz: the frames are sent at that offset from the baseband's 0 Hz (a radio tuned carrier_hz below
     1090 MHz), their phase turning by 2 pi carrier_hz / sample_rate per sample of the stream; 0, the
-    default, leaves them as they were.  dc=(i, q): a constant (a zero-IF radio's DC spike, in 8-bit LSB)
-    added to every sample; None, the default, adds nothing."""
+    default, leaves them as they were.  A frame tuple may carry a sixth element, the frame's own carrier
+    offset in Hz (its transmitter's offset from 1090 MHz), which adds to carrier_hz for that frame.
+    dc=(i, q): a constant (a zero-IF radio's DC spike, in 8-bit LSB) added to every sample; None, the
+    default, adds nothing."""
     i = noise(nsamples, sigma, seed * 2 + 11)
     q = noise(nsamples, sigma, seed * 2 + 12)
     if tone is not None:
@@ -193,7 +195,9 @@ def synth_stream_at(nsamples: int, frames, sigma: float = 1.5, seed: int = 1, sa
         w = 2 * np.pi * (offset_hz / sample_rate) * np.arange(nsamples, dtype=np.float64)
         i += tone_amp * np.cos(w)
         q += tone_amp * np.sin(w)
-    for pos, frame, amp, phase, frac in frames:
+    for fr in frames:
+        pos, frame, amp, phase, frac = fr[:5]
+        f_hz = carrier_hz + (fr[5] if len(fr) > 5 else 0.0)
         start, env = frame_envelope_at(frame, pos, frac, sample_rate)
         env = env * amp
         if sample_rate == 2_000_000:                       # synth_stream's envelope length
@@ -202,8 +206,8 @@ def synth_stream_at(nsamples: int, frames, sigma: float = 1.5, seed: int = 1, sa
         if start >= nsamples or end <= start:
             continue
         seg = env[: end - start]
-        if carrier_hz:
-            ph = phase + 2 * np.pi * (carrier_hz / sample_rate) * np.arange(start, end, dtype=np.float64)
+        if f_hz:
+            ph = phase + 2 * np.pi * (f_hz / sample_rate) * np.arange(start, end, dtype=np.float64)
             i[start:end] += seg * np.cos(ph)
             q[start:end] += seg * np.sin(ph)
         else:
@@ -228,19 +232,28 @@ def synth_stream_at(nsamples: int, frames, sigma: float = 1.5, seed: int = 1, sa
 def synth_stream(nsamples: int, frames, sigma: float = 1.5, seed: int = 1) -> np.ndarray:
     """Build a u8 interleaved I/Q stream of `nsamples` samples.
 
-    frames: iterable of (pos, frame_bytes, amplitude_lsb, carrier_phase_rad, frac).
-    Overlapping frames add coherently in I/Q.  Returns uint8 array of 2*nsamples.
+    frames: iterable of (pos, frame_bytes, amplitude_lsb, carrier_phase_rad, frac), optionally with a sixth
+    element, the frame's carrier offset in Hz from the centre of the stream (its phase then turns by
+    2 pi offset / 2 MHz per sample of the stream).  Overlapping frames add coherently in I/Q.  Returns
+    uint8 array of 2*nsamples.
     """
     i = noise(nsamples, sigma, seed * 2 + 11)
     q = noise(nsamples, sigma, seed * 2 + 12)
-    for pos, frame, amp, phase, frac in frames:
+    for fr in frames:
+        pos, frame, amp, phase, frac = fr[:5]
+        f_hz = fr[5] if len(fr) > 5 else 0.0
         env = frame_envelope(frame, frac) * amp
         end = min(nsamples, pos + len(env))
         if pos >= nsamples or end <= pos:
             continue
         seg = env[: end - pos]
-        i[pos:end] += seg * np.cos(phase)
-        q[pos:end] += seg * np.sin(phase)
+        if f_hz:
+            ph = phase + 2 * np.pi * (f_hz / 2_000_000) * np.arange(pos, end, dtype=np.float64)
+            i[pos:end] += seg * np.cos(ph)
+            q[pos:end] += seg * np.sin(ph)
+        else:
+            i[pos:end] += seg * np.cos(phase)
+            q[pos:end] += seg * np.sin(phase)
     out = np.empty(2 * nsamples, dtype=np.uint8)
     out[0::2] = np.clip(np.rint(127.0 + i), 0, 255).astype(np.uint8)
     out[1::2] = np.clip(np.rint(127.0 + q), 0, 255).astype(np.uint8)
@@ -365,39 +378,45 @@ def df17_grid(nsamples: int, period: int, seed: int, sigma: float = 1.5, amp: fl
     return synth_stream(nsamples, frames, sigma=sigma, seed=seed)
 
 
-def fleet_at(snr_db: float, nframes: int, seed: int, n_aircraft: int = 20, amp: float = 20.0, period: int = 400):
+def _fleet_frame(frames: list, fleet, rng: Counter, k: int, n_aircraft: int, amp: float, period: int, carrier_of):
+    """fleet_at's frame k (appended to frames, as its hex returned); carrier_of(address) -> Hz, when given, is
+    each aircraft's own carrier offset, carried as the frame tuple's sixth element."""
+    icao = fleet[rng.below(n_aircraft)]
+    me = [_me_ident, _me_airborne, _me_airborne, _me_velocity][rng.below(4)](rng)
+    frame = make_frame(17, 5, icao.to_bytes(3, "big") + me)
+    fr = (200 + k * period + rng.below(100), frame, amp, 2 * np.pi * rng.uniform(), 0.5 * rng.uniform())
+    frames.append(fr if carrier_of is None else fr + (float(carrier_of(icao)),))
+    return frame.hex()
+
+
+def fleet_at(snr_db: float, nframes: int, seed: int, n_aircraft: int = 20, amp: float = 20.0, period: int = 400,
+             carrier_of=None):
     """DF17 extended squitters (identification, airborne position, velocity) of a fleet of n_aircraft,
     each sending many frames, in noise at snr_db (pulse power / noise power = amp^2 / (2 sigma^2)), one
-    frame every ~period samples.  Returns (stream, set of the frames' hex)."""
+    frame every ~period samples.  carrier_of(address) -> Hz gives each aircraft its own carrier offset;
+    None, the default, sends every frame at 0 Hz.  Returns (stream, set of the frames' hex)."""
     sigma = amp / (np.sqrt(2.0) * 10 ** (snr_db / 20.0))
     rng = Counter(seed)
     fleet = [0x400000 + rng.below(0x3FFFFF) for _ in range(n_aircraft)]
     frames, truth = [], set()
     for k in range(nframes):
-        aa = fleet[rng.below(n_aircraft)].to_bytes(3, "big")
-        me = [_me_ident, _me_airborne, _me_airborne, _me_velocity][rng.below(4)](rng)
-        frame = make_frame(17, 5, aa + me)
-        frames.append((200 + k * period + rng.below(100), frame, amp, 2 * np.pi * rng.uniform(), 0.5 * rng.uniform()))
-        truth.add(frame.hex())
+        truth.add(_fleet_frame(frames, fleet, rng, k, n_aircraft, amp, period, carrier_of))
     return synth_stream(200 + nframes * period + 400, frames, sigma=sigma, seed=seed), truth
 
 
 def fleet_at_rate(snr_db: float, nframes: int, seed: int, sample_rate: int = 2_400_000, n_aircraft: int = 20,
                   amp: float = 20.0, period: int = 400, dtype: str = "uc8", scale: float = 1.0, tone=None,
-                  carrier_hz: float = 0.0, dc=None):
+                  carrier_hz: float = 0.0, dc=None, carrier_of=None):
     """fleet_at sampled at sample_rate (2.4 MS/s: what dump1090-fa and readsb record): the same frames,
     arrival times, amplitudes and carrier phases, over the same stretch of time, with the same noise per
-    sample; dtype, scale, tone, carrier_hz and dc as synth_stream_at.  Returns (stream, set of the frames' hex)."""
+    sample; dtype, scale, tone, carrier_hz and dc as synth_stream_at, carrier_of as fleet_at (each
+    aircraft's offset adds to carrier_hz).  Returns (stream, set of the frames' hex)."""
     sigma = amp / (np.sqrt(2.0) * 10 ** (snr_db / 20.0))
     rng = Counter(seed)
     fleet = [0x400000 + rng.below(0x3FFFFF) for _ in range(n_aircraft)]
     frames, truth = [], set()
     for k in range(nframes):
-        aa = fleet[rng.below(n_aircraft)].to_bytes(3, "big")
-        me = [_me_ident, _me_airborne, _me_airborne, _me_velocity][rng.below(4)](rng)
-        frame = make_frame(17, 5, aa + me)
-        frames.append((200 + k * period + rng.below(100), frame, amp, 2 * np.pi * rng.uniform(), 0.5 * rng.uniform()))
-        truth.add(frame.hex())
+        truth.add(_fleet_frame(frames, fleet, rng, k, n_aircraft, amp, period, carrier_of))
     a, b = _rate_ratio(sample_rate)
     n = -(-(200 + nframes * period + 400) * a // b)
     return synth_stream_at(n, frames, sigma=sigma, seed=seed, sample_rate=sample_rate, dtype=dtype, scale=scale,

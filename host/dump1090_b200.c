@@ -47,6 +47,12 @@
  * the 2 MHz band with the most power above the floor (where the channel most likely sits: the value for
  * --input-offset).  It combines with every --sample-rate, --iformat and --input-offset and leaves stdout
  * as it is.
+ * --carrier measures every decoded frame's carrier frequency on the GPU (modes_set_carrier) and prints one
+ * summary line on stderr at the end, as --levels does: the messages and aircraft measured and the receiver's
+ * offset, the median over aircraft of each aircraft's median carrier, in Hz and in ppm of 1090 MHz (the
+ * receiver's tuning error; carrier_summary in dump1090_b200/api.py is the same computation).  It combines with
+ * every --sample-rate, --iformat, --input-offset and output mode and leaves stdout as it is; the device
+ * resolve has no room for it, so it is refused together with --gpu-resolve.
  * The live-radio, networking and interactive options are out of scope.
  */
 #include <math.h>
@@ -57,7 +63,7 @@
 #include "modes_b200.h"
 
 static int opt_raw = 0, opt_onlyaddr = 0, opt_stats = 0, opt_check_crc = 1, opt_sbs = 0, opt_json = 0, opt_beast = 0;
-static int opt_levels = 0, opt_recover = 0, opt_weak = 0, opt_arrival = 0, opt_spectrum = 0;
+static int opt_levels = 0, opt_recover = 0, opt_weak = 0, opt_arrival = 0, opt_spectrum = 0, opt_carrier = 0;
 static modes_tracker *tracker = NULL;
 
 /* --levels: totals over the records taken so far */
@@ -131,10 +137,59 @@ static void print_spectrum(unsigned long fs) {
             (at + (w - 1) / 2.0 - N / 2) * (double)fs / N);
 }
 
+/* --carrier: (address, code) of every measured message, summarised at the end */
+static struct { uint64_t *v; size_t n, cap; } cr;
+
+static void take_carrier(const modes_message *mm) {
+    if (!mm->carrier) return;
+    if (cr.n == cr.cap) {
+        const size_t cap = cr.cap ? 2 * cr.cap : 4096;
+        uint64_t *v = (uint64_t *)realloc(cr.v, cap * sizeof(uint64_t));
+        if (!v) return;
+        cr.v = v; cr.cap = cap;
+    }
+    const uint32_t addr = ((uint32_t)mm->aa1 << 16) | ((uint32_t)mm->aa2 << 8) | (uint32_t)mm->aa3;
+    cr.v[cr.n++] = ((uint64_t)addr << 16) | (uint16_t)mm->carrier;
+}
+
+static int cmp_u64(const void *a, const void *b) {
+    const uint64_t x = *(const uint64_t *)a, y = *(const uint64_t *)b;
+    return x < y ? -1 : x > y;
+}
+
+static int cmp_double(const void *a, const void *b) {
+    const double x = *(const double *)a, y = *(const double *)b;
+    return x < y ? -1 : x > y;
+}
+
+/* the median of n sorted values (the mean of the middle two for even n) */
+static double median_of(const double *v, size_t n) { return n & 1 ? v[n / 2] : 0.5 * (v[n / 2 - 1] + v[n / 2]); }
+
+static void print_carrier(void) {
+    qsort(cr.v, cr.n, sizeof(uint64_t), cmp_u64);            /* by address, then by code */
+    double *per = (double *)malloc((cr.n ? cr.n : 1) * sizeof(double)), *hz = (double *)malloc((cr.n ? cr.n : 1) * sizeof(double));
+    size_t n_ac = 0;
+    for (size_t i = 0; per && hz && i < cr.n;) {
+        size_t k = 0;
+        for (const uint64_t a = cr.v[i] >> 16; i < cr.n && cr.v[i] >> 16 == a; i++)
+            hz[k++] = ((double)(cr.v[i] & 0xffffu) - 16384.0) * 100.0;
+        per[n_ac++] = median_of(hz, k);
+    }
+    fprintf(stderr, "carrier: %zu messages, %zu aircraft, ", cr.n, n_ac);
+    if (!n_ac) fprintf(stderr, "receiver offset n/a\n");
+    else {
+        qsort(per, n_ac, sizeof(double), cmp_double);
+        const double f = median_of(per, n_ac);
+        fprintf(stderr, "receiver offset %+.0f Hz (%+.3f ppm of 1090 MHz)\n", f, f / 1090.0);
+    }
+    free(per); free(hz); free(cr.v);
+}
+
 /* Message sink: the --raw / --onlyaddr forms of displayModesMessage
  * (dump1090.c:1318-1331) and, by default, the full text (:1314-1450) via modes_format_message(). */
 static void on_message(void *user, const modes_message *mm) {
     (void)user;
+    if (opt_carrier) take_carrier(mm);
     if (opt_stats) return;                                  /* dump1090.c:1803 */
     if (opt_beast) {
         uint8_t frame[64];
@@ -192,6 +247,7 @@ int main(int argc, char **argv) {
         else if (!strcmp(argv[j], "--arrival")) opt_arrival = 1;
         else if (!strcmp(argv[j], "--levels")) opt_levels = 1;
         else if (!strcmp(argv[j], "--spectrum")) opt_spectrum = 1;
+        else if (!strcmp(argv[j], "--carrier")) opt_carrier = 1;
         else if (!strcmp(argv[j], "--recover")) opt_recover = 1;
         else if (!strcmp(argv[j], "--recover-weak")) opt_recover = opt_weak = 1;
         else if (!strcmp(argv[j], "--gpu-resolve")) cfg.gpu_resolve = 1;
@@ -262,6 +318,10 @@ int main(int argc, char **argv) {
         fprintf(stderr, "--recover cannot be combined with --gpu-resolve: the device resolve has no recovery rule\n");
         return 1;
     }
+    if (opt_carrier && cfg.gpu_resolve) {
+        fprintf(stderr, "--carrier cannot be combined with --gpu-resolve: the device resolve's delivery records have no room for it\n");
+        return 1;
+    }
     FILE *f = (filename[0] == '-' && filename[1] == 0) ? stdin : fopen(filename, "rb");
     if (!f) { perror("Opening data file"); return 1; }
 
@@ -278,6 +338,7 @@ int main(int argc, char **argv) {
     if (opt_arrival) modes_set_arrival(ctx, 1);
     if (opt_levels) modes_set_levels(ctx, 1);
     if (opt_spectrum) modes_set_spectrum(ctx, 1);
+    if (opt_carrier && modes_set_carrier(ctx, 1)) { fprintf(stderr, "--carrier: %s\n", modes_last_error(ctx)); return 1; }
     if (opt_recover && modes_set_recovery(ctx, 1)) { fprintf(stderr, "--recover: %s\n", modes_last_error(ctx)); return 1; }
     if (opt_weak && modes_set_weak_preambles(ctx, 1)) { fprintf(stderr, "--recover-weak: %s\n", modes_last_error(ctx)); return 1; }
     modes_set_sink(ctx, on_message, NULL);
@@ -292,6 +353,7 @@ int main(int argc, char **argv) {
     if (modes_finish(ctx)) { fprintf(stderr, "modes_finish: %s\n", modes_last_error(ctx)); return 1; }
     if (opt_levels) { take_levels(ctx); print_levels(); }
     if (opt_spectrum) { take_spectra(ctx); print_spectrum(sample_rate); }
+    if (opt_carrier) print_carrier();
     if (opt_stats) {                                        /* dump1090.c:2993-3006 */
         modes_stats st;
         modes_get_stats(ctx, &st);

@@ -91,7 +91,9 @@ typedef struct modes_message {
     int32_t  metype, mesub, heading_is_valid, heading, aircraft_type;
     int32_t  fflag, tflag, raw_latitude, raw_longitude;
     char     flight[9];
-    char     pad1[3];
+    char     pad1[1];
+    int16_t  carrier;           /* carrier code of the delivered attempt (modes_set_carrier): 0 = not measured,
+                                   otherwise its frequency is (carrier - 16384) * 100 Hz above the bytes' centre */
     int32_t  ew_dir, ew_velocity, ns_dir, ns_velocity;
     int32_t  vert_rate_source, vert_rate_sign, vert_rate, velocity;
     int32_t  movement, movement_valid, ground_track, ground_track_valid;
@@ -603,6 +605,37 @@ size_t modes_format_beast(const modes_message *mm, uint8_t *buf, size_t capacity
  * contexts.  Returns 0, or -1 for a NULL handle. */
 int    modes_set_arrival(modes_ctx *ctx, int on);
 int    modes_pool_set_arrival(modes_pool *p, int on);
+
+/* ---- carrier frequency of each message ------------------------------------------------------------
+ * Where in frequency a frame arrived, relative to the centre of the 2 MHz bytes the scan reads: the median
+ * over many aircraft is the receiver's own tuning error (its crystal error in ppm of 1090 MHz), a 4-10 MS/s
+ * capture's offset shows whether modes_set_input_offset was right, and a frame far from its aircraft's usual
+ * offset stands out.  For a decoded attempt (MODES_EVAL_DECODED) at buffer position j with b bits (56 or 112,
+ * from msgtype), its frame bits = its msg after any CRC fix:
+ *   1. The pulse sample of bit i is j+16+2i when the bit is 1 and j+17+2i when it is 0; the preamble's
+ *      pulses are at j+0, 2, 7 and 9.
+ *   2. The pairs are the pulse samples exactly two samples (1 us) apart: the preamble pairs (0, 2) and
+ *      (7, 9), and the pulses of each two consecutive bits of equal value.
+ *   3. With z = (I - 127) + i (Q - 127) of the 2 MHz bytes (resampled, decimated, shifted or converted on
+ *      the other input paths), the record of the attempt is the sum of z_later conj(z_earlier) over the
+ *      pairs:  re = sum (Ia Ib + Qa Qb),  im = sum (Ia Qb - Qa Ib)  (a the earlier sample), in int32.
+ * The host converts the delivered attempt's record to f = atan2(im, re) / (2 pi 1 us), unambiguous within
+ * +-500 kHz, and to the code 16384 + round(f / 100 Hz) (halves away from zero) in modes_message.carrier; a
+ * frame above the centre of the bytes has f > 0.  The code is 0 (not measured) with the switch off, for
+ * re = im = 0, for recovered messages and for frames from the hex door.  csrc/modes_carrier_core.cuh has
+ * the arithmetic.
+ *
+ * Carrier measurement is off by default.  When it is on, every batch submitted afterwards runs the signal
+ * pass's kernel (one more launch per batch when signal and arrival measurement are off, none more when one
+ * is on), which writes one modes_carrier record per candidate to device memory; the records are copied to
+ * the host beside the candidate records.  On an n_gpus > 1 context the setting reaches every GPU; a pool
+ * applies it to all its device contexts.  It cannot be combined with gpu_resolve, whose delivery records
+ * have no room for it.  Returns 0, or -1 for a NULL handle or with gpu_resolve. */
+typedef struct modes_carrier {
+    int32_t re[2], im[2];       /* the record of pass[k]; 0, 0 for an attempt not decoded */
+} modes_carrier;
+int    modes_set_carrier(modes_ctx *ctx, int on);
+int    modes_pool_set_carrier(modes_pool *p, int on);
 
 /* ---- receiver levels: noise floor, peak and clipping per buffer --------------------------------
  * What an operator reads of a receiver besides its messages: how loud the channel is, how close the
