@@ -15,7 +15,7 @@ build/%.o: $(CSRC)/%.cu $(CSRC)/modes_internal.h $(CSRC)/modes_eval_serial.cuh $
 	@mkdir -p build
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@
 
-build/%.o: $(CSRC)/%.cpp $(CSRC)/modes_internal.h $(CSRC)/modes_carrier_core.cuh $(CSRC)/modes_input_core.cuh $(CSRC)/modes_resample_core.cuh $(CSRC)/modes_spectrum_core.cuh include/modes_b200.h
+build/%.o: $(CSRC)/%.cpp $(CSRC)/modes_internal.h $(CSRC)/modes_carrier_core.cuh $(CSRC)/modes_resolve_core.cuh $(CSRC)/modes_input_core.cuh $(CSRC)/modes_resample_core.cuh $(CSRC)/modes_spectrum_core.cuh include/modes_b200.h
 	@mkdir -p build
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 

@@ -1666,11 +1666,7 @@ int modes_resolver_tail_cache(const modes_resolver *r, const modes_candidate *ca
 int modes_resolver_run_tentative(modes_resolver *r, const modes_candidate *candidates, const modes_tile *tiles,
                                  size_t n_tiles, int64_t buffer_base) {
     if (!r || !tiles) return -1;
-    r->tentative = r->rs;
-    memset(r->tentative.stats, 0, sizeof(r->tentative.stats));
-    memset(&r->tentative.rstats, 0, sizeof(r->tentative.rstats));
-    memset(&r->tentative.wstats, 0, sizeof(r->tentative.wstats));
-    r->tentative.cur_buffer = -1; r->tentative.next_j = 0; r->tentative.next_j_recovered = 0;
+    r->tentative.start_part(r->rs, true);
     resolve_tentative(r->tentative, r->rc, candidates, tiles, n_tiles, buffer_base, r->scratch);
     r->has_tentative = true;
     return 0;
@@ -1679,10 +1675,7 @@ int modes_resolver_run_tentative(modes_resolver *r, const modes_candidate *candi
 int modes_resolver_commit(modes_resolver *r, modes_sink_fn sink, void *user) {
     if (!r || !r->has_tentative) return -1;
     r->out.sink = sink; r->out.user = user;
-    for (int i = 0; i < 8; i++) r->rs.stats[i] += r->tentative.stats[i];
-    add_recovery_stats(r->rs.rstats, r->tentative.rstats);
-    add_recovery_stats(r->rs.wstats, r->tentative.wstats);
-    memcpy(r->rs.icao, r->tentative.icao, sizeof(r->rs.icao));
+    r->rs.fold_part(r->tentative);
     r->rs.cur_buffer = r->tentative.cur_buffer; r->rs.next_j = r->tentative.next_j;
     r->rs.next_j_recovered = r->tentative.next_j_recovered;
     resolve_commit(r->out, r->scratch);

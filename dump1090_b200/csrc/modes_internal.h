@@ -269,6 +269,11 @@ struct ResolveState {
     modes_recovery_stats rstats;
     modes_recovery_stats wstats; // recoveries at weak preambles (modes_set_weak_preambles)
     void reset();
+    // A part of the stream judged on its own after `from`: from's cache and skip state, totals zeroed;
+    // at_buffer: the part starts at a buffer boundary (no skip state).
+    void start_part(const ResolveState &from, bool at_buffer);
+    // Take over a finished part's cache and add its totals.  The skip state is left to the caller.
+    void fold_part(const ResolveState &part);
 };
 
 // recover_signal: recovered messages carry their record's signal (else 0)
@@ -311,7 +316,6 @@ void resolve_commit(MessageOut &out, ResolveScratch *scratch);
 void deliver_gpu(const modes_delivery *d, size_t n, int64_t buffer_base, MessageOut &out);
 // The order-dependent tail of decodeModesMessage + field decode for one evaluated frame.
 int finish_message(ResolveState &st, const modes_frame_eval &p, modes_message *out);
-void add_recovery_stats(modes_recovery_stats &to, const modes_recovery_stats &from);
 
 // ---- host glue shared by the context (modes_api.cpp) and the receiver pool (modes_pool.cpp) ----
 // An owning, grow-only array of T in device memory (DevBuf) or pinned host memory (PinnedBuf).

@@ -28,6 +28,7 @@
 #include <vector>
 #include "modes_internal.h"
 #include "modes_carrier_core.cuh"
+#include "modes_resolve_core.cuh"
 
 namespace modes {
 
@@ -41,18 +42,32 @@ void ResolveState::reset() {
     std::memset(&wstats, 0, sizeof(wstats));
 }
 
-static inline uint32_t icao_slot(uint32_t a) {           // dump1090.c:898-905
-    a = ((a >> 16) ^ a) * 0x45d9f3bu;
-    a = ((a >> 16) ^ a) * 0x45d9f3bu;
-    a = (a >> 16) ^ a;
-    return a & 1023u;
+void ResolveState::start_part(const ResolveState &from, bool at_buffer) {
+    *this = from;
+    std::memset(stats, 0, sizeof(stats));
+    std::memset(&rstats, 0, sizeof(rstats));
+    std::memset(&wstats, 0, sizeof(wstats));
+    if (at_buffer) { cur_buffer = -1; next_j = 0; next_j_recovered = 0; }
 }
 
-static inline bool icao_seen(const ResolveState &st, uint32_t a) {
-    return a != 0 && st.icao[icao_slot(a)] == a;         // dump1090.c:919-925, TTL not modelled
+static void add_recovery_stats(modes_recovery_stats &to, const modes_recovery_stats &from) {
+    to.considered += from.considered; to.found += from.found; to.ambiguous += from.ambiguous;
+    to.unknown_address += from.unknown_address; to.dropped += from.dropped; to.delivered += from.delivered;
 }
 
-static inline int bits_by_type(int df) { return (df >= 16 && df <= 21) ? 112 : 56; }
+void ResolveState::fold_part(const ResolveState &part) {
+    for (int i = 0; i < 8; i++) stats[i] += part.stats[i];
+    add_recovery_stats(rstats, part.rstats);
+    add_recovery_stats(wstats, part.wstats);
+    std::memcpy(icao, part.icao, sizeof(icao));
+}
+
+// The host's address cache, for the rules of modes_resolve_core.cuh.
+struct IcaoCache {
+    uint32_t *slots;
+    uint32_t read(uint32_t s) const { return slots[s]; }
+    void write(uint32_t s, uint32_t a) { slots[s] = a; }
+};
 
 // struct modesMessage fields that are pure functions of the frame bytes.
 static void decode_fields(modes_message *o) {
@@ -140,38 +155,11 @@ static void decode_fields(modes_message *o) {
     }
 }
 
-// Order-dependent verdict of decodeModesMessage for one evaluated frame
-// (dump1090.c:1108-1128 statistics, :1183-1210 ICAO logic) without building the
-// message: returns crcok; *iid and *ap_addr receive the DF11 interrogator id and
-// the recovered address of an address/parity format (0 when not applicable).
-static inline int judge(ResolveState &st, const modes_frame_eval &p, uint32_t *iid, uint32_t *ap_addr) {
-    *iid = 0; *ap_addr = 0;
-    if (p.nfixed == 1) st.stats[6]++;                      // dump1090.c:1122-1126
-    else if (p.nfixed == 2) st.stats[7]++;
-    const int df = p.msgtype;
-    int crcok = p.crc == 0;
-    if (df == 11 || df == 17 || df == 18) {
-        const uint32_t addr = ((uint32_t)p.msg[1] << 16) | ((uint32_t)p.msg[2] << 8) | (uint32_t)p.msg[3];
-        if (crcok && p.nfixed == 0) st.icao[icao_slot(addr)] = addr;          // :1198-1200
-        if (df == 11 && !crcok && p.crc < 80 && icao_seen(st, addr)) {         // :1204-1209
-            *iid = p.crc;
-            crcok = 1;
-        }
-        return crcok;
-    }
-    // parity field = CRC ^ address, so the syndrome is the sender's address (:962-974)
-    if ((df == 0 || df == 4 || df == 5 || df == 16 || df == 20 || df == 21 || df == 24) && icao_seen(st, p.crc)) {
-        *ap_addr = p.crc;
-        return 1;
-    }
-    return 0;
-}
-
 static void build_message(const modes_frame_eval &p, int crcok, uint32_t iid, uint32_t ap_addr, modes_message *o) {
     std::memset(o, 0, sizeof(*o));
     std::memcpy(o->msg, p.msg, 14);
     o->msgtype = p.msgtype;
-    o->msgbits = bits_by_type(p.msgtype);
+    o->msgbits = (int32_t)rcore::bits_by_type(p.msgtype);
     o->crc = p.crc;
     o->nfixed = p.nfixed;
     o->signal = p.signal;
@@ -183,10 +171,15 @@ static void build_message(const modes_frame_eval &p, int crcok, uint32_t iid, ui
     if (ap_addr) { o->aa1 = (ap_addr >> 16) & 0xff; o->aa2 = (ap_addr >> 8) & 0xff; o->aa3 = ap_addr & 0xff; }
 }
 
+// A judged attempt's message fields: the DF11 interrogator id, the address of an address/parity format.
+static inline uint32_t iid_of(const rcore::Decision &d) { return d.extra_is_ap ? 0u : d.extra; }
+static inline uint32_t ap_addr_of(const rcore::Decision &d) { return d.extra_is_ap ? d.extra : 0u; }
+
 int finish_message(ResolveState &st, const modes_frame_eval &p, modes_message *o) {
-    uint32_t iid, ap;
-    const int crcok = judge(st, p, &iid, &ap);
-    build_message(p, crcok, iid, ap, o);
+    IcaoCache cache{st.icao};
+    rcore::Decision d{};
+    const int crcok = (int)rcore::judge(st, cache, p, d);
+    build_message(p, crcok, iid_of(d), ap_addr_of(d), o);
     return crcok;
 }
 
@@ -203,14 +196,6 @@ struct Delivery {
     uint8_t recovered;           // eval is a recovery record's frame (1: at a candidate, 2: at a weak preamble): crc 0, nfixed = its flips
     int16_t carrier;             // the attempt's carrier code (0: not measured)
 };
-
-static inline void materialise(const Delivery &d, modes_message *mm) {
-    build_message(d.eval, d.crcok, d.iid, d.ap_addr, mm);
-    mm->sample_pos = d.sample_pos;
-    mm->phase_corrected = d.phase_corrected;
-    if (d.recovered) { mm->recovered = d.recovered; mm->errorbit = -1; }
-    mm->carrier = d.carrier;
-}
 
 // Cores this process may actually keep busy: the CPUs it is allowed on, cut down to the CPU-time
 // quota of its control group (a container that sees 128 CPUs but is granted 16 CPUs' worth of time
@@ -299,25 +284,6 @@ class BuildPool {
     uint64_t gen_ = 0;
 };
 
-// One evaluated attempt, as detectModeS handles it after the delta gate; car: the candidate's carrier
-// record (nullptr: not measured), k: which of its attempts this is.
-// Returns true when the message is good (the scan skips past it).
-static inline bool attempt(ResolveState &st, const ResolveConfig &cfg, const modes_frame_eval &p, bool retry,
-                           int64_t sample_pos, std::vector<Delivery> &deliveries, const modes_carrier *car, int k) {
-    if (!(p.flags & MODES_EVAL_DECODED)) return false;
-    uint32_t iid, ap;
-    const int crcok = judge(st, p, &iid, &ap);
-    if (crcok || retry) {                                  // dump1090.c:1738-1753
-        if (!(p.flags & MODES_EVAL_ERRORS)) st.stats[2]++;
-        if (p.nfixed == 0) st.stats[crcok ? 3 : 4]++;
-        else { st.stats[4]++; st.stats[5]++; st.stats[6]++; }
-    }
-    if (cfg.check_crc == 0 || crcok)                       // dump1090.c:1803; :1772-1773
-        deliveries.push_back(Delivery{p, sample_pos, iid, ap, (uint8_t)crcok, (uint8_t)(crcok && retry), (uint8_t)0,
-                                      car ? carrier::code_of(car->re[k], car->im[k]) : (int16_t)0});
-    return crcok != 0;
-}
-
 // With recovery records (rec[k] belongs to cands[k]; include/modes_b200.h rules 1-6), a candidate the
 // walk visits where neither attempt was good may add a recovered message.  It goes into the list at
 // once, in stream order, and is taken out again if the reference delivers a good message within its
@@ -353,7 +319,8 @@ static inline void recovery_step(ResolveState &st, const ResolveConfig &cfg, con
     if (r.status != MODES_RECOVER_FOUND) return;                           // rule 4
     stats.found++;
     const uint32_t addr = ((uint32_t)r.msg[1] << 16) | ((uint32_t)r.msg[2] << 8) | (uint32_t)r.msg[3];
-    if (!icao_seen(st, addr)) { stats.unknown_address++; return; }         // rule 5
+    IcaoCache cache{st.icao};
+    if (!rcore::seen(cache, addr)) { stats.unknown_address++; return; }    // rule 5
     modes_frame_eval e{};
     std::memcpy(e.msg, r.msg, 14);
     e.msgtype = (uint8_t)(r.msg[0] >> 3);
@@ -417,6 +384,7 @@ static void walk_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_c
     // in stream order is a chain of cache misses (the records were just written by DMA).  Request
     // the lines of a tile well before it is reached.
     constexpr size_t kAhead = 24;
+    IcaoCache cache{st.icao};
     for (size_t ti = 0; ti < n_tiles; ti++) {
         if (ti + kAhead < n_tiles && tiles[ti + kAhead].count) {
             const char *p = reinterpret_cast<const char *>(cands + tiles[ti + kAhead].offset);
@@ -436,28 +404,16 @@ static void walk_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_c
             const int64_t buffer = buffer_base + rb;
             const uint32_t j = (uint32_t)(c->t & (kBufSamples - 1));
             if (buffer != st.cur_buffer) { st.cur_buffer = buffer; st.next_j = 0; st.next_j_recovered = 0; }
-            if (j < st.next_j) continue;                   // inside a message already taken (rule 1)
-            st.stats[0]++;                                 // dump1090.c:1651
+            rcore::Decision d[2] = {};
+            const int visit = rcore::candidate(st, cache, j, c->pass[0], c->pass[1], cfg.check_crc, d);
+            if (visit < 0) continue;                       // inside a message already taken (rule 1)
             const int64_t pos = buffer * (int64_t)kBufSamples + j - MODES_CARRY_SAMPLES;
-            bool good = false;
-            const modes_frame_eval &p1 = c->pass[0];
-            const modes_carrier *ck = car ? car + k0 + k : nullptr;
-            if (p1.flags & MODES_EVAL_GATE_OK) {           // dump1090.c:1723-1726
-                const uint32_t skip = (uint32_t)(8 + bits_by_type(p1.msgtype)) * 2 + 1;
-                if (attempt(st, cfg, p1, false, pos, deliveries, ck, 0)) {
-                    st.next_j = j + skip;
-                    good = true;
-                } else {
-                    if (j) st.stats[1]++;                  // dump1090.c:1660-1663
-                    const modes_frame_eval &p2 = c->pass[1];
-                    if (p2.flags & MODES_EVAL_GATE_OK) {
-                        const uint32_t skip2 = (uint32_t)(8 + bits_by_type(p2.msgtype)) * 2 + 1;
-                        if (attempt(st, cfg, p2, true, pos, deliveries, ck, 1)) { st.next_j = j + skip2; good = true; }
-                    }
-                }
-            }
-            if constexpr (kRecover) recovery_step(st, cfg, rec[k0 + k], good, buffer, j, pos, deliveries, pend, st.rstats, 1);
-            (void)good;
+            for (int a = 0; a < 2; a++)
+                if (d[a].deliver)
+                    deliveries.push_back(Delivery{c->pass[a], pos, iid_of(d[a]), ap_addr_of(d[a]), (uint8_t)d[a].crcok,
+                                                  (uint8_t)d[a].phase_corrected, (uint8_t)0,
+                                                  car ? carrier::code_of(car[k0 + k].re[a], car[k0 + k].im[a]) : (int16_t)0});
+            if constexpr (kRecover) recovery_step(st, cfg, rec[k0 + k], visit > 0, buffer, j, pos, deliveries, pend, st.rstats, 1);
         }
     }
     if (merge) weak_steps(st, cfg, wc, UINT64_MAX, b_hi, buffer_base, deliveries, pend);
@@ -471,54 +427,44 @@ static void judge_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_
     else walk_tiles<false>(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, b_lo, b_hi, nullptr, nullptr, car);
 }
 
-// Build the delivered structs: in place and in parallel for array output, then the callback
-// (if any) sequentially in stream order.
-static void deliver(const std::vector<Delivery> &deliveries, MessageOut &out) {
-    const size_t n = deliveries.size();
+// Build n delivered structs with build(i, struct): in place and in parallel for array output, then
+// the callback (if any) sequentially in stream order.
+template <class Build>
+static void deliver_each(size_t n, MessageOut &out, const Build &build) {
     size_t in_array = 0;
     if (out.array && out.count < out.capacity) {
         in_array = out.capacity - out.count < n ? out.capacity - out.count : n;
         modes_message *base = out.array + out.count;
-        const Delivery *d = deliveries.data();
-        BuildPool::get().run(in_array, [=](size_t b, size_t e) {
-            for (size_t i = b; i < e; i++) {
-                materialise(d[i], base + i);
-            }
-        });
+        BuildPool::get().run(in_array, [&](size_t b, size_t e) { for (size_t i = b; i < e; i++) build(i, base + i); });
     }
     if (out.sink) {
         for (size_t i = 0; i < n; i++) {
             if (i < in_array) { out.sink(out.user, out.array + out.count + i); continue; }
             modes_message tmp;
-            materialise(deliveries[i], &tmp);
+            build(i, &tmp);
             out.sink(out.user, &tmp);
         }
     }
     out.count += n;
 }
 
+static void deliver(const std::vector<Delivery> &deliveries, MessageOut &out) {
+    deliver_each(deliveries.size(), out, [d = deliveries.data()](size_t i, modes_message *mm) {
+        build_message(d[i].eval, d[i].crcok, d[i].iid, d[i].ap_addr, mm);
+        mm->sample_pos = d[i].sample_pos;
+        mm->phase_corrected = d[i].phase_corrected;
+        if (d[i].recovered) { mm->recovered = d[i].recovered; mm->errorbit = -1; }
+        mm->carrier = d[i].carrier;
+    });
+}
+
 void deliver_gpu(const modes_delivery *d, size_t n, int64_t buffer_base, MessageOut &out) {
-    auto build = [=](const modes_delivery &x, modes_message *mm) {
-        const bool is_ap = (x.bits >> 16) & 1u;
-        build_message(x.eval, (int)(x.bits & 1u), is_ap ? 0u : x.extra, is_ap ? x.extra : 0u, mm);
-        mm->sample_pos = (buffer_base << 17) + x.t - MODES_CARRY_SAMPLES;
-        mm->phase_corrected = (int)((x.bits >> 8) & 1u);
-    };
-    size_t in_array = 0;
-    if (out.array && out.count < out.capacity) {
-        in_array = out.capacity - out.count < n ? out.capacity - out.count : n;
-        modes_message *base = out.array + out.count;
-        BuildPool::get().run(in_array, [=](size_t b, size_t e) { for (size_t i = b; i < e; i++) build(d[i], base + i); });
-    }
-    if (out.sink) {
-        for (size_t i = 0; i < n; i++) {
-            if (i < in_array) { out.sink(out.user, out.array + out.count + i); continue; }
-            modes_message tmp;
-            build(d[i], &tmp);
-            out.sink(out.user, &tmp);
-        }
-    }
-    out.count += n;
+    deliver_each(n, out, [=](size_t i, modes_message *mm) {
+        const bool is_ap = (d[i].bits >> 16) & 1u;
+        build_message(d[i].eval, (int)(d[i].bits & 1u), is_ap ? 0u : d[i].extra, is_ap ? d[i].extra : 0u, mm);
+        mm->sample_pos = (buffer_base << 17) + d[i].t - MODES_CARRY_SAMPLES;
+        mm->phase_corrected = (int)((d[i].bits >> 8) & 1u);
+    });
 }
 
 // ---- parts of a stream judged concurrently, exactly
@@ -544,10 +490,10 @@ struct Part {
 };
 struct PartRun { ResolveState start, end; std::vector<Delivery> deliveries; };
 struct ResolveScratch {
-    std::vector<Delivery> deliveries;
+    std::vector<Part> parts;
     std::vector<PartRun> runs;   // kept between calls: delivery lists keep their capacity (growing them from nothing
                                  // in every call costs more in page faults, taken concurrently, than the verdicts)
-    size_t n_runs_held = 0;      // > 0: a tentative resolve left its deliveries in runs[0 .. n_runs_held)
+    size_t n_runs_held = 0;      // the last resolve's deliveries are in runs[0 .. n_runs_held) until delivered
 };
 ResolveScratch *scratch_create() { return new (std::nothrow) ResolveScratch(); }
 void scratch_destroy(ResolveScratch *s) { delete s; }
@@ -590,25 +536,22 @@ static void cut_parts(const modes_candidate *cands, const modes_tile *tiles, siz
     parts.push_back(p);
 }
 
-void add_recovery_stats(modes_recovery_stats &to, const modes_recovery_stats &from) {
-    to.considered += from.considered; to.found += from.found; to.ambiguous += from.ambiguous;
-    to.unknown_address += from.unknown_address; to.dropped += from.dropped; to.delivered += from.delivered;
-}
-
 // Judge the parts (rounds of guess and verify, see above); runs[k] receives part k's deliveries
-// and statistics, `st` the state after the last part.
+// and statistics, `st` the state after the last part.  A single part is judged in place on `st`.
 static int judge_parts(ResolveState &st, const ResolveConfig &cfg, const std::vector<Part> &parts, PartRun *runs) {
     const size_t n = parts.size();
+    if (n == 1) {
+        const Part &p = parts[0];
+        runs[0].deliveries.clear();
+        judge_tiles(st, cfg, p.cands, p.tiles, p.n_tiles, p.buffer_base, runs[0].deliveries, p.b_lo, p.b_hi, p.rec, p.weak, p.car);
+        return 1;
+    }
     ResolveState blank;
     blank.reset();
     auto run_part = [&](size_t k, const ResolveState &from) {
         PartRun &r = runs[k];
         const Part &p = parts[k];
-        r.start = from;
-        std::memset(r.start.stats, 0, sizeof(r.start.stats));
-        std::memset(&r.start.rstats, 0, sizeof(r.start.rstats));
-        std::memset(&r.start.wstats, 0, sizeof(r.start.wstats));
-        if (k) { r.start.cur_buffer = -1; r.start.next_j = 0; r.start.next_j_recovered = 0; }   // a part starts a buffer
+        r.start.start_part(from, k != 0);                  // a later part starts a buffer
         r.end = r.start;
         r.deliveries.clear();
         judge_tiles(r.end, cfg, p.cands, p.tiles + p.tile_lo, p.n_tiles - p.tile_lo, p.buffer_base, r.deliveries, p.b_lo, p.b_hi,
@@ -630,8 +573,8 @@ static int judge_parts(ResolveState &st, const ResolveConfig &cfg, const std::ve
             // part k-1 writes (addresses are re-confirmed every second or so, so the tail of a long
             // part has normally written every slot the whole part leaves changed).
             const Part &q = parts[k - 1];
-            ResolveState g = st;
-            g.cur_buffer = -1; g.next_j = 0; g.next_j_recovered = 0;   // (recovery never writes the cache: the guess skips it)
+            ResolveState g;
+            g.start_part(st, true);                        // (recovery never writes the cache: the guess skips it)
             const size_t end_tile = parts[k].first_of_shard ? q.n_tiles : (parts[k].tile_lo + 1 < q.n_tiles ? parts[k].tile_lo + 1 : q.n_tiles);
             const size_t len = end_tile - q.tile_lo;
             size_t tail = len / 16 > 128 ? len / 16 : 128;             // at least ~1 M samples (half a second of stream)
@@ -656,96 +599,26 @@ static int judge_parts(ResolveState &st, const ResolveConfig &cfg, const std::ve
             if (std::memcmp(truth.icao, runs[done].start.icao, sizeof(truth.icao)) != 0) break;
         }
     }
-    for (size_t k = 0; k < n; k++) {
-        for (int i = 0; i < 8; i++) st.stats[i] += runs[k].end.stats[i];
-        add_recovery_stats(st.rstats, runs[k].end.rstats);
-        add_recovery_stats(st.wstats, runs[k].end.wstats);
-    }
-    if (n) {
-        std::memcpy(st.icao, runs[n - 1].end.icao, sizeof(st.icao));
-        // the skip state is that of the last part that saw a candidate (an empty part leaves none)
-        for (size_t k = n; k-- > 0;)
-            if (runs[k].end.cur_buffer != -1 || k == 0) {
-                st.cur_buffer = runs[k].end.cur_buffer; st.next_j = runs[k].end.next_j;
-                st.next_j_recovered = runs[k].end.next_j_recovered;
-                break;
-            }
-    }
+    for (size_t k = 0; k < n; k++) st.fold_part(runs[k].end);
+    // the skip state is that of the last part that saw a candidate (an empty part leaves none)
+    for (size_t k = n; k-- > 0;)
+        if (runs[k].end.cur_buffer != -1 || k == 0) {
+            st.cur_buffer = runs[k].end.cur_buffer; st.next_j = runs[k].end.next_j;
+            st.next_j_recovered = runs[k].end.next_j_recovered;
+            break;
+        }
     return rounds;
 }
 
-static PartRun *runs_for(ResolveScratch *scratch, size_t n) {
-    if (scratch->runs.size() < n) scratch->runs.resize(n);
-    return scratch->runs.data();
-}
-
-void resolve_candidates(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands,
-                        const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, MessageOut &out,
-                        ResolveScratch *scratch, const modes_recovered *recovered, const WeakList &weak,
-                        const modes_carrier *carrier) {
-    const bool timing = std::getenv("MODES_RESOLVE_TIMING") != nullptr;
-    auto now = [] { return std::chrono::steady_clock::now(); };
-    auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) {
-        return std::chrono::duration<double, std::milli>(b - a).count(); };
-    const auto t0 = now();
-    scratch->n_runs_held = 0;
-    const size_t want = parts_for(n_tiles);
-    if (want <= 1) {
-        std::vector<Delivery> &deliveries = scratch->deliveries;
-        deliveries.clear();
-        judge_tiles(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, 0, UINT32_MAX, recovered, &weak, carrier);
-        const auto t1 = now();
-        deliver(deliveries, out);
-        if (timing) std::fprintf(stderr, "resolve_candidates: %zu tiles, verdicts %.2f ms, structs %.2f ms\n", n_tiles, ms(t0, t1), ms(t1, now()));
-        return;
-    }
-    std::vector<Part> parts;
-    cut_parts(cands, tiles, n_tiles, buffer_base, want, parts, recovered, &weak, carrier);
-    PartRun *runs = runs_for(scratch, parts.size());
-    const int rounds = judge_parts(st, cfg, parts, runs);
-    const auto t1 = now();
-    for (size_t k = 0; k < parts.size(); k++) deliver(runs[k].deliveries, out);
-    if (timing)
-        std::fprintf(stderr, "resolve_candidates: %zu tiles in %zu parts, %d rounds, verdicts %.2f ms, structs %.2f ms\n", n_tiles,
-                     parts.size(), rounds, ms(t0, t1), ms(t1, now()));
-}
-
-void resolve_tentative(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands, const modes_tile *tiles,
-                       size_t n_tiles, int64_t buffer_base, ResolveScratch *scratch) {
-    scratch->deliveries.clear();
-    scratch->n_runs_held = 0;
-    const size_t want = parts_for(n_tiles);
-    if (want <= 1) {
-        judge_tiles(st, cfg, cands, tiles, n_tiles, buffer_base, scratch->deliveries);
-        return;
-    }
-    std::vector<Part> parts;
-    cut_parts(cands, tiles, n_tiles, buffer_base, want, parts);
-    judge_parts(st, cfg, parts, runs_for(scratch, parts.size()));
-    scratch->n_runs_held = parts.size();
-}
-
-void resolve_commit(MessageOut &out, ResolveScratch *scratch) {
-    if (scratch->n_runs_held) {
-        for (size_t k = 0; k < scratch->n_runs_held; k++) { deliver(scratch->runs[k].deliveries, out); scratch->runs[k].deliveries.clear(); }
-        scratch->n_runs_held = 0;
-        return;
-    }
-    deliver(scratch->deliveries, out);
-    scratch->deliveries.clear();
-}
-
-// Several shards of one stream (e.g. one per GPU), resolved concurrently and exactly: every shard
-// is a part, long shards are cut once more (see judge_parts).
-void resolve_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards, const modes_candidate *const *cands,
-                    const modes_tile *const *tiles, const size_t *n_tiles, const int64_t *buffer_base,
-                    MessageOut &out, ResolveScratch *scratch, const modes_recovered *const *recovered, const WeakList *weak,
-                    const modes_carrier *const *carrier) {
-    const bool timing = std::getenv("MODES_RESOLVE_TIMING") != nullptr;
-    auto now = [] { return std::chrono::steady_clock::now(); };
-    auto t_start = now();
-    scratch->n_runs_held = 0;
-    std::vector<Part> parts;
+// Judge several shards of one stream (e.g. one per GPU) concurrently and exactly: every shard is a
+// part, long shards are cut once more (see judge_parts).  The deliveries are held in the scratch
+// until resolve_commit.  Returns the rounds judge_parts took.
+static int judge_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards, const modes_candidate *const *cands,
+                        const modes_tile *const *tiles, const size_t *n_tiles, const int64_t *buffer_base, ResolveScratch *scratch,
+                        const modes_recovered *const *recovered = nullptr, const WeakList *weak = nullptr,
+                        const modes_carrier *const *carrier = nullptr) {
+    std::vector<Part> &parts = scratch->parts;
+    parts.clear();
     size_t threads_left = parts_for((size_t)-1);
     for (size_t k = 0; k < n_shards; k++) {
         size_t want = parts_for(n_tiles[k]);
@@ -755,14 +628,44 @@ void resolve_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards,
                   recovered && weak ? weak + k : nullptr, carrier ? carrier[k] : nullptr);
         threads_left = threads_left > want ? threads_left - want : 0;
     }
-    PartRun *runs = runs_for(scratch, parts.size());
-    const int rounds = judge_parts(st, cfg, parts, runs);
-    auto t_judged = now();
-    for (size_t k = 0; k < parts.size(); k++) deliver(runs[k].deliveries, out);
+    if (scratch->runs.size() < parts.size()) scratch->runs.resize(parts.size());
+    const int rounds = judge_parts(st, cfg, parts, scratch->runs.data());
+    scratch->n_runs_held = parts.size();
+    return rounds;
+}
+
+void resolve_commit(MessageOut &out, ResolveScratch *scratch) {
+    for (size_t k = 0; k < scratch->n_runs_held; k++) { deliver(scratch->runs[k].deliveries, out); scratch->runs[k].deliveries.clear(); }
+    scratch->n_runs_held = 0;
+}
+
+void resolve_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards, const modes_candidate *const *cands,
+                    const modes_tile *const *tiles, const size_t *n_tiles, const int64_t *buffer_base,
+                    MessageOut &out, ResolveScratch *scratch, const modes_recovered *const *recovered, const WeakList *weak,
+                    const modes_carrier *const *carrier) {
+    const bool timing = std::getenv("MODES_RESOLVE_TIMING") != nullptr;
+    auto now = [] { return std::chrono::steady_clock::now(); };
+    const auto t_start = now();
+    const int rounds = judge_shards(st, cfg, n_shards, cands, tiles, n_tiles, buffer_base, scratch, recovered, weak, carrier);
+    const size_t n_parts = scratch->n_runs_held;
+    const auto t_judged = now();
+    resolve_commit(out, scratch);
     if (timing)
-        std::fprintf(stderr, "resolve_shards: %zu shards in %zu parts, %d rounds, verdicts %.2f ms, structs %.2f ms\n", n_shards,
-                     parts.size(), rounds, std::chrono::duration<double, std::milli>(t_judged - t_start).count(),
+        std::fprintf(stderr, "resolve: %zu shards in %zu parts, %d rounds, verdicts %.2f ms, structs %.2f ms\n", n_shards, n_parts,
+                     rounds, std::chrono::duration<double, std::milli>(t_judged - t_start).count(),
                      std::chrono::duration<double, std::milli>(now() - t_judged).count());
+}
+
+void resolve_candidates(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands,
+                        const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, MessageOut &out,
+                        ResolveScratch *scratch, const modes_recovered *recovered, const WeakList &weak,
+                        const modes_carrier *carrier) {
+    resolve_shards(st, cfg, 1, &cands, &tiles, &n_tiles, &buffer_base, out, scratch, &recovered, &weak, &carrier);
+}
+
+void resolve_tentative(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands, const modes_tile *tiles,
+                       size_t n_tiles, int64_t buffer_base, ResolveScratch *scratch) {
+    judge_shards(st, cfg, 1, &cands, &tiles, &n_tiles, &buffer_base, scratch);
 }
 
 }  // namespace modes
