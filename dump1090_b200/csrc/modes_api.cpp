@@ -511,20 +511,9 @@ int wait_batch(modes_ctx *ctx, Slot &s, uint64_t *n_out) {
     return 0;
 }
 
-// One finished batch's results in pinned host memory, as the host resolve takes them.
-struct ShardView {
-    const modes_candidate *cands = nullptr;
-    const modes_tile *tiles = nullptr;
-    size_t n_tiles = 0;
-    int64_t buffer_base = 0;
-    const modes_recovered *recovered = nullptr;   // the batch ran no recovery: nullptr
-    WeakList weak;
-    const modes_carrier *carrier = nullptr;       // the batch measured no carrier: nullptr
-};
-
 // Queue the copies of the slot's finished batch (n candidate records) to pinned memory on its
-// stream; the view is valid once the stream has been waited for.
-int fetch_async(modes_ctx *ctx, Slot &s, uint64_t n, ShardView &v) {
+// stream; the shard is valid once the stream has been waited for.
+int fetch_async(modes_ctx *ctx, Slot &s, uint64_t n, Shard &v) {
     const size_t nt = tiles_for((uint64_t)s.n_buffers * kBufSamples);
     CK(ctx, ensure_spare(s.h_records, n));
     CK(ctx, s.h_tiles.ensure(nt));
@@ -549,8 +538,8 @@ int fetch_async(modes_ctx *ctx, Slot &s, uint64_t n, ShardView &v) {
         if (n) CK(ctx, cudaMemcpyAsync(s.h_carrier.get(), s.d_carrier.get(), n * sizeof(modes_carrier), cudaMemcpyDeviceToHost, s.stream));
     }
     CK(ctx, cudaMemcpyAsync(s.h_tiles.get(), s.out_tiles, nt * sizeof(modes_tile), cudaMemcpyDeviceToHost, s.stream));
-    v = ShardView{s.h_records.get(), s.h_tiles.get(), nt, s.buffer_base, s.feat.recover ? s.h_recovered.get() : nullptr, wl,
-                  s.feat.carrier ? s.h_carrier.get() : nullptr};
+    v = Shard{s.h_records.get(), s.h_tiles.get(), nt, s.buffer_base, s.feat.recover ? s.h_recovered.get() : nullptr, wl,
+              s.feat.carrier ? s.h_carrier.get() : nullptr};
     return 0;
 }
 
@@ -588,13 +577,12 @@ int collect(modes_ctx *ctx, Slot &s) {
         deliver_gpu(s.h_deliveries.get(), nd, s.buffer_base, ctx->out);
         return 0;
     }
-    ShardView v;
+    Shard v;
     if (fetch_async(ctx, s, n, v)) return -1;
     CK(ctx, wait_stream(s.stream));
     const double t2 = dbg ? now_ms() : 0;
     ResolveConfig rc{ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->cfg.check_crc, s.feat.signal ? 1 : 0};
-    resolve_candidates(ctx->rs, rc, v.cands, v.tiles, v.n_tiles, v.buffer_base, ctx->out, ctx->scratch, v.recovered, v.weak,
-                       v.carrier);
+    resolve_candidates(ctx->rs, rc, v, ctx->out, ctx->scratch);
     if (dbg) fprintf(stderr, "[collect] %zu buffers, %llu cands: wait %.3f ms, d2h %.3f ms, resolve %.3f ms (t=%.3f)\n",
                      s.n_buffers, (unsigned long long)n, t1 - t0, t2 - t1, now_ms() - t2, now_ms());
     return 0;
@@ -606,14 +594,8 @@ int collect_group(modes_ctx *ctx, int parity) {
     const size_t n = ctx->group_n[parity];
     if (!n) return 0;
     ctx->group_n[parity] = 0;
-    std::vector<const modes_candidate *> cands(n);
-    std::vector<const modes_tile *> tiles(n);
-    std::vector<size_t> n_tiles(n);
-    std::vector<int64_t> base(n);
-    std::vector<const modes_recovered *> recovered(n, nullptr);
-    std::vector<WeakList> weak(n);
-    std::vector<const modes_carrier *> carrier(n, nullptr);
-    bool any_recover = false, signal = false, any_carrier = false;
+    std::vector<Shard> shards(n);
+    bool signal = false;
     for (size_t k = 0; k < n; k++) {
         modes_ctx *g = ctx->gpus[k];
         Slot &s = g->slot[parity];
@@ -624,27 +606,20 @@ int collect_group(modes_ctx *ctx, int parity) {
         s.busy = false;
         append_levels(ctx, s);                          // groups and GPUs in stream order
         append_spectra(ctx, s);
-        ShardView v;
-        if (fetch_async(g, s, nc, v)) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
-        cands[k] = v.cands; tiles[k] = v.tiles; n_tiles[k] = v.n_tiles; base[k] = v.buffer_base;
-        recovered[k] = v.recovered; weak[k] = v.weak; carrier[k] = v.carrier;
-        any_recover |= s.feat.recover;
-        any_carrier |= s.feat.carrier;
+        if (fetch_async(g, s, nc, shards[k])) return fail(ctx, "GPU %d: %s", g->cfg.device, g->err.c_str());
         signal = s.feat.signal;
     }
     for (size_t k = 0; k < n; k++) {
         CK(ctx, cudaSetDevice(ctx->gpus[k]->cfg.device));
         CK(ctx, wait_stream(ctx->gpus[k]->slot[parity].stream));
     }
+    // the switches are the same on every GPU of a group: all or none of the shards have records
+    for (size_t k = 1; k < n; k++)
+        if (!shards[k].recovered != !shards[0].recovered || !shards[k].carrier != !shards[0].carrier)
+            return fail(ctx, "internal: recovery or carrier records of GPU %d and GPU %d differ", ctx->gpus[0]->cfg.device,
+                        ctx->gpus[k]->cfg.device);
     ResolveConfig rc{ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->cfg.check_crc, signal ? 1 : 0};
-    if (any_recover)   // the switch is the same on every GPU of a group: all or none of the shards have records
-        for (size_t k = 0; k < n; k++)
-            if (!recovered[k]) return fail(ctx, "internal: recovery records missing for GPU %d", ctx->gpus[k]->cfg.device);
-    if (any_carrier)   // likewise
-        for (size_t k = 0; k < n; k++)
-            if (!carrier[k]) return fail(ctx, "internal: carrier records missing for GPU %d", ctx->gpus[k]->cfg.device);
-    resolve_shards(ctx->rs, rc, n, cands.data(), tiles.data(), n_tiles.data(), base.data(), ctx->out, ctx->scratch,
-                   any_recover ? recovered.data() : nullptr, weak.data(), any_carrier ? carrier.data() : nullptr);
+    resolve_shards(ctx->rs, rc, shards.data(), n, ctx->out, ctx->scratch);
     return 0;
 }
 
@@ -1156,15 +1131,13 @@ int modes_recover_device(modes_ctx *ctx, void *d_out, size_t capacity) {
 
 }  // extern "C"
 
-int modes::carrier_fetch(modes_ctx *ctx, modes_carrier *out) {
+int modes::detect_shard(modes_ctx *ctx, Shard &shard) {
     if (!ctx) return -1;
     Slot &s = ctx->detect;
-    if (!s.feat.carrier) return fail(ctx, "carrier records without modes_set_carrier");
-    if (!out) return fail(ctx, "carrier records: no output array");
+    if (!s.busy) return fail(ctx, "the batch's records without modes_detect_device");
     CK(ctx, cudaSetDevice(ctx->cfg.device));
     uint64_t n = 0;
-    if (wait_batch(ctx, s, &n)) return -1;
-    if (n) CK(ctx, cudaMemcpyAsync(out, s.d_carrier.get(), n * sizeof(modes_carrier), cudaMemcpyDeviceToHost, s.stream));
+    if (wait_batch(ctx, s, &n) || fetch_async(ctx, s, n, shard)) return -1;
     CK(ctx, wait_stream(s.stream));
     return 0;
 }
@@ -1522,7 +1495,7 @@ int modes_resolve(modes_ctx *ctx, const modes_candidate *candidates, const modes
                   int64_t buffer_base) {
     if (!ctx || !tiles) return -1;
     ResolveConfig rc{ctx->cfg.fix_errors, ctx->cfg.aggressive, ctx->cfg.check_crc, 0};
-    resolve_candidates(ctx->rs, rc, candidates, tiles, n_tiles, buffer_base, ctx->out, ctx->scratch);
+    resolve_candidates(ctx->rs, rc, Shard{candidates, tiles, n_tiles, buffer_base}, ctx->out, ctx->scratch);
     return 0;
 }
 
@@ -1530,14 +1503,7 @@ struct modes_resolver {
     ResolveState rs; ResolveConfig rc; MessageOut out; ResolveScratch *scratch = nullptr;
     ResolveState tentative;             // end state of the last modes_resolver_run_tentative
     bool has_tentative = false;
-    const modes_carrier *carrier = nullptr;   // the next modes_resolver_run_weak's carrier records (modes::resolver_set_carrier)
 };
-
-}  // extern "C"
-
-void modes::resolver_set_carrier(modes_resolver *r, const modes_carrier *carrier) { if (r) r->carrier = carrier; }
-
-extern "C" {
 
 modes_resolver *modes_resolver_create(const modes_config *cfg) {
     modes_resolver *r = new (std::nothrow) modes_resolver();
@@ -1557,7 +1523,7 @@ int modes_resolver_run(modes_resolver *r, const modes_candidate *candidates, con
                        size_t n_tiles, int64_t buffer_base, modes_sink_fn sink, void *user) {
     if (!r || !tiles) return -1;
     r->out.sink = sink; r->out.user = user;
-    resolve_candidates(r->rs, r->rc, candidates, tiles, n_tiles, buffer_base, r->out, r->scratch);
+    resolve_candidates(r->rs, r->rc, Shard{candidates, tiles, n_tiles, buffer_base}, r->out, r->scratch);
     return 0;
 }
 
@@ -1565,7 +1531,7 @@ int modes_resolver_run_recovered(modes_resolver *r, const modes_candidate *candi
                                  const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, modes_sink_fn sink, void *user) {
     if (!r || !tiles) return -1;
     r->out.sink = sink; r->out.user = user;
-    resolve_candidates(r->rs, r->rc, candidates, tiles, n_tiles, buffer_base, r->out, r->scratch, recovered);
+    resolve_candidates(r->rs, r->rc, Shard{candidates, tiles, n_tiles, buffer_base, recovered}, r->out, r->scratch);
     return 0;
 }
 
@@ -1573,11 +1539,13 @@ int modes_resolver_run_shards_recovered(modes_resolver *r, size_t n_shards, cons
                                         const modes_recovered *const *recovered, const modes_tile *const *tiles,
                                         const size_t *n_tiles, const int64_t *buffer_base, modes_sink_fn sink, void *user) {
     if (!r || (n_shards && (!candidates || !tiles || !n_tiles || !buffer_base))) return -1;
-    if (recovered)
-        for (size_t k = 0; k < n_shards; k++)
-            if (!recovered[k]) return -1;
+    std::vector<Shard> shards(n_shards);
+    for (size_t k = 0; k < n_shards; k++) {
+        if (recovered && !recovered[k]) return -1;
+        shards[k] = Shard{candidates[k], tiles[k], n_tiles[k], buffer_base[k], recovered ? recovered[k] : nullptr};
+    }
     r->out.sink = sink; r->out.user = user;
-    resolve_shards(r->rs, r->rc, n_shards, candidates, tiles, n_tiles, buffer_base, r->out, r->scratch, recovered);
+    resolve_shards(r->rs, r->rc, shards.data(), n_shards, r->out, r->scratch);
     return 0;
 }
 
@@ -1594,10 +1562,8 @@ int modes_resolver_run_weak(modes_resolver *r, const modes_candidate *candidates
     for (size_t k = 1; k < n_weak; k++)
         if (weak_t[k] <= weak_t[k - 1]) return -1;                   // stream order, each position once
     r->out.sink = sink; r->out.user = user;
-    const modes_carrier *carrier = r->carrier;
-    r->carrier = nullptr;
-    resolve_candidates(r->rs, r->rc, candidates, tiles, n_tiles, buffer_base, r->out, r->scratch, recovered,
-                       WeakList{weak_t, weak_rec, n_weak}, carrier);
+    resolve_candidates(r->rs, r->rc, Shard{candidates, tiles, n_tiles, buffer_base, recovered, WeakList{weak_t, weak_rec, n_weak}},
+                       r->out, r->scratch);
     return 0;
 }
 
@@ -1608,15 +1574,15 @@ int modes_resolver_run_shards_weak(modes_resolver *r, size_t n_shards, const mod
                                    void *user) {
     if (!r || (n_shards && (!candidates || !tiles || !n_tiles || !buffer_base || !recovered || !weak_t || !weak_rec || !n_weak)))
         return -1;
-    std::vector<WeakList> wl(n_shards);
+    std::vector<Shard> shards(n_shards);
     for (size_t k = 0; k < n_shards; k++) {
         if (!recovered[k] || (n_weak[k] && (!weak_t[k] || !weak_rec[k]))) return -1;
         for (size_t i = 1; i < n_weak[k]; i++)
             if (weak_t[k][i] <= weak_t[k][i - 1]) return -1;
-        wl[k] = WeakList{weak_t[k], weak_rec[k], n_weak[k]};
+        shards[k] = Shard{candidates[k], tiles[k], n_tiles[k], buffer_base[k], recovered[k], WeakList{weak_t[k], weak_rec[k], n_weak[k]}};
     }
     r->out.sink = sink; r->out.user = user;
-    resolve_shards(r->rs, r->rc, n_shards, candidates, tiles, n_tiles, buffer_base, r->out, r->scratch, recovered, wl.data());
+    resolve_shards(r->rs, r->rc, shards.data(), n_shards, r->out, r->scratch);
     return 0;
 }
 
@@ -1630,8 +1596,10 @@ int modes_resolver_run_shards(modes_resolver *r, size_t n_shards, const modes_ca
                               const modes_tile *const *tiles, const size_t *n_tiles, const int64_t *buffer_base,
                               modes_sink_fn sink, void *user) {
     if (!r || (n_shards && (!candidates || !tiles || !n_tiles || !buffer_base))) return -1;
+    std::vector<Shard> shards(n_shards);
+    for (size_t k = 0; k < n_shards; k++) shards[k] = Shard{candidates[k], tiles[k], n_tiles[k], buffer_base[k]};
     r->out.sink = sink; r->out.user = user;
-    resolve_shards(r->rs, r->rc, n_shards, candidates, tiles, n_tiles, buffer_base, r->out, r->scratch);
+    resolve_shards(r->rs, r->rc, shards.data(), n_shards, r->out, r->scratch);
     return 0;
 }
 
@@ -1657,7 +1625,7 @@ int modes_resolver_tail_cache(const modes_resolver *r, const modes_candidate *ca
     ResolveScratch *tmp = scratch_create();
     if (!tmp) return -1;
     if (n_tail_tiles > n_tiles) n_tail_tiles = n_tiles;
-    resolve_tentative(st, r->rc, candidates, tiles + (n_tiles - n_tail_tiles), n_tail_tiles, buffer_base, tmp);
+    resolve_tentative(st, r->rc, Shard{candidates, tiles + (n_tiles - n_tail_tiles), n_tail_tiles, buffer_base}, tmp);
     scratch_destroy(tmp);
     memcpy(cache, st.icao, sizeof(st.icao));
     return 0;
@@ -1667,7 +1635,7 @@ int modes_resolver_run_tentative(modes_resolver *r, const modes_candidate *candi
                                  size_t n_tiles, int64_t buffer_base) {
     if (!r || !tiles) return -1;
     r->tentative.start_part(r->rs, true);
-    resolve_tentative(r->tentative, r->rc, candidates, tiles, n_tiles, buffer_base, r->scratch);
+    resolve_tentative(r->tentative, r->rc, Shard{candidates, tiles, n_tiles, buffer_base}, r->scratch);
     r->has_tentative = true;
     return 0;
 }

@@ -208,12 +208,6 @@ void launch_weak_scan(const BatchView &in, const DeviceTables &tab, const WeakOu
 // search as launch_recover's).
 void launch_recover_weak(const BatchView &in, const DeviceTables &tab, const uint32_t *count, uint32_t capacity,
                          uint32_t scratch_cap, const uint32_t *pos, modes_recovered *out, int sm_count, cudaStream_t stream);
-// The carrier records of the last modes_detect_device batch (the receiver pool's slot contexts measure
-// them with modes_set_carrier): one per candidate, as many as modes_detect_fetch copies.
-int carrier_fetch(modes_ctx *ctx, modes_carrier *out);
-// The carrier records of the candidates of the resolver's next modes_resolver_run_weak call (nullptr: not
-// measured); the call clears them.
-void resolver_set_carrier(modes_resolver *r, const modes_carrier *carrier);
 // modes_weak_device over the buffers first_buffer + i * buffer_step of the last batch only (the
 // receiver pool: its data buffers, never its pad buffers); modes_weak_device is (0, 1).
 int weak_device_strided(modes_ctx *ctx, void *d_pos, void *d_rec, size_t capacity, uint32_t first_buffer, uint32_t buffer_step);
@@ -296,21 +290,28 @@ void scratch_destroy(ResolveScratch *s);
 // The weak positions of a record array (sorted t, as the candidates' t) and their recovery records.
 struct WeakList { const uint32_t *t = nullptr; const modes_recovered *rec = nullptr; size_t n = 0; };
 
-// recovered: one record per candidate (modes_recover.cu), or nullptr with recovery off; weak: the
-// weak positions merged into the walk (only with recovered); carrier: one carrier record per candidate
-// (modes_signal.cu), or nullptr with carrier measurement off
-void resolve_candidates(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands,
-                        const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, MessageOut &out,
-                        ResolveScratch *scratch, const modes_recovered *recovered = nullptr, const WeakList &weak = WeakList(),
-                        const modes_carrier *carrier = nullptr);
-void resolve_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards, const modes_candidate *const *cands,
-                    const modes_tile *const *tiles, const size_t *n_tiles, const int64_t *buffer_base,
-                    MessageOut &out, ResolveScratch *scratch, const modes_recovered *const *recovered = nullptr,
-                    const WeakList *weak = nullptr, const modes_carrier *const *carrier = nullptr);
+// One record array as the resolve takes it: a batch's candidate records and tile table, and the stream's
+// buffer number of the array's buffer 0 (buffer numbers in the records: t >> 17).  recovered: one record
+// per candidate (modes_recover.cu), or nullptr with recovery off; weak: the weak positions merged into the
+// walk (only with recovered); carrier: one carrier record per candidate (modes_signal.cu), or nullptr with
+// carrier measurement off.  Only the candidates and weak positions of the buffers [b_lo, b_hi) are judged.
+struct Shard {
+    const modes_candidate *cands = nullptr;
+    const modes_tile *tiles = nullptr;
+    size_t n_tiles = 0;
+    int64_t buffer_base = 0;
+    const modes_recovered *recovered = nullptr;
+    WeakList weak{};
+    const modes_carrier *carrier = nullptr;
+    uint32_t b_lo = 0, b_hi = UINT32_MAX;
+};
+
+void resolve_candidates(ResolveState &st, const ResolveConfig &cfg, const Shard &shard, MessageOut &out, ResolveScratch *scratch);
+void resolve_shards(ResolveState &st, const ResolveConfig &cfg, const Shard *shards, size_t n_shards, MessageOut &out,
+                    ResolveScratch *scratch);
 // A shard resolved from a GUESSED address cache (one rank / one GPU thread of a sharded decode):
 // verdicts only, deliveries held back in the scratch until the guess is verified.
-void resolve_tentative(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands, const modes_tile *tiles,
-                       size_t n_tiles, int64_t buffer_base, ResolveScratch *scratch);
+void resolve_tentative(ResolveState &st, const ResolveConfig &cfg, const Shard &shard, ResolveScratch *scratch);
 void resolve_commit(MessageOut &out, ResolveScratch *scratch);
 // Messages from the device resolve's delivery records (structs built in parallel, sink called in order).
 void deliver_gpu(const modes_delivery *d, size_t n, int64_t buffer_base, MessageOut &out);
@@ -358,6 +359,11 @@ template <typename T> using PinnedBuf = CudaBuf<T, true>;
 
 // The optional measurements and searches of a decode (modes_set_* / modes_pool_set_*).
 struct Features { bool signal = false, arrival = false, levels = false, recover = false, weak = false, spectrum = false, carrier = false; };
+
+// The last modes_detect_device batch's records (the receiver pool's slot contexts), in the context's pinned
+// memory, with those of the passes it ran with its own arrays (recovery, weak preambles, carrier): waits for
+// the batch, copies them and waits once.  The shard is valid until the context's next batch.
+int detect_shard(modes_ctx *ctx, Shard &shard);
 
 // Level or spectrum records not taken yet, oldest first.
 template <typename T>

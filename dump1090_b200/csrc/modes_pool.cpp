@@ -18,9 +18,11 @@
 // receiver's own stream; whatever the scan finds inside the pad buffers is dropped.  The price is a
 // second scan over constant buffers (the scan runs at 2 T samples/s; the link delivers 25 G samples/s).
 //
-// The order-dependent half is the existing host resolver, one per receiver: the records of a data
-// buffer are re-based to that receiver's own stream position and replayed with its own address
-// cache.  Built on the public C ABI only (modes_detect_device / _fetch, modes_resolver_*).
+// The order-dependent half is the host resolve, one resolve state per receiver: the records of a data
+// buffer are judged where they lie in the batch's record array, at that receiver's own stream position
+// and with its own address cache.  Built on the public C ABI (modes_detect_device, modes_recover_device,
+// modes_levels_device) and three internal calls: the host resolve itself, detect_shard, which brings a
+// batch's records to the host with one wait, and weak_device_strided, the weak scan over the data buffers.
 //
 // A receiver at 2.4 MS/s (modes_pool_set_input_rate) brings 131072 input samples per call, and its 2 MHz
 // buffers complete at their own pace (157286.4 input samples each): at most one per call, none in the
@@ -67,7 +69,7 @@ constexpr uint32_t kRate2M = 2000000, kRate24 = 2400000;
 constexpr size_t kHistBytes = 2 * ((size_t)6 * (kBufSamples + kCarrySamples) / 5 + 2 * modes::resample::kTaps + 16) + kBuf;
 
 struct Receiver {
-    modes_resolver *res = nullptr;
+    modes::ResolveState rs;                    // its address cache, skip state and statistics
     int64_t buffers = 0;                       // buffers of this receiver decoded so far
     int64_t submitted = 0;                     // buffers of this receiver submitted so far (2 MHz buffers)
     uint8_t carry[MODES_CARRY_BYTES];
@@ -212,20 +214,9 @@ struct modes_pool {
         modes::DevBuf<modes_spectrum> d_spectra;
     } slot[2];
     unsigned submitted = 0, collected = 0;     // batches so far: slot = number & 1
-    std::vector<modes_candidate> cands;
-    std::vector<modes_recovered> recovered;    // with recovery: one record per candidate
-    std::vector<modes_carrier> carrier;        // with carrier measurement: one record per candidate
-    std::vector<uint32_t> weak_t;              // with weak preambles: the batch's weak positions and records
-    std::vector<modes_recovered> weak_rec;
-    std::vector<modes_tile> tiles;
     // the per-receiver resolve: one block of the receiver list per host thread
     struct Block {
-        std::vector<modes_candidate> local;    // one receiver's records, re-based to its buffer
-        std::vector<modes_recovered> local_rec;   // and their recovery records
-        std::vector<modes_carrier> local_car;     // and their carrier records
-        std::vector<uint32_t> local_wt;        // the receiver's weak positions, re-based, and their records
-        std::vector<modes_recovered> local_wrec;
-        std::vector<modes_tile> local_tiles;
+        std::unique_ptr<modes::ResolveScratch, void (*)(modes::ResolveScratch *)> scratch{nullptr, modes::scratch_destroy};
         std::vector<modes_message> msgs;       // the block's messages, receiver by receiver
         std::vector<size_t> counts;            // messages of each receiver of the block
         size_t used = 0, at = 0;               // messages of the block; where they start in the call's sequence
@@ -391,16 +382,14 @@ modes_pool *modes_pool_create(const modes_config *cfg, size_t n_receivers, size_
     p->max_batch = max_batch_receivers && max_batch_receivers < n_receivers ? max_batch_receivers : n_receivers;
     p->rx.resize(n_receivers);
     for (Receiver &r : p->rx) {
-        r.res = modes_resolver_create(cfg);
+        r.rs.reset();
         memset(r.carry, 127, sizeof r.carry);
-        if (!r.res) { modes_pool_destroy(p); return nullptr; }
     }
     return p;
 }
 
 void modes_pool_destroy(modes_pool *p) {
     if (!p) return;
-    for (Receiver &r : p->rx) if (r.res) modes_resolver_destroy(r.res);
     for (modes_pool::Slot &sl : p->slot) {
         if (sl.rate_done) cudaEventDestroy(sl.rate_done);
         if (sl.ctx) modes_destroy(sl.ctx);     // waits for the slot's stream
@@ -410,19 +399,18 @@ void modes_pool_destroy(modes_pool *p) {
 
 const char *modes_pool_last_error(const modes_pool *p) { return p ? p->err.c_str() : "no pool"; }
 
-// The per-receiver resolve; recovered: the batch's recovery records (nullptr: off), whose signal the
-// messages carry only when the batch measured signals; weak_t / weak_rec / n_weak: its weak positions;
-// carrier: the batch's carrier records (nullptr: off).
-static int pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, const modes_candidate *candidates,
-                        const modes_recovered *recovered, bool signal, const modes_tile *tiles, modes_pool_sink_fn sink,
-                        void *user, const uint32_t *weak_t = nullptr, const modes_recovered *weak_rec = nullptr,
-                        size_t n_weak = 0, const modes_carrier *carrier = nullptr) {
+// The per-receiver resolve of a batch of n pairs (its records, recovery records, weak positions and carrier
+// records); recovered messages carry their record's signal only when the batch measured signals.
+static int pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, const modes::Shard &batch, bool signal,
+                        modes_pool_sink_fn sink, void *user) {
     if (!p) return -1;
     if (check_ids(p, receivers, n)) return -1;
     if (!n) return 0;
-    if (!tiles) return fail(p, "no tile table");
-    const size_t n_tiles = modes_tile_count(2 * n);
-    const size_t n_local = modes_tile_count(1);
+    if (!batch.tiles) return fail(p, "no tile table");
+    const modes_tile *tiles = batch.tiles;
+    const uint32_t *weak_t = batch.weak.t;
+    const size_t n_tiles = modes_tile_count(2 * n), n_weak = batch.weak.n;
+    const modes::ResolveConfig rc{p->cfg.fix_errors, p->cfg.aggressive, p->cfg.check_crc, signal ? 1 : 0};
     // Receivers are independent: the list is cut into blocks, one host thread each; a block's messages
     // land in its own array and are moved to the caller's array / handed to the sink in list order.
     size_t n_blocks = pool_threads();
@@ -445,60 +433,31 @@ static int pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, cons
         tile_range(i0, ga, gb); tile_range(i1 - 1, gc, gd);
         // a candidate delivers at most two messages of the reference (both attempts without --check-crc,
         // dump1090.c:1803) and, with recovery, one recovered message after them; a weak position one
-        const size_t per_candidate = recovered ? 3 : 2;
+        const size_t per_candidate = batch.recovered ? 3 : 2;
         for (size_t g = ga; g <= gd; g++) room += per_candidate * (size_t)tiles[g].count;
         const uint32_t *wlo = std::lower_bound(weak_t, weak_t + n_weak, (uint32_t)(kBufSamples * (2 * i0 + 1)));
         const uint32_t *whi = std::lower_bound(weak_t, weak_t + n_weak, (uint32_t)(kBufSamples * (2 * i1)));
         room += (size_t)(whi - wlo);
         if (bl.msgs.size() < room) bl.msgs.resize(room);
-        bl.local_tiles.resize(n_local);
+        if (!bl.scratch) bl.scratch.reset(modes::scratch_create());
+        if (!bl.scratch) { bl.failed = (int64_t)i0; return; }
         size_t used = 0;
         for (size_t i = i0; i < i1; i++) {
             Receiver &r = p->rx[receivers[i]];
-            const int64_t t0 = kBufSamples * (int64_t)(2 * i + 1), t1 = t0 + kBufSamples;
+            // the receiver's data buffer, batch buffer 2i+1, judged in place as its own buffer r.buffers
+            modes::Shard s = batch;
             size_t g0, g1;
             tile_range(i, g0, g1);
-            bl.local.clear();
-            bl.local_rec.clear();
-            bl.local_car.clear();
-            for (modes_tile &lt : bl.local_tiles) { lt.offset = 0; lt.count = 0; }
-            for (size_t g = g0; g <= g1; g++) {
-                const modes_candidate *c = candidates + tiles[g].offset;
-                for (uint32_t k = 0; k < tiles[g].count; k++) {
-                    if (c[k].t < t0 || c[k].t >= t1) continue;
-                    modes_candidate lc = c[k];
-                    lc.t -= t0;                           // position inside the receiver's own buffer
-                    const size_t lg = (size_t)((lc.t + 2) / MODES_TILE_SAMPLES);
-                    if (lg >= n_local) { bl.failed = (int64_t)i; return; }
-                    bl.local_tiles[lg].count++;
-                    bl.local.push_back(lc);
-                    if (recovered) {
-                        modes_recovered rc = recovered[tiles[g].offset + k];
-                        if (!signal) rc.signal = 0;
-                        bl.local_rec.push_back(rc);
-                    }
-                    if (carrier) bl.local_car.push_back(carrier[tiles[g].offset + k]);
-                }
-            }
-            uint32_t off = 0;
-            for (modes_tile &lt : bl.local_tiles) { lt.offset = off; off += lt.count; }
-            bl.local_wt.clear();
-            bl.local_wrec.clear();
-            for (const uint32_t *w = std::lower_bound(weak_t, weak_t + n_weak, (uint32_t)t0); w < weak_t + n_weak && *w < t1; w++) {
-                modes_recovered rc = weak_rec[w - weak_t];
-                if (!signal) rc.signal = 0;
-                bl.local_wt.push_back(*w - (uint32_t)t0);
-                bl.local_wrec.push_back(rc);
-            }
-            modes_resolver_set_output(r.res, bl.msgs.data() + used, room - used);
-            modes::resolver_set_carrier(r.res, carrier ? bl.local_car.data() : nullptr);
-            if (modes_resolver_run_weak(r.res, bl.local.data(), recovered ? bl.local_rec.data() : nullptr, bl.local_tiles.data(),
-                                        n_local, r.buffers, bl.local_wt.data(), bl.local_wrec.data(), bl.local_wt.size(),
-                                        nullptr, nullptr)) {
-                bl.failed = (int64_t)i; return;
-            }
-            const size_t k = modes_resolver_output_count(r.res);
-            modes_resolver_set_output(r.res, nullptr, 0);
+            s.tiles = tiles + g0;
+            s.n_tiles = g1 - g0 + 1;
+            s.buffer_base = r.buffers - (int64_t)(2 * i + 1);
+            s.b_lo = (uint32_t)(2 * i + 1);
+            s.b_hi = s.b_lo + 1;
+            modes::MessageOut out;
+            out.array = bl.msgs.data() + used;
+            out.capacity = room - used;
+            modes::resolve_candidates(r.rs, rc, s, out, bl.scratch.get());
+            const size_t k = out.count;
             if (k > room - used) { bl.failed = (int64_t)i; return; }   // the bound above is exact: never reached
             bl.counts[i - i0] = k;
             used += k;
@@ -542,7 +501,7 @@ static int pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, cons
 
 int modes_pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, const modes_candidate *candidates,
                        const modes_tile *tiles, modes_pool_sink_fn sink, void *user) {
-    return pool_resolve(p, receivers, n, candidates, nullptr, false, tiles, sink, user);
+    return pool_resolve(p, receivers, n, modes::Shard{candidates, tiles}, false, sink, user);
 }
 
 // One buffer of each listed receiver.  A receiver gets a pair when it decodes a buffer in this call: a 2 MHz
@@ -692,27 +651,9 @@ int modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user) {
         p->collected++;
         return 0;
     }
-    uint64_t n_cand = 0;
-    if (modes_detect_wait(sl.ctx, &n_cand)) return fail(p, "%s", modes_last_error(sl.ctx));
+    modes::Shard batch;
+    if (modes::detect_shard(sl.ctx, batch)) return fail(p, "%s", modes_last_error(sl.ctx));
     const size_t n = sl.ids.size();
-    p->cands.resize(n_cand ? n_cand : 1);
-    p->tiles.resize(modes_tile_count(2 * n));
-    if (modes_detect_fetch(sl.ctx, p->cands.data(), p->tiles.data())) return fail(p, "%s", modes_last_error(sl.ctx));
-    if (sl.feat.recover) {
-        p->recovered.resize(n_cand ? n_cand : 1);
-        if (modes_recover_fetch(sl.ctx, p->recovered.data())) return fail(p, "%s", modes_last_error(sl.ctx));
-    }
-    if (sl.feat.carrier) {
-        p->carrier.resize(n_cand ? n_cand : 1);
-        if (modes::carrier_fetch(sl.ctx, p->carrier.data())) return fail(p, "%s", modes_last_error(sl.ctx));
-    }
-    uint64_t n_weak = 0;
-    if (sl.feat.weak) {
-        if (modes_weak_fetch(sl.ctx, nullptr, nullptr, &n_weak)) return fail(p, "%s", modes_last_error(sl.ctx));
-        p->weak_t.resize(n_weak ? n_weak : 1);
-        p->weak_rec.resize(n_weak ? n_weak : 1);
-        if (modes_weak_fetch(sl.ctx, p->weak_t.data(), p->weak_rec.data(), &n_weak)) return fail(p, "%s", modes_last_error(sl.ctx));
-    }
     if (sl.feat.levels) {
         sl.level_out.resize(n);
         if (modes_levels_fetch(sl.ctx, sl.level_out.data())) return fail(p, "%s", modes_last_error(sl.ctx));
@@ -729,9 +670,7 @@ int modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user) {
     }
     sl.busy = false;
     p->collected++;
-    return pool_resolve(p, sl.ids.data(), n, p->cands.data(), sl.feat.recover ? p->recovered.data() : nullptr, sl.feat.signal,
-                        p->tiles.data(), sink, user, p->weak_t.data(), p->weak_rec.data(), (size_t)n_weak,
-                        sl.feat.carrier ? p->carrier.data() : nullptr);
+    return pool_resolve(p, sl.ids.data(), n, batch, sl.feat.signal, sink, user);
 }
 
 int modes_pool_ingest(modes_pool *p, const uint32_t *receivers, const uint8_t *const *iq, size_t n,
@@ -745,7 +684,8 @@ int modes_pool_ingest(modes_pool *p, const uint32_t *receivers, const uint8_t *c
 
 int modes_pool_stats(const modes_pool *p, uint32_t receiver, modes_stats *out) {
     if (!p || receiver >= p->rx.size() || !out) return -1;
-    return modes_resolver_stats(p->rx[receiver].res, out);
+    memcpy(out->v, p->rx[receiver].rs.stats, sizeof(out->v));
+    return 0;
 }
 
 int modes_pool_reset(modes_pool *p, uint32_t receiver) {
@@ -758,7 +698,8 @@ int modes_pool_reset(modes_pool *p, uint32_t receiver) {
     r.levels.clear();
     r.spectra.clear();
     memset(r.carry, 127, sizeof r.carry);
-    return modes_resolver_reset(r.res);
+    r.rs.reset();
+    return 0;
 }
 
 int modes_pool_set_input_rate(modes_pool *p, uint32_t receiver, uint32_t hz) {
@@ -811,14 +752,16 @@ int modes_pool_set_recovery(modes_pool *p, int on) { return set_feature(p, &mode
 
 int modes_pool_recovery_stats(const modes_pool *p, uint32_t receiver, modes_recovery_stats *out) {
     if (!p || receiver >= p->rx.size() || !out) return -1;
-    return modes_resolver_recovery_stats(p->rx[receiver].res, out);
+    *out = p->rx[receiver].rs.rstats;
+    return 0;
 }
 
 int modes_pool_set_weak_preambles(modes_pool *p, int on) { return set_feature(p, &modes::Features::weak, on); }
 
 int modes_pool_weak_stats(const modes_pool *p, uint32_t receiver, modes_recovery_stats *out) {
     if (!p || receiver >= p->rx.size() || !out) return -1;
-    return modes_resolver_weak_stats(p->rx[receiver].res, out);
+    *out = p->rx[receiver].rs.wstats;
+    return 0;
 }
 
 int modes_pool_set_levels(modes_pool *p, int on) { return set_feature(p, &modes::Features::levels, on); }

@@ -359,24 +359,36 @@ static inline void weak_steps(ResolveState &st, const ResolveConfig &cfg, WeakCu
     }
 }
 
-// The verdict pass over one run of tiles: everything order-dependent, no message structs yet.
-// `b_lo`, `b_hi`: only the candidates of the buffers [b_lo, b_hi) of this record array are judged (buffer
-// numbers as in the records: t >> 17); the walk ends at the first candidate of buffer b_hi or later
-// (records are in stream order).  The whole array: 0, UINT32_MAX.  kRecover: apply the recovery rules
-// with `rec` and merge the weak positions `weak` (may be nullptr) into the walk (the walk without
-// them has no trace of them).  car: the carrier records of the candidates (nullptr: not measured).
+// A run of a shard's record array judged in one sequence (see "parts" below).
+struct Part {
+    const Shard *shard;
+    size_t tile_lo;              // first tile that can hold one of its candidates
+    uint32_t b_lo, b_hi;         // its buffers, as numbered in the records (t >> 17)
+    bool first_of_shard;         // the tail pass for a shard's first part walks the previous SHARD's array
+};
+
+// The verdict pass over the tiles of a part from tile_lo on: everything order-dependent, no message
+// structs yet.  Only the candidates of the part's buffers [b_lo, b_hi) are judged; the walk ends at the
+// first candidate of buffer b_hi or later (records are in stream order).  kRecover: apply the recovery
+// rules with the shard's recovery records and merge its weak positions into the walk (the walk without
+// them has no trace of them).
 template <bool kRecover>
-static void walk_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands, const modes_tile *tiles,
-                       size_t n_tiles, int64_t buffer_base, std::vector<Delivery> &deliveries, uint32_t b_lo, uint32_t b_hi,
-                       const modes_recovered *rec, const WeakList *weak, const modes_carrier *car) {
+static void walk_tiles(ResolveState &st, const ResolveConfig &cfg, const Part &p, std::vector<Delivery> &deliveries) {
+    const Shard &s = *p.shard;
+    const modes_candidate *cands = s.cands;
+    const modes_tile *tiles = s.tiles + p.tile_lo;
+    const size_t n_tiles = s.n_tiles - p.tile_lo;
+    const uint32_t b_lo = p.b_lo, b_hi = p.b_hi;
+    const int64_t buffer_base = s.buffer_base;
+    const modes_carrier *car = s.carrier;
     RecoveryPending pend;
     WeakCursor wc;
-    const bool merge = kRecover && weak && weak->n;
+    const bool merge = kRecover && s.weak.n;
     if (merge) {                                           // the first weak position of buffer b_lo or later
-        wc.w = weak;
+        wc.w = &s.weak;
         const uint64_t lo = (uint64_t)b_lo << 17;
-        size_t a = 0, b = weak->n;
-        while (a < b) { const size_t m = (a + b) / 2; if (weak->t[m] < lo) a = m + 1; else b = m; }
+        size_t a = 0, b = s.weak.n;
+        while (a < b) { const size_t m = (a + b) / 2; if (s.weak.t[m] < lo) a = m + 1; else b = m; }
         wc.next = a;
     }
     // The kernels append a tile's records wherever the global cursor stands when the tile finishes:
@@ -413,18 +425,16 @@ static void walk_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_c
                     deliveries.push_back(Delivery{c->pass[a], pos, iid_of(d[a]), ap_addr_of(d[a]), (uint8_t)d[a].crcok,
                                                   (uint8_t)d[a].phase_corrected, (uint8_t)0,
                                                   car ? carrier::code_of(car[k0 + k].re[a], car[k0 + k].im[a]) : (int16_t)0});
-            if constexpr (kRecover) recovery_step(st, cfg, rec[k0 + k], visit > 0, buffer, j, pos, deliveries, pend, st.rstats, 1);
+            if constexpr (kRecover)
+                recovery_step(st, cfg, s.recovered[k0 + k], visit > 0, buffer, j, pos, deliveries, pend, st.rstats, 1);
         }
     }
     if (merge) weak_steps(st, cfg, wc, UINT64_MAX, b_hi, buffer_base, deliveries, pend);
 }
 
-static void judge_tiles(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands, const modes_tile *tiles,
-                        size_t n_tiles, int64_t buffer_base, std::vector<Delivery> &deliveries,
-                        uint32_t b_lo = 0, uint32_t b_hi = UINT32_MAX, const modes_recovered *rec = nullptr,
-                        const WeakList *weak = nullptr, const modes_carrier *car = nullptr) {
-    if (rec) walk_tiles<true>(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, b_lo, b_hi, rec, weak, car);
-    else walk_tiles<false>(st, cfg, cands, tiles, n_tiles, buffer_base, deliveries, b_lo, b_hi, nullptr, nullptr, car);
+static void judge_tiles(ResolveState &st, const ResolveConfig &cfg, const Part &p, std::vector<Delivery> &deliveries) {
+    if (p.shard->recovered) walk_tiles<true>(st, cfg, p, deliveries);
+    else walk_tiles<false>(st, cfg, p, deliveries);
 }
 
 // Build n delivered structs with build(i, struct): in place and in parallel for array output, then
@@ -478,16 +488,6 @@ void deliver_gpu(const modes_delivery *d, size_t n, int64_t buffer_base, Message
 // cache part k-1 really ended with, and a part whose guess was wrong is simply judged again.  One
 // round normally suffices; in the worst case the loop degenerates to the sequential order, never
 // to a wrong result.
-struct Part {
-    const modes_candidate *cands; const modes_tile *tiles; size_t n_tiles;   // the record array the part lies in
-    size_t tile_lo;              // first tile that can hold one of its candidates
-    uint32_t b_lo, b_hi;         // its buffers, as numbered in the records (t >> 17)
-    int64_t buffer_base;
-    bool first_of_shard;         // the tail pass for a shard's first part walks the previous SHARD's array
-    const modes_recovered *rec;  // the array's recovery records, or nullptr
-    const WeakList *weak;        // the array's weak positions, or nullptr
-    const modes_carrier *car;    // the array's carrier records, or nullptr
-};
 struct PartRun { ResolveState start, end; std::vector<Delivery> deliveries; };
 struct ResolveScratch {
     std::vector<Part> parts;
@@ -516,22 +516,21 @@ static size_t parts_for(size_t n_tiles) {
     return p < 1 ? 1 : p;
 }
 
-// Cut one record array into up to `want` parts at buffer boundaries.  The boundary of part k is
-// read from the records themselves: the buffer after the one the first candidate at or behind tile
-// k * n_tiles / want lies in (tiles do not line up with buffers; records are in stream order).
-static void cut_parts(const modes_candidate *cands, const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, size_t want,
-                      std::vector<Part> &parts, const modes_recovered *rec = nullptr, const WeakList *weak = nullptr,
-                      const modes_carrier *car = nullptr) {
-    Part p{cands, tiles, n_tiles, 0, 0, UINT32_MAX, buffer_base, true, rec, weak, car};
+// Cut a shard's buffers [b_lo, b_hi) into up to `want` parts at buffer boundaries.  The boundary of
+// part k is read from the records themselves: the buffer after the one the first candidate at or behind
+// tile k * n_tiles / want lies in (tiles do not line up with buffers; records are in stream order).
+static void cut_parts(const Shard &s, size_t want, std::vector<Part> &parts) {
+    Part p{&s, 0, s.b_lo, s.b_hi, true};
     for (size_t k = 1; k < want; k++) {
-        size_t ti = k * n_tiles / want;
-        while (ti < n_tiles && tiles[ti].count == 0) ti++;
-        if (ti >= n_tiles) break;
-        const uint32_t b = (uint32_t)(cands[tiles[ti].offset].t >> 17) + 1;      // first buffer of the next part
+        size_t ti = k * s.n_tiles / want;
+        while (ti < s.n_tiles && s.tiles[ti].count == 0) ti++;
+        if (ti >= s.n_tiles) break;
+        const uint32_t b = (uint32_t)(s.cands[s.tiles[ti].offset].t >> 17) + 1;  // first buffer of the next part
         if (b <= p.b_lo) continue;                                                 // (a gap longer than a part)
+        if (b >= s.b_hi) break;
         p.b_hi = b;
         parts.push_back(p);
-        p.tile_lo = ti; p.b_lo = b; p.b_hi = UINT32_MAX; p.first_of_shard = false;
+        p.tile_lo = ti; p.b_lo = b; p.b_hi = s.b_hi; p.first_of_shard = false;
     }
     parts.push_back(p);
 }
@@ -541,21 +540,18 @@ static void cut_parts(const modes_candidate *cands, const modes_tile *tiles, siz
 static int judge_parts(ResolveState &st, const ResolveConfig &cfg, const std::vector<Part> &parts, PartRun *runs) {
     const size_t n = parts.size();
     if (n == 1) {
-        const Part &p = parts[0];
         runs[0].deliveries.clear();
-        judge_tiles(st, cfg, p.cands, p.tiles, p.n_tiles, p.buffer_base, runs[0].deliveries, p.b_lo, p.b_hi, p.rec, p.weak, p.car);
+        judge_tiles(st, cfg, parts[0], runs[0].deliveries);
         return 1;
     }
     ResolveState blank;
     blank.reset();
     auto run_part = [&](size_t k, const ResolveState &from) {
         PartRun &r = runs[k];
-        const Part &p = parts[k];
         r.start.start_part(from, k != 0);                  // a later part starts a buffer
         r.end = r.start;
         r.deliveries.clear();
-        judge_tiles(r.end, cfg, p.cands, p.tiles + p.tile_lo, p.n_tiles - p.tile_lo, p.buffer_base, r.deliveries, p.b_lo, p.b_hi,
-                    p.rec, p.weak, p.car);
+        judge_tiles(r.end, cfg, parts[k], r.deliveries);
     };
     int rounds = 0;
     size_t done = 0;                                       // parts [0, done) are final
@@ -572,16 +568,17 @@ static int judge_parts(ResolveState &st, const ResolveConfig &cfg, const std::ve
             // First guess: the cache this call started with, overwritten by what the LAST SIXTEENTH of
             // part k-1 writes (addresses are re-confirmed every second or so, so the tail of a long
             // part has normally written every slot the whole part leaves changed).
-            const Part &q = parts[k - 1];
+            Part q = parts[k - 1];
             ResolveState g;
-            g.start_part(st, true);                        // (recovery never writes the cache: the guess skips it)
-            const size_t end_tile = parts[k].first_of_shard ? q.n_tiles : (parts[k].tile_lo + 1 < q.n_tiles ? parts[k].tile_lo + 1 : q.n_tiles);
+            g.start_part(st, true);
+            const size_t n_tiles = q.shard->n_tiles;
+            const size_t end_tile = parts[k].first_of_shard ? n_tiles : (parts[k].tile_lo + 1 < n_tiles ? parts[k].tile_lo + 1 : n_tiles);
             const size_t len = end_tile - q.tile_lo;
             size_t tail = len / 16 > 128 ? len / 16 : 128;             // at least ~1 M samples (half a second of stream)
             if (tail > len) tail = len;
+            q.tile_lo = end_tile - tail;
             runs[k].deliveries.clear();
-            judge_tiles(g, cfg, q.cands, q.tiles + (end_tile - tail), q.n_tiles - (end_tile - tail), q.buffer_base, runs[k].deliveries,
-                        q.b_lo, q.b_hi);
+            walk_tiles<false>(g, cfg, q, runs[k].deliveries);          // recovery never writes the cache: the guess skips it
             run_part(k, g);
         };
         std::vector<std::thread> th;
@@ -613,19 +610,15 @@ static int judge_parts(ResolveState &st, const ResolveConfig &cfg, const std::ve
 // Judge several shards of one stream (e.g. one per GPU) concurrently and exactly: every shard is a
 // part, long shards are cut once more (see judge_parts).  The deliveries are held in the scratch
 // until resolve_commit.  Returns the rounds judge_parts took.
-static int judge_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards, const modes_candidate *const *cands,
-                        const modes_tile *const *tiles, const size_t *n_tiles, const int64_t *buffer_base, ResolveScratch *scratch,
-                        const modes_recovered *const *recovered = nullptr, const WeakList *weak = nullptr,
-                        const modes_carrier *const *carrier = nullptr) {
+static int judge_shards(ResolveState &st, const ResolveConfig &cfg, const Shard *shards, size_t n_shards, ResolveScratch *scratch) {
     std::vector<Part> &parts = scratch->parts;
     parts.clear();
     size_t threads_left = parts_for((size_t)-1);
     for (size_t k = 0; k < n_shards; k++) {
-        size_t want = parts_for(n_tiles[k]);
+        size_t want = parts_for(shards[k].n_tiles);
         const size_t share = threads_left / (n_shards - k) > 0 ? threads_left / (n_shards - k) : 1;
         if (want > share) want = share;
-        cut_parts(cands[k], tiles[k], n_tiles[k], buffer_base[k], want, parts, recovered ? recovered[k] : nullptr,
-                  recovered && weak ? weak + k : nullptr, carrier ? carrier[k] : nullptr);
+        cut_parts(shards[k], want, parts);
         threads_left = threads_left > want ? threads_left - want : 0;
     }
     if (scratch->runs.size() < parts.size()) scratch->runs.resize(parts.size());
@@ -639,14 +632,12 @@ void resolve_commit(MessageOut &out, ResolveScratch *scratch) {
     scratch->n_runs_held = 0;
 }
 
-void resolve_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards, const modes_candidate *const *cands,
-                    const modes_tile *const *tiles, const size_t *n_tiles, const int64_t *buffer_base,
-                    MessageOut &out, ResolveScratch *scratch, const modes_recovered *const *recovered, const WeakList *weak,
-                    const modes_carrier *const *carrier) {
+void resolve_shards(ResolveState &st, const ResolveConfig &cfg, const Shard *shards, size_t n_shards, MessageOut &out,
+                    ResolveScratch *scratch) {
     const bool timing = std::getenv("MODES_RESOLVE_TIMING") != nullptr;
     auto now = [] { return std::chrono::steady_clock::now(); };
     const auto t_start = now();
-    const int rounds = judge_shards(st, cfg, n_shards, cands, tiles, n_tiles, buffer_base, scratch, recovered, weak, carrier);
+    const int rounds = judge_shards(st, cfg, shards, n_shards, scratch);
     const size_t n_parts = scratch->n_runs_held;
     const auto t_judged = now();
     resolve_commit(out, scratch);
@@ -656,16 +647,12 @@ void resolve_shards(ResolveState &st, const ResolveConfig &cfg, size_t n_shards,
                      std::chrono::duration<double, std::milli>(now() - t_judged).count());
 }
 
-void resolve_candidates(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands,
-                        const modes_tile *tiles, size_t n_tiles, int64_t buffer_base, MessageOut &out,
-                        ResolveScratch *scratch, const modes_recovered *recovered, const WeakList &weak,
-                        const modes_carrier *carrier) {
-    resolve_shards(st, cfg, 1, &cands, &tiles, &n_tiles, &buffer_base, out, scratch, &recovered, &weak, &carrier);
+void resolve_candidates(ResolveState &st, const ResolveConfig &cfg, const Shard &shard, MessageOut &out, ResolveScratch *scratch) {
+    resolve_shards(st, cfg, &shard, 1, out, scratch);
 }
 
-void resolve_tentative(ResolveState &st, const ResolveConfig &cfg, const modes_candidate *cands, const modes_tile *tiles,
-                       size_t n_tiles, int64_t buffer_base, ResolveScratch *scratch) {
-    judge_shards(st, cfg, 1, &cands, &tiles, &n_tiles, &buffer_base, scratch);
+void resolve_tentative(ResolveState &st, const ResolveConfig &cfg, const Shard &shard, ResolveScratch *scratch) {
+    judge_shards(st, cfg, &shard, 1, scratch);
 }
 
 }  // namespace modes
