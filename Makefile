@@ -86,7 +86,7 @@ tests/_build/libeval_serial_host.so: tests/host_shim/eval_serial_host.cpp $(CSRC
 # test infrastructure: device harness over the product's own kernel objects (recovery and signal
 # passes on constructed corpora, and the exhaustive sweeps of the core headers' device build)
 DSHIM_OBJS := build/modes_recover.o build/modes_signal.o build/modes_levels.o build/modes_tables.o
-dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so tests/_build/libscan_eval_device.so tests/_build/libresample_pool_device.so tests/_build/libresolve_device.so tests/_build/libinput_device.so tests/_build/libconvert_pool_device.so tests/_build/librate_spectrum_device.so tests/_build/libcarrier_device.so
+dshim: tests/_build/libkernels_device.so tests/_build/libarrival_device.so tests/_build/libscan_eval_device.so tests/_build/libresample_pool_device.so tests/_build/libresolve_device.so tests/_build/libinput_device.so tests/_build/libconvert_pool_device.so tests/_build/librate_spectrum_device.so tests/_build/libcarrier_device.so tests/_build/libgather_pool_device.so
 tests/_build/libkernels_device.so: tests/device_shim/kernels_device.cu $(DSHIM_OBJS) $(CSRC)/modes_internal.h $(CSRC)/modes_signal_core.cuh $(CSRC)/modes_levels_core.cuh include/modes_b200.h
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/kernels_device.cu -o tests/_build/kernels_device.o
@@ -117,6 +117,11 @@ tests/_build/libconvert_pool_device.so: tests/device_shim/convert_pool_device.cu
 	@mkdir -p tests/_build
 	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/convert_pool_device.cu -o tests/_build/convert_pool_device.o
 	$(NVCC) $(ARCH) -shared -o $@ tests/_build/convert_pool_device.o build/modes_resample.o -cudart static
+# the receiver pool's gather launch on constructed jobs (tests/test_pool_device_input.py)
+tests/_build/libgather_pool_device.so: tests/device_shim/gather_pool_device.cu build/modes_resample.o $(CSRC)/modes_internal.h include/modes_b200.h
+	@mkdir -p tests/_build
+	$(NVCC) $(NVFLAGS) -I$(CSRC) -c tests/device_shim/gather_pool_device.cu -o tests/_build/gather_pool_device.o
+	$(NVCC) $(ARCH) -shared -o $@ tests/_build/gather_pool_device.o build/modes_resample.o -cudart static
 # the 16-bit input launches on chosen spans, and their timing (tests/test_input_format.py, scripts/input_format_time.py)
 tests/_build/libinput_device.so: tests/device_shim/input_device.cu build/modes_resample.o $(CSRC)/modes_internal.h include/modes_b200.h
 	@mkdir -p tests/_build

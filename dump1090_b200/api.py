@@ -292,7 +292,8 @@ EXPORTS = ["modes_abi_version", "modes_default_config", "modes_create", "modes_d
            "modes_set_input_rate", "modes_resample_device", "modes_pool_set_input_rate", "modes_set_input_format",
            "modes_pool_set_input_format", "modes_resample_device_at", "modes_set_input_offset",
            "modes_resample_device_shift", "modes_set_spectrum", "modes_take_spectra", "modes_pool_set_spectrum",
-           "modes_pool_take_spectra", "modes_process_device", "modes_set_carrier", "modes_pool_set_carrier"]
+           "modes_pool_take_spectra", "modes_process_device", "modes_set_carrier", "modes_pool_set_carrier",
+           "modes_pool_submit_device", "modes_pool_ingest_device"]
 
 INPUT_RATES = (2_000_000, 2_400_000, 4_000_000, 6_000_000, 8_000_000, 10_000_000)      # modes_set_input_rate
 INPUT_FORMATS = {"uc8": 0, "sc16": 1, "sc16q11": 2}     # modes_set_input_format: MODES_INPUT_*
@@ -391,6 +392,8 @@ def lib():
         L.modes_pool_last_error.argtypes = [C.c_void_p]
         L.modes_pool_ingest.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, POOL_SINK_FN, C.c_void_p]
         L.modes_pool_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
+        L.modes_pool_ingest_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, POOL_SINK_FN, C.c_void_p]
+        L.modes_pool_submit_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
         L.modes_pool_collect.argtypes = [C.c_void_p, POOL_SINK_FN, C.c_void_p]
         L.modes_pool_resolve.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, POOL_SINK_FN, C.c_void_p]
         L.modes_pool_stats.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(Stats)]
@@ -1119,7 +1122,12 @@ class ReceiverPool:
     set_input_format(receiver, fmt, shift) one receiver (modes_pool_set_input_format).  A buffer is the
     receiver's next BUFFER_SAMPLES samples as uint8 bytes: BUFFER_BYTES for a UC8 receiver, 2 * BUFFER_BYTES
     of little-endian int16 I/Q for an SC16 or SC16Q11 one; everything delivered for a 16-bit receiver
-    equals what a UC8 receiver at its rate delivers on the converted bytes."""
+    equals what a UC8 receiver at its rate delivers on the converted bytes.
+    ingest() and submit() also take CUDA torch tensors on the pool's device, either a list of one tensor per
+    receiver or a 2-D tensor of one row per receiver, each read as its raw bytes (e.g. int16 SC16 I/Q), and
+    decode them where they are (modes_pool_submit_device): the output is what the same bytes give from host
+    memory, without their two trips across PCIe.  A receiver is fed from one kind of memory until
+    reset(receiver)."""
 
     def __init__(self, n_receivers: int, max_batch: int = 0, signal: bool = False, levels: bool = False,
                  recover: bool = False, weak_preambles: bool = False, arrival: bool = False,
@@ -1172,8 +1180,49 @@ class ReceiverPool:
                 raise ValueError(f"receiver {r}: a buffer of {b.size} bytes, its input format takes {want}")
         return ids, bufs
 
+    def _device_buffers(self, receivers, buffers):
+        """The ids, the device addresses of the CUDA tensors (a list of one per receiver, or the rows of a 2-D
+        tensor), each read as its raw bytes and of its receiver's size, and the tensors to keep alive until the
+        batch is collected; their writers finished.  ValueError otherwise."""
+        ids = np.ascontiguousarray(receivers, dtype=np.uint32)
+        if _is_cuda_tensor(buffers):
+            t = self._on_device(buffers)
+            if t.dim() != 2 or t.shape[0] != ids.size:
+                raise ValueError(f"a tensor of shape {tuple(t.shape)} for {ids.size} receivers: one row per receiver")
+            row = t.shape[1] * t.element_size()
+            ptrs, sizes, keep = [t.data_ptr() + i * row for i in range(ids.size)], [row] * ids.size, [t]
+        else:
+            if not all(_is_cuda_tensor(b) for b in buffers):
+                raise ValueError("a list that mixes CUDA tensors with host buffers: one kind of memory per call")
+            keep = [self._on_device(b) for b in buffers]
+            if len(keep) != ids.size:
+                raise ValueError(f"{len(keep)} buffers for {ids.size} receivers")
+            ptrs, sizes = [t.data_ptr() for t in keep], [t.numel() * t.element_size() for t in keep]
+        for r, n in zip(ids.tolist(), sizes):
+            want = self._bytes[r] if r < self.n else BUFFER_BYTES
+            if n != want:
+                raise ValueError(f"receiver {r}: a buffer of {n} bytes, its input format takes {want}")
+        if keep:
+            _sync_stream(keep[0])                            # one device, so one current stream for all
+        return ids, (C.c_void_p * len(ptrs))(*ptrs), keep
+
+    def _on_device(self, t):
+        """The CUDA tensor as a contiguous tensor on this pool's device."""
+        if t.device.index != self.cfg.device:
+            raise ValueError(f"the tensor is on {t.device}, the pool on cuda:{self.cfg.device}")
+        return t if t.is_contiguous() else t.contiguous()
+
+    @staticmethod
+    def _on_gpu(buffers) -> bool:
+        return _is_cuda_tensor(buffers) or any(_is_cuda_tensor(b) for b in buffers)
+
     def ingest(self, receivers, buffers) -> None:
-        """buffers[i]: the next buffer of receivers[i], uint8 bytes (numpy) of its format (class docstring)."""
+        """buffers[i]: the next buffer of receivers[i], uint8 bytes (numpy) of its format (class docstring),
+        or CUDA tensors of those bytes (a list, or a 2-D tensor of one row per receiver)."""
+        if self._on_gpu(buffers):
+            ids, ptrs, _keep = self._device_buffers(receivers, buffers)
+            self._check(lib().modes_pool_ingest_device(self._h, _ptr(ids), ptrs, ids.size, self._fn, None))
+            return
         ids, bufs = self._buffers(receivers, buffers)
         ptrs = (C.c_void_p * len(bufs))(*[b.ctypes.data for b in bufs])
         self._check(lib().modes_pool_ingest(self._h, _ptr(ids), ptrs, ids.size, self._fn, None))
@@ -1183,8 +1232,18 @@ class ReceiverPool:
         fn = sink if sink is not None else C.cast(None, POOL_SINK_FN)
         self._check(lib().modes_pool_ingest(self._h, _ptr(receivers), ptrs, receivers.size, fn, None))
 
+    def ingest_device_ptrs(self, receivers: np.ndarray, ptrs, sink=None) -> None:
+        """modes_pool_ingest_device: the same from raw device addresses of the pool's device, written before the call."""
+        fn = sink if sink is not None else C.cast(None, POOL_SINK_FN)
+        self._check(lib().modes_pool_ingest_device(self._h, _ptr(receivers), ptrs, receivers.size, fn, None))
+
     def submit(self, receivers, buffers) -> None:
         """Upload + kernels, no waiting; `buffers` are kept alive until the matching collect()."""
+        if self._on_gpu(buffers):
+            ids, ptrs, keep = self._device_buffers(receivers, buffers)
+            self._check(lib().modes_pool_submit_device(self._h, _ptr(ids), ptrs, ids.size))
+            self._inflight = getattr(self, "_inflight", []) + [(ids, keep)]
+            return
         ids, bufs = self._buffers(receivers, buffers)
         ptrs = (C.c_void_p * len(bufs))(*[b.ctypes.data for b in bufs])
         self._check(lib().modes_pool_submit(self._h, _ptr(ids), ptrs, ids.size))
@@ -1192,6 +1251,10 @@ class ReceiverPool:
 
     def submit_ptrs(self, receivers: np.ndarray, ptrs) -> None:
         self._check(lib().modes_pool_submit(self._h, _ptr(receivers), ptrs, receivers.size))
+
+    def submit_device_ptrs(self, receivers: np.ndarray, ptrs) -> None:
+        """modes_pool_submit_device: raw device addresses, which must stay valid and unchanged until collect()."""
+        self._check(lib().modes_pool_submit_device(self._h, _ptr(receivers), ptrs, receivers.size))
 
     def collect(self, sink="collect") -> None:
         """Wait for the oldest submitted batch, resolve it, deliver its messages (sink=None: only to the output array)."""

@@ -1303,26 +1303,41 @@ int modes_finish(modes_ctx *ctx) {
     return run_buffers(ctx, dev ? device_buffers(ctx->d_pending.get(), ctx->d_carry.get()) : host_buffers(ctx->pending.get()), 1);
 }
 
-// modes_process_device's refusal of memory that is not the context's device memory, naming what it is.
-static int check_device_input(modes_ctx *ctx, const void *p) {
+}  // extern "C"
+
+namespace modes {
+
+std::string device_input_refusal(const void *p, int device, const char *owner, const char *host_call) {
+    char buf[256];
     cudaPointerAttributes a;
     const cudaError_t e = cudaPointerGetAttributes(&a, p);
     if (e != cudaSuccess) {
         (void)cudaGetLastError();
-        return fail(ctx, "modes_process_device: cudaPointerGetAttributes failed: %s", cudaGetErrorString(e));
+        snprintf(buf, sizeof buf, "cudaPointerGetAttributes failed: %s", cudaGetErrorString(e));
+        return buf;
     }
     const char *what = nullptr;
     switch (a.type) {
     case cudaMemoryTypeDevice:
-        if (a.device == ctx->cfg.device) return 0;
-        return fail(ctx, "modes_process_device: the bytes are in memory of device %d, not of the context's device %d",
-                    a.device, ctx->cfg.device);
+        if (a.device == device) return std::string();
+        snprintf(buf, sizeof buf, "the bytes are in memory of device %d, not of the %s's device %d", a.device, owner, device);
+        return buf;
     case cudaMemoryTypeManaged: what = "managed memory"; break;
     case cudaMemoryTypeHost: what = "pinned host memory"; break;
     default: what = "host memory"; break;
     }
-    return fail(ctx, "modes_process_device: the bytes are in %s, not in memory of the context's device %d (use modes_process)",
-                what, ctx->cfg.device);
+    snprintf(buf, sizeof buf, "the bytes are in %s, not in memory of the %s's device %d (use %s)", what, owner, device, host_call);
+    return buf;
+}
+
+}  // namespace modes
+
+extern "C" {
+
+// modes_process_device's refusal of memory that is not the context's device memory, naming what it is.
+static int check_device_input(modes_ctx *ctx, const void *p) {
+    const std::string no = modes::device_input_refusal(p, ctx->cfg.device, "context", "modes_process");
+    return no.empty() ? 0 : fail(ctx, "modes_process_device: %s", no.c_str());
 }
 
 int modes_process_device(modes_ctx *ctx, const void *d_iq, size_t nbytes) {

@@ -5,6 +5,7 @@
 #include <cstddef>
 #include <cstdint>
 #include <cstring>
+#include <string>
 #include <vector>
 #include <cuda_runtime.h>
 #include "modes_b200.h"
@@ -158,6 +159,24 @@ struct PoolConvertJob {
     int32_t        shift;
 };
 void launch_convert_pool(const PoolConvertJob *d_jobs, uint32_t n_jobs, cudaStream_t stream);
+// The receiver pool's device-fed 2 MHz receivers (modes_pool_submit_device): one launch for one job per such
+// pair of the batch, after the conversion.  A job copies the MODES_BUFFER_BYTES UC8 bytes at in (the caller's
+// buffer; nullptr: data already holds them, converted) to data, writes the pad tail from carry_in (the
+// receiver's device carry; nullptr: its stream starts, the tail is no signal) and stores the last
+// MODES_CARRY_BYTES of the buffer to carry_out.  in and data are 16-byte aligned, the three carry spans
+// 4-byte aligned; carry_out is never carry_in.
+struct PoolGatherJob {
+    const uint8_t *in;
+    uint8_t       *data;
+    const uint8_t *carry_in;
+    uint8_t       *carry_out;
+    uint8_t       *pad_tail;
+};
+void launch_gather_pool(const PoolGatherJob *d_jobs, uint32_t n_jobs, cudaStream_t stream);
+// A device-fed call's refusal of memory that is not device memory of `device` (modes_process_device,
+// modes_pool_submit_device): empty when p is such memory, else what it is, for the caller's message
+// (`owner`: whose device; `host_call`: the call for host memory).
+std::string device_input_refusal(const void *p, int device, const char *owner, const char *host_call);
 // The input spectrum pass (modes_spectrum.cu, K13; arithmetic in modes_spectrum_core.cuh): out[k] = the record of
 // reference buffer first_buffer + k, k < n_buffers, of a stream at the ratio out : in (InputRate) whose input
 // span the job holds (in, in_bytes, in_first: as launch_decimate reads them, UC8 with shift < 0, else int16

@@ -38,6 +38,14 @@
 // area, and one launch ahead of the others (K10's pool form) converts each to its UC8 buffer, straight into
 // the pair's data buffer at 2 MHz, into the receiver's slot of the UC8 staging area at 2.4 MS/s.  From there
 // on the receiver is a UC8 receiver at its rate; its carry (2 MHz) is converted on the host.
+//
+// A device-fed call (modes_pool_submit_device) reads the callers' buffers where they are: the conversion
+// reads its 16-bit buffers in place, and the resampling and history launches read the 2.4 MS/s UC8
+// receivers' buffers in place.  The 2 MHz receivers' carries stay on the device, in ping-pong halves of
+// one array: one more launch (gather_pool_kernel), after the conversion, moves each 2 MHz buffer into its
+// pair, its receiver's carry into the pad tail (no signal for a stream's first buffer) and the buffer's
+// last 476 bytes into the other half.  Only the 16-bit 2.4 MS/s receivers still use a staging area, the
+// UC8 one they are converted into.
 #include <algorithm>
 #include <cstdarg>
 #include <cstdio>
@@ -84,6 +92,9 @@ struct Receiver {
     int64_t in_total = 0, hist0 = 0;
     modes::DevBuf<uint8_t> hist[2];            // kHistBytes each, made on the receiver's first 2.4 MS/s call
     int cur = 0;
+    // which memory its stream is fed from (modes_pool_submit or modes_pool_submit_device), fixed by its
+    // first call until modes_pool_reset
+    enum class Feed : uint8_t { none, host, device } feed = Feed::none;
 };
 
 // 2.4 MS/s: what a call of one buffer's bytes does to receiver r: whether it completes the 2 MHz buffer
@@ -196,7 +207,8 @@ struct modes_pool {
         bool busy = false;
         // staged calls (a 2.4 MS/s or a 16-bit receiver): the call's UC8 buffers [max_batch], the jobs of
         // the resampling and history launches (pinned and device), and an event after the launches, which
-        // the other slot's next staged call waits for (a receiver in both batches)
+        // the other slot's next staged call waits for (a receiver in both batches).  A device-fed call
+        // records it too, after its gather launch, and waits for it first: its carries are the other slot's.
         modes::DevBuf<uint8_t> d_stage;
         RateJobs<true> h_jobs;
         RateJobs<false> d_jobs;
@@ -207,6 +219,9 @@ struct modes_pool {
         modes::PinnedBuf<modes::PoolConvertJob> h_cjobs;
         modes::DevBuf<modes::PoolConvertJob> d_cjobs;
         std::vector<const uint8_t *> iq8, iq16;   // the call's UC8 and 16-bit buffers, each group in call order
+        // device-fed calls: the gather jobs of their 2 MHz pairs
+        modes::PinnedBuf<modes::PoolGatherJob> h_gjobs;
+        modes::DevBuf<modes::PoolGatherJob> d_gjobs;
         // with spectra: one job and one record per pair
         modes::PinnedBuf<modes::PoolSpectrumJob> h_sjobs;
         modes::DevBuf<modes::PoolSpectrumJob> d_sjobs;
@@ -214,6 +229,9 @@ struct modes_pool {
         modes::DevBuf<modes_spectrum> d_spectra;
     } slot[2];
     unsigned submitted = 0, collected = 0;     // batches so far: slot = number & 1
+    // device-fed 2 MHz receivers' carries: [2][n_receivers][MODES_CARRY_BYTES], made on the first device-fed
+    // call; the call of a receiver's buffer k reads half k & 1 and writes half (k + 1) & 1
+    modes::DevBuf<uint8_t> d_carries;
     // the per-receiver resolve: one block of the receiver list per host thread
     struct Block {
         std::unique_ptr<modes::ResolveScratch, void (*)(modes::ResolveScratch *)> scratch{nullptr, modes::scratch_destroy};
@@ -281,8 +299,9 @@ int out_of_memory(modes_pool *p) {
     return fail(p, "out of memory for %zu receivers per batch", p->max_batch);
 }
 
-// The slot contexts that are missing and the batches' buffers, with the pool's device current.
-int ensure_device(modes_pool *p) {
+// The slot contexts that are missing and the batches' buffers, with the pool's device current; the
+// carries' pinned staging only for host-fed calls.
+int ensure_device(modes_pool *p, bool host_fed) {
     if (cudaSetDevice(p->cfg.device) != cudaSuccess) return fail(p, "cudaSetDevice failed: %s", cudaGetErrorString(cudaGetLastError()));
     modes_config c = p->cfg;
     c.n_gpus = 1; c.gpu_resolve = 0;
@@ -300,7 +319,7 @@ int ensure_device(modes_pool *p) {
                 return fail(p, "device memset failed");
             }
         }
-        if (sl.h_carry.ensure(p->max_batch * MODES_CARRY_BYTES)) return out_of_memory(p);
+        if (host_fed && sl.h_carry.ensure(p->max_batch * MODES_CARRY_BYTES)) return out_of_memory(p);
     }
     return 0;
 }
@@ -511,39 +530,73 @@ int modes_pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, const
 // buffers (into their pairs at 2 MHz, into the staging area at 2.4 MS/s), resample the completing
 // receivers / move the 2 MHz ones into their pairs, and advance the histories.  Staging slots: the UC8
 // buffers in call order, then the 16-bit 2.4 MS/s receivers'.
-int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *const *iq, size_t n) {
+//
+// device: the buffers are device memory of cfg.device (modes_pool_submit_device), read in place by the same
+// launches, and the 2 MHz pairs are filled by the gather launch; the staging area holds only the 16-bit
+// 2.4 MS/s receivers' converted bytes.
+static int submit(modes_pool *p, const uint32_t *receivers, const uint8_t *const *iq, size_t n, bool device) {
     namespace input = modes::input;
+    using Feed = Receiver::Feed;
     if (!p) return -1;
     if (check_ids(p, receivers, n)) return -1;
     if (!n) return fail(p, "an empty batch");
     if (!iq) return fail(p, "no buffers");
-    if (ensure_device(p)) return -1;
+    if (device)
+        for (size_t i = 0; i < n; i++) {
+            if (!iq[i]) return fail(p, "modes_pool_submit_device: receiver %u: null pointer", receivers[i]);
+            if (reinterpret_cast<uintptr_t>(iq[i]) & 15)
+                return fail(p, "modes_pool_submit_device: receiver %u: the buffer at %p is not 16-byte aligned", receivers[i],
+                            static_cast<const void *>(iq[i]));
+            const std::string no = modes::device_input_refusal(iq[i], p->cfg.device, "pool", "modes_pool_submit");
+            if (!no.empty()) return fail(p, "modes_pool_submit_device: receiver %u: %s", receivers[i], no.c_str());
+        }
+    for (size_t i = 0; i < n; i++)
+        if (p->rx[receivers[i]].feed == (device ? Feed::host : Feed::device))
+            return fail(p, "%s: receiver %u has a stream fed from %s memory in progress; call modes_pool_reset first",
+                        device ? "modes_pool_submit_device" : "modes_pool_submit", receivers[i], device ? "host" : "device");
+    if (ensure_device(p, !device)) return -1;
     modes_pool::Slot &sl = p->slot[p->submitted & 1];
     if (sl.busy) return fail(p, "two batches are in flight: modes_pool_collect first");
-    bool staged = false, wide = false;
+    bool staged = false, wide = false, two_mhz = false, rated = false, wide24 = false;
     for (size_t i = 0; i < n; i++) {
         if (!iq[i]) return fail(p, "receiver %u: no buffer", receivers[i]);
         const Receiver &r = p->rx[receivers[i]];
         wide |= r.format != input::kUC8;
         staged |= wide || r.rate != kRate2M;
+        two_mhz |= r.rate == kRate2M;
+        rated |= r.rate != kRate2M;
+        wide24 |= r.format != input::kUC8 && r.rate != kRate2M;
     }
+    if (device) staged = false;                // a device-fed call stages only wide24's conversions
     const size_t mb = p->max_batch;
     const bool spectra = p->feat.spectrum;
     if (staged && (sl.d_stage.ensure(mb * kBuf) || sl.h_jobs.ensure(mb) || sl.d_jobs.ensure(mb))) return out_of_memory(p);
-    if (wide && (sl.d_stage16.ensure(mb * 2 * kBuf) || sl.h_cjobs.ensure(mb) || sl.d_cjobs.ensure(mb))) return out_of_memory(p);
+    if (wide && !device && (sl.d_stage16.ensure(mb * 2 * kBuf) || sl.h_cjobs.ensure(mb) || sl.d_cjobs.ensure(mb)))
+        return out_of_memory(p);
+    if (device) {
+        if ((two_mhz && (p->d_carries.ensure(2 * p->rx.size() * MODES_CARRY_BYTES) || sl.h_gjobs.ensure(mb) || sl.d_gjobs.ensure(mb))) ||
+            (rated && (sl.h_jobs.ensure(mb) || sl.d_jobs.ensure(mb))) || (wide24 && sl.d_stage.ensure(mb * kBuf)) ||
+            (wide && (sl.h_cjobs.ensure(mb) || sl.d_cjobs.ensure(mb))))
+            return out_of_memory(p);
+    }
     if (spectra && (sl.h_sjobs.ensure(mb) || sl.d_sjobs.ensure(mb) || sl.h_spectra.ensure(mb) || sl.d_spectra.ensure(mb)))
         return out_of_memory(p);
-    if (staged && !sl.rate_done && cudaEventCreateWithFlags(&sl.rate_done, cudaEventDisableTiming) != cudaSuccess)
+    if ((staged || device) && !sl.rate_done && cudaEventCreateWithFlags(&sl.rate_done, cudaEventDisableTiming) != cudaSuccess)
         return fail(p, "event creation failed: %s", cudaGetErrorString(cudaGetLastError()));
 
     modes::PoolResampleJob *rj = sl.h_jobs.resample();
     modes::PoolHistoryJob *hj = sl.h_jobs.history();
-    size_t n_pairs = 0, n_rj = 0, n_hist = 0, n_conv = 0;
+    // a device-fed receiver's carry: half k & 1 holds what its buffer k - 1 left
+    auto device_carry = [p](uint32_t id, int64_t k) {
+        return p->d_carries.get() + ((size_t)(k & 1) * p->rx.size() + id) * MODES_CARRY_BYTES;
+    };
+    size_t n_pairs = 0, n_rj = 0, n_hist = 0, n_conv = 0, n_gather = 0;
     uint64_t hist_max = 0;
     bool carries = false;
     sl.iq8.clear();
     sl.iq16.clear();
-    for (size_t i = 0; i < n; i++) (p->rx[receivers[i]].format == input::kUC8 ? sl.iq8 : sl.iq16).push_back(iq[i]);
+    if (!device)
+        for (size_t i = 0; i < n; i++) (p->rx[receivers[i]].format == input::kUC8 ? sl.iq8 : sl.iq16).push_back(iq[i]);
     size_t n_stage = sl.iq8.size();
     sl.ids.clear();
     sl.buf_index.clear();
@@ -551,14 +604,23 @@ int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *c
         Receiver &r = p->rx[receivers[i]];
         const bool uc8 = r.format == input::kUC8;
         uint8_t *data = sl.d_batch.get() + (2 * n_pairs + 1) * kBuf;    // the data buffer of its pair, if it gets one
-        // staged: where its call's UC8 bytes are staged (none for a 16-bit 2 MHz receiver, converted into its pair)
-        uint8_t *stage = staged && (uc8 || r.rate != kRate2M) ? sl.d_stage.get() + (uc8 ? k8++ : n_stage++) * kBuf : nullptr;
+        // staged: where its call's UC8 bytes are staged (none for a 16-bit 2 MHz receiver, converted into its pair);
+        // device-fed: only a 16-bit 2.4 MS/s receiver's
+        const bool staging = device ? !uc8 && r.rate != kRate2M : staged && (uc8 || r.rate != kRate2M);
+        uint8_t *stage = staging ? sl.d_stage.get() + (uc8 ? k8++ : n_stage++) * kBuf : nullptr;
+        // the UC8 bytes the resampling reads: a device-fed UC8 receiver's own buffer
+        const uint8_t *in8 = device && uc8 ? iq[i] : stage;
         if (!uc8) {
-            sl.h_cjobs[n_conv] = modes::PoolConvertJob{sl.d_stage16.get() + n_conv * 2 * kBuf, stage ? stage : data, r.shift};
+            const uint8_t *in16 = device ? iq[i] : sl.d_stage16.get() + n_conv * 2 * kBuf;
+            sl.h_cjobs[n_conv] = modes::PoolConvertJob{in16, stage ? stage : data, r.shift};
             n_conv++;
         }
         bool pair = true;
-        if (r.rate == kRate2M) {
+        if (r.rate == kRate2M && device) {
+            sl.h_gjobs[n_gather++] = modes::PoolGatherJob{uc8 ? iq[i] : nullptr, data,
+                                                          r.submitted ? device_carry(receivers[i], r.submitted) : nullptr,
+                                                          device_carry(receivers[i], r.submitted + 1), data - MODES_CARRY_BYTES};
+        } else if (r.rate == kRate2M) {
             memcpy(sl.h_carry.get() + n_pairs * MODES_CARRY_BYTES, r.carry, MODES_CARRY_BYTES);
             carries = true;
             if (stage) rj[n_rj++] = modes::PoolResampleJob{nullptr, stage, 0, 0, -1, nullptr, data};
@@ -571,23 +633,38 @@ int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *c
             const RatePlan pl = rate_plan(r);
             pair = pl.completes;
             if (pair)
-                rj[n_rj++] = modes::PoolResampleJob{r.hist[r.cur].get(), stage, r.hist0, r.in_total, r.submitted * kBufSamples,
+                rj[n_rj++] = modes::PoolResampleJob{r.hist[r.cur].get(), in8, r.hist0, r.in_total, r.submitted * kBufSamples,
                                                     data - MODES_CARRY_BYTES, data};
             const uint64_t bytes = (uint64_t)(r.in_total + (int64_t)kBuf - pl.keep);
             if (bytes > kHistBytes)
                 return fail(p, "internal: 2.4 MS/s input history of %llu bytes for receiver %u", (unsigned long long)bytes, receivers[i]);
-            hj[n_hist++] = modes::PoolHistoryJob{r.hist[r.cur].get(), stage, r.hist0, r.in_total, pl.keep, r.hist[r.cur ^ 1].get()};
+            hj[n_hist++] = modes::PoolHistoryJob{r.hist[r.cur].get(), in8, r.hist0, r.in_total, pl.keep, r.hist[r.cur ^ 1].get()};
             if (bytes > hist_max) hist_max = bytes;
         }
         if (!pair) continue;
-        if (spectra) sl.h_sjobs[n_pairs] = spectrum_job(r, r.submitted, data, stage);
+        if (spectra) sl.h_sjobs[n_pairs] = spectrum_job(r, r.submitted, data, in8);
         n_pairs++;
         sl.ids.push_back(receivers[i]);
         sl.buf_index.push_back(r.submitted);
     }
 
     cudaStream_t st = static_cast<cudaStream_t>(modes_stream(sl.ctx));
-    if (!staged) {
+    const modes_pool::Slot &other = p->slot[(p->submitted & 1) ^ 1];
+    if (device) {
+        if ((n_gather && cudaMemcpyAsync(sl.d_gjobs.get(), sl.h_gjobs.get(), n_gather * sizeof(modes::PoolGatherJob),
+                                         cudaMemcpyHostToDevice, st) != cudaSuccess) ||
+            (rated && cudaMemcpyAsync(sl.d_jobs.resample(), rj, sl.h_jobs.bytes(), cudaMemcpyHostToDevice, st) != cudaSuccess) ||
+            (n_conv && cudaMemcpyAsync(sl.d_cjobs.get(), sl.h_cjobs.get(), n_conv * sizeof(modes::PoolConvertJob),
+                                       cudaMemcpyHostToDevice, st) != cudaSuccess))
+            return fail(p, "job upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+        modes::launch_convert_pool(sl.d_cjobs.get(), (uint32_t)n_conv, st);
+        // the other batch in flight may name the same receivers: its carries, reads and history step first
+        if (other.rate_recorded && cudaStreamWaitEvent(st, other.rate_done, 0) != cudaSuccess)
+            return fail(p, "stream wait failed: %s", cudaGetErrorString(cudaGetLastError()));
+        modes::launch_gather_pool(sl.d_gjobs.get(), (uint32_t)n_gather, st);
+        modes::launch_resample_pool(sl.d_jobs.resample(), (uint32_t)n_rj, st);
+        modes::launch_history_pool(sl.d_jobs.history(), (uint32_t)n_hist, hist_max, st);
+    } else if (!staged) {
         if (upload_carries(p, sl, st, n_pairs) || upload_buffers(p, st, iq, n, sl.d_batch.get() + kBuf, 2 * kBuf, kBuf)) return -1;
     } else {
         if (!sl.iq8.empty() && upload_buffers(p, st, sl.iq8.data(), sl.iq8.size(), sl.d_stage.get(), kBuf, kBuf)) return -1;
@@ -602,7 +679,6 @@ int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *c
         // the conversion writes only this slot's pairs and staging area: it need not wait for the other slot
         modes::launch_convert_pool(sl.d_cjobs.get(), (uint32_t)n_conv, st);
         // the other batch in flight may name the same receivers: its reads and its history step first
-        const modes_pool::Slot &other = p->slot[(p->submitted & 1) ^ 1];
         if (other.rate_recorded && cudaStreamWaitEvent(st, other.rate_done, 0) != cudaSuccess)
             return fail(p, "stream wait failed: %s", cudaGetErrorString(cudaGetLastError()));
         modes::launch_resample_pool(sl.d_jobs.resample(), (uint32_t)n_rj, st);
@@ -611,7 +687,7 @@ int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *c
     // the spectra read the histories too: before rate_done, after which the other slot's history step may
     // overwrite them
     if (spectra && n_pairs && launch_pool_spectra(p, sl, st, n_pairs)) return -1;
-    if (staged) {
+    if (staged || device) {
         if (cudaGetLastError() != cudaSuccess || cudaEventRecord(sl.rate_done, st) != cudaSuccess)
             return fail(p, "resampling launch failed: %s", cudaGetErrorString(cudaGetLastError()));
         sl.rate_recorded = true;
@@ -620,8 +696,10 @@ int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *c
 
     for (size_t i = 0; i < n; i++) {
         Receiver &r = p->rx[receivers[i]];
+        r.feed = device ? Feed::device : Feed::host;
         if (r.rate == kRate2M) {
             r.submitted++;
+            if (device) continue;              // its carry is on the device
             // what it carries into its next buffer (dump1090.c:481)
             if (r.format == input::kUC8) memcpy(r.carry, iq[i] + kBuf - MODES_CARRY_BYTES, MODES_CARRY_BYTES);
             else input::convert_samples(iq[i] + 2 * (kBuf - MODES_CARRY_BYTES), MODES_CARRY_BYTES / 2, r.shift, r.carry);
@@ -636,6 +714,14 @@ int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *c
     sl.busy = true;
     p->submitted++;
     return 0;
+}
+
+int modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *const *iq, size_t n) {
+    return submit(p, receivers, iq, n, false);
+}
+
+int modes_pool_submit_device(modes_pool *p, const uint32_t *receivers, const void *const *d_iq, size_t n) {
+    return submit(p, receivers, reinterpret_cast<const uint8_t *const *>(d_iq), n, true);
 }
 
 int modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user) {
@@ -682,6 +768,15 @@ int modes_pool_ingest(modes_pool *p, const uint32_t *receivers, const uint8_t *c
     return modes_pool_collect(p, sink, user);
 }
 
+int modes_pool_ingest_device(modes_pool *p, const uint32_t *receivers, const void *const *d_iq, size_t n,
+                             modes_pool_sink_fn sink, void *user) {
+    if (!p) return -1;
+    if (p->collected != p->submitted) return fail(p, "a submitted batch is in flight: modes_pool_collect first");
+    if (!n) return check_ids(p, receivers, n);
+    if (modes_pool_submit_device(p, receivers, d_iq, n)) return -1;
+    return modes_pool_collect(p, sink, user);
+}
+
 int modes_pool_stats(const modes_pool *p, uint32_t receiver, modes_stats *out) {
     if (!p || receiver >= p->rx.size() || !out) return -1;
     memcpy(out->v, p->rx[receiver].rs.stats, sizeof(out->v));
@@ -698,6 +793,7 @@ int modes_pool_reset(modes_pool *p, uint32_t receiver) {
     r.levels.clear();
     r.spectra.clear();
     memset(r.carry, 127, sizeof r.carry);
+    r.feed = Receiver::Feed::none;             // its device carry is not read again: the next buffer is a first
     r.rs.reset();
     return 0;
 }

@@ -13,7 +13,8 @@
 // filter sees exactly the bytes it would see on the converted stream; at 2 MHz K10 (convert_kernel)
 // converts the batch's span straight into its body and carry block.  UC8 keeps its own loader, chosen
 // at compile time.  The receiver pool's 16-bit receivers have K10's pool form (convert_pool_kernel): one
-// launch converts every 16-bit buffer of a call, ahead of the pool's resampling launches.
+// launch converts every 16-bit buffer of a call, ahead of the pool's resampling launches.  A device-fed pool
+// call (modes_pool_submit_device) moves its 2 MHz receivers' buffers and carries with gather_pool_kernel.
 //
 // K11 (decimate_kernel): 4, 6, 8 and 10 MS/s input decimated by M = 2..5, in K10's groups of 8 output
 // samples, from either staging loader.  K12 (its Shift form): the same with each input sample first
@@ -271,7 +272,40 @@ __global__ void __launch_bounds__(kThreads) convert_pool_kernel(const PoolConver
     reinterpret_cast<uint4 *>(j.out)[g] = o;
 }
 
+// Device-fed 2 MHz receivers: job blockIdx.y's buffer moves from the caller's memory to its pair in
+// kGatherBlocks blocks of 16-byte copies, kGatherWords per thread; block 0 also moves the two carries,
+// one 4-byte word per thread (476 bytes: 119 words).
+constexpr int kGatherWords = 4;
+constexpr int kGatherBlocks = kBufWords / (kGatherWords * kThreads);
+static_assert(kGatherBlocks * kGatherWords * kThreads == kBufWords, "whole blocks of words");
+constexpr int kCarryWords = MODES_CARRY_BYTES / 4;
+static_assert(kCarryWords * 4 == MODES_CARRY_BYTES && kCarryWords <= kThreads, "one carry word per thread");
+
+__global__ void __launch_bounds__(kThreads) gather_pool_kernel(const PoolGatherJob *jobs) {
+    const PoolGatherJob j = jobs[blockIdx.y];
+    if (j.in) {
+        const uint4 *in = reinterpret_cast<const uint4 *>(j.in);
+        uint4 *out = reinterpret_cast<uint4 *>(j.data);
+        const int w0 = (int)blockIdx.x * kGatherWords * kThreads + threadIdx.x;
+        uint4 v[kGatherWords];
+#pragma unroll
+        for (int k = 0; k < kGatherWords; k++) v[k] = __ldg(in + w0 + k * kThreads);
+#pragma unroll
+        for (int k = 0; k < kGatherWords; k++) out[w0 + k * kThreads] = v[k];
+    }
+    if (blockIdx.x != 0 || threadIdx.x >= kCarryWords) return;
+    const int t = threadIdx.x;
+    const uint32_t *tail = reinterpret_cast<const uint32_t *>((j.in ? j.in : j.data) + MODES_BUFFER_BYTES - MODES_CARRY_BYTES);
+    const uint32_t c = j.carry_in ? __ldg(reinterpret_cast<const uint32_t *>(j.carry_in) + t) : 0x7f7f7f7fu;
+    reinterpret_cast<uint32_t *>(j.pad_tail)[t] = c;
+    reinterpret_cast<uint32_t *>(j.carry_out)[t] = j.in ? __ldg(tail + t) : tail[t];
+}
+
 }  // namespace
+
+void launch_gather_pool(const PoolGatherJob *d_jobs, uint32_t n_jobs, cudaStream_t stream) {
+    if (n_jobs) gather_pool_kernel<<<dim3(kGatherBlocks, n_jobs), kThreads, 0, stream>>>(d_jobs);
+}
 
 void launch_convert_pool(const PoolConvertJob *d_jobs, uint32_t n_jobs, cudaStream_t stream) {
     if (n_jobs) convert_pool_kernel<<<dim3(kConvertBlocks, n_jobs), kThreads, 0, stream>>>(d_jobs);

@@ -545,6 +545,25 @@ int  modes_pool_ingest(modes_pool *p, const uint32_t *receivers, const uint8_t *
  * A receiver may be named in both. */
 int  modes_pool_submit(modes_pool *p, const uint32_t *receivers, const uint8_t *const *iq, size_t n);
 int  modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user);
+/* modes_pool_submit / modes_pool_ingest for buffers in device memory of the pool's device (cfg.device): a CUDA
+ * SDR front end, a GPU ingest of remote feeds or a torch pipeline feeds its receivers without a copy through
+ * the host.  d_iq[i] is what iq[i] is for a host-fed call: MODES_BUFFER_BYTES for a UC8 receiver, twice that
+ * for an SC16 or SC16Q11 one, at either input rate.
+ *   Same output: the same messages and every field, sample_pos, statistics, modes_pool_buffers, and level,
+ *     spectrum, recovery and weak records as host-fed calls of the same bytes in the same calls, with every
+ *     switch and with two batches in flight.
+ *   The bytes must be fully written before the call, which does not order itself after the caller's
+ *     streams, and must not change until the matching modes_pool_collect returns (as a host-fed buffer).
+ *   One kind of memory per receiver: from its first call until modes_pool_reset a receiver is fed either by
+ *     host-fed calls or by device-fed calls; naming it in a call of the other kind is refused ("in progress").
+ *   Refused, with a message naming the receiver: a NULL pointer, a buffer that is not 16-byte aligned, and
+ *     memory that cudaPointerGetAttributes does not report as device memory of cfg.device (host, pinned,
+ *     managed, or another device's).
+ * The 2 MHz receivers' carries then live on the device (2 x 476 bytes per receiver of the pool, made on
+ * the first device-fed call); host-fed calls make none of it. */
+int  modes_pool_submit_device(modes_pool *p, const uint32_t *receivers, const void *const *d_iq, size_t n);
+int  modes_pool_ingest_device(modes_pool *p, const uint32_t *receivers, const void *const *d_iq, size_t n,
+                              modes_pool_sink_fn sink, void *user);
 /* The host half alone, for candidate records produced elsewhere over a batch laid out as the pool lays
  * it out: buffer 2i = pad buffer of receivers[i] (no signal, last MODES_CARRY_BYTES = its carry), buffer
  * 2i+1 = its new buffer; candidates/tiles as modes_detect_fetch returns them for those 2n buffers.  The
