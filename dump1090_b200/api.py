@@ -10,6 +10,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import os
 from pathlib import Path
 
 import numpy as np
@@ -293,7 +294,7 @@ EXPORTS = ["modes_abi_version", "modes_default_config", "modes_create", "modes_d
            "modes_pool_set_input_format", "modes_resample_device_at", "modes_set_input_offset",
            "modes_resample_device_shift", "modes_set_spectrum", "modes_take_spectra", "modes_pool_set_spectrum",
            "modes_pool_take_spectra", "modes_process_device", "modes_set_carrier", "modes_pool_set_carrier",
-           "modes_pool_submit_device", "modes_pool_ingest_device"]
+           "modes_pool_submit_device", "modes_pool_ingest_device", "modes_pool_finish", "modes_pool_finish_device"]
 
 INPUT_RATES = (2_000_000, 2_400_000, 4_000_000, 6_000_000, 8_000_000, 10_000_000)      # modes_set_input_rate
 INPUT_FORMATS = {"uc8": 0, "sc16": 1, "sc16q11": 2}     # modes_set_input_format: MODES_INPUT_*
@@ -395,6 +396,10 @@ def lib():
         L.modes_pool_ingest_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, POOL_SINK_FN, C.c_void_p]
         L.modes_pool_submit_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
         L.modes_pool_collect.argtypes = [C.c_void_p, POOL_SINK_FN, C.c_void_p]
+        L.modes_pool_finish.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, POOL_SINK_FN,
+                                        C.c_void_p]
+        L.modes_pool_finish_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, POOL_SINK_FN,
+                                               C.c_void_p]
         L.modes_pool_resolve.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, POOL_SINK_FN, C.c_void_p]
         L.modes_pool_stats.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(Stats)]
         L.modes_pool_reset.argtypes = [C.c_void_p, C.c_uint32]
@@ -1127,7 +1132,10 @@ class ReceiverPool:
     receiver or a 2-D tensor of one row per receiver, each read as its raw bytes (e.g. int16 SC16 I/Q), and
     decode them where they are (modes_pool_submit_device): the output is what the same bytes give from host
     memory, without their two trips across PCIe.  A receiver is fed from one kind of memory until
-    reset(receiver)."""
+    reset(receiver).
+    finish(receivers, tails) ends the listed receivers' streams with their last bytes (modes_pool_finish):
+    everything delivered for a receiver then equals Decoder(same settings).decode(all its bytes), the EOF
+    buffer included unless drop_eof_buffer=1.  decode_captures() decodes many finite captures this way."""
 
     def __init__(self, n_receivers: int, max_batch: int = 0, signal: bool = False, levels: bool = False,
                  recover: bool = False, weak_preambles: bool = False, arrival: bool = False,
@@ -1226,6 +1234,32 @@ class ReceiverPool:
         ids, bufs = self._buffers(receivers, buffers)
         ptrs = (C.c_void_p * len(bufs))(*[b.ctypes.data for b in bufs])
         self._check(lib().modes_pool_ingest(self._h, _ptr(ids), ptrs, ids.size, self._fn, None))
+
+    def finish(self, receivers, tails) -> None:
+        """tails[i]: the last bytes of receivers[i]'s stream, 0 up to its buffer size, uint8 bytes (numpy) or a
+        CUDA tensor read as its raw bytes (for a device-fed or never-fed receiver); the streams then end as
+        Decoder.finish() ends one.  Until reset(receiver), the receiver takes no more buffers."""
+        ids = np.ascontiguousarray(receivers, dtype=np.uint32)
+        if len(tails) != ids.size:
+            raise ValueError(f"{len(tails)} tails for {ids.size} receivers")
+        on_gpu = [_is_cuda_tensor(t) for t in tails]
+        if any(on_gpu) and not all(on_gpu):
+            raise ValueError("a list that mixes CUDA tensors with host buffers: one kind of memory per call")
+        if any(on_gpu):
+            keep = [self._on_device(t) for t in tails]
+            ptrs, sizes = [t.data_ptr() for t in keep], [t.numel() * t.element_size() for t in keep]
+        else:
+            keep = [np.ascontiguousarray(t, dtype=np.uint8).reshape(-1) for t in tails]
+            ptrs, sizes = [t.ctypes.data for t in keep], [t.size for t in keep]
+        for r, n in zip(ids.tolist(), sizes):
+            most = self._bytes[r] if r < self.n else BUFFER_BYTES
+            if n > most:
+                raise ValueError(f"receiver {r}: a tail of {n} bytes, its input format takes at most {most}")
+        if any(on_gpu) and keep:
+            _sync_stream(keep[0])
+        fn = lib().modes_pool_finish_device if any(on_gpu) else lib().modes_pool_finish
+        sizes = np.asarray(sizes, dtype=np.uintp)
+        self._check(fn(self._h, _ptr(ids), (C.c_void_p * len(ptrs))(*ptrs), _ptr(sizes), ids.size, self._fn, None))
 
     def ingest_ptrs(self, receivers: np.ndarray, ptrs, sink=None) -> None:
         """The same from raw host addresses (pinned memory); sink: a POOL_SINK_FN or None to drop the messages."""
@@ -1382,6 +1416,44 @@ class ReceiverPool:
             self.close()
         except Exception:
             pass
+
+
+def decode_captures(captures, *, input_rate: int = 2_000_000, input_format: str = "uc8", input_shift: int | None = None,
+                    max_batch: int = 0, **switches_and_flags) -> list:
+    """Decode many finite captures at once, each as one receiver of a ReceiverPool: returns each capture's
+    messages, equal to Decoder(same settings).decode(capture).  captures: file paths or uint8 arrays, all of
+    one rate and format.  Every capture is fed one buffer per call, in calls of up to max_batch receivers (0:
+    all of them) with two batches in flight, and then finished with its tail.  switches_and_flags: the
+    ReceiverPool switches (signal, levels, recover, ...) and modes_config flags (fix_errors, aggressive,
+    check_crc, drop_eof_buffer, device)."""
+    data = [np.fromfile(c, dtype=np.uint8) if isinstance(c, (str, os.PathLike)) else
+            (np.frombuffer(c, dtype=np.uint8) if isinstance(c, (bytes, bytearray)) else
+             np.ascontiguousarray(c, dtype=np.uint8).reshape(-1)) for c in captures]
+    n = len(data)
+    if not n:
+        return []
+    full = BUFFER_BYTES * (1 if input_format == "uc8" else 2)
+    mb = max_batch if 0 < max_batch < n else n
+    with ReceiverPool(n, max_batch=mb, input_rate=input_rate, input_format=input_format, input_shift=input_shift,
+                      **switches_and_flags) as pool:
+        whole = [d.size // full for d in data]
+        in_flight = 0
+        for k in range(max(whole)):
+            ids = [i for i in range(n) if whole[i] > k]
+            for g in range(0, len(ids), mb):
+                group = ids[g: g + mb]
+                if in_flight == 2:
+                    pool.collect()
+                    in_flight -= 1
+                pool.submit(group, [data[i][k * full: (k + 1) * full] for i in group])
+                in_flight += 1
+        while in_flight:
+            pool.collect()
+            in_flight -= 1
+        for g in range(0, n, mb):
+            group = list(range(g, min(g + mb, n)))
+            pool.finish(group, [data[i][whole[i] * full:] for i in group])
+        return [pool.take(i) for i in range(n)]
 
 
 # ---- SURVEY.md 8(f) item 3: aircraft tracker (host only) -------------------------------------

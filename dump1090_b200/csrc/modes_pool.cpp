@@ -46,6 +46,10 @@
 // pair, its receiver's carry into the pad tail (no signal for a stream's first buffer) and the buffer's
 // last 476 bytes into the other half.  Only the 16-bit 2.4 MS/s receivers still use a staging area, the
 // UC8 one they are converted into.
+//
+// A finite capture ends with modes_pool_finish: each listed receiver's tail is staged as a whole buffer padded
+// with 127 and goes through the same submit path as at most two internal batches (the whole buffer the tail
+// completes, then the EOF buffer), with a few memsets that set what lies past the stream's end to no signal.
 #include <algorithm>
 #include <cstdarg>
 #include <cstdio>
@@ -95,6 +99,7 @@ struct Receiver {
     // which memory its stream is fed from (modes_pool_submit or modes_pool_submit_device), fixed by its
     // first call until modes_pool_reset
     enum class Feed : uint8_t { none, host, device } feed = Feed::none;
+    bool finished = false;                     // modes_pool_finish ended its stream (until modes_pool_reset)
 };
 
 // 2.4 MS/s: what a call of one buffer's bytes does to receiver r: whether it completes the 2 MHz buffer
@@ -114,6 +119,18 @@ RatePlan rate_plan(const Receiver &r) {
     pl.keep = keep < r.hist0 ? r.hist0 : keep;
     return pl;
 }
+
+// A pair of a finish batch (modes_pool_finish): the receiver's tail, staged as a whole buffer padded with 127,
+// makes 2 MHz buffer `buffer`.  A 2.4 MS/s receiver's pair is resampled from its history and the staged tail
+// (no history step: a finish runs at most two batches, both reading the same history); a 2 MHz one is the
+// staged tail itself.  Bytes past real8 of the staged buffer's UC8 bytes (a 16-bit tail's, once converted)
+// and past out_real of the pair's data buffer (2.4 MS/s) are set to 127: input past the stream's end and
+// output past N_out are no signal, as modes_finish pads them.  buffer < 0: an ordinary buffer of the call.
+struct EofPair {
+    int64_t buffer = -1;
+    size_t real8 = kBuf, out_real = kBuf;
+    uint32_t samples = (uint32_t)kBufSamples;  // the real samples of the buffer, for its level record
+};
 
 // The job arrays of a slot's resampling and history launches (pinned or device): PoolResampleJob[n], then
 // PoolHistoryJob[n], in one allocation, so that one copy uploads both.
@@ -202,6 +219,7 @@ struct modes_pool {
         modes::PinnedBuf<uint8_t> h_carry;     // [max_batch][MODES_CARRY_BYTES]
         std::vector<uint32_t> ids;             // the receivers of the batch in flight
         std::vector<int64_t> buf_index;        // with levels: each one's own index of its buffer
+        std::vector<uint32_t> samples;         // with levels: the real samples of each one's buffer
         std::vector<modes_level> level_out;
         modes::Features feat;                  // the switches as they were at submit
         bool busy = false;
@@ -232,6 +250,10 @@ struct modes_pool {
     // device-fed 2 MHz receivers' carries: [2][n_receivers][MODES_CARRY_BYTES], made on the first device-fed
     // call; the call of a receiver's buffer k reads half k & 1 and writes half (k + 1) & 1
     modes::DevBuf<uint8_t> d_carries;
+    // modes_pool_finish: the listed receivers' tails, each staged as a whole buffer of its format padded with
+    // 127 (pinned for host tails, device memory for device tails), made on the first finish
+    modes::PinnedBuf<uint8_t> h_tails;
+    modes::DevBuf<uint8_t> d_tails;
     // the per-receiver resolve: one block of the receiver list per host thread
     struct Block {
         std::unique_ptr<modes::ResolveScratch, void (*)(modes::ResolveScratch *)> scratch{nullptr, modes::scratch_destroy};
@@ -390,6 +412,15 @@ int detect_pairs(modes_pool *p, modes_pool::Slot &sl, size_t n) {
     return 0;
 }
 
+// A finish batch's padding: every span set to 127 on the slot's stream.
+using Spans = std::vector<std::pair<uint8_t *, size_t>>;
+int fill_no_signal(modes_pool *p, const Spans &spans, cudaStream_t st) {
+    for (const auto &sp : spans)
+        if (cudaMemsetAsync(sp.first, 127, sp.second, st) != cudaSuccess)
+            return fail(p, "EOF padding failed: %s", cudaGetErrorString(cudaGetLastError()));
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -534,7 +565,10 @@ int modes_pool_resolve(modes_pool *p, const uint32_t *receivers, size_t n, const
 // device: the buffers are device memory of cfg.device (modes_pool_submit_device), read in place by the same
 // launches, and the 2 MHz pairs are filled by the gather launch; the staging area holds only the 16-bit
 // 2.4 MS/s receivers' converted bytes.
-static int submit(modes_pool *p, const uint32_t *receivers, const uint8_t *const *iq, size_t n, bool device) {
+//
+// eof (modes_pool_finish's batches, else nullptr): per listed receiver, the pair its staged tail makes.
+static int submit(modes_pool *p, const uint32_t *receivers, const uint8_t *const *iq, size_t n, bool device,
+                  const EofPair *eof = nullptr) {
     namespace input = modes::input;
     using Feed = Receiver::Feed;
     if (!p) return -1;
@@ -550,10 +584,14 @@ static int submit(modes_pool *p, const uint32_t *receivers, const uint8_t *const
             const std::string no = modes::device_input_refusal(iq[i], p->cfg.device, "pool", "modes_pool_submit");
             if (!no.empty()) return fail(p, "modes_pool_submit_device: receiver %u: %s", receivers[i], no.c_str());
         }
+    const char *call = device ? "modes_pool_submit_device" : "modes_pool_submit";
+    for (size_t i = 0; i < n; i++)
+        if (p->rx[receivers[i]].finished)
+            return fail(p, "%s: receiver %u after modes_pool_finish; call modes_pool_reset first", call, receivers[i]);
     for (size_t i = 0; i < n; i++)
         if (p->rx[receivers[i]].feed == (device ? Feed::host : Feed::device))
             return fail(p, "%s: receiver %u has a stream fed from %s memory in progress; call modes_pool_reset first",
-                        device ? "modes_pool_submit_device" : "modes_pool_submit", receivers[i], device ? "host" : "device");
+                        call, receivers[i], device ? "host" : "device");
     if (ensure_device(p, !device)) return -1;
     modes_pool::Slot &sl = p->slot[p->submitted & 1];
     if (sl.busy) return fail(p, "two batches are in flight: modes_pool_collect first");
@@ -593,6 +631,7 @@ static int submit(modes_pool *p, const uint32_t *receivers, const uint8_t *const
     size_t n_pairs = 0, n_rj = 0, n_hist = 0, n_conv = 0, n_gather = 0;
     uint64_t hist_max = 0;
     bool carries = false;
+    Spans fill_in, fill_out;                   // a finish batch's padding after the conversion / the resampling
     sl.iq8.clear();
     sl.iq16.clear();
     if (!device)
@@ -600,9 +639,12 @@ static int submit(modes_pool *p, const uint32_t *receivers, const uint8_t *const
     size_t n_stage = sl.iq8.size();
     sl.ids.clear();
     sl.buf_index.clear();
+    sl.samples.clear();
     for (size_t i = 0, k8 = 0; i < n; i++) {
         Receiver &r = p->rx[receivers[i]];
         const bool uc8 = r.format == input::kUC8;
+        const EofPair *e = eof && eof[i].buffer >= 0 ? &eof[i] : nullptr;
+        const int64_t buffer = e ? e->buffer : r.submitted;   // the 2 MHz buffer of its pair, if it gets one
         uint8_t *data = sl.d_batch.get() + (2 * n_pairs + 1) * kBuf;    // the data buffer of its pair, if it gets one
         // staged: where its call's UC8 bytes are staged (none for a 16-bit 2 MHz receiver, converted into its pair);
         // device-fed: only a 16-bit 2.4 MS/s receiver's
@@ -614,6 +656,7 @@ static int submit(modes_pool *p, const uint32_t *receivers, const uint8_t *const
             const uint8_t *in16 = device ? iq[i] : sl.d_stage16.get() + n_conv * 2 * kBuf;
             sl.h_cjobs[n_conv] = modes::PoolConvertJob{in16, stage ? stage : data, r.shift};
             n_conv++;
+            if (e && e->real8 < kBuf) fill_in.emplace_back((stage ? stage : data) + e->real8, kBuf - e->real8);
         }
         bool pair = true;
         if (r.rate == kRate2M && device) {
@@ -630,22 +673,27 @@ static int submit(modes_pool *p, const uint32_t *receivers, const uint8_t *const
                     cudaGetLastError();
                     return fail(p, "out of memory for the input history of receiver %u", receivers[i]);
                 }
-            const RatePlan pl = rate_plan(r);
+            // a finish batch's pair reads the history as it is and leaves it so: no history step
+            const RatePlan pl = e ? RatePlan{true, r.hist0} : rate_plan(r);
             pair = pl.completes;
             if (pair)
-                rj[n_rj++] = modes::PoolResampleJob{r.hist[r.cur].get(), in8, r.hist0, r.in_total, r.submitted * kBufSamples,
+                rj[n_rj++] = modes::PoolResampleJob{r.hist[r.cur].get(), in8, r.hist0, r.in_total, buffer * kBufSamples,
                                                     data - MODES_CARRY_BYTES, data};
-            const uint64_t bytes = (uint64_t)(r.in_total + (int64_t)kBuf - pl.keep);
-            if (bytes > kHistBytes)
-                return fail(p, "internal: 2.4 MS/s input history of %llu bytes for receiver %u", (unsigned long long)bytes, receivers[i]);
-            hj[n_hist++] = modes::PoolHistoryJob{r.hist[r.cur].get(), in8, r.hist0, r.in_total, pl.keep, r.hist[r.cur ^ 1].get()};
-            if (bytes > hist_max) hist_max = bytes;
+            if (e && e->out_real < kBuf) fill_out.emplace_back(data + e->out_real, kBuf - e->out_real);
+            if (!e) {
+                const uint64_t bytes = (uint64_t)(r.in_total + (int64_t)kBuf - pl.keep);
+                if (bytes > kHistBytes)
+                    return fail(p, "internal: 2.4 MS/s input history of %llu bytes for receiver %u", (unsigned long long)bytes, receivers[i]);
+                hj[n_hist++] = modes::PoolHistoryJob{r.hist[r.cur].get(), in8, r.hist0, r.in_total, pl.keep, r.hist[r.cur ^ 1].get()};
+                if (bytes > hist_max) hist_max = bytes;
+            }
         }
         if (!pair) continue;
-        if (spectra) sl.h_sjobs[n_pairs] = spectrum_job(r, r.submitted, data, in8);
+        if (spectra) sl.h_sjobs[n_pairs] = spectrum_job(r, buffer, data, in8);
         n_pairs++;
         sl.ids.push_back(receivers[i]);
-        sl.buf_index.push_back(r.submitted);
+        sl.buf_index.push_back(buffer);
+        sl.samples.push_back(e ? e->samples : (uint32_t)kBufSamples);
     }
 
     cudaStream_t st = static_cast<cudaStream_t>(modes_stream(sl.ctx));
@@ -658,11 +706,13 @@ static int submit(modes_pool *p, const uint32_t *receivers, const uint8_t *const
                                        cudaMemcpyHostToDevice, st) != cudaSuccess))
             return fail(p, "job upload failed: %s", cudaGetErrorString(cudaGetLastError()));
         modes::launch_convert_pool(sl.d_cjobs.get(), (uint32_t)n_conv, st);
+        if (fill_no_signal(p, fill_in, st)) return -1;
         // the other batch in flight may name the same receivers: its carries, reads and history step first
         if (other.rate_recorded && cudaStreamWaitEvent(st, other.rate_done, 0) != cudaSuccess)
             return fail(p, "stream wait failed: %s", cudaGetErrorString(cudaGetLastError()));
         modes::launch_gather_pool(sl.d_gjobs.get(), (uint32_t)n_gather, st);
         modes::launch_resample_pool(sl.d_jobs.resample(), (uint32_t)n_rj, st);
+        if (fill_no_signal(p, fill_out, st)) return -1;
         modes::launch_history_pool(sl.d_jobs.history(), (uint32_t)n_hist, hist_max, st);
     } else if (!staged) {
         if (upload_carries(p, sl, st, n_pairs) || upload_buffers(p, st, iq, n, sl.d_batch.get() + kBuf, 2 * kBuf, kBuf)) return -1;
@@ -678,10 +728,12 @@ static int submit(modes_pool *p, const uint32_t *receivers, const uint8_t *const
             return fail(p, "job upload failed: %s", cudaGetErrorString(cudaGetLastError()));
         // the conversion writes only this slot's pairs and staging area: it need not wait for the other slot
         modes::launch_convert_pool(sl.d_cjobs.get(), (uint32_t)n_conv, st);
+        if (fill_no_signal(p, fill_in, st)) return -1;
         // the other batch in flight may name the same receivers: its reads and its history step first
         if (other.rate_recorded && cudaStreamWaitEvent(st, other.rate_done, 0) != cudaSuccess)
             return fail(p, "stream wait failed: %s", cudaGetErrorString(cudaGetLastError()));
         modes::launch_resample_pool(sl.d_jobs.resample(), (uint32_t)n_rj, st);
+        if (fill_no_signal(p, fill_out, st)) return -1;
         modes::launch_history_pool(sl.d_jobs.history(), (uint32_t)n_hist, hist_max, st);
     }
     // the spectra read the histories too: before rate_done, after which the other slot's history step may
@@ -697,6 +749,10 @@ static int submit(modes_pool *p, const uint32_t *receivers, const uint8_t *const
     for (size_t i = 0; i < n; i++) {
         Receiver &r = p->rx[receivers[i]];
         r.feed = device ? Feed::device : Feed::host;
+        if (eof && eof[i].buffer >= 0) {       // a finish batch: the stream ends after it
+            r.submitted = eof[i].buffer + 1;
+            continue;
+        }
         if (r.rate == kRate2M) {
             r.submitted++;
             if (device) continue;              // its carry is on the device
@@ -746,6 +802,7 @@ int modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user) {
         for (size_t i = 0; i < n; i++) {
             modes_level r = sl.level_out[i];
             r.buffer = sl.buf_index[i];
+            r.n_samples = sl.samples[i];
             p->rx[sl.ids[i]].levels.push(r);
         }
     }
@@ -777,6 +834,169 @@ int modes_pool_ingest_device(modes_pool *p, const uint32_t *receivers, const voi
     return modes_pool_collect(p, sink, user);
 }
 
+}  // extern "C"
+
+namespace {
+
+// The end of a receiver's stream (modes_pool_finish), tests/pool_finish_model.py.  At 2 MHz as modes_finish ends
+// one: a tail of a whole buffer is an ordinary buffer (batch 1), the rest of it the EOF buffer, r.submitted or the
+// one after.  At 2.4 MS/s by finish_held's rule: the whole stream has n_in = in_total / 2 + the tail's samples
+// (ceil(bytes / 2) UC8, floor(bytes / 4) 16-bit) and N_out = ceil(5 n_in / 6), so buffer N_out / B is the EOF
+// buffer and the buffers before it from r.submitted are whole: at most one, the buffer whose filter lookahead
+// had not arrived.
+struct FinishPlan {
+    bool whole;                                // batch 1: buffer r.submitted, whole
+    bool eof;                                  // batch 2: the EOF buffer (not with drop_eof_buffer)
+    EofPair pair;                              // batch 2's pair
+    size_t staged;                             // the tail bytes staged (at 2 MHz a whole tail goes to batch 1 as it is)
+};
+FinishPlan finish_plan(const Receiver &r, size_t tail, bool drop) {
+    const bool uc8 = r.format == modes::input::kUC8;
+    auto samples_of = [uc8](size_t bytes) { return uc8 ? ((int64_t)bytes + 1) / 2 : (int64_t)bytes / 4; };
+    FinishPlan f;
+    f.eof = !drop;
+    if (r.rate == kRate2M) {
+        f.whole = tail == (uc8 ? kBuf : 2 * kBuf);
+        f.staged = f.whole ? 0 : tail;
+        f.pair.buffer = r.submitted + (f.whole ? 1 : 0);
+        f.pair.samples = (uint32_t)samples_of(f.staged);
+    } else {
+        const int64_t n_out = modes::resample::n_out(r.in_total / 2 + samples_of(tail));
+        f.pair.buffer = n_out / kBufSamples;
+        f.whole = f.pair.buffer > r.submitted;
+        f.staged = tail;
+        f.pair.samples = (uint32_t)(n_out - f.pair.buffer * kBufSamples);
+    }
+    // the staged buffer's real UC8 bytes (a 16-bit tail's once converted; a trailing odd UC8 byte is an I whose Q,
+    // the padding, is 127) and the EOF pair's real output bytes
+    f.pair.real8 = 2 * (size_t)samples_of(f.staged);
+    f.pair.out_real = 2 * (size_t)f.pair.samples;
+    return f;
+}
+
+}  // namespace
+
+static int finish_batches(modes_pool *p, const uint32_t *receivers, const uint8_t *const *tails, const size_t *tail_bytes,
+                          size_t n, bool device, modes_pool_sink_fn sink, void *user);
+
+static int finish(modes_pool *p, const uint32_t *receivers, const uint8_t *const *tails, const size_t *tail_bytes,
+                  size_t n, bool device, modes_pool_sink_fn sink, void *user) {
+    using Feed = Receiver::Feed;
+    const char *call = device ? "modes_pool_finish_device" : "modes_pool_finish";
+    if (!p) return -1;
+    if (p->collected != p->submitted) return fail(p, "%s: a submitted batch is in flight: modes_pool_collect first", call);
+    if (check_ids(p, receivers, n)) return -1;
+    if (!n) return 0;
+    if (!tails || !tail_bytes) return fail(p, "%s: no tails", call);
+    size_t staging = 0;
+    for (size_t i = 0; i < n; i++) {
+        const Receiver &r = p->rx[receivers[i]];
+        const size_t full = r.format == modes::input::kUC8 ? kBuf : 2 * kBuf;
+        if (r.finished) return fail(p, "%s: receiver %u after modes_pool_finish; call modes_pool_reset first", call, receivers[i]);
+        if (tail_bytes[i] > full)
+            return fail(p, "%s: receiver %u: a tail of %zu bytes, more than its buffer of %zu", call, receivers[i], tail_bytes[i], full);
+        if (r.feed == (device ? Feed::host : Feed::device))
+            return fail(p, "%s: receiver %u has a stream fed from %s memory in progress; call modes_pool_reset first", call,
+                        receivers[i], device ? "host" : "device");
+        if (!tail_bytes[i]) continue;
+        if (!tails[i]) return fail(p, "%s: receiver %u: null pointer with %zu bytes", call, receivers[i], tail_bytes[i]);
+        if (!device) continue;
+        if (reinterpret_cast<uintptr_t>(tails[i]) & 15)
+            return fail(p, "%s: receiver %u: the tail at %p is not 16-byte aligned", call, receivers[i],
+                        static_cast<const void *>(tails[i]));
+        const std::string no = modes::device_input_refusal(tails[i], p->cfg.device, "pool", "modes_pool_finish");
+        if (!no.empty()) return fail(p, "%s: receiver %u: %s", call, receivers[i], no.c_str());
+    }
+    for (size_t i = 0; i < n; i++) staging += p->rx[receivers[i]].format == modes::input::kUC8 ? kBuf : 2 * kBuf;
+    if (ensure_device(p, !device)) return -1;
+    if (device ? p->d_tails.ensure(staging) != cudaSuccess : p->h_tails.ensure(staging) != cudaSuccess) return out_of_memory(p);
+
+    const int rc = finish_batches(p, receivers, tails, tail_bytes, n, device, sink, user);
+    // every listed receiver's stream has ended, whether or not its last buffers could be decoded
+    for (size_t i = 0; i < n; i++) p->rx[receivers[i]].finished = true;
+    return rc;
+}
+
+// The tails staged and decoded (checked by finish).
+static int finish_batches(modes_pool *p, const uint32_t *receivers, const uint8_t *const *tails, const size_t *tail_bytes,
+                          size_t n, bool device, modes_pool_sink_fn sink, void *user) {
+    const char *call = device ? "modes_pool_finish_device" : "modes_pool_finish";
+    std::vector<FinishPlan> plan(n);
+    std::vector<const uint8_t *> staged(n);
+    for (size_t i = 0; i < n; i++) {
+        const Receiver &r = p->rx[receivers[i]];
+        plan[i] = finish_plan(r, tail_bytes[i], p->cfg.drop_eof_buffer != 0);
+        if (plan[i].pair.buffer > r.submitted + 1)
+            return fail(p, "internal: receiver %u: a finish of buffers %lld to %lld", receivers[i], (long long)r.submitted,
+                        (long long)plan[i].pair.buffer);
+    }
+    // Each tail into a whole buffer of its format, padded with 127: the pool's launches load whole buffers.
+    cudaStream_t st = static_cast<cudaStream_t>(modes_stream(p->slot[p->submitted & 1].ctx));
+    for (size_t i = 0, at = 0; i < n; i++) {
+        const size_t full = p->rx[receivers[i]].format == modes::input::kUC8 ? kBuf : 2 * kBuf, t = plan[i].staged;
+        if (device) {
+            uint8_t *d = p->d_tails.get() + at;
+            if ((t && cudaMemcpyAsync(d, tails[i], t, cudaMemcpyDeviceToDevice, st) != cudaSuccess) ||
+                cudaMemsetAsync(d + t, 127, full - t, st) != cudaSuccess)
+                return fail(p, "%s: staging the tails failed: %s", call, cudaGetErrorString(cudaGetLastError()));
+            staged[i] = d;
+        } else {
+            uint8_t *h = p->h_tails.get() + at;
+            if (t) memcpy(h, tails[i], t);
+            memset(h + t, 127, full - t);
+            staged[i] = h;
+        }
+        at += full;
+    }
+    if (device && cudaStreamSynchronize(st) != cudaSuccess)
+        return fail(p, "%s: staging the tails failed: %s", call, cudaGetErrorString(cudaGetLastError()));
+
+    // Batch 1, the whole buffers: a 2 MHz receiver's tail as an ordinary buffer, a 2.4 MS/s receiver's buffer
+    // r.submitted from its staged tail.  Batch 2, the EOF buffers.  Each keeps one pair per receiver and batch.
+    std::vector<uint32_t> ids;
+    std::vector<const uint8_t *> iq;
+    std::vector<EofPair> pairs;
+    for (int batch = 1; batch <= 2; batch++) {
+        ids.clear(); iq.clear(); pairs.clear();
+        for (size_t i = 0; i < n; i++) {
+            const Receiver &r = p->rx[receivers[i]];
+            const FinishPlan &f = plan[i];
+            if (batch == 1 ? !f.whole : !f.eof) continue;
+            ids.push_back(receivers[i]);
+            if (batch == 2) {
+                iq.push_back(staged[i]);
+                pairs.push_back(f.pair);
+            } else if (r.rate == kRate2M) {
+                iq.push_back(tails[i]);
+                pairs.push_back(EofPair());
+            } else {
+                EofPair e = f.pair;
+                e.buffer = r.submitted;
+                e.out_real = kBuf;
+                e.samples = (uint32_t)kBufSamples;
+                iq.push_back(staged[i]);
+                pairs.push_back(e);
+            }
+        }
+        if (ids.empty()) continue;
+        if (submit(p, ids.data(), iq.data(), ids.size(), device, pairs.data())) return -1;
+        if (modes_pool_collect(p, sink, user)) return -1;
+    }
+    return 0;
+}
+
+extern "C" {
+
+int modes_pool_finish(modes_pool *p, const uint32_t *receivers, const uint8_t *const *tails, const size_t *tail_bytes,
+                      size_t n, modes_pool_sink_fn sink, void *user) {
+    return finish(p, receivers, tails, tail_bytes, n, false, sink, user);
+}
+
+int modes_pool_finish_device(modes_pool *p, const uint32_t *receivers, const void *const *d_tails,
+                             const size_t *tail_bytes, size_t n, modes_pool_sink_fn sink, void *user) {
+    return finish(p, receivers, reinterpret_cast<const uint8_t *const *>(d_tails), tail_bytes, n, true, sink, user);
+}
+
 int modes_pool_stats(const modes_pool *p, uint32_t receiver, modes_stats *out) {
     if (!p || receiver >= p->rx.size() || !out) return -1;
     memcpy(out->v, p->rx[receiver].rs.stats, sizeof(out->v));
@@ -794,6 +1014,7 @@ int modes_pool_reset(modes_pool *p, uint32_t receiver) {
     r.spectra.clear();
     memset(r.carry, 127, sizeof r.carry);
     r.feed = Receiver::Feed::none;             // its device carry is not read again: the next buffer is a first
+    r.finished = false;
     r.rs.reset();
     return 0;
 }
@@ -804,7 +1025,7 @@ int modes_pool_set_input_rate(modes_pool *p, uint32_t receiver, uint32_t hz) {
         return fail(p, "modes_pool_set_input_rate: %u samples/s is not supported (2000000 or 2400000)", hz);
     if (receiver >= p->rx.size()) return fail(p, "receiver %u out of range (%zu receivers)", receiver, p->rx.size());
     Receiver &r = p->rx[receiver];
-    if (r.submitted || r.in_total)
+    if (r.submitted || r.in_total || r.finished)
         return fail(p, "modes_pool_set_input_rate: receiver %u has a stream in progress; call modes_pool_reset first", receiver);
     r.rate = hz;
     return 0;
@@ -823,7 +1044,7 @@ int modes_pool_set_input_format(modes_pool *p, uint32_t receiver, uint32_t forma
         return fail(p, "modes_pool_set_input_format: shift %d is not supported with UC8 (0, or negative)", (int)shift);
     if (receiver >= p->rx.size()) return fail(p, "receiver %u out of range (%zu receivers)", receiver, p->rx.size());
     Receiver &r = p->rx[receiver];
-    if (r.submitted || r.in_total)
+    if (r.submitted || r.in_total || r.finished)
         return fail(p, "modes_pool_set_input_format: receiver %u has a stream in progress; call modes_pool_reset first", receiver);
     r.format = format;
     r.shift = shift < 0 ? input::default_shift(format) : (int)shift;

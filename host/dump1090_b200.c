@@ -53,6 +53,12 @@
  * receiver's tuning error; carrier_summary in dump1090_b200/api.py is the same computation).  It combines with
  * every --sample-rate, --iformat, --input-offset and output mode and leaves stdout as it is; the device
  * resolve has no room for it, so it is refused together with --gpu-resolve.
+ * --pool decodes every --ifile (given once per file) at once, each as one receiver of a receiver pool
+ * (modes_pool_*: one buffer of every file per batch, each file finished with its tail by modes_pool_finish),
+ * and prints exactly what one run per file prints, file by file in command-line order.  It takes the text
+ * outputs (the default, --raw, --onlyaddr), --stats, --no-fix, --no-crc-check, --aggressive,
+ * --drop-eof-buffer, --sample-rate 2000000 or 2400000, --iformat, --iformat-shift and --device; every other
+ * option, and --ifile - (stdin), is refused with it.  Without --pool a repeated --ifile means the last one.
  * The live-radio, networking and interactive options are out of scope.
  */
 #include <math.h>
@@ -222,6 +228,103 @@ static void on_message(void *user, const modes_message *mm) {
     if (opt_raw) return;
 }
 
+/* The reference's --stats lines (dump1090.c:2993-3006). */
+static void print_stats(const modes_stats *st) {
+    printf("%lld valid preambles\n", (long long)st->v[0]);
+    printf("%lld demodulated again after phase correction\n", (long long)st->v[1]);
+    printf("%lld demodulated with zero errors\n", (long long)st->v[2]);
+    printf("%lld with good crc\n", (long long)st->v[3]);
+    printf("%lld with bad crc\n", (long long)st->v[4]);
+    printf("%lld errors corrected\n", (long long)st->v[5]);
+    printf("%lld single bit errors\n", (long long)st->v[6]);
+    printf("%lld two bits errors\n", (long long)st->v[7]);
+    printf("%lld total usable messages\n", (long long)(st->v[3] + st->v[5]));
+}
+
+/* --pool: each file's lines, held until every file is done */
+static struct text { char *v; size_t n, cap; } *pool_text;
+
+static void on_pool_message(void *user, uint32_t receiver, const modes_message *mm) {
+    (void)user;
+    if (opt_stats) return;                                  /* dump1090.c:1803 */
+    char line[2048];
+    size_t n = 0;
+    if (opt_onlyaddr) n = (size_t)snprintf(line, sizeof(line), "%02x%02x%02x\n", mm->aa1, mm->aa2, mm->aa3);
+    else if (!opt_raw) {
+        n = modes_format_message(mm, opt_check_crc, line, sizeof(line));
+        if (n >= sizeof(line)) n = sizeof(line) - 1;
+    } else {
+        line[n++] = '*';
+        for (int j = 0; j < mm->msgbits / 8; j++) n += (size_t)snprintf(line + n, sizeof(line) - n, "%02x", mm->msg[j]);
+        line[n++] = ';';
+        line[n++] = '\n';
+    }
+    struct text *t = &pool_text[receiver];
+    if (t->n + n > t->cap) {
+        const size_t cap = 2 * (t->n + n) + 4096;
+        char *v = (char *)realloc(t->v, cap);
+        if (!v) { fprintf(stderr, "out of memory\n"); exit(1); }
+        t->v = v; t->cap = cap;
+    }
+    memcpy(t->v + t->n, line, n);
+    t->n += n;
+}
+
+/* --pool: every file one receiver, fed one buffer per file and call, then finished with its tail. */
+static int run_pool(const modes_config *cfg, char **files, size_t n, uint32_t rate, uint32_t format, int32_t shift) {
+    const size_t full = (size_t)MODES_BUFFER_BYTES * (format == MODES_INPUT_UC8 ? 1 : 2);
+    FILE **f = (FILE **)calloc(n, sizeof(FILE *));
+    if (!f) { fprintf(stderr, "out of memory\n"); return 1; }
+    for (size_t i = 0; i < n; i++) {
+        f[i] = fopen(files[i], "rb");
+        if (!f[i]) { perror("Opening data file"); return 1; }
+    }
+    size_t *tail = (size_t *)calloc(n, sizeof(size_t));
+    uint32_t *ids = (uint32_t *)malloc(n * sizeof(uint32_t));
+    const uint8_t **iq = (const uint8_t **)malloc(n * sizeof(uint8_t *));
+    int *done = (int *)calloc(n, sizeof(int));
+    pool_text = (struct text *)calloc(n, sizeof(struct text));
+    unsigned char *bufs = (unsigned char *)modes_host_alloc(n * full);
+    unsigned char *tails = (unsigned char *)malloc(n * full);
+    if (!tail || !ids || !iq || !done || !pool_text || !bufs || !tails) { fprintf(stderr, "out of memory\n"); return 1; }
+    modes_pool *p = modes_pool_create(cfg, n, n);
+    if (!p) { fprintf(stderr, "modes_pool_create failed\n"); return 1; }
+    for (uint32_t i = 0; i < n; i++) {
+        if (modes_pool_set_input_rate(p, i, rate)) { fprintf(stderr, "--sample-rate: %s\n", modes_pool_last_error(p)); return 1; }
+        if (modes_pool_set_input_format(p, i, format, shift)) { fprintf(stderr, "--iformat: %s\n", modes_pool_last_error(p)); return 1; }
+    }
+    for (;;) {
+        size_t k = 0;
+        for (uint32_t i = 0; i < n; i++) {
+            if (done[i]) continue;
+            unsigned char *b = bufs + k * full;
+            const size_t got = fread(b, 1, full, f[i]);
+            if (got == full) { ids[k] = i; iq[k++] = b; continue; }
+            memcpy(tails + i * full, b, got);                  /* a short read: the file's tail */
+            tail[i] = got;
+            done[i] = 1;
+        }
+        if (!k) break;
+        if (modes_pool_ingest(p, ids, iq, k, on_pool_message, NULL)) { fprintf(stderr, "modes_pool_ingest: %s\n", modes_pool_last_error(p)); return 1; }
+    }
+    for (uint32_t i = 0; i < n; i++) { ids[i] = i; iq[i] = tails + i * full; }
+    if (modes_pool_finish(p, ids, iq, tail, n, on_pool_message, NULL)) { fprintf(stderr, "modes_pool_finish: %s\n", modes_pool_last_error(p)); return 1; }
+    for (uint32_t i = 0; i < n; i++) {
+        fwrite(pool_text[i].v, 1, pool_text[i].n, stdout);
+        if (opt_stats) {
+            modes_stats st;
+            modes_pool_stats(p, i, &st);
+            print_stats(&st);
+        }
+        free(pool_text[i].v);
+        fclose(f[i]);
+    }
+    modes_pool_destroy(p);
+    modes_host_free(bufs);
+    free(tails); free(pool_text); free(done); free(iq); free(ids); free(tail); free(f);
+    return 0;
+}
+
 int main(int argc, char **argv) {
     modes_config cfg;
     const char *filename = NULL;
@@ -230,10 +333,22 @@ int main(int argc, char **argv) {
     const char *iformat = "UC8";
     const char *iformat_shift = NULL;
     const char *input_offset = NULL;
+    int opt_pool = 0;
+    const char *pool_refused = NULL;                        /* the first option --pool does not take */
+    char **files = (char **)malloc((size_t)argc * sizeof(char *));
+    size_t n_files = 0;
+    if (!files) { fprintf(stderr, "out of memory\n"); return 1; }
     modes_default_config(&cfg);
     for (int j = 1; j < argc; j++) {
         int more = j + 1 < argc;
-        if (!strcmp(argv[j], "--ifile") && more) filename = argv[++j];
+        if (!pool_refused && (!strcmp(argv[j], "--sbs") || !strcmp(argv[j], "--aircraft-json") || !strcmp(argv[j], "--beast") ||
+                              !strcmp(argv[j], "--arrival") || !strcmp(argv[j], "--levels") || !strcmp(argv[j], "--spectrum") ||
+                              !strcmp(argv[j], "--carrier") || !strcmp(argv[j], "--recover") ||
+                              !strcmp(argv[j], "--recover-weak") || !strcmp(argv[j], "--gpu-resolve") ||
+                              !strcmp(argv[j], "--gpus") || !strcmp(argv[j], "--chunk") || !strcmp(argv[j], "--input-offset")))
+            pool_refused = argv[j];
+        if (!strcmp(argv[j], "--ifile") && more) filename = files[n_files++] = argv[++j];
+        else if (!strcmp(argv[j], "--pool")) opt_pool = 1;
         else if (!strcmp(argv[j], "--raw")) opt_raw = 1;
         else if (!strcmp(argv[j], "--onlyaddr")) opt_onlyaddr = 1;
         else if (!strcmp(argv[j], "--no-fix")) cfg.fix_errors = 0;
@@ -264,6 +379,22 @@ int main(int argc, char **argv) {
         }
     }
     if (!filename) { fprintf(stderr, "--ifile <filename> is required (use '-' for stdin)\n"); return 1; }
+    if (opt_pool) {
+        if (pool_refused) {
+            fprintf(stderr, "--pool cannot be combined with %s: it takes the text outputs, --stats, --no-fix, --no-crc-check, "
+                            "--aggressive, --drop-eof-buffer, --sample-rate, --iformat, --iformat-shift and --device\n", pool_refused);
+            return 1;
+        }
+        for (size_t i = 0; i < n_files; i++)
+            if (!strcmp(files[i], "-")) {
+                fprintf(stderr, "--pool decodes files: --ifile - (stdin) cannot be combined with --pool\n");
+                return 1;
+            }
+        if (sample_rate != 2000000 && sample_rate != 2400000) {
+            fprintf(stderr, "--pool takes --sample-rate 2000000 or 2400000\n");
+            return 1;
+        }
+    }
     if (sample_rate != 2000000 && sample_rate != 2400000 && sample_rate != 4000000 && sample_rate != 6000000 &&
         sample_rate != 8000000 && sample_rate != 10000000) {
         fprintf(stderr, "--sample-rate takes 2000000, 2400000, 4000000, 6000000, 8000000 or 10000000\n");
@@ -322,6 +453,12 @@ int main(int argc, char **argv) {
         fprintf(stderr, "--carrier cannot be combined with --gpu-resolve: the device resolve's delivery records have no room for it\n");
         return 1;
     }
+    if (opt_pool) {
+        const int rc = run_pool(&cfg, files, n_files, (uint32_t)sample_rate, format, shift);
+        free(files);
+        return rc;
+    }
+    free(files);
     FILE *f = (filename[0] == '-' && filename[1] == 0) ? stdin : fopen(filename, "rb");
     if (!f) { perror("Opening data file"); return 1; }
 
@@ -357,15 +494,7 @@ int main(int argc, char **argv) {
     if (opt_stats) {                                        /* dump1090.c:2993-3006 */
         modes_stats st;
         modes_get_stats(ctx, &st);
-        printf("%lld valid preambles\n", (long long)st.v[0]);
-        printf("%lld demodulated again after phase correction\n", (long long)st.v[1]);
-        printf("%lld demodulated with zero errors\n", (long long)st.v[2]);
-        printf("%lld with good crc\n", (long long)st.v[3]);
-        printf("%lld with bad crc\n", (long long)st.v[4]);
-        printf("%lld errors corrected\n", (long long)st.v[5]);
-        printf("%lld single bit errors\n", (long long)st.v[6]);
-        printf("%lld two bits errors\n", (long long)st.v[7]);
-        printf("%lld total usable messages\n", (long long)(st.v[3] + st.v[5]));
+        print_stats(&st);
         if (opt_recover) {
             modes_recovery_stats rs;
             modes_get_recovery_stats(ctx, &rs);

@@ -262,7 +262,8 @@ int  modes_set_input_offset(modes_ctx *ctx, int32_t offset_hz);
  * delivers nothing and is still collected.  modes_pool_buffers counts the 2 MHz buffers decoded, and the
  * receiver's messages, sample_pos (2 MHz samples), statistics and level records (their buffer index a
  * 2 MHz buffer's) equal those of the 2 MHz decode, without the EOF buffer, of the first
- * modes_pool_buffers buffers of the receiver's resampled stream, with every switch.  The pool's device
+ * modes_pool_buffers buffers of the receiver's resampled stream, with every switch, until
+ * modes_pool_finish ends the stream with the buffers whose lookahead never arrives and the EOF buffer.  The pool's device
  * memory grows by a staging area (2 x 256 KiB per receiver of a batch) and about 1.1 MiB of input
  * history per 2.4 MS/s receiver. */
 typedef struct modes_pool modes_pool;                /* the receiver pool: "many receivers on one GPU" below */
@@ -564,6 +565,35 @@ int  modes_pool_collect(modes_pool *p, modes_pool_sink_fn sink, void *user);
 int  modes_pool_submit_device(modes_pool *p, const uint32_t *receivers, const void *const *d_iq, size_t n);
 int  modes_pool_ingest_device(modes_pool *p, const uint32_t *receivers, const void *const *d_iq, size_t n,
                               modes_pool_sink_fn sink, void *user);
+/* Ends the streams of the listed receivers: tails[i] holds tail_bytes[i] more bytes of receiver receivers[i]'s
+ * stream (0 up to its buffer size: MODES_BUFFER_BYTES for a UC8 receiver, twice that for a 16-bit one), after
+ * which its stream ends as modes_finish ends one.  A finite capture of any length is fed as its whole buffers
+ * (modes_pool_submit / _ingest) and then its tail; a capture shorter than one buffer is a tail alone.
+ *   Same output: after it, everything the pool has delivered for a receiver (messages and every field,
+ *     sample_pos, signal, arrival and carrier, statistics, recovery and weak statistics, level and spectrum
+ *     records, modes_pool_buffers) equals modes_process + modes_finish of a single-stream context with the same
+ *     modes_config, rate, format, shift and switches on all the bytes the receiver was given.  cfg.drop_eof_buffer
+ *     takes effect here: the EOF buffer is decoded (127 past the stream's end, its level record counting the real
+ *     samples only) unless it is set.
+ *   Synchronous, like modes_pool_ingest, and refused while a submitted batch is in flight.  It runs as at most
+ *     two batches: first the whole 2 MHz buffers the tails complete (at 2 MHz a tail of a whole buffer, at
+ *     2.4 MS/s the buffer whose filter lookahead had not arrived), then the EOF buffers.  Messages go to the sink
+ *     and the output array batch by batch, each batch's in list order; each receiver's are in its stream order.
+ *   Refused as modes_pool_ingest refuses (a receiver out of range or listed twice, more than max_batch
+ *     receivers, a receiver fed from the other kind of memory), and for a tail longer than the receiver's buffer,
+ *     a NULL tail of more than 0 bytes, and a receiver already finished.  Afterwards the receiver is finished:
+ *     modes_pool_submit* and modes_pool_finish* naming it, and its rate and format setters, are refused until
+ *     modes_pool_reset starts a new stream.  A receiver never fed may be finished (a capture shorter than a buffer).
+ *   Staging: each tail is copied into a whole buffer padded with 127 (pinned host memory for modes_pool_finish,
+ *     device memory for modes_pool_finish_device, one buffer of its format per listed receiver, kept for later
+ *     calls). */
+int  modes_pool_finish(modes_pool *p, const uint32_t *receivers, const uint8_t *const *tails, const size_t *tail_bytes,
+                       size_t n, modes_pool_sink_fn sink, void *user);
+/* The same with the tails in device memory of cfg.device, for receivers fed by modes_pool_submit_device (or never
+ * fed): each is copied on the device, so it may end anywhere in its allocation; refused as a device-fed buffer is
+ * (NULL, not 16-byte aligned, not device memory of cfg.device). */
+int  modes_pool_finish_device(modes_pool *p, const uint32_t *receivers, const void *const *d_tails,
+                              const size_t *tail_bytes, size_t n, modes_pool_sink_fn sink, void *user);
 /* The host half alone, for candidate records produced elsewhere over a batch laid out as the pool lays
  * it out: buffer 2i = pad buffer of receivers[i] (no signal, last MODES_CARRY_BYTES = its carry), buffer
  * 2i+1 = its new buffer; candidates/tiles as modes_detect_fetch returns them for those 2n buffers.  The
